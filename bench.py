@@ -1,17 +1,20 @@
 #!/usr/bin/env python
-"""bench.py — SA-SSD inference hot path on B200: frames/sec on synthetic KITTI-shaped clouds.
+"""bench.py — SA-SSD inference hot path on H100: frames/sec on synthetic KITTI-shaped clouds.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the whole hot path (voxelize -> anchors_mask -> 13 sparse convs ->
 BEV neck -> heads -> guided anchors -> PSWarp -> rotated NMS) over one batch of B frames
 (default B=1 = BASELINE.json configs[1]: car_cfg.py, batch 1, ~20 k points per frame).
-Rank 0 prints ONE JSON line (see the driver contract): `value` = whole-job frames/s with
+Rank 0 prints ONE JSON line: `value` = whole-job frames/s with
 inputs resident in HBM, `e2e` = the same through the public API from host buffers (pinned
 H2D of the raw points, D2H of the detections inside the timed region), `roofline` for the
 dominant kernel, `roofline_sparse` for the 13 ruled sparse convs (pair-model bytes, SURVEY
 §8d), `cpu_baseline` = the CPU oracle port timed on the host cores.
+--dump-outputs DIR writes what the timed path returned in its last timed step (detections
+[B, det_cap, 9] with the rows past each frame's count zeroed, and the per-frame counts) as
+.npy files; inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -67,7 +70,8 @@ def load_peaks():
             d = json.load(f)
         return dict(hbm_gbs=float(d["hbm_gbs"]), bf16_tflops=float(d["bf16_tflops"]),
                     bf16_tflops_sustained=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s - not reached rates
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -229,14 +233,6 @@ def algorithmic_work(aux, batch):
     return tot_b, tot_f, pairs, exec_over_pairs, exec_chunks
 
 
-# DRAM bytes of one B=1 launch of the roofline kernel with the constant-region tile skipping ON, from the committed
-# `ncu --set full` capture profiles/r2_ncu_full_conv2d_tma.md (dram__bytes_read.sum + dram__bytes_write.sum)
-NCU_DRAM_BYTES_PER_LAUNCH = {      # launch 3 of the capture: 22 799 104 B read + 748 544 B written (cold L2, B=1)
-    "tma::conv2d_tma_kernel<128> (half-width units)": 23547648,
-    "tma::conv2d_tma_kernel<256>": 23547648,      # same layer, same tiles; not captured separately at N = 256
-}
-
-
 def profile_step(model, points, pt_off, batch, maxpts, iters=3):
     """Per-C-ABI-call CUDA-event timing of one step (events on the launching stream)."""
     from sassd_b200 import ops
@@ -322,7 +318,16 @@ def parity_check(model, sd, batches, batch, maxpts, n_frames=2):
     return res
 
 
-MIN_TIMED_S = 1.0      # the timed region repeats the K steps until it is at least this long
+def dump_outputs(out_dir, det, nd, rank, world):
+    """The timed path's results of its last step as float32 / float64 .npy files (rank-suffixed when world > 1)."""
+    os.makedirs(out_dir, exist_ok=True)
+    det = det.float().cpu().numpy().astype(np.float32)
+    nd = nd.cpu().numpy().astype(np.int64).reshape(-1)
+    for b, n in enumerate(nd):
+        det[b, max(0, min(int(n), det.shape[1])):] = 0.0      # rows past the count hold whatever a former step left
+    sfx = "" if world == 1 else "_rank%d" % rank
+    np.save(os.path.join(out_dir, "detections%s.npy" % sfx), det)
+    np.save(os.path.join(out_dir, "num_detections%s.npy" % sfx), nd.astype(np.float64))
 
 
 def run_ours(args, rank, world, local):
@@ -351,7 +356,7 @@ def run_ours(args, rank, world, local):
     for fb in batches:
         hp, ho, counts = model.stage_points(fb)
         staged.append((hp.to(dev).clone(), ho.to(dev).clone(), max(counts)))
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > the 50 MB L2
 
     maxpts = ops.next_pow2(max(max(p.shape[0] for p in fb) for fb in batches))
     graph = None
@@ -365,22 +370,18 @@ def run_ours(args, rank, world, local):
             return graph.replay() + (None,)
         return model.forward_device(p, o, B, mx)
 
-    t_est0 = time.perf_counter()
     for i in range(max(3, args.warmup)):
         det, nd, status, aux = step(i)
     torch.cuda.synchronize()
-    est_step_s = (time.perf_counter() - t_est0) / max(3, args.warmup)
     word = int(status.item())
     assert word == 0, "device status flags %s" % ops._lib.decode_flags(word)
     # the shard's single exchange step: pre-allocated, warmed before anything is timed
     gather = D.DetectionGather(det.shape[0], det.shape[1], dev)
     gather.warm()
 
-    # ---- timed region: K steps (repeated `rounds` times until >= MIN_TIMED_S), CUDA events on the launching
-    # stream around every step, L2 flushed (untimed) between steps, + the result gather, max over ranks
-    rounds = max(1, int(np.ceil(MIN_TIMED_S / max(args.steps * est_step_s, 1e-6))))
-    rounds = int(D.max_over_ranks(rounds, dev))
-    nsteps = args.steps * rounds
+    # ---- timed region: K = --steps steps, CUDA events on the launching stream around every step, L2 flushed
+    # (untimed) between steps, + the result gather, max over ranks
+    nsteps = args.steps
     sampler = ClockSampler(local)
     D.barrier(); torch.cuda.synchronize()
     sampler.start()
@@ -403,6 +404,8 @@ def run_ours(args, rank, world, local):
     torch.cuda.synchronize()
     D.barrier(); torch.cuda.synchronize()
     t_wall = time.perf_counter() - t_wall0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, det, nd, rank, world)
     clocks = sampler.stop()
     launches = (ops.LAUNCHES - l0)
     if graph is not None:      # launches are inside the captured graph: count the kernels of one eager step
@@ -469,9 +472,6 @@ def run_ours(args, rank, world, local):
         tile_counts, sp_counts = count_step(model, *staged[0][:2], B, staged[0][2])
     finally:
         _ops.CONV2D_TILE_ORDER = order0
-    tiles_map = B * 25 * 11
-    nsplit_on = args.precision == "f16x3" and tiles_map <= (_ops.CONV2D_NSPLIT_MAX_TILES if graph is not None else
-                                                             _ops.CONV2D_NSPLIT_MAX_TILES_STREAM)
     peaks = load_peaks()
     H, W = 200, 176
     dom = max(prof.items(), key=lambda kv: kv[1]["ms_total_per_step"])
@@ -487,21 +487,17 @@ def run_ours(args, rank, world, local):
         per_launch_ms = bev["ms_total_per_step"] / bev["calls_per_step"]
         ach = flops / (per_launch_ms * 1e-3) / 1e12
         peak = peaks["bf16_tflops_sustained"]
-        kname = {"fp32": "gconv_ffma_kernel<CONV2D,128,16>", "tf32x3": "tc::gconv_tc_kernel<CONV2D,256,1,TF32X3>",
-                 "mixed": "tc::gconv_tc_kernel<CONV2D,256,1,TF32X3>",
-                 "f16x3": ("tma::conv2d_tma_kernel<128> (half-width units)" if nsplit_on else "tma::conv2d_tma_kernel<256>")
+        kname = {"fp32": "gconv_ffma_kernel<CONV2D,128,16>", "tf32x3": "tc::gconv_tc_kernel<CONV2D,64,TF32X3>",
+                 "mixed": "tc::gconv_tc_kernel<CONV2D,64,TF32X3>",
+                 "f16x3": "tma::conv2d_tma_kernel<128> (two 128-channel units per tile)"
                           if bev_key.startswith("conv2d_tma") else
-                          "tc::gconv_tc_kernel<CONV2D,256,1,F16X3>"}[args.precision]
+                          "tc::gconv_tc_kernel<CONV2D,64,F16X3>"}[args.precision]
         passes = {"fp32": "fp32 FFMA (no tensor cores)", "tf32x3": "3 TF32 MMA passes per algorithmic flop",
                   "mixed": "3 TF32 MMA passes per algorithmic flop",
                   "f16x3": "3 FP16 MMA passes per algorithmic flop (ceiling 1/3 of the fp16/bf16 peak)"}[args.precision]
-        ncu_b1 = NCU_DRAM_BYTES_PER_LAUNCH.get(kname)
         roofline = dict(kernel="%s (BEVNet 3x3 256->256, %d launches/step)" % (kname, bev["calls_per_step"]),
                         bound="tensor", achieved=ach, peak=peak, unit="TFLOP/s", frac=ach / peak,
-                        traffic=(ncu_b1 * B) if ncu_b1 else None,
-                        traffic_unit="bytes per launch: dram__bytes_read.sum + dram__bytes_write.sum of the B=1 launch "
-                                     "(conv2d_tma_kernel<128>, tile skipping on, cold L2) in "
-                                     "profiles/r2_ncu_full_conv2d_tma.md, scaled by the batch",
+                        traffic=None,
                         tiles_computed=tc[0] if tc else None, tiles_total=tc[1] if tc else None,
                         tiles_computed_frac=tiles_frac,
                         peak_source="%s bf16 dense, sustained" % peaks["source"],
@@ -513,9 +509,9 @@ def run_ours(args, rank, world, local):
     sp_bytes, sp_flops, pairs, exec_over_pairs, exec_chunks = algorithmic_work(aux, B)
     sp_ms = sum(v["ms_total_per_step"] for k, v in prof.items() if k.startswith("gconv[table") or k.startswith("spconv_split[taps=27"))
     sp_kernel = {"fp32": "gconv_ffma_kernel<TABLE,...>", "mixed": "gconv_ffma_kernel<TABLE,...>"}.get(
-        args.precision, "tc::gconv_tc_kernel<TABLE,BN,1,%s>" % args.precision.upper())
+        args.precision, "tc::gconv_tc_kernel<TABLE,BN,%s>" % args.precision.upper())
     if any(k.startswith("spconv_split") for k in prof):
-        sp_kernel = ("sps::spconv_split_kernel<TABLE,BN> (cp.async gather of split fp16 rows, tap-packed tcgen05 FP16x3, "
+        sp_kernel = ("sps::spconv_split_kernel<TABLE,BN> (cp.async gather of split fp16 rows, tap-packed wgmma FP16x3, "
                      "tile-level tap skipping, 2-CTA tap split for small layers)")
     sp_ach = sp_bytes / (sp_ms * 1e-3) / 1e9 if sp_ms > 0 else 0.0
     roofline_sparse = dict(kernel=sp_kernel + " x13 ruled sparse convs", bound="hbm", achieved=sp_ach,
@@ -550,15 +546,15 @@ def run_ours(args, rank, world, local):
                           "rotated NMS)" % nsamp)
 
     line = dict(metric=METRIC, value=value, unit="frames/s", n_gpus=world, steps=args.steps, warmup=max(3, args.warmup),
-                ms_per_step=dev_ms / nsteps, steps_timed=nsteps, rounds=rounds, higher_is_better=True, scaling="weak",
+                ms_per_step=dev_ms / nsteps, steps_timed=nsteps, higher_is_better=True, scaling="weak",
                 vs_baseline=None, dtype="f32", data="synthetic", impl="ours", config=workload_config(B),
                 details=dict(weights="synthetic (seed 0, BN calibrated)",
                              l2="flushed between steps (256 MiB memset, untimed)", precision=args.precision,
                              bev_tile_skipping=bool(ops.TILE_OCCUPANCY), sparse_tap_skipping=bool(ops.SPCONV_TAP_SKIP),
                              sparse_tap_split=bool(ops.SPCONV_TAP_SPLIT), cuda_graph=graph is not None,
                              parallelism="frames sharded, dp%d" % world,
-                             timed_region="%d x %d steps (>= %.1f s), per-step CUDA events + the result all_gather "
-                                          "(%.3f ms)" % (rounds, args.steps, MIN_TIMED_S, gather_ms)),
+                             timed_region="%d steps, per-step CUDA events + the result all_gather "
+                                          "(%.3f ms)" % (nsteps, gather_ms)),
                 clocks=clocks, gpu_launches=launches,
                 e2e=dict(value=e2e, unit="frames/s", h2d_bytes_per_step=h2d, d2h_bytes_per_step=d2h,
                          api="SingleStageDetector.detect_stream (host numpy points in, numpy detections out) + the "
@@ -572,7 +568,7 @@ def run_ours(args, rank, world, local):
 
 # ------------------------------------------------------------------------------------------- reference dataflow on the GPU
 def run_reference_gpu(args, rank, world, local):
-    """Comparator, never product: the REFERENCE'S GPU DATAFLOW on this B200, built from library kernels the way the
+    """Comparator, never product: the REFERENCE'S GPU DATAFLOW on this GPU, built from library kernels the way the
     reference runs it - spconv v1.0 `indice_conv` as per-offset gather (index_select) -> SGEMM (mm) -> scatter-add
     (index_add_) with a host copy of indice_pair_num per layer, BatchNorm1d/ReLU as torch ops, `dense()`, BEVNet and the
     heads through cuDNN fp32 (TF32 off), decode / guided anchors / PSWarp (`grid_sample`) as the reference's torch ops
@@ -725,7 +721,7 @@ def run_reference_gpu(args, rank, world, local):
                 ms_per_step=1e3 * dt / done, steps_timed=done, higher_is_better=True, scaling="weak", vs_baseline=None,
                 dtype="f32", data="synthetic", impl="reference-gpu", config=workload_config(B), clocks=clocks,
                 detections=ndet,
-                note="comparator: the reference's GPU dataflow from library kernels on this B200 (torch "
+                note="comparator: the reference's GPU dataflow from library kernels on this GPU (torch "
                      "index_select/mm/index_add_ per offset, cuDNN fp32 with TF32 off, torch head ops with their syncs, the "
                      "unmodified reference NMS kernel + host sweep); rulebooks, voxels and anchor masks precomputed and "
                      "NOT timed (the reference builds rulebooks inside spconv on the GPU and the rest in DataLoader "
@@ -746,6 +742,8 @@ def main():
     ap.add_argument("--density", default="20k", choices=["5k", "10k", "20k", "40k", "80k", "120k", "mix"],
                     help="points per synthetic frame (mix = the 5k-120k sweep interleaved)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the timed path's outputs of its last timed step to DIR/<name>.npy")
     ap.add_argument("--no-parity", action="store_true", help="skip the oracle comparison of streamed frames")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel from Python instead of one CUDA graph")
     ap.add_argument("--serial-stream", action="store_true",

@@ -1,4 +1,4 @@
-/* sassd_b200 — C ABI of the B200-native SA-SSD inference hot path.
+/* sassd_b200 — C ABI of the SA-SSD inference hot path for the H100 (sm_90a).
  *
  * Drop-in boundary (DESIGN.md §Boundary, SURVEY.md §8b): these are the entry
  * points a binding of the reference's native extensions for this path would
@@ -152,7 +152,7 @@ int sassd_rulebook_pairs(const int32_t* nbr, const int32_t* d_rows_out, int rows
  * mode CONV2D: rows are pixels of a [batch,H,W] NHWC map, taps = 3x3 window, zero padding
  * mode ROWS  : taps == 1, row(m,0) = m                (1x1 convs / plain GEMM)
  * weight [taps, Cin, Cout] f32; scale/shift [Cout] (folded BatchNorm or bias); Cin % 4 == 0.
- * precision: SASSD_PREC_FP32 = CUDA-core FFMA; SASSD_PREC_TF32X3 / SASSD_PREC_F16X3 = tcgen05 tensor cores with a
+ * precision: SASSD_PREC_FP32 = CUDA-core FFMA; SASSD_PREC_TF32X3 / SASSD_PREC_F16X3 = Hopper tensor cores (wgmma) with a
  * 3-product hi/lo split of both operands (tf32: 21 bits, any range; fp16: 22 bits, |x| < 65504, 2x the MMA rate).
  * ---------------------------------------------------------------------- */
 enum { SASSD_GCONV_TABLE = 0, SASSD_GCONV_CONV2D = 1, SASSD_GCONV_ROWS = 2 };
@@ -189,10 +189,9 @@ typedef struct {
     int32_t tile_order;            /* sassd_conv2d_f16x3_occ: 0 = tiles round-robin over the CTAs (best with several steps
                                       in flight), 1 = computed tiles first, constant tiles after (best for one step at a
                                       time: no CTA gets two computed tiles while others only store constants) */
-    int32_t n_split;               /* 0 / 1 = a work unit is a whole tile (all cout channels); 2 (cout > 128 only) = a unit
-                                      is one half of a tile's output channels, N = 128 instructions: finer units for one
-                                      step at a time on maps of a few hundred tiles (B <= 4), where whole tiles quantise
-                                      badly over 148 SMs; costs a second read of the activation tile from L2 */
+    int32_t n_split;               /* accepted for ABI compatibility and ignored: a work unit is a tile and at most 128 of
+                                      its output channels (the register accumulators' budget), so cout > 128 always runs
+                                      as two units per tile */
 } sassd_conv2d_desc;
 int sassd_conv2d_f16x3(const sassd_conv2d_desc* host_desc, const void* in_split, const void* wpack, const float* scale,
                        const float* shift, float* out_f32, void* out_split, sassd_stream_t stream);

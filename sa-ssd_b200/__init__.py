@@ -1,7 +1,7 @@
-"""sassd_b200 — B200-native implementation of the SA-SSD point-cloud inference
+"""sassd_b200 — H100 (sm_90a) implementation of the SA-SSD point-cloud inference
 hot path (voxelize -> sparse 3D conv backbone -> BEV neck -> SSD rotate head ->
 PSWarp rescoring -> rotated NMS) behind the reference's mmdet.models operator
-API.  Hand-written sm_100a CUDA lives in ``csrc/`` behind the C ABI declared in
+API.  Hand-written sm_90a CUDA lives in ``csrc/`` behind the C ABI declared in
 ``include/sassd_b200.h``; this package is the host-side mirror of the reference
 interface.  Import name: ``sassd_b200`` (alias of the ``sa-ssd_b200/`` directory).
 """

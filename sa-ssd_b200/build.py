@@ -1,9 +1,9 @@
-"""Build libsassd_b200.so (all CUDA kernels + the C ABI) in-tree with nvcc for sm_100a.
+"""Build libsassd_b200.so (all CUDA kernels + the C ABI) in-tree with nvcc for sm_90a (H100).
 
     python -m sassd_b200.build [--force]
 
-nvcc cross-compiles without a GPU; the shared object is git-ignored but travels
-to the GPU box with the repo snapshot."""
+nvcc cross-compiles without a GPU; the shared object and the object files under
+build/ are build products (git-ignored)."""
 import os
 import subprocess
 import sys
@@ -12,7 +12,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsassd_b200.so")
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-diag-suppress", "550"]
 
 
@@ -50,21 +50,9 @@ def build(force=False, verbose=False):
         return obj
     with ThreadPoolExecutor(max_workers=8) as ex:
         objs = list(ex.map(cc, sources()))
-    cmd = ["nvcc", "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs
+    cmd = ["nvcc", "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs
     subprocess.check_call(cmd)
-    build_probe(force)
     return LIB
-
-
-def build_probe(force=False):
-    """tests/tools/ts_probe: the tcgen05 instruction-rate microbenchmark (measurement tool, not part of the library)."""
-    root = os.path.dirname(HERE)
-    src = os.path.join(root, "tests", "tools", "ts_probe.cu")
-    exe = src[:-3]
-    if os.path.exists(src) and (force or not os.path.exists(exe) or os.path.getmtime(exe) < os.path.getmtime(src)):
-        subprocess.check_call(["nvcc", "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-I", CSRC,
-                               src, "-o", exe])
-    return exe
 
 
 if __name__ == "__main__":

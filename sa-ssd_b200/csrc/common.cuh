@@ -1,4 +1,4 @@
-// Shared helpers for the sassd_b200 CUDA kernels (sm_100a only).
+// Shared helpers for the sassd_b200 CUDA kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -15,11 +15,24 @@ static inline int sassd_check_launch() {
 
 static inline int sassd_div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// Streaming multiprocessors of the current device (132 on an H100 SXM), queried once per process.
+static inline int sassd_num_sms() {
+    static const int n = [] {
+        int dev = 0, v = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v < 1) {
+            cudaGetLastError();
+            v = 132;
+        }
+        return v;
+    }();
+    return n;
+}
+
 // Persistent-style grid sizing: enough CTAs to cover `work` items, capped at
-// `waves` resident waves of the 148-SM part (grid-stride loops pick up the rest).
+// `ctas_per_sm` resident CTAs per SM (grid-stride loops pick up the rest).
 static inline int sassd_grid(long long work, int block, int ctas_per_sm = 8) {
     long long need = (work + block - 1) / block;
-    long long cap = 148LL * ctas_per_sm;
+    long long cap = (long long)sassd_num_sms() * ctas_per_sm;
     if (need < 1) need = 1;
     return (int)(need < cap ? need : cap);
 }

@@ -1,27 +1,21 @@
 // Dense NHWC 3x3 / 1x1 convolution + folded BatchNorm + ReLU for the BEV neck and the heads
 // (BEVNet cmn.py:233-282, SSDRotateHead ssd_rotate_head.py:218-231, PSWarpHead.convs :424-429),
-// tcgen05 FP16x3, with the activation operand moved by TMA.
+// Hopper tensor cores (wgmma) on FP16x3, with the activation operand moved by TMA.
 //
 // Why a second tensor-core kernel: in gconv_tc.cu the A operand is gathered by producer warps
-// (LDG -> split -> STS), nine times per element for a 3x3 conv; ncu shows that kernel bound by the
-// L1TEX/shared-memory pipe (85 % of peak) with the tensor pipe at 67 %.  Here
+// (LDG -> split -> STS), nine times per element for a 3x3 conv.  Here
 //   * activations live in HBM already split: two fp16 planes [2][B][H][W][C] (hi, lo*2048), written
 //     once by the epilogue of the producing layer (or by the sparse->BEV scatter);
 //   * a tile is an 8x16-pixel patch; for tap (dy,dx) and a 64-channel chunk the A operand is ONE
 //     cp.async.bulk.tensor.4d box {64 ch, 16 x, 8 y, 1} at (y0+dy, x0+dx) — TMA writes it 128B-swizzled
-//     straight into the UMMA layout and zero-fills out-of-image pixels (= the conv's zero padding);
-//   * no producer warps: warp 4 lane 0 issues the TMA boxes (A hi, A lo) and the weight bulk copies,
-//     warp 5 lane 0 issues the MMAs (one operand of each K=16 step is read once for two of the three
-//     products: weight-stationary B collector at N=256, A collector otherwise), warps 0-3 drain TMEM,
-//     stage the next layer's split planes in 64B-swizzled shared memory and write them with TMA stores.
-// The LSU / shared-memory store path is out of the main loop entirely.  Where the time goes and what was
-// tried (stale loads, CTA pairs, N=128 instructions, collectors): profiles/r1_ncu_full_conv2d_tma.md.
+//     straight into the wgmma operand layout and zero-fills out-of-image pixels (= the conv's zero padding);
+//   * no producer warps: warp 8 lane 0 issues the TMA boxes (A hi, A lo) and the weight bulk copies, two consumer
+//     warpgroups (pixel rows 0-63 / 64-127 of the tile) issue the MMAs and store the outputs from registers.
+// A work unit is a tile and up to 128 of its output channels: the two register accumulators (big, small) of a
+// 64 x 128 block are 128 floats per thread, so 256-channel layers run each tile as two units on the same weight pack.
 #include <cuda.h>
 
 #include <cstdlib>
-
-#include <cstdio>
-#include <vector>
 
 #include "tc_common.cuh"
 
@@ -32,29 +26,18 @@ using namespace tc;
 constexpr int TILE_H = SASSD_CONV2D_TILE_H, TILE_W = SASSD_CONV2D_TILE_W;   // 8 x 16 = 128 output pixels per tile
 constexpr int BKC = 64;                         // channels per chunk (one 128-byte fp16 row)
 constexpr int kConstTile = 1 << 30;             // tile reference flag: the tile only stores the layer's constant vector
-constexpr int EPI_WARPS = 4;
-constexpr int THREADS2 = (EPI_WARPS + 2) * 32;  // 192
-constexpr int WARP_LOAD = EPI_WARPS, WARP_ISSUE = EPI_WARPS + 1;
+constexpr int CONS_WARPS = CONS_THREADS / 32;   // 8
+constexpr int THREADS2 = CONS_THREADS + 32;     // + the TMA / bulk-copy issuing warp
+constexpr int W_LOAD = CONS_WARPS;
 
 template <int BN>
 struct Cfg2 {
     static constexpr int B_TILE_BYTES = BN * 128;
     static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-    static constexpr int STAGES = (BN >= 256) ? 2 : (BN >= 128 ? 3 : 4);
-    static constexpr int ACC_BUFS = (4 * BN <= 512) ? 2 : 1;
-    // Epilogue warps.  BN = 256 has a single accumulator buffer (2 x 256 columns = all of TMEM), so the next tile's MMAs
-    // wait until the epilogue has READ the accumulators: eight warps (two per TMEM lane quarter, 128 columns each) pull
-    // everything into registers first - ~1.5k clk instead of ~10k (profiles/r2_dense_epilogue.md) - then do the math.
-    static constexpr int EW = (BN >= 256) ? 8 : 4;
-    static constexpr int CPW = BN * 4 / EW;                  // accumulator columns per epilogue warp
-    static constexpr int THREADS = (EW + 2) * 32;
-    static constexpr int W_LOAD = EW, W_ISSUE = EW + 1;
-    static constexpr int TMEM_COLS = (ACC_BUFS * 2 * BN < 32) ? 32 : ACC_BUFS * 2 * BN;
-    // epilogue staging for the TMA store of the split output: per warp 2 buffers x (hi 2 KB + lo 2 KB)
-    static constexpr int OUT_STAGE_BYTES = EPI_WARPS * 2 * 4096;
+    static constexpr int STAGES = (BN >= 128) ? 3 : (BN >= 64 ? 4 : 5);
     // tile order (active tiles first) when the map carries constant-region information: uint16 per tile
     static constexpr int ORDER_CAP = 832;
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + OUT_STAGE_BYTES + 1024 + 256 + ORDER_CAP * 2;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256 + ORDER_CAP * 2;
 };
 
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
@@ -64,18 +47,6 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
         ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar)
         : "memory");
 }
-
-__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, int c0, int c1, int c2, int c3, uint32_t src) {
-    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.tile.bulk_group [%0, {%1, %2, %3, %4}], [%5];"
-                 ::"l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(src)
-                 : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_group_read() {
-    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void bulk_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 struct Conv2dArgs {
     const void* wpack;
@@ -88,13 +59,9 @@ struct Conv2dArgs {
     const float* cvec;    // output constant of the tiles that see a constant input (tile_dist > reach, not on the border)
     int reach;
     int* counters;        // optional [2]: += tiles computed (not stored as a constant), += tiles (bench instrumentation)
-    long long* trace;     // optional [grid][16] clock64 sums / globaltimer stamps per CTA (SASSD_TMA_TRACE=n: n-th launch, timing experiments)
-    int tile_order;       // 1: computed tiles first (SASSD_TMA_ORDER=1), 0: round-robin
+    int tile_order;       // 1: computed tiles first, 0: round-robin
     int nsplit;           // work units per tile: 1, or 2 = each unit computes BN of the 2*BN output channels (the weight
-                          // pack is the 2*BN-wide one; small maps, where whole tiles are too coarse to balance 148 SMs)
-    int dbg;              // SASSD_TMA_DBG (timing experiments only): 1 = reuse stale B stages, 2 = reuse stale A stages,
-                          // 4 = plain MMAs (no operand collector), 8 = no TMA stores, 16 = no wait for the staging buffer,
-                          // 32 = constant tiles through the staged TMA path
+                          // pack is the 2*BN-wide one)
 };
 
 // True when tile (ty, tx) sees a constant input and its output is p.cvec (see sassd_conv2d_f16x3_occ in the header).
@@ -103,249 +70,10 @@ __device__ __forceinline__ bool tile_is_constant(const Conv2dArgs& p, int tile, 
     return p.reach < 2 || !(ty == 0 || ty == tiles_y - 1 || tx == 0 || tx == tiles_x - 1);
 }
 
-// Epilogue of one 8x16-pixel tile, run by the four epilogue warps.  Thread r owns pixel (py, px) = (r / 16, r % 16)
-// and TMEM lane r.  The split output goes TMEM -> registers -> a 64B-swizzled staging box [2 rows][16 px][32 ch] per
-// warp -> one TMA tensor store per fp16 plane (coalesced 64-B pixel segments, image-edge clipping by the TMA unit);
-// the LSU only sees conflict-free STS.128.  f32 outputs (the small head convs) are stored directly.  `release()` is
-// called by lane 0 once the accumulators are in registers, so the next tile's MMAs may start.
-template <int BN, class Release>
-__device__ __forceinline__ void drain_tile(const Conv2dArgs& p, const CUtensorMap* omap, uint32_t tmem_acc, int warp,
-                                           int lane, int b, int ty, int tx, bool store, uint32_t my_stage,
-                                           uint32_t& store_it, Release&& release, bool const_tile = false) {
-    const int r = warp * 32 + lane;
-    const int py = r / TILE_W, px = r % TILE_W;
-    const int y = ty * TILE_H + py, x = tx * TILE_W + px;
-    const bool valid = store && y < p.H && x < p.W;
-    const size_t pix = ((size_t)b * p.H + y) * p.W + x;
-    const uint32_t row_off = (uint32_t)lane * 64u, sw = ((uint32_t)lane >> 1) & 3u;
-    const bool vec_ss = p.scale && p.shift && (p.cout & 3) == 0;
-    constexpr int CW = 32;
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += CW) {
-        uint32_t v[CW], u[CW];
-        const uint32_t taddr = tmem_acc + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-        if (!const_tile) {
-            tmem_ld<CW>(v, taddr);
-            tmem_ld<CW>(u, taddr + (uint32_t)BN);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (c0 + CW >= BN) {      // accumulators are in registers: the next tile's MMAs may start
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) release();
-            }
-        }
-        float o[CW];
-        if (const_tile) {         // constant input region: the output is the layer's precomputed constant vector
-#pragma unroll
-            for (int j = 0; j < CW; ++j) o[j] = (c0 + j) < p.cout ? __ldg(&p.cvec[c0 + j]) : 0.f;
-        } else
-#pragma unroll
-        for (int j = 0; j < CW; j += 4) {
-            const int n = c0 + j;
-            float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (vec_ss) {
-                if (n < p.cout) {
-                    sc = __ldg((const float4*)(p.scale + n));
-                    sh = __ldg((const float4*)(p.shift + n));
-                }
-            } else {
-                if (p.scale) {
-                    if (n + 0 < p.cout) sc.x = __ldg(&p.scale[n + 0]);
-                    if (n + 1 < p.cout) sc.y = __ldg(&p.scale[n + 1]);
-                    if (n + 2 < p.cout) sc.z = __ldg(&p.scale[n + 2]);
-                    if (n + 3 < p.cout) sc.w = __ldg(&p.scale[n + 3]);
-                }
-                if (p.shift) {
-                    if (n + 0 < p.cout) sh.x = __ldg(&p.shift[n + 0]);
-                    if (n + 1 < p.cout) sh.y = __ldg(&p.shift[n + 1]);
-                    if (n + 2 < p.cout) sh.z = __ldg(&p.shift[n + 2]);
-                    if (n + 3 < p.cout) sh.w = __ldg(&p.shift[n + 3]);
-                }
-            }
-            const float scs[4] = {sc.x, sc.y, sc.z, sc.w}, shs[4] = {sh.x, sh.y, sh.z, sh.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                float val = fmaf(__fadd_rn(__uint_as_float(v[j + e]), __uint_as_float(u[j + e]) * (1.f / kF16LoScale)),
-                                 scs[e], shs[e]);
-                if (p.relu) val = fmaxf(val, 0.f);
-                o[j + e] = (n + e) < p.cout ? val : 0.f;
-            }
-        }
-        if (p.out_f32 && valid) {
-            float* orow = p.out_f32 + pix * p.out_f32_stride;
-#pragma unroll
-            for (int j = 0; j < CW; j += 4) {
-                const int n = c0 + j;
-                if (n + 3 < p.out_f32_stride) *(float4*)(orow + n) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
-                else
-                    for (int e = 0; e < 4; ++e)
-                        if (n + e < p.out_f32_stride) orow[n + e] = o[j + e];
-            }
-        }
-        if (p.out_split && store && c0 < p.out_split_ch) {
-            const uint32_t buf = my_stage + (store_it & 1u) * 4096u;
-            if (store_it >= 2) {      // the store issued two iterations ago has finished reading this buffer
-                if (lane == 0) bulk_wait_group_read<1>();
-                __syncwarp();
-            }
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                uint32_t h0, h1, h2, h3, l0, l1, l2, l3;
-                split_f16x2(o[8 * q + 0], o[8 * q + 1], h0, l0);
-                split_f16x2(o[8 * q + 2], o[8 * q + 3], h1, l1);
-                split_f16x2(o[8 * q + 4], o[8 * q + 5], h2, l2);
-                split_f16x2(o[8 * q + 6], o[8 * q + 7], h3, l3);
-                const uint32_t dst = buf + row_off + (((uint32_t)q ^ sw) << 4);
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(h0), "r"(h1), "r"(h2), "r"(h3) : "memory");
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst + 2048u), "r"(l0), "r"(l1), "r"(l2), "r"(l3) : "memory");
-            }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) {
-                const int oy = ty * TILE_H + 2 * warp, ox = tx * TILE_W;
-                tma_store_4d(omap, c0, ox, oy, b, buf);
-                tma_store_4d(omap, c0, ox, oy, p.batch + b, buf + 2048u);
-                bulk_commit_group();
-            }
-            ++store_it;
-        }
-    }
-}
-
-// Epilogue of the columns [col0, col0 + CPW) of one 8x16-pixel tile for the warp that owns TMEM lane quarter `quad`
-// (same arithmetic and store path as drain_tile).  double_buf: this warp owns two staging buffers.
-//   ROLLED = false (BN = 256, single accumulator buffer): ALL of the warp's accumulator columns are read into registers
-//     first (big + small/2048 combined: CPW fp32 registers), the accumulator is released to the MMA warp, then the
-//     slices are processed - four unrolled copies of the slice code.
-//   ROLLED = true (double-buffered accumulators): one slice at a time in a rolled loop.  At B = 1 a CTA runs this code
-//     once or twice per launch, so it executes at instruction-fetch speed: the unrolled form's first pass cost 19-25k
-//     clk against 6.5k for a warm one (profiles/r2_dense_epilogue.md).
-// BN scale / shift: lane l holds column c0 + l of the slice (two loads per slice, issued before the TMEM loads) and
-// the FMAs take them by shuffle - instead of 16 broadcast float4 loads per slice in the dependent chain.
-template <int BN, int CPW, bool ROLLED, class Release>
-__device__ __forceinline__ void drain_cols(const Conv2dArgs& p, const CUtensorMap* omap, uint32_t tmem_acc, int quad,
-                                           int col0, int lane, int b, int ty, int tx, uint32_t my_stage, bool double_buf,
-                                           uint32_t& store_it, Release&& release, bool const_tile, int n_off = 0,
-                                           long long* ph = nullptr) {
-    const int r = quad * 32 + lane;
-    const int py = r / TILE_W, px = r % TILE_W;
-    const int y = ty * TILE_H + py, x = tx * TILE_W + px;
-    const bool valid = y < p.H && x < p.W;
-    const size_t pix = ((size_t)b * p.H + y) * p.W + x;
-    const uint32_t row_off = (uint32_t)lane * 64u, sw = ((uint32_t)lane >> 1) & 3u;
-    constexpr int CW = 32, NS = CPW / CW;
-    long long tq = ph ? clock64() : 0;
-    auto stamp = [&](int i) { if (ph) { const long long t = clock64(); ph[i] += t - tq; tq = t; } };
-    const uint32_t tbase = tmem_acc + ((uint32_t)(quad * 32) << 16) + (uint32_t)col0;
-    // this lane's column of slice s: folded-BN scale and shift (1, 0 beyond cout: those accumulators are exact zeros)
-    auto lane_scale = [&](int s) { const int n = n_off + col0 + s * CW + lane; return (p.scale && n < p.cout) ? __ldg(&p.scale[n]) : 1.f; };
-    auto lane_shift = [&](int s) { const int n = n_off + col0 + s * CW + lane; return (p.shift && n < p.cout) ? __ldg(&p.shift[n]) : 0.f; };
-    // one 32-column slice: BN + ReLU (or the layer constant), fp32 store and / or split -> staging -> TMA store
-    auto emit = [&](const float (&a)[CW], float scl, float shl, int s) {
-        const int c0 = n_off + col0 + s * CW;       // output channel of this slice's first column
-        float o[CW];
-        if (const_tile) {         // constant input region: the output is the layer's precomputed constant vector
-            const float cv = (c0 + lane) < p.cout ? __ldg(&p.cvec[c0 + lane]) : 0.f;
-#pragma unroll
-            for (int j = 0; j < CW; ++j) o[j] = __shfl_sync(0xffffffffu, cv, j);
-        } else {
-#pragma unroll
-            for (int j = 0; j < CW; ++j) {
-                float val = fmaf(a[j], __shfl_sync(0xffffffffu, scl, j), __shfl_sync(0xffffffffu, shl, j));
-                if (p.relu) val = fmaxf(val, 0.f);
-                o[j] = val;
-            }
-        }
-        stamp(1);
-        if (p.out_f32 && valid) {
-            float* orow = p.out_f32 + pix * p.out_f32_stride;
-#pragma unroll
-            for (int j = 0; j < CW; j += 4) {
-                const int n = c0 + j;
-                if (n + 3 < p.out_f32_stride) *(float4*)(orow + n) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
-                else
-                    for (int e = 0; e < 4; ++e)
-                        if (n + e < p.out_f32_stride) orow[n + e] = o[j + e];
-            }
-        }
-        if (p.out_split && c0 < p.out_split_ch) {
-            const uint32_t buf = my_stage + (double_buf ? (store_it & 1u) * 4096u : 0u);
-            if (store_it >= (double_buf ? 2u : 1u) && !(p.dbg & 16)) {   // the store that last used this buffer has read it
-                if (lane == 0) { if (double_buf) bulk_wait_group_read<1>(); else bulk_wait_group_read<0>(); }
-                __syncwarp();
-            }
-            stamp(2);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                uint32_t h0, h1, h2, h3, l0, l1, l2, l3;
-                split_f16x2(o[8 * q + 0], o[8 * q + 1], h0, l0);
-                split_f16x2(o[8 * q + 2], o[8 * q + 3], h1, l1);
-                split_f16x2(o[8 * q + 4], o[8 * q + 5], h2, l2);
-                split_f16x2(o[8 * q + 6], o[8 * q + 7], h3, l3);
-                const uint32_t dst = buf + row_off + (((uint32_t)q ^ sw) << 4);
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(h0), "r"(h1), "r"(h2), "r"(h3) : "memory");
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst + 2048u), "r"(l0), "r"(l1), "r"(l2), "r"(l3) : "memory");
-            }
-            stamp(3);
-            fence_proxy_async();
-            __syncwarp();
-            stamp(4);
-            if (lane == 0 && !(p.dbg & 8)) {
-                const int oy = ty * TILE_H + 2 * quad, ox = tx * TILE_W;
-                tma_store_4d(omap, c0, ox, oy, b, buf);
-                tma_store_4d(omap, c0, ox, oy, p.batch + b, buf + 2048u);
-                bulk_commit_group();
-            }
-            stamp(5);
-            ++store_it;
-        }
-    };
-    auto load_slice = [&](float (&a)[CW], int s) {      // big + small / 2048 of 32 accumulator columns
-        uint32_t v[CW], u[CW];
-        tmem_ld<CW>(v, tbase + (uint32_t)(s * CW));
-        tmem_ld<CW>(u, tbase + (uint32_t)(s * CW) + (uint32_t)BN);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int j = 0; j < CW; ++j) a[j] = __fadd_rn(__uint_as_float(v[j]), __uint_as_float(u[j]) * (1.f / kF16LoScale));
-    };
-    if constexpr (ROLLED) {
-#pragma unroll 1
-        for (int s = 0; s < NS; ++s) {
-            float a[CW];
-            float scl = 1.f, shl = 0.f;
-            if (!const_tile) {
-                scl = lane_scale(s); shl = lane_shift(s);
-                load_slice(a, s);
-                if (s == NS - 1) {          // the last columns are in registers: the MMA warp may reuse this buffer
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) release();
-                }
-            }
-            stamp(0);
-            emit(a, scl, shl, s);
-        }
-    } else {
-        float acc[NS][CW], scl[NS], shl[NS];
-        if (!const_tile) {
-#pragma unroll
-            for (int s = 0; s < NS; ++s) { scl[s] = lane_scale(s); shl[s] = lane_shift(s); }
-#pragma unroll
-            for (int s = 0; s < NS; ++s) load_slice(acc[s], s);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) release();           // accumulators are in registers: the next tile's MMAs may start
-        }
-        stamp(0);
-#pragma unroll
-        for (int s = 0; s < NS; ++s) emit(acc[s], scl[s], shl[s], s);
-    }
-}
-
 // A unit of a constant-region tile: every pixel gets the layer's constant vector (channels [n_off, n_off + ncols) of it).
-// No staging and no TMA: lane g of a pixel's group holds 8 channels of the split constant in registers and the EW
-// epilogue warps write whole pixels with 16-byte stores (ncols / 8 lanes cover one pixel: 512 contiguous bytes at
-// ncols = 256).  Same values, bit for bit, as drain_cols(const_tile = true).  Requires vpp = ncols / 8 in {8, 16, 32}.
+// Lane g of a pixel's group holds 8 channels of the split constant in registers and the EW consumer warps write
+// whole pixels with 16-byte stores (ncols / 8 lanes cover one pixel: 512 contiguous bytes at ncols = 256).  Same
+// values, bit for bit, as the register epilogue of a constant tile.  Requires vpp = ncols / 8 in {8, 16, 32}.
 template <int EW>
 __device__ __forceinline__ void store_constant_unit(const Conv2dArgs& p, int b, int ty, int tx, int n_off, int ncols,
                                                     int warp, int lane) {
@@ -373,25 +101,18 @@ __device__ __forceinline__ void store_constant_unit(const Conv2dArgs& p, int b, 
 }
 
 template <int BN>
-__global__ void __launch_bounds__(Cfg2<BN>::THREADS, 1)
-conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap omap, const Conv2dArgs p) {
+__global__ void __launch_bounds__(THREADS2, 1)
+conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p) {
     using C = Cfg2<BN>;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    const uint32_t ostage_base = base + C::STAGES * C::STAGE_BYTES;       // 1024-aligned
-    const uint32_t bar_base = ostage_base + C::OUT_STAGE_BYTES;
+    const uint32_t bar_base = base + C::STAGES * C::STAGE_BYTES;
     auto full = [&](int s) { return bar_base + 8u * s; };
     auto empty = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-    auto tmem_full = [&](int a) { return bar_base + 8u * (2 * C::STAGES + a); };
-    auto tmem_empty = [&](int a) { return bar_base + 8u * (2 * C::STAGES + 2 + a); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4);
-    volatile uint32_t* tmem_slot_ptr =
-        (volatile uint32_t*)(base_ptr + C::STAGES * C::STAGE_BYTES + C::OUT_STAGE_BYTES + 8 * (2 * C::STAGES + 4));
 
     pdl_launch_dependents();      // the next layer may be scheduled as this grid's CTAs retire
-    if (p.trace && threadIdx.x == 0) p.trace[(size_t)blockIdx.x * 16 + 7] = (long long)globaltimer_ns();
-    // warp index through a shuffle so that the compiler knows it is warp-uniform (role loops on the uniform datapath)
+    // warp index through a shuffle so that the compiler knows it is warp-uniform
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
     const int tiles_x = (p.W + TILE_W - 1) / TILE_W, tiles_y = (p.H + TILE_H - 1) / TILE_H;
     const int ntiles = p.batch * tiles_y * tiles_x;
@@ -400,30 +121,19 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constan
     const int nchunks = p.taps * kchunks;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < C::STAGES; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(tmem_full(a), 1); mbar_init(tmem_empty(a), C::EW); }
+        for (int s = 0; s < C::STAGES; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 2); }
         fence_barrier_init();
         asm volatile("prefetch.tensormap [%0];" ::"l"(&amap) : "memory");
-        if (p.out_split) asm volatile("prefetch.tensormap [%0];" ::"l"(&omap) : "memory");
     }
-    if (warp == C::W_ISSUE) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                     "r"((uint32_t)C::TMEM_COLS)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
     pdl_wait();                   // the producing layer has completed; nothing above touched global data
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
     // With constant-region information most tiles only store a constant.  Static round-robin leaves some CTAs with
-    // two computed tiles and others with none; with SASSD_TMA_ORDER=1 (for maps of up to ORDER_CAP tiles) every CTA
+    // two computed tiles and others with none; with tile_order = 1 (for maps of up to ORDER_CAP tiles) every CTA
     // builds the same order - computed tiles first, constant tiles after - and all roles walk
-    // order[blockIdx.x + i * gridDim.x].  Measured: one step at a time 705 -> 776 frames/s, but four steps in flight
-    // 1470 -> 1290 (the freed SMs are what the other frames' kernels run on), so round-robin is the default.
-    uint16_t* order = (uint16_t*)(base_ptr + C::STAGES * C::STAGE_BYTES + C::OUT_STAGE_BYTES + 256);
+    // order[blockIdx.x + i * gridDim.x].  Round-robin is the default: with several steps in flight the SMs that
+    // only store constants are what the other frames' kernels run on.
+    uint16_t* order = (uint16_t*)(base_ptr + C::STAGES * C::STAGE_BYTES + 256);
     const bool small_map = p.tile_dist != nullptr && ntiles <= C::ORDER_CAP;
     const bool use_order = p.tile_order && small_map;
     // For maps of up to ORDER_CAP tiles warp 0 fetches every tile's distance in one batch of loads (one memory latency
@@ -431,7 +141,6 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constan
     if (small_map) {
         if (warp == 0) {
             // verdicts of tiles lane, lane + 32, ... as bits of one word; the distances are fetched four at a time
-            // (rolled: at B = 1 this code runs once per launch, at instruction-fetch speed)
             uint32_t cst_bits = 0u;
             int ty = (lane / tiles_x) % tiles_y, tx = lane % tiles_x;      // tile `lane`; advanced by 32 tiles per slot
 #pragma unroll 1
@@ -473,17 +182,16 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constan
         }
         __syncthreads();
     }
-    // tile_ref(k): the k-th tile in walking order, bit 15 set when it only stores the layer's constant
+    // tile_ref(k): the k-th tile in walking order, bit 30 set when it only stores the layer's constant
     auto tile_ref = [&](int k) -> int {
         if (small_map) { const int v = order[k]; return (v & 0x7fff) | ((v & 0x8000) << 15); }
         if (!p.tile_dist) return k;
         return tile_is_constant(p, k, (k / tiles_x) % tiles_y, k % tiles_x, tiles_y, tiles_x) ? (k | kConstTile) : k;
     };
-    if (p.trace && threadIdx.x == 0) p.trace[(size_t)blockIdx.x * 16 + 8] = (long long)globaltimer_ns();
 
-    if (warp == C::W_LOAD) {
+    if (warp == W_LOAD) {
         if (lane == 0) {
-            int stage = 0, issued = 0;
+            int stage = 0;
             uint32_t phase = 0;
             for (int k = blockIdx.x; k < nunits; k += gridDim.x) {
                 const int ref = tile_ref(k / nsplit), half = k % nsplit;
@@ -498,377 +206,115 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constan
                         mbar_wait(empty(stage), phase ^ 1u);
                         const uint32_t a_hi = base + stage * C::STAGE_BYTES, a_lo = a_hi + A_TILE_BYTES;
                         const uint32_t b_dst = a_hi + 2 * A_TILE_BYTES;
-                        const bool warm = issued >= C::STAGES;
-                        const bool load_a = !(warm && (p.dbg & 2)), load_b = !(warm && (p.dbg & 1));
-                        ++issued;
-                        mbar_expect_tx(full(stage), (load_a ? 2 * A_TILE_BYTES : 0) + (load_b ? 2 * C::B_TILE_BYTES : 0));
+                        mbar_expect_tx(full(stage), 2 * A_TILE_BYTES + 2 * C::B_TILE_BYTES);
                         // coordinates innermost first: {channel, x, y, plane*B + b}; out-of-image pixels arrive as zeros
-                        if (load_a) {
-                            tma_load_4d(a_hi, &amap, kc * BKC, x0 + dx, y0 + dy, b, full(stage));
-                            tma_load_4d(a_lo, &amap, kc * BKC, x0 + dx, y0 + dy, p.batch + b, full(stage));
-                        }
+                        tma_load_4d(a_hi, &amap, kc * BKC, x0 + dx, y0 + dy, b, full(stage));
+                        tma_load_4d(a_lo, &amap, kc * BKC, x0 + dx, y0 + dy, p.batch + b, full(stage));
                         // pack: per (tap, chunk) [hi | lo], each nsplit * BN rows of 128 bytes; this unit's BN rows of each
                         const uint8_t* src = (const uint8_t*)p.wpack +
                                              (size_t)(t * kchunks + kc) * (size_t)(2 * nsplit) * C::B_TILE_BYTES +
                                              (size_t)half * C::B_TILE_BYTES;
-                        constexpr uint32_t kPiece = (C::B_TILE_BYTES >= 16384) ? 16384u : (uint32_t)C::B_TILE_BYTES;
-                        if (load_b) {
+                        constexpr uint32_t kPiece = (C::B_TILE_BYTES >= 8192) ? 8192u : (uint32_t)C::B_TILE_BYTES;
 #pragma unroll 1
-                            for (int part = 0; part < 2; ++part)
+                        for (int part = 0; part < 2; ++part)
 #pragma unroll 1
-                                for (uint32_t o = 0; o < (uint32_t)C::B_TILE_BYTES; o += kPiece)
-                                    bulk_g2s(b_dst + part * C::B_TILE_BYTES + o,
-                                             src + (size_t)part * nsplit * C::B_TILE_BYTES + o, kPiece, full(stage));
-                        }
+                            for (uint32_t o = 0; o < (uint32_t)C::B_TILE_BYTES; o += kPiece)
+                                bulk_g2s(b_dst + part * C::B_TILE_BYTES + o,
+                                         src + (size_t)part * nsplit * C::B_TILE_BYTES + o, kPiece, full(stage));
                         if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
                     }
                 }
             }
         }
-    } else if (warp == C::W_ISSUE) {
-        // Warp-convergent loop (uniform datapath), one elected lane issues.  Round 2: this loop, not the tensor pipe,
-        // was the bound - rebuilding four 64-bit descriptors per K=16 step plus a run-time debug variant cost ~60 SASS
-        // instructions per three MMAs (profiles/r2_mma_issue_probe.md) - so a descriptor is now a per-stage low word
-        // plus immediates and the three products are straight-line code.
-        constexpr uint32_t idesc = make_idesc(BM, BN, 0u /*F16*/);
-        constexpr uint32_t kStageLo = (uint32_t)C::STAGE_BYTES >> 4, kATileLo = (uint32_t)A_TILE_BYTES >> 4,
-                           kBTileLo = (uint32_t)C::B_TILE_BYTES >> 4;
-        const bool leader = elect_one();
-        const uint32_t lo0 = desc_lo(base);
+    } else {
+        // ===================== consumers: warpgroup wg owns pixel rows 64 wg .. 64 wg + 63 of the tile =====================
+        const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+        const int rl0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);        // tile rows rl0 and rl0 + 8 (= pixel py * 16 + px)
+        const size_t plane = (size_t)p.batch * p.H * p.W * p.out_split_ch;
+        float big[BN / 2], small[BN / 2];
         int stage = 0;
         uint32_t phase = 0;
-        int acc = 0;
-        uint32_t acc_phase = 0;
         int computed = 0;
-        long long* tr = p.trace ? p.trace + (size_t)blockIdx.x * 16 : nullptr;
-        long long t_acc = 0, t_full = 0, t_iss = 0;
-        const long long t_begin = tr ? clock64() : 0;
-        for (int k = blockIdx.x; k < nunits; k += gridDim.x) {
-            if (tile_ref(k / nsplit) & kConstTile) continue;
-            if (k % nsplit == 0) ++computed;
-            long long c0 = tr ? clock64() : 0;
-            mbar_wait(tmem_empty(acc), acc_phase ^ 1u);
-            tc_fence_after();
-            if (tr) t_acc += clock64() - c0;
-            const uint32_t d_big = tmem_base + (uint32_t)(acc * 2 * BN), d_small = d_big + (uint32_t)BN;
-            uint32_t first = 0u;
-            for (int ch = 0; ch < nchunks; ++ch) {
-                c0 = tr ? clock64() : 0;
-                mbar_wait(full(stage), phase);
-                tc_fence_after();
-                const long long c1 = tr ? clock64() : 0;
-                const uint32_t ah = lo0 + (uint32_t)stage * kStageLo, al = ah + kATileLo;
-                const uint32_t bh = al + kATileLo, bl = bh + kBTileLo;
-                if (leader) {
-                    // Each K=16 step reads one operand once for two of its three products: bh through the
-                    // weight-stationary form's B collector when N = 256 (B is the larger operand), ah through the A
-                    // collector otherwise.
-                    if (BN == 256 && !(p.dbg & 4)) {
-#pragma unroll
-                        for (uint32_t k16 = 0; k16 < 4; ++k16) {
-                            const uint32_t ko = k16 * kDescK16;
-                            const uint32_t f = k16 ? 1u : first;
-                            mma_f16_ws_lo<1>(d_big, ah + ko, bh + ko, idesc, f);
-                            mma_f16_ws_lo<2>(d_small, al + ko, bh + ko, idesc, f);
-                            mma_f16_ws_lo<0>(d_small, ah + ko, bl + ko, idesc, 1u);
-                        }
-                    } else {
-#pragma unroll
-                        for (uint32_t k16 = 0; k16 < 4; ++k16) {
-                            const uint32_t ko = k16 * kDescK16;
-                            const uint32_t f = k16 ? 1u : first;
-                            mma_f16_lo(d_small, al + ko, bh + ko, idesc, f);
-                            mma_f16_acoll_lo<1>(d_big, ah + ko, bh + ko, idesc, f);
-                            mma_f16_acoll_lo<2>(d_small, ah + ko, bl + ko, idesc, 1u);
-                        }
-                    }
-                    mma_commit(empty(stage));
-                }
-                __syncwarp();
-                if (tr) { t_full += c1 - c0; t_iss += clock64() - c1; }
-                first = 1u;
-                if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
-            }
-            if (leader) mma_commit(tmem_full(acc));
-            __syncwarp();
-            if (++acc == C::ACC_BUFS) { acc = 0; acc_phase ^= 1u; }
-        }
-        if (tr && leader) { tr[0] = t_acc; tr[1] = t_full; tr[2] = t_iss; tr[3] = clock64() - t_begin; tr[4] = computed; }
-        if (p.counters && leader) {
-            if (computed) atomicAdd(&p.counters[0], computed);
-            if (blockIdx.x == 0) atomicAdd(&p.counters[1], ntiles);
-        }
-    } else if (warp < C::EW) {
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        uint32_t store_it = 0;
-        const int quad = warp & 3, col0 = (warp >> 2) * C::CPW;          // TMEM lane quarter, first column of this warp
-        constexpr bool kDoubleBuf = C::EW == 4;                          // 32 KB of staging: 4 x 2 x 4 KB or 8 x 4 KB
-        const uint32_t my_stage = ostage_base + (uint32_t)warp * (uint32_t)(C::OUT_STAGE_BYTES / C::EW);
-        long long* tr = (p.trace && threadIdx.x == 0) ? p.trace + (size_t)blockIdx.x * 16 : nullptr;
-        long long e_wait = 0, e_drain = 0;
-        long long phase_clk[6] = {0, 0, 0, 0, 0, 0};
         for (int k = blockIdx.x; k < nunits; k += gridDim.x) {
             const int ref = tile_ref(k / nsplit), n_off = (k % nsplit) * BN;
             const int tile = ref & ~kConstTile;
+            const bool const_tile = (ref & kConstTile) != 0;
             const int b = tile / (tiles_y * tiles_x);
             const int ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
-            if (ref & kConstTile) {                                         // no MMAs ran for this tile
+            if (const_tile) {                                               // no MMAs run for this tile
                 const int ncols = min(BN, p.out_split_ch - n_off);
-                if (p.out_split && !p.out_f32 && (ncols == 64 || ncols == 128 || ncols == 256) && !(p.dbg & 32))
-                    store_constant_unit<C::EW>(p, b, ty, tx, n_off, ncols, warp, lane);
-                else
-                    drain_cols<BN, C::CPW, (C::ACC_BUFS == 2)>(p, &omap, 0u, quad, col0, lane, b, ty, tx, my_stage, kDoubleBuf, store_it, [] {},
-                                           true, n_off);
-                continue;
-            }
-            const long long c0 = tr ? clock64() : 0;
-            if (lane == 0) mbar_wait(tmem_full(acc), acc_phase);
-            __syncwarp();
-            tc_fence_after();
-            const long long c1 = tr ? clock64() : 0;
-            const uint32_t bar = tmem_empty(acc);
-            drain_cols<BN, C::CPW, (C::ACC_BUFS == 2)>(p, &omap, tmem_base + (uint32_t)(acc * 2 * BN), quad, col0, lane, b, ty, tx, my_stage,
-                                   kDoubleBuf, store_it, [bar] { mbar_arrive(bar); }, false, n_off, tr ? phase_clk : nullptr);
-            if (tr) { e_wait += c1 - c0; e_drain += clock64() - c1; }
-            if (++acc == C::ACC_BUFS) { acc = 0; acc_phase ^= 1u; }
-        }
-        if (tr) {
-            tr[5] = e_wait; tr[6] = e_drain;
-            for (int i = 0; i < 6; ++i) tr[10 + i] = phase_clk[i];
-        }
-        if (lane == 0) bulk_wait_group_all();
-        __syncwarp();
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (p.trace && threadIdx.x == 0) p.trace[(size_t)blockIdx.x * 16 + 9] = (long long)globaltimer_ns();
-    if (warp == C::W_ISSUE) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)C::TMEM_COLS)
-                     : "memory");
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// CTA-pair variant for Cout = 256 (the BEV neck): tcgen05.mma.cta_group::2, M = 256 (two 128-pixel tiles, one per
-// CTA), N = 256 with each CTA holding half of the weight block.  A single-CTA SS-mode MMA of 128x256x16 reads
-// 4 KB (A) + 8 KB (B) of shared memory and the operand read port delivers ~64 B/clk, so it takes ~192 clk instead
-// of the 128-clk tensor floor (ncu: tensor pipe 62 % active with or without any global loads).  In a pair each SM
-// reads 4 KB + 4 KB per MMA, which is the floor, and a stage shrinks to 64 KB so three stages fit.
-// Protocol (same as CUTLASS' 2-SM pipelines): only the leader's full[] barriers are used; the leader arms them with
-// the bytes of BOTH CTAs and the peer's TMA loads complete_tx on them (.cta_group::2 loads may signal either CTA of
-// the pair); tcgen05.commit multicasts the stage-free / accumulator-ready arrivals to both CTAs; the peer's epilogue
-// warps release the accumulator with a remote arrive on the leader's tmem_empty barrier.
-constexpr int STAGES_2CTA = 3;
-constexpr int B_HALF_BYTES = 128 * 128;                                   // 128 of the 256 weight rows, one plane
-constexpr int STAGE_2CTA_BYTES = 2 * A_TILE_BYTES + 2 * B_HALF_BYTES;     // 64 KB
-constexpr int OUT_STAGE_2CTA_BYTES = EPI_WARPS * 2 * 4096;
-constexpr int SMEM_2CTA_BYTES = STAGES_2CTA * STAGE_2CTA_BYTES + OUT_STAGE_2CTA_BYTES + 1024 + 256;
-
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "WAIT_LOOP_C:\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra.uni WAIT_DONE_C;\n\t"
-        "bra.uni WAIT_LOOP_C;\n\t"
-        "WAIT_DONE_C:\n\t"
-        "}\n" ::"r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
-                                                 uint32_t bar_cluster) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-        ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar_cluster)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar_cluster) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-        ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar_cluster)
-        : "memory");
-}
-__device__ __forceinline__ void mma_f16_pair(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accum)
-        : "memory");
-}
-__device__ __forceinline__ void mma_f16_pair_lo(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "mov.b64 da, {%1, %5};\n\t"
-        "mov.b64 db, {%2, %5};\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accum), "r"(kDescHi)
-        : "memory");
-}
-__device__ __forceinline__ void mma_commit_pair(uint32_t bar) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-        "h"((uint16_t)3)
-        : "memory");
-}
-
-__global__ void __launch_bounds__(THREADS2, 1)
-conv2d_tma_pair_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
-                       const __grid_constant__ CUtensorMap omap, const Conv2dArgs p) {
-    constexpr int BN = 256;
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    const uint32_t ostage_base = base + STAGES_2CTA * STAGE_2CTA_BYTES;
-    const uint32_t bar_base = ostage_base + OUT_STAGE_2CTA_BYTES;
-    auto full = [&](int s) { return bar_base + 8u * s; };
-    auto empty = [&](int s) { return bar_base + 8u * (STAGES_2CTA + s); };
-    const uint32_t tmem_full = bar_base + 8u * (2 * STAGES_2CTA), tmem_empty = tmem_full + 8u;
-    const uint32_t tmem_slot = tmem_full + 16u;
-    volatile uint32_t* tmem_slot_ptr = (volatile uint32_t*)(base_ptr + (tmem_slot - base));
-
-    const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const int cluster_id = blockIdx.x >> 1, nclusters = gridDim.x >> 1;
-    const int tiles_x = (p.W + TILE_W - 1) / TILE_W, tiles_y = (p.H + TILE_H - 1) / TILE_H;
-    const int ntiles = p.batch * tiles_y * tiles_x;
-    const int npairs = (ntiles + 1) / 2;
-    const int kchunks = (p.cin + BKC - 1) / BKC;
-    const int nchunks = p.taps * kchunks;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES_2CTA; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 1); }
-        mbar_init(tmem_full, 1);
-        mbar_init(tmem_empty, 2 * EPI_WARPS);
-        fence_barrier_init();
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&amap) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&bmap) : "memory");
-        if (p.out_split) asm volatile("prefetch.tensormap [%0];" ::"l"(&omap) : "memory");
-    }
-    if (warp == WARP_ISSUE) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();      // both CTAs' barriers are initialised before any remote arrive / complete_tx
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
-
-    if (warp == WARP_LOAD) {
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int pair = cluster_id; pair < npairs; pair += nclusters) {
-                const int tile = 2 * pair + (int)rank;
-                const bool real = tile < ntiles;
-                const int b = real ? tile / (tiles_y * tiles_x) : 0;
-                const int ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
-                // a pair's odd slot past the last tile loads a box that is wholly outside the image (all zeros)
-                const int y0 = real ? ty * TILE_H : p.H + 1, x0 = real ? tx * TILE_W : 0;
-                for (int t = 0; t < p.taps; ++t) {
-                    const int dy = p.taps == 9 ? t / 3 - 1 : 0, dx = p.taps == 9 ? t % 3 - 1 : 0;
-                    for (int kc = 0; kc < kchunks; ++kc) {
-                        mbar_wait(empty(stage), phase ^ 1u);
-                        const uint32_t a_hi = base + stage * STAGE_2CTA_BYTES, a_lo = a_hi + A_TILE_BYTES;
-                        const uint32_t b_hi = a_hi + 2 * A_TILE_BYTES, b_lo = b_hi + B_HALF_BYTES;
-                        const uint32_t bar = mapa_rank(full(stage), 0);
-                        if (leader) mbar_expect_tx(full(stage), 2 * STAGE_2CTA_BYTES);
-                        tma_load_4d_pair(a_hi, &amap, kc * BKC, x0 + dx, y0 + dy, b, bar);
-                        tma_load_4d_pair(a_lo, &amap, kc * BKC, x0 + dx, y0 + dy, p.batch + b, bar);
-                        // weight rows of this CTA's half: block (t, kc) = [hi 256 rows][lo 256 rows]
-                        const int row = (t * kchunks + kc) * 2 * BN + (int)rank * 128;
-                        tma_load_2d_pair(b_hi, &bmap, 0, row, bar);
-                        tma_load_2d_pair(b_lo, &bmap, 0, row + BN, bar);
-                        if (++stage == STAGES_2CTA) { stage = 0; phase ^= 1u; }
-                    }
+                if (p.out_split && !p.out_f32 && (ncols == 64 || ncols == 128 || ncols == 256)) {
+                    store_constant_unit<CONS_WARPS>(p, b, ty, tx, n_off, ncols, warp, lane);
+                    continue;
                 }
-            }
-        }
-    } else if (warp == WARP_ISSUE) {
-        if (leader) {       // leader CTA: warp-convergent loop, one elected lane issues for the pair (see conv2d_tma_kernel)
-            constexpr uint32_t idesc = make_idesc(2 * BM, BN, 0u /*F16*/);
-            constexpr uint32_t kStageLo = (uint32_t)STAGE_2CTA_BYTES >> 4, kATileLo = (uint32_t)A_TILE_BYTES >> 4,
-                               kBHalfLo = (uint32_t)B_HALF_BYTES >> 4;
-            const bool issuer = elect_one();
-            const uint32_t lo0 = desc_lo(base);
-            int stage = 0;
-            uint32_t phase = 0, acc_phase = 0;
-            const uint32_t d_big = tmem_base, d_small = tmem_base + (uint32_t)BN;
-            for (int pair = cluster_id; pair < npairs; pair += nclusters) {
-                mbar_wait_cluster(tmem_empty, acc_phase ^ 1u);
-                tc_fence_after();
-                uint32_t first = 0u;
+            } else {
+                if (k % nsplit == 0) ++computed;
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) { big[i] = 0.f; small[i] = 0.f; }
+                int prev = -1;
                 for (int ch = 0; ch < nchunks; ++ch) {
                     mbar_wait(full(stage), phase);
-                    tc_fence_after();
-                    const uint32_t ah = lo0 + (uint32_t)stage * kStageLo, al = ah + kATileLo;
-                    const uint32_t bh = al + kATileLo, bl = bh + kBHalfLo;
-                    if (issuer) {
-#pragma unroll
-                        for (uint32_t k16 = 0; k16 < 4; ++k16) {
-                            const uint32_t ko = k16 * kDescK16, f = k16 ? 1u : first;
-                            mma_f16_pair_lo(d_small, al + ko, bh + ko, idesc, f);
-                            mma_f16_pair_lo(d_small, ah + ko, bl + ko, idesc, 1u);
-                            mma_f16_pair_lo(d_big, ah + ko, bh + ko, idesc, f);
-                        }
-                        mma_commit_pair(empty(stage));
-                    }
-                    __syncwarp();
-                    first = 1u;
-                    if (++stage == STAGES_2CTA) { stage = 0; phase ^= 1u; }
+                    const uint32_t ah = base + stage * C::STAGE_BYTES + (uint32_t)wg * (A_TILE_BYTES / 2);
+                    const uint32_t bh = base + stage * C::STAGE_BYTES + 2 * A_TILE_BYTES;
+                    wgmma_fence();
+                    mma_chunk_x3<1, BN>(big, small, ah, ah + A_TILE_BYTES, bh, bh + C::B_TILE_BYTES);
+                    wgmma_commit();
+                    wgmma_wait<1>();            // the previous chunk's MMAs have read their stage
+                    if (prev >= 0 && t == 0) mbar_arrive(empty(prev));
+                    prev = stage;
+                    if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
                 }
-                if (issuer) mma_commit_pair(tmem_full);
-                __syncwarp();
-                acc_phase ^= 1u;
+                wgmma_wait<0>();
+                fence_regs<BN / 2>(big);
+                fence_regs<BN / 2>(small);
+                if (prev >= 0 && t == 0) mbar_arrive(empty(prev));
+            }
+            // epilogue from registers: folded BN + ReLU (or the layer constant), fp32 and / or split-plane stores
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int n = n_off + 8 * j + 2 * (t & 3);
+                float c0, c1, sc0 = 1.f, sc1 = 1.f, sh0 = 0.f, sh1 = 0.f;
+                if (const_tile) {
+                    c0 = n < p.cout ? __ldg(&p.cvec[n]) : 0.f;
+                    c1 = n + 1 < p.cout ? __ldg(&p.cvec[n + 1]) : 0.f;
+                } else {
+                    if (p.scale && n < p.cout) sc0 = __ldg(&p.scale[n]);
+                    if (p.scale && n + 1 < p.cout) sc1 = __ldg(&p.scale[n + 1]);
+                    if (p.shift && n < p.cout) sh0 = __ldg(&p.shift[n]);
+                    if (p.shift && n + 1 < p.cout) sh1 = __ldg(&p.shift[n + 1]);
+                }
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int rl = rl0 + 8 * i;
+                    const int y = ty * TILE_H + rl / TILE_W, x = tx * TILE_W + rl % TILE_W;
+                    float o0 = c0, o1 = c1;
+                    if (!const_tile) {
+                        o0 = fmaf(__fadd_rn(big[4 * j + 2 * i], small[4 * j + 2 * i] * (1.f / kF16LoScale)), sc0, sh0);
+                        o1 = fmaf(__fadd_rn(big[4 * j + 2 * i + 1], small[4 * j + 2 * i + 1] * (1.f / kF16LoScale)), sc1, sh1);
+                        if (p.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+                        if (n >= p.cout) o0 = 0.f;
+                        if (n + 1 >= p.cout) o1 = 0.f;
+                    }
+                    if (y >= p.H || x >= p.W) continue;
+                    const size_t pix = ((size_t)b * p.H + y) * p.W + x;
+                    if (p.out_f32 && n < p.out_f32_stride)
+                        *(float2*)(p.out_f32 + pix * p.out_f32_stride + n) = make_float2(o0, o1);
+                    if (p.out_split && n < p.out_split_ch) {
+                        uint32_t h, l;
+                        split_f16x2(o0, o1, h, l);
+                        __half* dst = p.out_split + pix * p.out_split_ch + n;
+                        *(uint32_t*)dst = h;
+                        *(uint32_t*)(dst + plane) = l;
+                    }
+                }
             }
         }
-    } else if (warp < EPI_WARPS) {
-        uint32_t acc_phase = 0, store_it = 0;
-        const uint32_t my_stage = ostage_base + (uint32_t)warp * 8192u;
-        const uint32_t release_bar = mapa_rank(tmem_empty, 0);
-        for (int pair = cluster_id; pair < npairs; pair += nclusters) {
-            const int tile = 2 * pair + (int)rank;
-            const bool real = tile < ntiles;
-            const int b = real ? tile / (tiles_y * tiles_x) : 0;
-            const int ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
-            if (lane == 0) mbar_wait(tmem_full, acc_phase);
-            __syncwarp();
-            tc_fence_after();
-            drain_tile<BN>(p, &omap, tmem_base, warp, lane, b, ty, tx, real, my_stage, store_it,
-                           [release_bar] { mbar_arrive_remote(release_bar); });
-            acc_phase ^= 1u;
+        if (p.counters && threadIdx.x == 0) {
+            if (computed) atomicAdd(&p.counters[0], computed);
+            if (blockIdx.x == 0) atomicAdd(&p.counters[1], ntiles);
         }
-        if (lane == 0) bulk_wait_group_all();
-        __syncwarp();
-    }
-
-    __syncwarp();
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();      // the leader's MMAs read the peer's shared memory and write its TMEM until here
-    if (warp == WARP_ISSUE) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
     }
 }
-
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -889,7 +335,7 @@ static EncodeTiledFn get_encode() {
 }
 
 template <int BN>
-static int launch2(const CUtensorMap& map, const CUtensorMap& omap, const Conv2dArgs& a, cudaStream_t stream) {
+static int launch2(const CUtensorMap& map, const Conv2dArgs& a, cudaStream_t stream) {
     using C = Cfg2<BN>;
     auto kern = conv2d_tma_kernel<BN>;
     static bool configured = false;
@@ -899,8 +345,8 @@ static int launch2(const CUtensorMap& map, const CUtensorMap& omap, const Conv2d
         configured = true;
     }
     const int units = a.batch * sassd_div_up(a.H, TILE_H) * sassd_div_up(a.W, TILE_W) * a.nsplit;
-    const int grid = units < 148 ? units : 148;
-    if (launch_pdl(kern, dim3(grid), dim3(C::THREADS), C::SMEM_BYTES, stream, map, omap, a) != cudaSuccess) return SASSD_ERR_LAUNCH;
+    const int grid = units < sassd_num_sms() ? units : sassd_num_sms();
+    if (launch_pdl(kern, dim3(grid), dim3(THREADS2), C::SMEM_BYTES, stream, map, a) != cudaSuccess) return SASSD_ERR_LAUNCH;
     return sassd_check_launch();
 }
 
@@ -951,110 +397,15 @@ extern "C" int sassd_conv2d_f16x3_occ(const sassd_conv2d_desc* d, const void* in
     a.batch = d->batch; a.H = d->H; a.W = d->W; a.cin = d->cin; a.cout = d->cout; a.taps = d->taps; a.relu = d->relu;
     a.out_f32_stride = d->out_f32_stride; a.out_split_ch = d->out_split_ch;
     a.tile_dist = tile_dist; a.reach = reach; a.cvec = const_out; a.counters = counters;
-    a.trace = nullptr;
+    a.tile_order = d->tile_order;
     a.nsplit = 1;
-    static const int trace_call = [] { const char* e = getenv("SASSD_TMA_TRACE"); return e ? atoi(e) : 0; }();
-    static long long* trace_buf = nullptr;
-    static int trace_calls = 0;
-    bool tracing = false;
-    if (trace_call && d->cout == 256 && ++trace_calls == trace_call) {
-        if (!trace_buf) cudaMalloc(&trace_buf, 148 * 16 * sizeof(long long));
-        cudaMemsetAsync(trace_buf, 0, 148 * 16 * sizeof(long long), (cudaStream_t)stream_);
-        a.trace = trace_buf;
-        tracing = true;
-    }
-    static const int tile_order_env = [] { const char* e = getenv("SASSD_TMA_ORDER"); return e ? atoi(e) : -1; }();
-    a.tile_order = tile_order_env >= 0 ? tile_order_env : d->tile_order;      // the environment overrides (experiments)
-    static const int dbg = [] { const char* e = getenv("SASSD_TMA_DBG"); return e ? atoi(e) : 0; }();
-    a.dbg = dbg;
     cudaStream_t stream = (cudaStream_t)stream_;
-    CUtensorMap omap = map;    // placeholder when there is no split output (never dereferenced)
-    if (out_split) {
-        // the split output as the epilogue stores it: one box = 32 channels of 2 rows x 16 pixels (one warp)
-        cuuint64_t odims[4] = {(cuuint64_t)d->out_split_ch, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)(2 * d->batch)};
-        cuuint64_t ostrides[3] = {(cuuint64_t)d->out_split_ch * 2, (cuuint64_t)d->W * d->out_split_ch * 2,
-                                  (cuuint64_t)d->H * d->W * d->out_split_ch * 2};
-        cuuint32_t obox[4] = {32u, (cuuint32_t)TILE_W, 2u, 1u};
-        rc = enc(&omap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, out_split, odims, ostrides, obox, estr,
-                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (rc != CUDA_SUCCESS) return SASSD_ERR_LAUNCH;
-    }
-    if (d->cout <= 32) return launch2<32>(map, omap, a, stream);
-    if (d->cout <= 64) return launch2<64>(map, omap, a, stream);
-    if (d->cout <= 128) return launch2<128>(map, omap, a, stream);
-    // opt-in: measured equal to the single-CTA kernel (both sit at the chip's sustained tensor rate, DESIGN.md section 7)
-    static const bool use_pair = [] { const char* e = getenv("SASSD_TMA_PAIR"); return e && atoi(e) != 0; }();
-    // Small maps (B = 1: 275 tiles of which about half are computed) leave 148 SMs with one or two whole tiles each;
-    // in halves of 128 output channels (same weight pack, N = 128 instructions at their 64-clk floor, double-buffered
-    // accumulators, three operand stages) the computed work spreads evenly and the last epilogue is half as long:
-    // one step at a time +5 % (B=1), +15 % (B=4, 7.4 -> 7.5 waves instead of 8).  Nothing at B >= 8, and with several
-    // steps in flight it costs 2-4 % (a half-width unit re-reads the activation tile: 85 B/clk/SM from L2), so
-    // the throughput slots and the 1x1 layer (load/store bound: 0.036 -> 0.044 ms) keep whole tiles.
-    // Selected per launch by the caller (desc.n_split = 2); SASSD_TMA_NSPLIT_TILES=n forces it for maps of <= n tiles.
-    static const int nsplit_tiles = [] { const char* e = getenv("SASSD_TMA_NSPLIT_TILES"); return e ? atoi(e) : -1; }();
-    const int map_tiles = a.batch * sassd_div_up(a.H, TILE_H) * sassd_div_up(a.W, TILE_W);
-    auto dump_trace = [&] {      // timing experiment: per-CTA clock sums / time stamps of this launch -> stderr
-        std::vector<long long> h(148 * 16);
-        cudaStreamSynchronize(stream);
-        cudaMemcpy(h.data(), trace_buf, h.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-        long long t0 = 0, t1 = 0;
-        for (int c = 0; c < 148; ++c) {
-            const long long* q = &h[(size_t)c * 16];
-            if (!q[7]) continue;
-            if (!t0 || q[7] < t0) t0 = q[7];
-            if (q[9] > t1) t1 = q[9];
-        }
-        fprintf(stderr, "TMA_TRACE B=%d nsplit=%d: first CTA start -> last CTA end %.2f us\n", d->batch, a.nsplit, (t1 - t0) * 1e-3);
-        fprintf(stderr, "TMA_TRACE cta | mma: wait_acc wait_full issue total units | epi(warp0): wait_full drain | ns: start prologue end\n");
-        for (int c = 0; c < 148; c += (c < 3 ? 1 : 48)) {
-            const long long* q = &h[(size_t)c * 16];
-            fprintf(stderr, "TMA_TRACE %3d | %8lld %8lld %8lld %8lld %3lld | %8lld %8lld | %6lld %6lld %6lld | epi phases: tmem %lld math %lld bufwait %lld split+sts %lld fence %lld tma %lld\n", c, q[0], q[1], q[2],
-                    q[3], q[4], q[5], q[6], q[7] - t0, q[8] - t0, q[9] - t0, q[10], q[11], q[12], q[13], q[14], q[15]);
-        }
-    };
-    if (!use_pair && (nsplit_tiles >= 0 ? map_tiles <= nsplit_tiles : d->n_split == 2)) {
-        a.nsplit = 2;
-        const int rc = launch2<128>(map, omap, a, stream);
-        if (tracing) dump_trace();
-        return rc;
-    }
-    if (!use_pair) {
-        const int rc = launch2<256>(map, omap, a, stream);
-        if (tracing) dump_trace();
-        return rc;
-    }
-    // weight pack as a 2-D tensor of 128-byte rows (already in UMMA swizzled order: no TMA swizzle)
-    const int kchunks = sassd_div_up(d->cin, BKC);
-    CUtensorMap bmap;
-    cuuint64_t bdims[2] = {64u, (cuuint64_t)d->taps * kchunks * 2 * 256};
-    cuuint64_t bstrides[1] = {128u};
-    cuuint32_t bbox[2] = {64u, 128u};
-    rc = enc(&bmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(wpack), bdims, bstrides, bbox, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (rc != CUDA_SUCCESS) return SASSD_ERR_LAUNCH;
-    static bool configured = false;
-    if (!configured) {
-        if (cudaFuncSetAttribute(conv2d_tma_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_2CTA_BYTES) !=
-            cudaSuccess)
-            return SASSD_ERR_LAUNCH;
-        configured = true;
-    }
-    const int tiles = a.batch * sassd_div_up(a.H, TILE_H) * sassd_div_up(a.W, TILE_W);
-    const int npairs = (tiles + 1) / 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * (npairs < 74 ? npairs : 74));
-    cfg.blockDim = dim3(THREADS2);
-    cfg.dynamicSmemBytes = SMEM_2CTA_BYTES;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (cudaLaunchKernelEx(&cfg, conv2d_tma_pair_kernel, map, bmap, omap, a) != cudaSuccess) return SASSD_ERR_LAUNCH;
-    return sassd_check_launch();
+    if (d->cout <= 32) return launch2<32>(map, a, stream);
+    if (d->cout <= 64) return launch2<64>(map, a, stream);
+    if (d->cout <= 128) return launch2<128>(map, a, stream);
+    // 128 < cout <= 256: two units per tile, each 128 output channels of the 256-wide weight pack
+    a.nsplit = 2;
+    return launch2<128>(map, a, stream);
 }
 
 // SparseConvTensor.dense() into the split BEV map: hi / lo*2048 fp16 planes [2,B,H,W,D*C] (channel d*C + c).

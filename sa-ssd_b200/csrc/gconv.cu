@@ -203,7 +203,7 @@ template <int MODE, int BN, int BK>
 static int launch_ffma(const sassd_gconv_desc* d, const float* in, const float* w, const float* scale,
                        const float* shift, const int* nbr, const int* d_rows, float* out, cudaStream_t stream) {
     int gx = sassd_div_up(d->rows_cap, GC_BM);
-    if (gx > 148 * 4) gx = 148 * 4;
+    if (gx > sassd_num_sms() * 4) gx = sassd_num_sms() * 4;
     dim3 grid(gx, sassd_div_up(d->cout, BN));
     gconv_ffma_kernel<MODE, BN, BK><<<grid, GC_THREADS, 0, stream>>>(in, w, scale, shift, nbr, d_rows, out, d->cin,
                                                                      d->cout, d->taps, d->in_stride, d->out_stride,

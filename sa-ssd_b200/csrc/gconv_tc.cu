@@ -1,24 +1,24 @@
-// Gathered implicit-GEMM convolution on the 5th-gen tensor cores (tcgen05, sm_100a),
-// fp32-accurate through a 3xTF32 split (SASSD_PREC_TF32X3).
+// Gathered implicit-GEMM convolution on the Hopper tensor cores (wgmma, sm_90a),
+// fp32-accurate through a 3-product hi/lo operand split (SASSD_PREC_TF32X3 / SASSD_PREC_F16X3).
 //
 //   out[m, :] = act( (sum_t  in[row(m,t), :] @ W[t]) * scale + shift )
 //
 // One persistent CTA per SM, warp-specialised:
-//   warps 0-3  epilogue  : tcgen05.ld accumulator (TMEM) -> BN scale/shift, ReLU -> global rows
-//   warps 4-7  A producer: each thread owns one of the tile's 128 output rows; per (tap, 32-channel
-//                          chunk) it gathers the 128 B of its input row (neighbour table / 3x3
-//                          window / identity), splits every fp32 into tf32 hi + lo and stores both
-//                          into 128B-swizzled K-major shared-memory tiles (generic proxy ->
-//                          fence.proxy.async -> mbarrier)
-//   warp  8    MMA issuer: one elected lane issues tcgen05.mma.kind::tf32 (M=128, N=BN, K=8):
-//                          lo*hi + hi*lo + hi*hi per K step, accumulating in TMEM across all taps
-//   warp  9    B loader  : cp.async.bulk (TMA 1-D) of the pre-split, pre-swizzled weight block
-// Pipelines: smem stages (full_a/full_b/empty mbarriers) and two TMEM accumulators
-// (tmem_full/tmem_empty) so the epilogue of tile i overlaps the MMAs of tile i+1.
+//   warps 0-7   consumers : two warpgroups, warpgroup g owns rows 64g..64g+63 of the 128-row tile; they issue
+//                           wgmma (M=64, N=NB, K=8 tf32 / 16 f16) from shared memory, lo*hi + hi*lo + hi*hi per
+//                           K step into register accumulators, then BN scale/shift, ReLU -> global rows
+//   warps 8-15  A producer: two threads per tile row; per (tap, channel chunk) they gather the row's 128 B
+//                           (neighbour table / 3x3 window / identity), split every fp32 into hi + lo and store both
+//                           into 128B-swizzled K-major shared-memory tiles (generic proxy -> mbarrier; the
+//                           consumers fence the proxies before their MMAs read the tiles)
+//                           lane 0 of producer warp 8 also issues the cp.async.bulk of the stage's pre-split,
+//                           pre-swizzled weight block (16 warps: the register file's four quarters split evenly)
+// A work unit is one tile and NB <= 64 of its output channels (two register accumulators of NB/2 floats per thread
+// must fit beside the producers' register budget); wider layers walk the tile once per 64-channel part.
 //
-// Why 3xTF32: tcgen05 has no fp32-input MMA and one TF32 pass (10-bit mantissa) cannot hold the
-// 1e-4 parity bar across 22 layers; hi = tf32_rn(x), lo = tf32_rn(x - hi), and
-// a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi leaves ~2^-21 relative error per product.
+// Why 3 products: one TF32 pass (10-bit mantissa) cannot hold the 1e-4 parity bar across 22 layers;
+// hi = tf32_rn(x), lo = tf32_rn(x - hi), and a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi leaves ~2^-21 relative
+// error per product (fp16: lo carries a factor 2048, 22 bits survive).
 #include <cstdlib>
 
 #include "common.cuh"
@@ -42,86 +42,54 @@ struct RowMapTC {
     }
 };
 
-template <int BN>
+constexpr int GC_PROD_WARPS = 8;
+constexpr int GC_THREADS = CONS_THREADS + GC_PROD_WARPS * 32;   // 512
+constexpr int GC_WARP_PROD = CONS_THREADS / 32;
+
+template <int NB>
 struct Cfg {
-    static constexpr int B_TILE_BYTES = BN * 128;                         // per hi / lo
+    static constexpr int B_TILE_BYTES = NB * 128;                         // per hi / lo
     static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-    static constexpr int STAGES = (BN >= 256) ? 2 : (BN >= 128 ? 3 : 4);
-    // per tile two fp32 accumulators of BN columns each: "big" (hi*hi) and "small" (lo*hi + hi*lo).
-    // Tensor-core accumulation truncates (measured: error grows linearly with the number of
-    // accumulate steps, ~2^-24 each); keeping the 2^-11-smaller terms out of the big accumulator
-    // cuts its step count by 3x, and the two are summed once, in fp32 RN, by the epilogue.
-    static constexpr int ACC_BUFS = (4 * BN <= 512) ? 2 : 1;             // double-buffer when TMEM allows
-    static constexpr int TMEM_COLS = (ACC_BUFS * 2 * BN < 32) ? 32 : ACC_BUFS * 2 * BN;   // power of two
+    static constexpr int STAGES = 4;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
 
-// CL = thread-block cluster size (1, 2 or 4).  With CL > 1 the CTAs of a cluster walk the same
-// (tap, chunk) sequence on different row tiles and share the weight stream: CTA r fetches the r-th
-// 1/CL slice of every weight block and multicasts it to all CTAs of the cluster, which divides the
-// L2 -> SM weight traffic (the dominant term at M=128 tiles: 64 KB of B per 16 KB of A) by CL.
-template <int MODE, int BN, int CL, int PREC>
-__global__ void __launch_bounds__(THREADS, 1)
+// NB = output channels per work unit, bn = padded width of the weight pack (a multiple of NB), nparts = bn / NB
+template <int MODE, int NB, int PREC>
+__global__ void __launch_bounds__(GC_THREADS, 1)
 gconv_tc_kernel(const float* __restrict__ in, const float* __restrict__ wpack, const float* __restrict__ scale,
                 const float* __restrict__ shift, const int* __restrict__ nbr, const int* __restrict__ d_rows,
                 float* __restrict__ out, int cin, int cout, int taps, int in_stride, int out_stride, int rows_cap,
-                int H, int W, int relu) {
-    using C = Cfg<BN>;
+                int H, int W, int relu, int bn, int nparts) {
+    using C = Cfg<NB>;
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment is required by the 128B swizzle
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
     const uint32_t bar_base = base + C::STAGES * C::STAGE_BYTES;
-    // barriers: full_a[S], full_b[S], empty[S], tmem_full[2], tmem_empty[2], then the TMEM address word
     auto full_a = [&](int s) { return bar_base + 8u * s; };
     auto full_b = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
     auto empty = [&](int s) { return bar_base + 8u * (2 * C::STAGES + s); };
-    auto empty_a = [&](int s) { return bar_base + 8u * (3 * C::STAGES + s); };   // CTA-local release (A producers)
-    auto tmem_full = [&](int a) { return bar_base + 8u * (4 * C::STAGES + a); };
-    auto tmem_empty = [&](int a) { return bar_base + 8u * (4 * C::STAGES + 2 + a); };
-    const uint32_t tmem_slot = bar_base + 8u * (4 * C::STAGES + 4);
-    volatile uint32_t* tmem_slot_ptr = (volatile uint32_t*)(base_ptr + C::STAGES * C::STAGE_BYTES + 8 * (4 * C::STAGES + 4));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int M = d_rows ? min(__ldg(d_rows), rows_cap) : rows_cap;
-    const int ntiles_real = (M + BM - 1) / BM;
-    // every CTA of a cluster must run the same number of tile iterations (they hand each other weight
-    // slices and stage-release signals); tiles past the end are computed on zero rows and never stored
-    const int ntiles = CL > 1 ? ((ntiles_real + (int)gridDim.x - 1) / (int)gridDim.x) * (int)gridDim.x : ntiles_real;
+    const int nunits = (M + BM - 1) / BM * nparts;
     using PR = Prec<PREC>;
     const int kchunks = (cin + PR::BKC - 1) / PR::BKC;
     const int nchunks = taps * kchunks;
-    const uint32_t cta_rank = CL > 1 ? cluster_ctarank() : 0u;
-    constexpr uint16_t kClusterMask = (uint16_t)((1u << CL) - 1u);
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < C::STAGES; ++s) {
-            mbar_init(full_a(s), NUM_PROD_WARPS);   // one elected arrive per producer warp
+            mbar_init(full_a(s), GC_PROD_WARPS);   // one elected arrive per producer warp
             mbar_init(full_b(s), 1);
-            mbar_init(empty(s), CL);      // one tcgen05.commit per CTA of the cluster (weight slices)
-            mbar_init(empty_a(s), 1);     // this CTA's own commit (A tiles are private)
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tmem_full(a), 1);
-            mbar_init(tmem_empty(a), NUM_EPI_WARPS);
+            mbar_init(empty(s), 2);                // one arrive per consumer warpgroup
         }
         fence_barrier_init();
     }
-    if (warp == WARP_MMA) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                     "r"((uint32_t)C::TMEM_COLS)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    if (CL > 1) cluster_sync_all();      // peers' barriers must exist before anything is multicast to them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
-    if (warp >= NUM_EPI_WARPS && warp < NUM_EPI_WARPS + NUM_PROD_WARPS) {
+    if (warp >= GC_WARP_PROD) {
         // ===================== A producers =====================
-        const int pt = threadIdx.x - NUM_EPI_WARPS * 32;
+        const int pt = threadIdx.x - CONS_THREADS;
         const int r = pt & 127;                           // tile row 0..127
         const int hf = pt >> 7;                           // which half of the row's 128-byte chunk this thread fills
         RowMapTC<MODE> rowmap{nbr, taps, M, H, W};
@@ -129,8 +97,10 @@ gconv_tc_kernel(const float* __restrict__ in, const float* __restrict__ wpack, c
         const uint32_t sw = (uint32_t)(r & 7);
         int stage = 0;
         uint32_t phase = 0;
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-            const int m = tile * BM + r;
+        for (int unit = blockIdx.x; unit < nunits; unit += gridDim.x) {
+            const int m = (unit / nparts) * BM + r;
+            // pack block of chunk ch: [hi: bn rows][lo: bn rows] of 128 bytes; this unit's NB rows of each
+            const uint8_t* wsrc = (const uint8_t*)wpack + (size_t)(unit % nparts) * C::B_TILE_BYTES;
             int x = 0, y = 0;
             if (MODE == SASSD_GCONV_CONV2D) { x = m % W; y = (m / W) % H; }
             // software pipeline: the global loads of the next PF chunks are in flight (register ring) while
@@ -169,7 +139,7 @@ gconv_tc_kernel(const float* __restrict__ in, const float* __restrict__ wpack, c
                     if (ch >= nchunks) break;
                     float4 (&vn)[NF4H] = ring[u];
                     uint4 ph[4], pl[4];       // this thread's 4 of the 8 16-byte chunks of the hi / lo rows
-                    if (!ring_live[u]) {      // missing neighbour (65 % of the sparse (row, offset) slots): no split math
+                    if (!ring_live[u]) {      // missing neighbour (most sparse (row, offset) slots): no split math
 #pragma unroll
                         for (int c = 0; c < 4; ++c) { ph[c] = make_uint4(0u, 0u, 0u, 0u); pl[c] = ph[c]; }
                     } else if constexpr (PREC == 0) {
@@ -197,9 +167,18 @@ gconv_tc_kernel(const float* __restrict__ in, const float* __restrict__ wpack, c
                         }
                     }
                     if (ch + PF < nchunks) fetch(vn, ring_live[u]);        // refill this ring slot
-                    if (lane == 0) mbar_wait(empty_a(stage), phase ^ 1u);   // one polling lane per warp
+                    if (lane == 0) {                                        // one polling lane per warp
+                        mbar_wait(empty(stage), phase ^ 1u);
+                        if (warp == GC_WARP_PROD) {                         // the stage's weight block
+                            const uint32_t dst = base + stage * C::STAGE_BYTES + 2 * A_TILE_BYTES;
+                            const uint8_t* src = wsrc + (size_t)ch * (2 * bn * 128);
+                            mbar_expect_tx(full_b(stage), 2 * C::B_TILE_BYTES);
+                            bulk_g2s(dst, src, C::B_TILE_BYTES, full_b(stage));
+                            bulk_g2s(dst + C::B_TILE_BYTES, src + (size_t)bn * 128, C::B_TILE_BYTES, full_b(stage));
+                        }
+                    }
                     __syncwarp();
-                    uint8_t* a_hi = base_ptr + stage * C::STAGE_BYTES;
+                    uint8_t* a_hi = smem_raw + (base - smem_u32(smem_raw)) + stage * C::STAGE_BYTES;
                     uint8_t* a_lo = a_hi + A_TILE_BYTES;
 #pragma unroll
                     for (int c = 0; c < 4; ++c) {
@@ -207,193 +186,106 @@ gconv_tc_kernel(const float* __restrict__ in, const float* __restrict__ wpack, c
                         *(uint4*)(a_hi + off) = ph[c];
                         *(uint4*)(a_lo + off) = pl[c];
                     }
-                    // no proxy fence here (it lowers to MEMBAR.ALL.CTA and would wait for the prefetch ring's
-                    // loads still in flight); the MMA lane fences after its mbarrier wait
-                    __syncwarp();               // one arrive per warp (256 arrivals on one mbarrier per chunk
-                    if (lane == 0) mbar_arrive(full_a(stage));   // serialise for ~1-2k cycles)
+                    // no proxy fence here (it would wait for the prefetch ring's loads still in flight); the
+                    // consumers fence after their mbarrier wait
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(full_a(stage));
                     if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
                 }
-            }
-        }
-    } else if (warp == WARP_BLOAD) {
-        // ===================== B loader (weights) =====================
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-                for (int ch = 0; ch < nchunks; ++ch) {
-                    mbar_wait(empty(stage), phase ^ 1u);
-                    const uint32_t dst = base + stage * C::STAGE_BYTES + 2 * A_TILE_BYTES;
-                    const uint8_t* src = (const uint8_t*)wpack + (size_t)ch * (2 * C::B_TILE_BYTES);
-                    mbar_expect_tx(full_b(stage), 2 * C::B_TILE_BYTES);      // all slices, own and peers'
-                    if (CL == 1) {
-                        // several medium-sized bulk copies in flight move a block faster than one big one
-                        constexpr uint32_t kPiece = (2 * C::B_TILE_BYTES >= 8192) ? 8192u : (uint32_t)(2 * C::B_TILE_BYTES);
-#pragma unroll 1
-                        for (uint32_t o = 0; o < 2u * C::B_TILE_BYTES; o += kPiece)
-                            bulk_g2s(dst + o, src + o, kPiece, full_b(stage));
-                    } else {
-                        constexpr uint32_t kSlice = 2 * C::B_TILE_BYTES / CL;
-                        bulk_g2s_mc(dst + cta_rank * kSlice, src + cta_rank * kSlice, kSlice, full_b(stage), kClusterMask);
-                    }
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == WARP_MMA) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            constexpr uint32_t idesc = make_idesc(BM, BN, PR::FMT);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-                mbar_wait(tmem_empty(acc), acc_phase ^ 1u);     // epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t d_big = tmem_base + (uint32_t)(acc * 2 * BN), d_small = d_big + (uint32_t)BN;
-                for (int ch = 0; ch < nchunks; ++ch) {
-                    mbar_wait(full_a(stage), phase);
-                    fence_proxy_async();        // producers' generic-proxy stores -> visible to the async proxy
-                    mbar_wait(full_b(stage), phase);
-                    tc_fence_after();
-                    const uint32_t a_hi = base + stage * C::STAGE_BYTES, a_lo = a_hi + A_TILE_BYTES;
-                    const uint32_t b_hi = a_hi + 2 * A_TILE_BYTES, b_lo = b_hi + C::B_TILE_BYTES;
-#pragma unroll
-                    for (int k8 = 0; k8 < 4; ++k8) {
-                        const uint32_t ko = (uint32_t)k8 * 32u;     // 8 tf32 / 16 fp16 = 32 bytes along K in the swizzle row
-                        const uint64_t dah = make_desc(a_hi + ko), dal = make_desc(a_lo + ko);
-                        const uint64_t dbh = make_desc(b_hi + ko), dbl = make_desc(b_lo + ko);
-                        mma_any<PREC>(d_small, dal, dbh, idesc, (ch | k8) ? 1u : 0u);
-                        mma_any<PREC>(d_small, dah, dbl, idesc, 1u);
-                        mma_any<PREC>(d_big, dah, dbh, idesc, (ch | k8) ? 1u : 0u);
-                    }
-                    // frees the smem stage (in every CTA of the cluster) when the MMAs retire
-                    mma_commit(empty_a(stage));
-                    if (CL == 1) mma_commit(empty(stage)); else mma_commit_mc(empty(stage), kClusterMask);
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
-                }
-                mma_commit(tmem_full(acc));                    // accumulator complete -> epilogue
-                if (++acc == C::ACC_BUFS) { acc = 0; acc_phase ^= 1u; }
             }
         }
     } else {
-        // ===================== epilogue (warps 0-3; TMEM lane quarter = warp id) =====================
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        const int r = warp * 32 + lane;
-        for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-            if (lane == 0) mbar_wait(tmem_full(acc), acc_phase);
-            __syncwarp();
-            tc_fence_after();
-            const int m = tile * BM + r;
-            float* orow = out + (size_t)m * out_stride;
-            constexpr int CW = (BN >= 32) ? 32 : 16;           // columns per tcgen05.ld
-#pragma unroll 1
-            for (int c0 = 0; c0 < BN; c0 += CW) {
-                uint32_t v[CW], u[CW];
-                const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(acc * 2 * BN + c0);
-                tmem_ld<CW>(v, taddr);
-                tmem_ld<CW>(u, taddr + (uint32_t)BN);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (m < M) {
+        // ===================== consumers: MMAs + epilogue =====================
+        const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+        // big: hi*hi of the current chunk, added to sum in fp32 RN after every chunk (the tensor core's accumulation
+        // truncates: over the 2304-term K of a 3x3 256-channel layer that alone cost 4x the FFMA kernel's error);
+        // small: the cross terms of all chunks, 2^-11 smaller
+        float big[NB / 2], small[NB / 2], sum[NB / 2];
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int unit = blockIdx.x; unit < nunits; unit += gridDim.x) {
+            const int tile = unit / nparts, n0 = (unit % nparts) * NB;
 #pragma unroll
-                    for (int j = 0; j < CW; j += 4) {
-                        const int n = c0 + j;
-                        if (n >= cout) break;
-                        float o[4];
+            for (int i = 0; i < NB / 2; ++i) { small[i] = 0.f; sum[i] = 0.f; }
+            for (int ch = 0; ch < nchunks; ++ch) {
+                mbar_wait(full_a(stage), phase);
+                fence_proxy_async();        // producers' generic-proxy stores -> visible to the MMAs' async proxy
+                mbar_wait(full_b(stage), phase);
+                const uint32_t a_hi = base + stage * C::STAGE_BYTES + (uint32_t)wg * (A_TILE_BYTES / 2);
+                const uint32_t b_hi = base + stage * C::STAGE_BYTES + 2 * A_TILE_BYTES;
+                wgmma_fence();
+                mma_chunk_x3<PREC, NB>(big, small, a_hi, a_hi + A_TILE_BYTES, b_hi, b_hi + C::B_TILE_BYTES, true);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs<NB / 2>(big);
+                if (t == 0) mbar_arrive(empty(stage));
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const int ne = n + e;
-                            const float sc = (scale && ne < cout) ? __ldg(&scale[ne]) : 1.f;
-                            const float sh = (shift && ne < cout) ? __ldg(&shift[ne]) : 0.f;
-                            const float small = PREC == 0 ? __uint_as_float(u[j + e])
-                                                          : __uint_as_float(u[j + e]) * (1.f / kF16LoScale);
-                            float val = fmaf(__fadd_rn(__uint_as_float(v[j + e]), small), sc, sh);
-                            if (relu) val = fmaxf(val, 0.f);
-                            o[e] = val;
-                        }
-                        if (n + 3 < cout && (out_stride & 3) == 0) {
-                            *(float4*)(orow + n) = make_float4(o[0], o[1], o[2], o[3]);
-                        } else {
+                for (int i = 0; i < NB / 2; ++i) sum[i] = __fadd_rn(sum[i], big[i]);
+                if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
+            }
+            fence_regs<NB / 2>(small);
+            const int r0 = tile * BM + wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
 #pragma unroll
-                            for (int e = 0; e < 4; ++e)
-                                if (n + e < cout) orow[n + e] = o[e];
-                        }
+            for (int j = 0; j < NB / 8; ++j) {
+                const int n = n0 + 8 * j + 2 * (t & 3);
+                float sc[2], sh[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    sc[e] = (scale && n + e < cout) ? __ldg(&scale[n + e]) : 1.f;
+                    sh[e] = (shift && n + e < cout) ? __ldg(&shift[n + e]) : 0.f;
+                }
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int m = r0 + 8 * i;
+                    if (m >= M || n >= cout) continue;
+                    float o[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float sm = PREC == 0 ? small[4 * j + 2 * i + e] : small[4 * j + 2 * i + e] * (1.f / kF16LoScale);
+                        float val = fmaf(__fadd_rn(sum[4 * j + 2 * i + e], sm), sc[e], sh[e]);
+                        if (relu) val = fmaxf(val, 0.f);
+                        o[e] = val;
+                    }
+                    float* orow = out + (size_t)m * out_stride;
+                    if (n + 1 < cout && (out_stride & 1) == 0) *(float2*)(orow + n) = make_float2(o[0], o[1]);
+                    else {
+                        orow[n] = o[0];
+                        if (n + 1 < cout) orow[n + 1] = o[1];
                     }
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tmem_empty(acc));
-            if (++acc == C::ACC_BUFS) { acc = 0; acc_phase ^= 1u; }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (CL > 1) cluster_sync_all();      // no CTA may exit while a peer can still signal its barriers
-    if (warp == WARP_MMA) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)C::TMEM_COLS)
-                     : "memory");
     }
 }
 
-template <int MODE, int BN, int CL, int PREC>
-static int launch_cl(const sassd_gconv_desc* d, const float* in, const float* w, const float* scale, const float* shift,
-                     const int* nbr, const int* d_rows, float* out, cudaStream_t stream, int grid) {
-    using C = Cfg<BN>;
-    auto kern = gconv_tc_kernel<MODE, BN, CL, PREC>;
+template <int MODE, int NB, int PREC>
+static int launch(const sassd_gconv_desc* d, const float* in, const float* w, const float* scale, const float* shift,
+                  const int* nbr, const int* d_rows, float* out, cudaStream_t stream, int bn) {
+    using C = Cfg<NB>;
+    auto kern = gconv_tc_kernel<MODE, NB, PREC>;
     static bool configured = false;
     if (!configured) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) != cudaSuccess)
             return SASSD_ERR_LAUNCH;
         configured = true;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = C::SMEM_BYTES;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CL;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (cudaLaunchKernelEx(&cfg, kern, in, w, scale, shift, nbr, d_rows, out, d->cin, d->cout, d->taps, d->in_stride,
-                           d->out_stride, d->rows_cap, d->H, d->W, d->relu) != cudaSuccess)
-        return SASSD_ERR_LAUNCH;
+    const int nparts = bn / NB;
+    const int units = sassd_div_up(d->rows_cap, BM) * nparts;
+    const int grid = units < sassd_num_sms() ? (units > 0 ? units : 1) : sassd_num_sms();
+    kern<<<grid, GC_THREADS, C::SMEM_BYTES, stream>>>(in, w, scale, shift, nbr, d_rows, out, d->cin, d->cout, d->taps,
+                                                      d->in_stride, d->out_stride, d->rows_cap, d->H, d->W, d->relu,
+                                                      bn, nparts);
     return sassd_check_launch();
-}
-
-template <int MODE, int BN, int PREC>
-static int launch(const sassd_gconv_desc* d, const float* in, const float* w, const float* scale, const float* shift,
-                  const int* nbr, const int* d_rows, float* out, cudaStream_t stream) {
-    const int tiles = sassd_div_up(d->rows_cap, BM);
-    // Dense maps with at least one tile per SM can share the weight stream inside a cluster (CTA r multicasts the
-    // r-th slice of every weight block).  Measured on B200 (round 1, 3xTF32, BEV 3x3 256->256): cluster 2 = same
-    // time as independent CTAs, cluster 4 = 1.8x slower (lock-step stage release with 2 stages) — the kernel is
-    // MMA/shared-memory bound, not L2 bound — so it stays opt-in: SASSD_TC_CLUSTER=2.
-    if constexpr (MODE == SASSD_GCONV_CONV2D && BN == 256) {
-        static int cl = -1;
-        if (cl < 0) { const char* e = getenv("SASSD_TC_CLUSTER"); cl = e ? atoi(e) : 1; }
-        if (cl == 2 && tiles >= 148)
-            return launch_cl<MODE, BN, 2, PREC>(d, in, w, scale, shift, nbr, d_rows, out, stream, 148);
-    }
-    return launch_cl<MODE, BN, 1, PREC>(d, in, w, scale, shift, nbr, d_rows, out, stream, tiles < 148 ? tiles : 148);
 }
 
 template <int MODE, int PREC>
 static int dispatch(const sassd_gconv_desc* d, const float* in, const float* w, const float* scale, const float* shift,
                     const int* nbr, const int* d_rows, float* out, cudaStream_t s) {
-    if (d->cout <= 16) return launch<MODE, 16, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s);
-    if (d->cout <= 32) return launch<MODE, 32, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s);
-    if (d->cout <= 64) return launch<MODE, 64, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s);
-    if (d->cout <= 128) return launch<MODE, 128, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s);
-    if (d->cout <= 256) return launch<MODE, 256, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s);
+    if (d->cout <= 16) return launch<MODE, 16, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s, 16);
+    if (d->cout <= 32) return launch<MODE, 32, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s, 32);
+    if (d->cout <= 64) return launch<MODE, 64, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s, 64);
+    if (d->cout <= 128) return launch<MODE, 64, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s, 128);
+    if (d->cout <= 256) return launch<MODE, 64, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s, 256);
     return SASSD_ERR_UNSUPPORTED;
 }
 

@@ -223,7 +223,7 @@ extern "C" int sassd_pswarp(const float* feat, int feat_stride, int batch, int H
     if (!feat || !boxes || !d_k || !scores || feat_stride < 28 || batch < 1 || k_cap < 1) return SASSD_ERR_ARG;
     const int wpb = 8;
     int gx = (k_cap + wpb - 1) / wpb;
-    if (gx > 148 * 4) gx = 148 * 4;
+    if (gx > sassd_num_sms() * 4) gx = sassd_num_sms() * 4;
     dim3 grid(gx, batch);
     pswarp_kernel<<<grid, wpb * 32, 0, (cudaStream_t)stream_>>>(feat, feat_stride, H, W, boxes, d_k, k_cap, off_x,
                                                                 off_y, spatial_scale, scores);

@@ -144,8 +144,8 @@ __device__ __forceinline__ float rotated_iou(const float* box_a, const float* bo
 // The grid is fixed (CUDA-graph friendly); each CTA walks the frame's live upper-triangle work items, whose number
 // depends on the device-side candidate count.  A work item is a QUARTER of a 64x64 tile - 64 rows x 16 columns, one
 // pair per thread: the guided anchors of an object overlap each other heavily, so many pairs take the slow rotated
-// polygon-clipping path, and with four pairs per thread (round 1) a frame's handful of tiles kept six SMs busy for
-// ~40 us (profiles/r2_ncu_small_kernels.md).  Each item writes its own 16-bit quarter of the 64-bit mask words.
+// polygon-clipping path, and with four pairs per thread a frame's handful of tiles would keep a few SMs busy while
+// the rest idle.  Each item writes its own 16-bit quarter of the 64-bit mask words.
 #define NMS_MASK_THREADS 1024   // 64 rows x 16 columns
 __global__ void __launch_bounds__(NMS_MASK_THREADS)
 nms_mask_kernel(const float* __restrict__ boxes5, const int* __restrict__ d_n, int n_fixed, int n_cap, int colb_cap,
@@ -419,7 +419,7 @@ extern "C" int sassd_nms_mask(const float* boxes5, int n, float thr, uint64_t* m
     const int colb = (n + 63) / 64;
     cudaMemsetAsync(mask, 0, (size_t)n * colb * 8, (cudaStream_t)stream_);
     const long long nitems = 4ll * colb * (colb + 1) / 2;    // quarter tiles
-    dim3 grid((unsigned)(nitems < 148 * 16 ? nitems : 148 * 16), 1);
+    dim3 grid((unsigned)(nitems < sassd_num_sms() * 16 ? nitems : sassd_num_sms() * 16), 1);
     nms_mask_kernel<<<grid, NMS_MASK_THREADS, 0, (cudaStream_t)stream_>>>(boxes5, nullptr, n, n, colb, thr,
                                                             (unsigned long long*)mask);
     return sassd_check_launch();

@@ -121,7 +121,7 @@ nbr_fill_kernel(const int4* __restrict__ coors_out, const int* __restrict__ d_ro
 
 static int nbr_grid(int rows_cap) {
     const int tiles = sassd_div_up(rows_cap, NBR_TILE_ROWS);
-    return tiles < 148 * 2 ? (tiles > 0 ? tiles : 1) : 148 * 2;
+    return tiles < sassd_num_sms() * 2 ? (tiles > 0 ? tiles : 1) : sassd_num_sms() * 2;
 }
 
 extern "C" int sassd_rulebook_subm(const int32_t* coors, const int32_t* d_rows, int rows_cap, int D, int H, int W,

@@ -1,28 +1,21 @@
 // Ruled sparse convolution (SubMConv3d / SparseConv3d / 1x1x1; spconv v1.0 indice_conv semantics, call sites
-// mmdet/models/necks/cmn.py:145-173,192-231) on tcgen05 FP16x3 with the features kept in "split rows":
-// two fp16 planes [2][rows_cap][C] (hi = half(x), lo = half((x - hi) * 2048)), C a multiple of 8.
+// mmdet/models/necks/cmn.py:145-173,192-231) on the Hopper tensor cores (wgmma) with FP16x3 and the features kept in
+// "split rows": two fp16 planes [2][rows_cap][C] (hi = half(x), lo = half((x - hi) * 2048)), C a multiple of 8.
 //
 // Structure (one CTA = one 128-row output tile at a time, output-stationary, no atomics, deterministic):
 //   * 8 producer warps only *issue* 16-byte cp.async gathers (zero fill for missing neighbours) straight into the
-//     128B-swizzled operand tiles plus an asynchronous mbarrier arrive; nobody waits for data.  The tile's [128,27]
-//     neighbour indices arrive by one bulk copy.
-//   * a helper warp does the generic->async proxy fence, one lane streams the weight blocks with cp.async.bulk.
-//   * the MMA warp runs its loop warp-convergent (uniform datapath), one elected lane issues
-//     x*w = ah*bh + (ah*bl + al*bh)/2048 as TWO instructions per K=16 step: ah x [bh | bl] (N = 2*BN) and al x bh.
-//     Round 2: the issue loop itself was the bound (profiles/r2_mma_issue_probe.md: ~20 SASS instructions per UTCHMMA
-//     = 100-130 clk against a 32-64 clk tensor floor), so descriptors are a per-stage low word + immediates.
+//     128B-swizzled operand tiles plus an asynchronous mbarrier arrive; nobody waits for data.  Lane 0 of the first
+//     producer warp also streams the weight blocks and the tile's [128,27] neighbour indices with cp.async.bulk.
+//   * two consumer warpgroups (64 rows each) wait for the gathers, fence the generic->async proxy and issue
+//     x*w = ah*bh + (ah*bl + al*bh)/2048 as wgmma (M = 64, N = BN, K = 16) into two register accumulators, then
+//     run the epilogue (folded BN, ReLU, next layer's split planes and / or fp32 rows) from registers.
 //   * narrow layers pack 2/4/8 taps into one 64-wide K chunk.
-//   * tap skipping (round 2): the rulebook kernel records, per 128-row tile, which of the 27 taps have a neighbour
+//   * tap skipping: the rulebook kernel records, per 128-row tile, which of the 27 taps have a neighbour
 //     at all (tile_mask); chunks whose taps are all absent are skipped by every role - reference semantics only need
 //     the listed pairs (spconv's indice_pairs), an absent pair contributes exactly zero.
 //   * small layers (2 * tiles <= CTAs, i.e. one frame at a time): the two CTAs of a cluster split the active chunks
-//     of ONE tile (split-K over taps); the peer hands its fp32 partial sums to the leader through an L2-resident
-//     scratch row block and a remote mbarrier arrive (release/acquire at cluster scope), the leader adds them in a
-//     fixed order and runs the epilogue.  A 45-tile layer then occupies 90 SMs with half the chunk chain each.
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
-
+//     of ONE tile (split-K over taps); each hands the fp32 partial sums of the rows it does not finalise to its peer
+//     through an L2-resident scratch row block and a remote mbarrier arrive (release/acquire at cluster scope).
 #include "tc_common.cuh"
 
 namespace sps {
@@ -30,23 +23,19 @@ namespace sps {
 using namespace tc;
 
 constexpr int BKC = 64;                 // channels per chunk
-constexpr int EPI_WARPS = 4, PROD_WARPS = 8;
-constexpr int THREADS3 = (EPI_WARPS + PROD_WARPS + 3) * 32;   // 480
-constexpr int W_MMA = EPI_WARPS + PROD_WARPS, W_BLOAD = W_MMA + 1, W_FENCE = W_MMA + 2;
+constexpr int PROD_WARPS = 8;
+constexpr int THREADS3 = CONS_THREADS + PROD_WARPS * 32;   // 512: 16 warps split evenly over the register file
+constexpr int W_PROD = CONS_THREADS / 32;
 constexpr int CLUSTER = 2;              // CTAs per cluster (tap split for small layers)
-constexpr int SPLIT_TILES_MAX = 74;     // tiles of the scratch block (148 SMs / CLUSTER)
+constexpr int SPLIT_TILES_MAX = 74;     // tiles of the scratch block (one per cluster: up to 148 CTAs per grid)
 
 template <int BN>
 struct Cfg3 {
     static constexpr int B_TILE_BYTES = BN * 128;
     static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
     static constexpr int STAGES = 4;
-    static constexpr int ACC_BUFS = 2;
-    // per accumulator buffer: [big | small1] written by the N = 2*BN instruction, then small2
-    static constexpr int ACC_COLS = 3 * BN;
-    static constexpr int TMEM_COLS = ACC_BUFS * ACC_COLS <= 128 ? 128 : (ACC_BUFS * ACC_COLS <= 256 ? 256 : 512);
     static constexpr int NBR_TILE_BYTES = BM * 27 * 4;                    // one tile's rows of the [rows, 27] table
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * NBR_TILE_BYTES + 1024 + 256;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * NBR_TILE_BYTES + 1024 + 512 + 256;
 };
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
@@ -93,10 +82,7 @@ struct Args {
     float* out_f32;         // [rows_cap][out_f32_stride] or null
     float* scratch;         // [SPLIT_TILES_MAX][128][BN] fp32 partial sums of the peer CTA (null: no tap split)
     int* counters;          // optional [2]: executed (tile, chunk) pairs, tiles (bench instrumentation)
-    long long* trace;       // optional [grid][16] clock64 sums per CTA (SASSD_SPS_TRACE=1, timing experiments only)
     int cin, cout, taps, rows_cap, relu, out_ch, out_f32_stride;
-    int dbg;                // SASSD_SPS_DBG (timing experiments only): 1 = no tap skipping, 2 = no tap split,
-                            // 16 = no MMAs, 32 = no gather copies
 };
 
 // The chunks of one tile this CTA executes, identical in every role: chunk g is active when one of its taps is in the
@@ -134,20 +120,13 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
     auto full_a = [&](int s, int w) { return bar_base + 512u + 8u * (s * PROD_WARPS + w); };   // one per producer warp:
                                                                    // 32 async arrivals each, on separate words
     auto full_b = [&](int s) { return bar_base + 8u * (C::STAGES + s); };         // weight block landed
-    auto ready_a = [&](int s) { return bar_base + 8u * (2 * C::STAGES + s); };    // full_a + proxy fence done
     auto empty = [&](int s) { return bar_base + 8u * (3 * C::STAGES + s); };
-    auto tmem_full = [&](int a) { return bar_base + 8u * (4 * C::STAGES + a); };
-    auto tmem_empty = [&](int a) { return bar_base + 8u * (4 * C::STAGES + 2 + a); };
     auto nbr_full = [&](int b) { return bar_base + 8u * (4 * C::STAGES + 4 + b); };
     auto nbr_empty = [&](int b) { return bar_base + 8u * (4 * C::STAGES + 6 + b); };
     const uint32_t peer_done = bar_base + 8u * (4 * C::STAGES + 8);               // the peer's partial sums of my rows are in L2
-    const uint32_t tmem_slot = bar_base + 8u * (4 * C::STAGES + 9);
-    volatile uint32_t* tmem_slot_ptr = (volatile uint32_t*)(base_ptr + (tmem_slot - base));
 
-    const long long t_start = p.trace ? clock64() : 0;
     pdl_launch_dependents();      // the next layer may be scheduled as this grid's CTAs retire
-    // warp index through a shuffle: the compiler then knows it is warp-uniform and keeps the role loops on the
-    // uniform datapath
+    // warp index through a shuffle: the compiler then knows it is warp-uniform
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
     // Tap packing: a chunk is 64 K-columns = `tpg` taps of `cin` stored channels each (cin 8/16/32 -> 8/4/2 taps per
     // chunk), so the narrow early layers run 4/7/14 chunks per tile instead of 27.  The weight pack has the same
@@ -163,40 +142,26 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
         for (int s = 0; s < C::STAGES; ++s) {
             for (int w = 0; w < PROD_WARPS; ++w) mbar_init(full_a(s, w), 32);
             mbar_init(full_b(s), 1);
-            mbar_init(ready_a(s), 1);
-            mbar_init(empty(s), 1);
+            mbar_init(empty(s), 2);                      // one arrive per consumer warpgroup
         }
-        for (int a = 0; a < 2; ++a) { mbar_init(tmem_full(a), 1); mbar_init(tmem_empty(a), EPI_WARPS); }
         for (int b = 0; b < 2; ++b) { mbar_init(nbr_full(b), 1); mbar_init(nbr_empty(b), PROD_WARPS); }
-        mbar_init(peer_done, (EPI_WARPS / 2) * 32);      // the peer's two giver warps
+        mbar_init(peer_done, 128);                       // the peer's giver warpgroup
         fence_barrier_init();
     }
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot),
-                     "r"((uint32_t)C::TMEM_COLS)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
     cluster_sync_all();           // the peer's barriers exist before anyone arrives on them remotely
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
     pdl_wait();                   // producing layer / rulebook complete; nothing above touched global data
     const int M = p.d_rows ? min(__ldg(p.d_rows), p.rows_cap) : p.rows_cap;
     const int ntiles = (M + BM - 1) / BM;
-    long long* tr = p.trace ? p.trace + (size_t)blockIdx.x * 16 : nullptr;
-    if (tr && threadIdx.x == 0) { tr[0] = t_start; tr[1] = clock64(); }
     // Work decomposition, uniform over the grid: R full rounds of one tile per CTA, then the remaining `rem` tiles.  A
-    // layer that has at most half as many tiles as there are CTAs (one frame at a time: 42-74 tiles) runs as a TAP
-    // SPLIT: cluster q owns tile q and its two CTAs share that tile's chunks, so a 45-tile layer occupies 90 SMs with
-    // half the chunk chain each.  (Splitting only the last partial round of a LARGE layer was measured too - 933
-    // tiles: 6.5 instead of 7 rounds - and lost what it gained to the hand-over at the very end of the kernel, where
-    // nothing overlaps it: B=16 sparse stage 1.178 -> 1.233 ms.  Hence R == 0.)
+    // layer that has at most half as many tiles as there are CTAs (one frame at a time) runs as a TAP SPLIT: cluster q
+    // owns tile q and its two CTAs share that tile's chunks, so a 45-tile layer occupies 90 SMs with half the chunk
+    // chain each.  Splitting only the last partial round of a large layer does not pay: the hand-over at the very end
+    // of the kernel overlaps nothing.  Hence R == 0.
     const uint32_t crank = cluster_ctarank();
     const int G = (int)gridDim.x;
     const int R = ntiles / G, rem = ntiles - R * G;
-    const bool tail_split = TABLE && p.scratch && !(p.dbg & 2) && nchunks > 1 && R == 0 && rem > 0 && 2 * rem <= G &&
+    const bool tail_split = TABLE && p.scratch && nchunks > 1 && R == 0 && rem > 0 && 2 * rem <= G &&
                             rem <= SPLIT_TILES_MAX;
     const int n_items = R + ((tail_split ? (int)(blockIdx.x >> 1) < rem : (int)blockIdx.x < rem) ? 1 : 0);
     struct Item { int tile, part, nparts; };
@@ -209,7 +174,7 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
     };
     auto chunks_of = [&](const Item& it) {
         uint32_t tm = all_taps;
-        if (TABLE && p.tile_mask && !(p.dbg & 1)) {
+        if (TABLE && p.tile_mask) {
             tm = (uint32_t)__ldg(&p.tile_mask[it.tile]) & all_taps;
             if (!tm) tm = 1u;       // a tile without any pair still has to produce act(shift): run one (all-zero) chunk
         }
@@ -219,19 +184,16 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
     // same few L2 lines for the same 16 KB at the same time; each tile therefore starts at a different tap
     // (rotation by a tile-dependent offset, identical in all roles; the sum over taps is order-independent up to fp32
     // rounding and deterministic per tile).
-    auto rot_of = [&](int tile) { return (p.dbg & 4) ? 0 : (int)(((unsigned)tile * 11u) % (unsigned)nchunks); };
+    auto rot_of = [&](int tile) { return (int)(((unsigned)tile * 11u) % (unsigned)nchunks); };
 
-    if (warp >= EPI_WARPS && warp < EPI_WARPS + PROD_WARPS) {
+    if (warp >= W_PROD) {
         // ===================== A producers: cp.async gather of split rows =====================
         // Nothing in this instruction stream waits for data: every thread issues its eight 16-byte copies (hardware
         // zero fill for a missing neighbour) and an asynchronous mbarrier arrive that fires when they have landed, so
-        // the gather runs STAGES chunks ahead.
-        // Lane mapping (round 2, tests/tools/ldgsts_probe.cu): the 8 lanes of an octet copy the 8 pieces of ONE
-        // 128-byte row, so an LDGSTS instruction touches 4 rows = 4 cache lines and costs ~7 clk whatever the rows hold
-        // (463 clk per 32 KB chunk).  With lane = row (round 1) an instruction touched 32 lines and the L1 serves about
-        // one line per clock: 725 clk per chunk at 35 % neighbour density, 2044 clk at 100 %.  Skipping absent rows
-        // (votes, dirty bits, ballot compaction) was measured too: the extra instructions cost more than they save.
-        const int pw = warp - EPI_WARPS;                    // rows 16 pw .. 16 pw + 15
+        // the gather runs STAGES chunks ahead.  The 8 lanes of an octet copy the 8 pieces of ONE 128-byte row, so a
+        // copy instruction touches 4 rows = 4 cache lines whatever the rows hold.
+        const int pw = warp - W_PROD;                       // rows 16 pw .. 16 pw + 15
+        const bool loader = pw == 0 && lane == 0;           // also streams weights and neighbour-table tiles
         const int piece = lane & 7, oct = lane >> 3;
         const int tl = piece / ppt, pc8 = (piece - tl * ppt) * 8;     // my tap within the chunk, element offset in it
         uint32_t offs[4];                                   // shared-memory offset of my 16 bytes of row j (any stage)
@@ -248,23 +210,30 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
         uint32_t phase = 0;
         int nb = 0;                    // neighbour-table buffer of this tile
         uint32_t nb_phase = 0;
-        long long tw = 0, ti = 0, tn = 0;
-        const bool trp = tr && pw == 0 && lane == 0;
+        int ld_nb = 0;                 // loader: next neighbour-table buffer to fill
+        uint32_t ld_nb_phase = 0;
+        auto load_nbr = [&](int tile) {     // one bulk copy: the tile's rows of the table are contiguous
+            const int rows_here = min(BM, p.rows_cap - tile * BM);
+            const uint32_t bytes = (uint32_t)(rows_here * p.taps * 4) & ~15u;
+            mbar_wait(nbr_empty(ld_nb), ld_nb_phase ^ 1u);
+            mbar_expect_tx(nbr_full(ld_nb), bytes);
+            if (bytes) bulk_g2s(nbr_base + ld_nb * C::NBR_TILE_BYTES, p.nbr + (size_t)tile * BM * p.taps, bytes, nbr_full(ld_nb));
+            if (++ld_nb == 2) { ld_nb = 0; ld_nb_phase ^= 1u; }
+        };
+        if (loader && nbr_tiles && n_items > 0) load_nbr(item_at(0).tile);
         for (int ii = 0; ii < n_items; ++ii) {
             const Item item = item_at(ii);
             const int tile = item.tile;
-            // rows of the table the loader thread copied for this tile (whole 16-byte units only)
+            // rows of the table the loader copied for this tile (whole 16-byte units only)
             const int rows_here = min(BM, p.rows_cap - tile * BM);
             const int rows_copied = nbr_tiles ? ((rows_here * p.taps * 4) & ~15) / (p.taps * 4) : 0;
             const int* ntile = nbr_smem + nb * (C::NBR_TILE_BYTES / 4);
             const uint32_t cmask = chunks_of(item);
             const int m0 = tile * BM + pw * 16 + oct;       // global row of j = 0
-            long long c0 = trp ? clock64() : 0;
             if (nbr_tiles) {
                 if (lane == 0) mbar_wait(nbr_full(nb), nb_phase);
                 __syncwarp();
             }
-            if (trp) tn += clock64() - c0;
             const int rot = rot_of(tile);
             auto chunk_at = [&](int gi) { return gi + rot < nchunks ? gi + rot : gi + rot - nchunks; };
             auto next_active = [&](int gi) {            // next position of the rotated walk whose chunk is executed
@@ -272,13 +241,11 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
                     if ((cmask >> chunk_at(gi)) & 1u) break;
                 return gi;
             };
-            // The neighbour indices are shared-memory loads, i.e. they go through the same LSU queue as the cp.async
-            // copies: issued after a chunk's copies they return only when those have drained (~a chunk period - the
-            // trace showed ~850 clk per chunk of this thread waiting for four LDS).  So the indices of the NEXT chunk are
-            // requested BEFORE this chunk's copies are queued.
+            // The neighbour indices are shared-memory loads through the same LSU queue as the cp.async copies, so
+            // the indices of the NEXT chunk are requested BEFORE this chunk's copies are queued.
             auto load_srcs = [&](int g, int (&dst)[4]) {
                 const int t = g * tpg + tl;
-                const bool tap_ok = tl < tpg && t < p.taps && !(p.dbg & 32);
+                const bool tap_ok = tl < tpg && t < p.taps;
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     const int m = m0 + 4 * j;
@@ -294,10 +261,16 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
             while (gi < nchunks) {
                 const int gi_next = next_active(gi);
                 // one lane polls the mbarrier, the warp follows
-                c0 = trp ? clock64() : 0;
-                if (lane == 0) mbar_wait(empty(stage), phase ^ 1u);
+                if (lane == 0) {
+                    mbar_wait(empty(stage), phase ^ 1u);
+                    if (loader) {
+                        const uint32_t dst = base + stage * C::STAGE_BYTES + 2 * A_TILE_BYTES;
+                        const uint8_t* src = (const uint8_t*)p.wpack + (size_t)chunk_at(gi) * (2 * C::B_TILE_BYTES);
+                        mbar_expect_tx(full_b(stage), 2 * C::B_TILE_BYTES);
+                        bulk_g2s(dst, src, 2 * C::B_TILE_BYTES, full_b(stage));
+                    }
+                }
                 __syncwarp();
-                const long long c1 = trp ? clock64() : 0;
                 int nxt[4] = {-1, -1, -1, -1};
                 if (gi_next < nchunks) load_srcs(chunk_at(gi_next), nxt);
                 const uint32_t a_hi = base + stage * C::STAGE_BYTES, a_lo = a_hi + A_TILE_BYTES;
@@ -309,7 +282,6 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
                     cp_async16(a_lo + offs[j], in_lo + eo, nbytes);
                 }
                 cp_async_arrive_noinc(full_a(stage, pw));
-                if (trp) { tw += c1 - c0; ti += clock64() - c1; }
                 if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
 #pragma unroll
                 for (int j = 0; j < 4; ++j) srcs[j] = nxt[j];
@@ -320,265 +292,110 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
                 if (lane == 0) mbar_arrive(nbr_empty(nb));
                 if (++nb == 2) { nb = 0; nb_phase ^= 1u; }
             }
-        }
-        if (trp) { tr[2] = tw; tr[3] = ti; tr[4] = tn; tr[5] = clock64(); }
-    } else if (warp == W_BLOAD) {
-        // ===================== weights + neighbour-table tiles (bulk copies) =====================
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            int nb = 0;
-            uint32_t nb_phase = 0;
-            auto load_nbr = [&](int tile) {     // one bulk copy: the tile's rows of the table are contiguous
-                const int rows_here = min(BM, p.rows_cap - tile * BM);
-                const uint32_t bytes = (uint32_t)(rows_here * p.taps * 4) & ~15u;
-                mbar_wait(nbr_empty(nb), nb_phase ^ 1u);
-                mbar_expect_tx(nbr_full(nb), bytes);
-                if (bytes) bulk_g2s(nbr_base + nb * C::NBR_TILE_BYTES, p.nbr + (size_t)tile * BM * p.taps, bytes, nbr_full(nb));
-                if (++nb == 2) { nb = 0; nb_phase ^= 1u; }
-            };
-            if (nbr_tiles && n_items > 0) load_nbr(item_at(0).tile);
-            for (int ii = 0; ii < n_items; ++ii) {
-                const Item item = item_at(ii);
-                const int tile = item.tile;
-                if (nbr_tiles && ii + 1 < n_items) load_nbr(item_at(ii + 1).tile);
-                const uint32_t cmask = chunks_of(item);
-                const int rot = rot_of(tile);
-                for (int ci = 0; ci < nchunks; ++ci) {
-                    const int ch = ci + rot < nchunks ? ci + rot : ci + rot - nchunks;
-                    if (!((cmask >> ch) & 1u)) continue;
-                    mbar_wait(empty(stage), phase ^ 1u);
-                    const uint32_t dst = base + stage * C::STAGE_BYTES + 2 * A_TILE_BYTES;
-                    const uint8_t* src = (const uint8_t*)p.wpack + (size_t)ch * (2 * C::B_TILE_BYTES);
-                    mbar_expect_tx(full_b(stage), 2 * C::B_TILE_BYTES);
-                    bulk_g2s(dst, src, 2 * C::B_TILE_BYTES, full_b(stage));
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == W_FENCE) {
-        // ===================== proxy fence on behalf of the MMA lane =====================
-        // The producers write shared memory through the generic proxy (cp.async), tcgen05.mma reads it through the
-        // async proxy, so a fence.proxy.async has to sit between.  In the producers it lowers to MEMBAR.ALL.CTA and
-        // stalls on their own in-flight copies; in the MMA lane it costs 130-650 clk per chunk that are serial with
-        // MMA issue (round-1 timeline trace).  This lane has nothing else to do.
-        // Lanes 0..7 each wait for one producer warp's barrier (in parallel), lane 0 then fences and signals.
-        {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int ii = 0; ii < n_items; ++ii) {
-                const Item item = item_at(ii);
-                const int tile = item.tile;
-                const uint32_t cmask = chunks_of(item);
-                const int rot = rot_of(tile);
-                for (int ci = 0; ci < nchunks; ++ci) {
-                    const int ch = ci + rot < nchunks ? ci + rot : ci + rot - nchunks;
-                    if (!((cmask >> ch) & 1u)) continue;
-                    if (lane < PROD_WARPS) mbar_wait(full_a(stage, lane), phase);
-                    __syncwarp();
-                    if (lane == 0) {
-                        fence_proxy_async();
-                        mbar_arrive(ready_a(stage));
-                    }
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
-                }
-            }
-        }
-    } else if (warp == W_MMA) {
-        // ===================== MMA issue: warp-convergent loop, one elected lane issues =====================
-        // x*w = ah*bh + (ah*bl + al*bh)/2048 as TWO instructions per K=16 step: ah x [bh | bl] (N = 2*BN, the weight
-        // block's hi and lo rows are contiguous) -> big and small1, al x bh (N = BN) -> small2.
-        constexpr uint32_t idesc2 = make_idesc(BM, 2 * BN, 0u /*F16*/), idesc1 = make_idesc(BM, BN, 0u);
-        constexpr uint32_t kStageLo = (uint32_t)C::STAGE_BYTES >> 4, kTileLo = (uint32_t)A_TILE_BYTES >> 4;
-        const bool leader = elect_one();
-        const uint32_t lo0 = desc_lo(base);
-        int stage = 0;
-        uint32_t phase = 0;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        int executed = 0, tiles_done = 0;
-        long long mw = 0, mi = 0, me = 0, mwb = 0;
-        const bool trm = tr && leader;
-        for (int ii = 0; ii < n_items; ++ii) {
-            const Item item = item_at(ii);
-            const int tile = item.tile, part = item.part;
-            const uint32_t cmask = chunks_of(item);
-            long long c0 = trm ? clock64() : 0;
-            mbar_wait(tmem_empty(acc), acc_phase ^ 1u);
-            tc_fence_after();
-            if (trm) me += clock64() - c0;
-            const uint32_t d_big = tmem_base + (uint32_t)(acc * C::ACC_COLS), d_small2 = d_big + (uint32_t)(2 * BN);
-            uint32_t accum = 0u;
-            const int rot = rot_of(tile);
-            for (int ci = 0; ci < nchunks; ++ci) {
-                const int ch = ci + rot < nchunks ? ci + rot : ci + rot - nchunks;
-                if (!((cmask >> ch) & 1u)) continue;
-                c0 = trm ? clock64() : 0;
-                mbar_wait(ready_a(stage), phase);
-                const long long cb = trm ? clock64() : 0;
-                mbar_wait(full_b(stage), phase);
-                tc_fence_after();
-                const long long c1 = trm ? clock64() : 0;
-                if (trm) mwb += c1 - cb;
-                // channels beyond cin are zero in both operands: issue only the K=16 steps that carry data
-                const int ksteps = (p.dbg & 16) ? 0 : min(4, (min(tpg, p.taps - ch * tpg) * cin + 15) / 16);
-                const uint32_t ah = lo0 + (uint32_t)stage * kStageLo, al = ah + kTileLo, bh = al + kTileLo;
-                if (leader) {
-                    if (ksteps == 4) {          // the common case, straight-line
-                        mma_f16_lo(d_big, ah, bh, idesc2, accum);
-                        mma_f16_lo(d_small2, al, bh, idesc1, accum);
-#pragma unroll
-                        for (uint32_t k = 1; k < 4; ++k) {
-                            mma_f16_lo(d_big, ah + k * kDescK16, bh + k * kDescK16, idesc2, 1u);
-                            mma_f16_lo(d_small2, al + k * kDescK16, bh + k * kDescK16, idesc1, 1u);
-                        }
-                    } else {
-                        for (int k = 0; k < ksteps; ++k) {
-                            mma_f16_lo(d_big, ah + (uint32_t)k * kDescK16, bh + (uint32_t)k * kDescK16, idesc2, k ? 1u : accum);
-                            mma_f16_lo(d_small2, al + (uint32_t)k * kDescK16, bh + (uint32_t)k * kDescK16, idesc1, k ? 1u : accum);
-                        }
-                    }
-                    mma_commit(empty(stage));
-                }
-                __syncwarp();
-                if (trm) { mw += c1 - c0; mi += clock64() - c1; }
-                if (ksteps) accum = 1u;
-                ++executed;
-                if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
-            }
-            if (leader) mma_commit(tmem_full(acc));
-            __syncwarp();
-            if (part == 0) ++tiles_done;
-            if (++acc == C::ACC_BUFS) { acc = 0; acc_phase ^= 1u; }
-        }
-        if (trm) { tr[6] = mw; tr[7] = mi; tr[8] = me; tr[9] = clock64(); tr[10] = executed; tr[12] = mwb; }
-        if (p.counters && leader && executed) {
-            atomicAdd(&p.counters[0], executed);
-            atomicAdd(&p.counters[1], tiles_done);
+            // The next tile's table goes into the buffer of tile ii - 1, which every producer warp has released long
+            // before this warp has issued all of tile ii's copies: requested here, the wait costs nothing and warp 0
+            // starts tile ii without waiting for the slowest warp of tile ii - 1.
+            if (loader && nbr_tiles && ii + 1 < n_items) load_nbr(item_at(ii + 1).tile);
         }
     } else {
-        // ===================== epilogue =====================
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        const int r = warp * 32 + lane;
+        // ===================== consumers: MMAs, then the epilogue from registers =====================
+        const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+        float big[BN / 2], small[BN / 2];
+        int stage = 0;
+        uint32_t phase = 0;
+        int executed = 0, tiles_done = 0;
         for (int ii = 0; ii < n_items; ++ii) {
             const Item item = item_at(ii);
             const int tile = item.tile, part = item.part;
             const bool split = item.nparts == 2;
             const uint32_t cmask = chunks_of(item);
-            const bool have_acc = cmask != 0;       // a split peer may have been dealt no chunk at all
-            if (have_acc) {
-                if (lane == 0) mbar_wait(tmem_full(acc), acc_phase);
-                __syncwarp();
-                tc_fence_after();
-            }
-            const int m = tile * BM + r;
-            // Tap split: the two CTAs hold partial sums of the SAME 128 rows.  Each finalises half of them - CTA 0
-            // rows 0..63 (its epilogue warps 0, 1), CTA 1 rows 64..127 (warps 2, 3) - and its other two warps
-            // ("givers") hand the partial sums of the rows it does not own to the peer: fp32 rows in an L2-resident
-            // scratch block, then a remote mbarrier arrive (release / acquire at cluster scope).  Half the bytes
-            // cross, in both directions at once, and the BN / split / store work is shared.
-            float* prow = split ? p.scratch + ((size_t)(tile - R * G) * BM + r) * BN : nullptr;
-            const bool giver = split && ((warp >> 1) != part);
-            if (split && !giver) {              // keeper: the peer's partial sums of my rows must be visible
-                if (lane == 0) mbar_wait_cluster(peer_done, 0u);
-                __syncwarp();
-            }
-            constexpr int CW = 16;
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) { big[i] = 0.f; small[i] = 0.f; }
+            const int rot = rot_of(tile);
+            int prev = -1;
+            for (int ci = 0; ci < nchunks; ++ci) {
+                const int ch = ci + rot < nchunks ? ci + rot : ci + rot - nchunks;
+                if (!((cmask >> ch) & 1u)) continue;
+                // the gathers are generic-proxy writes (cp.async): fence before the MMAs read them
 #pragma unroll 1
-            for (int c0 = 0; c0 < BN; c0 += CW) {
-                uint32_t v[CW], u[CW], w[CW];
-                const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(acc * C::ACC_COLS + c0);
-                const int nl = c0 + (lane & (CW - 1));
-                const float scl = (p.scale && nl < p.cout) ? __ldg(&p.scale[nl]) : 1.f;
-                const float shl = (p.shift && nl < p.cout) ? __ldg(&p.shift[nl]) : 0.f;
-                float4 q4[CW / 4];              // keeper: the peer's partial sums, requested before the TMEM loads
-                if (split && !giver) {
+                for (int w = 0; w < PROD_WARPS; ++w) mbar_wait(full_a(stage, w), phase);
+                fence_proxy_async();
+                mbar_wait(full_b(stage), phase);
+                const uint32_t ah = base + stage * C::STAGE_BYTES + (uint32_t)wg * (A_TILE_BYTES / 2);
+                const uint32_t bh = base + stage * C::STAGE_BYTES + 2 * A_TILE_BYTES;
+                wgmma_fence();
+                // K columns past the chunk's last tap are zero in both operands (zero-filled gather, zero weight rows)
+                mma_chunk_x3<1, BN>(big, small, ah, ah + A_TILE_BYTES, bh, bh + C::B_TILE_BYTES);
+                wgmma_commit();
+                wgmma_wait<1>();            // the previous chunk's MMAs have read their stage
+                if (prev >= 0 && t == 0) mbar_arrive(empty(prev));
+                prev = stage;
+                ++executed;
+                if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
+            }
+            wgmma_wait<0>();
+            fence_regs<BN / 2>(big);
+            fence_regs<BN / 2>(small);
+            if (prev >= 0 && t == 0) mbar_arrive(empty(prev));
+            if (part == 0) ++tiles_done;
+            // Tap split: the two CTAs hold partial sums of the SAME 128 rows.  Each finalises half of them - CTA 0
+            // rows 0..63 (warpgroup 0), CTA 1 rows 64..127 (warpgroup 1) - and its other warpgroup ("giver") hands
+            // the partial sums of the rows it does not own to the peer: fp32 values in an L2-resident scratch block
+            // at the positions of the (identical) register layout, then a remote mbarrier arrive (release / acquire
+            // at cluster scope).  Half the bytes cross, in both directions at once, and the epilogue work is shared.
+            const bool giver = split && wg != part;
+            const int rl0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);    // tile rows rl0 and rl0 + 8
+            float* prow = split ? p.scratch + (size_t)(tile - R * G) * BM * BN : nullptr;
+            if (split && !giver) {              // keeper: the peer's partial sums of my rows must be visible
+                mbar_wait_cluster(peer_done, 0u);
+            }
 #pragma unroll
-                    for (int j = 0; j < CW / 4; ++j) q4[j] = __ldcg((const float4*)(prow + c0 + 4 * j));   // L2
-                }
-                if (have_acc) {
-                    tmem_ld<CW>(v, taddr);
-                    tmem_ld<CW>(u, taddr + (uint32_t)BN);
-                    tmem_ld<CW>(w, taddr + (uint32_t)(2 * BN));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    if (c0 + CW >= BN) {      // accumulators are in registers: release the buffer to the MMA lane
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(tmem_empty(acc));
+            for (int j = 0; j < BN / 8; ++j) {
+                const int n = 8 * j + 2 * (t & 3);
+                const float scl0 = (p.scale && n < p.cout) ? __ldg(&p.scale[n]) : 1.f;
+                const float scl1 = (p.scale && n + 1 < p.cout) ? __ldg(&p.scale[n + 1]) : 1.f;
+                const float shl0 = (p.shift && n < p.cout) ? __ldg(&p.shift[n]) : 0.f;
+                const float shl1 = (p.shift && n + 1 < p.cout) ? __ldg(&p.shift[n + 1]) : 0.f;
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int rl = rl0 + 8 * i, m = tile * BM + rl;
+                    float a0 = __fadd_rn(big[4 * j + 2 * i], small[4 * j + 2 * i] * (1.f / kF16LoScale));
+                    float a1 = __fadd_rn(big[4 * j + 2 * i + 1], small[4 * j + 2 * i + 1] * (1.f / kF16LoScale));
+                    float2* q = split ? (float2*)(prow + (size_t)rl * BN + n) : nullptr;
+                    if (giver) {                    // hand the partial sums over, no epilogue for these rows here
+                        *q = make_float2(a0, a1);
+                        continue;
                     }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < CW; ++j) v[j] = u[j] = w[j] = 0u;
-                }
-                float a[CW];
-#pragma unroll
-                for (int j = 0; j < CW; ++j) {
-                    const float small = __fadd_rn(__uint_as_float(u[j]), __uint_as_float(w[j]));
-                    a[j] = __fadd_rn(__uint_as_float(v[j]), small * (1.f / kF16LoScale));
-                }
-                if (giver) {                    // hand the partial sums over, no epilogue for these rows here
-#pragma unroll
-                    for (int j = 0; j < CW; j += 4) *(float4*)(prow + c0 + j) = make_float4(a[j], a[j + 1], a[j + 2], a[j + 3]);
-                    continue;
-                }
-                if (split) {
-#pragma unroll
-                    for (int j = 0; j < CW; j += 4) {
-                        const float4 q = q4[j / 4];
-                        a[j] = __fadd_rn(a[j], q.x); a[j + 1] = __fadd_rn(a[j + 1], q.y);
-                        a[j + 2] = __fadd_rn(a[j + 2], q.z); a[j + 3] = __fadd_rn(a[j + 3], q.w);
+                    if (split) {
+                        const float2 pq = __ldcg(q);    // L2
+                        a0 = __fadd_rn(a0, pq.x);
+                        a1 = __fadd_rn(a1, pq.y);
                     }
-                }
-                // folded BN: lane l holds scale / shift of column c0 + (l & 15) (loaded above, before the TMEM loads) and
-                // every lane takes them by shuffle - instead of 8 dependent float4 loads behind branches per slice
-                float o[CW];
-#pragma unroll
-                for (int j = 0; j < CW; ++j) {
-                    float val = fmaf(a[j], __shfl_sync(0xffffffffu, scl, j), __shfl_sync(0xffffffffu, shl, j));
-                    if (p.relu) val = fmaxf(val, 0.f);
-                    o[j] = val;                  // columns >= cout: zero weights, scale 1, shift 0 -> exactly 0
-                }
-                if (m < M) {
-                    if (p.out_f32) {
-                        float* orow = p.out_f32 + (size_t)m * p.out_f32_stride;
-#pragma unroll
-                        for (int j = 0; j < CW; j += 4)
-                            if (c0 + j + 3 < p.out_f32_stride)
-                                *(float4*)(orow + c0 + j) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
-                    }
-                    if (p.out_split) {
-                        __half* ohi = p.out_split + (size_t)m * p.out_ch;
-                        __half* olo = ohi + p.out_plane;
-#pragma unroll
-                        for (int j = 0; j < CW; j += 8) {
-                            const int n = c0 + j;
-                            if (n + 7 < p.out_ch) {
-                                uint32_t h0, h1, h2, h3, l0, l1, l2, l3;
-                                split_f16x2(o[j + 0], o[j + 1], h0, l0);
-                                split_f16x2(o[j + 2], o[j + 3], h1, l1);
-                                split_f16x2(o[j + 4], o[j + 5], h2, l2);
-                                split_f16x2(o[j + 6], o[j + 7], h3, l3);
-                                *(uint4*)(ohi + n) = make_uint4(h0, h1, h2, h3);
-                                *(uint4*)(olo + n) = make_uint4(l0, l1, l2, l3);
-                            }
+                    // columns >= cout: zero weights, scale 1, shift 0 -> exactly 0
+                    float o0 = fmaf(a0, scl0, shl0), o1 = fmaf(a1, scl1, shl1);
+                    if (p.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+                    if (m < M) {
+                        if (p.out_f32 && n < p.out_f32_stride)
+                            *(float2*)(p.out_f32 + (size_t)m * p.out_f32_stride + n) = make_float2(o0, o1);
+                        if (p.out_split && 8 * j < p.out_ch) {
+                            uint32_t h, l;
+                            split_f16x2(o0, o1, h, l);
+                            __half* ohi = p.out_split + (size_t)m * p.out_ch + n;
+                            *(uint32_t*)ohi = h;
+                            *(uint32_t*)(ohi + p.out_plane) = l;
                         }
                     }
                 }
             }
             if (giver) mbar_arrive_remote(peer_done, (uint32_t)(part ^ 1));    // every thread releases its own stores
-            if (have_acc && ++acc == C::ACC_BUFS) { acc = 0; acc_phase ^= 1u; }
         }
-        if (tr && threadIdx.x == 0) tr[11] = clock64();
+        if (p.counters && threadIdx.x == 0 && executed) {
+            atomicAdd(&p.counters[0], executed);
+            atomicAdd(&p.counters[1], tiles_done);
+        }
     }
 
-    tc_fence_before();
     __syncthreads();
-    if (warp == W_MMA) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)C::TMEM_COLS)
-                     : "memory");
-    }
     cluster_sync_all();           // no CTA of the cluster exits while its peer may still arrive on its barriers
 }
 
@@ -586,7 +403,7 @@ template <int TABLE, int BN>
 static int launch3(const Args& a, cudaStream_t stream) {
     using C = Cfg3<BN>;
     auto kern = spconv_split_kernel<TABLE, BN>;
-    // Persistent CTAs in clusters of two, one CTA per SM (225 KB of shared memory): the grid must not exceed what is
+    // Persistent CTAs in clusters of two, one CTA per SM (~200 KB of shared memory): the grid must not exceed what is
     // co-resident - GPCs with an odd number of free SMs cannot host a last cluster, and a cluster left over for a
     // second wave would double the kernel's time.
     static int max_ctas = 0;
@@ -594,13 +411,14 @@ static int launch3(const Args& a, cudaStream_t stream) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) != cudaSuccess)
             return SASSD_ERR_LAUNCH;
         cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(148); cfg.blockDim = dim3(THREADS3); cfg.dynamicSmemBytes = C::SMEM_BYTES;
+        cfg.gridDim = dim3(CLUSTER * sassd_div_up(sassd_num_sms(), CLUSTER)); cfg.blockDim = dim3(THREADS3);
+        cfg.dynamicSmemBytes = C::SMEM_BYTES;
         int clusters = 0;
         if (cudaOccupancyMaxActiveClusters(&clusters, kern, &cfg) != cudaSuccess || clusters < 1) {
             cudaGetLastError();
-            clusters = 64;
+            clusters = sassd_num_sms() / (2 * CLUSTER);
         }
-        max_ctas = CLUSTER * (clusters < 74 ? clusters : 74);
+        max_ctas = CLUSTER * (clusters < SPLIT_TILES_MAX ? clusters : SPLIT_TILES_MAX);
     }
     // one CTA per tile up to the resident CTAs; with a tap split two CTAs per tile; always whole clusters
     int grid = CLUSTER * sassd_div_up(a.rows_cap, BM);
@@ -685,34 +503,6 @@ extern "C" int sassd_spconv_f16x3(const sassd_spconv_desc* d, const void* in_spl
     a.scratch = (float*)ws; a.counters = counters;
     a.cin = d->cin; a.cout = d->cout; a.taps = d->taps; a.rows_cap = d->rows_cap; a.relu = d->relu;
     a.out_ch = d->out_ch; a.out_f32_stride = d->out_f32_stride;
-    static const int dbg = [] { const char* e = getenv("SASSD_SPS_DBG"); return e ? atoi(e) : 0; }();
-    a.dbg = dbg;
-    a.trace = nullptr;
-    static const int trace_call = [] { const char* e = getenv("SASSD_SPS_TRACE"); return e ? atoi(e) : 0; }();
-    if (trace_call && d->taps > 1) {      // timing experiment: per-CTA clock sums of the trace_call-th ruled launch -> stderr
-        static long long* trace = nullptr;
-        static int calls = 0;
-        const size_t n = (size_t)148 * 16;
-        if (!trace) cudaMalloc(&trace, n * sizeof(long long));
-        if (++calls == trace_call) {
-            cudaMemsetAsync(trace, 0, n * sizeof(long long), (cudaStream_t)stream_);
-            a.trace = trace;
-            const int rc = sps::dispatch3<1>(a, (cudaStream_t)stream_);
-            std::vector<long long> h(n);
-            cudaStreamSynchronize((cudaStream_t)stream_);
-            cudaMemcpy(h.data(), trace, n * sizeof(long long), cudaMemcpyDeviceToHost);
-            fprintf(stderr, "SPS_TRACE rows_cap %d cin %d cout %d: cta  prologue  kernel | prod: wait_empty issue wait_nbr end | "
-                            "mma: wait_data(of which B) issue wait_acc end chunks | epi_end\n", d->rows_cap, d->cin, d->cout);
-            for (int c = 0; c < 148; c += (c < 4 ? 1 : 37)) {
-                const long long* q = &h[(size_t)c * 16];
-                if (!q[0]) continue;
-                fprintf(stderr, "SPS_TRACE %3d %8lld %8lld | %8lld %8lld %8lld %8lld | %8lld (%lld) %8lld %8lld %8lld %4lld | %8lld\n", c,
-                        q[1] - q[0], (q[11] ? q[11] : q[9]) - q[0], q[2], q[3], q[4], q[5] ? q[5] - q[0] : 0, q[6], q[12], q[7], q[8],
-                        q[9] ? q[9] - q[0] : 0, q[10], q[11] ? q[11] - q[0] : 0);
-            }
-            return rc;
-        }
-    }
     return d->taps > 1 ? sps::dispatch3<1>(a, (cudaStream_t)stream_) : sps::dispatch3<0>(a, (cudaStream_t)stream_);
 }
 

@@ -1,5 +1,5 @@
-// Device-side helpers shared by the tcgen05 kernels (gconv_tc.cu, conv2d_tma.cu): mbarrier / bulk-copy /
-// tcgen05 PTX wrappers, UMMA descriptors, TMEM loads and the hi/lo operand splits.
+// Device-side helpers shared by the tensor-core kernels (gconv_tc.cu, conv2d_tma.cu, spconv_split.cu) on sm_90a:
+// mbarrier / bulk-copy / cluster PTX wrappers, warpgroup MMA (wgmma) descriptors and issue, the hi/lo operand splits.
 #pragma once
 #include <cuda_fp16.h>
 
@@ -10,19 +10,12 @@
 
 namespace tc {
 
-constexpr int BM = 128;
+constexpr int BM = 128;                  // output rows per tile: two consumer warpgroups of 64 rows each
 constexpr int BK = 32;                   // fp32 elements per chunk = one 128-byte swizzle row
 constexpr int A_TILE_BYTES = BM * 128;   // 16 KB (hi) ; same for lo
-constexpr int NUM_EPI_WARPS = 4, NUM_PROD_WARPS = 8;   // two producer threads per tile row
-constexpr int THREADS = (NUM_EPI_WARPS + NUM_PROD_WARPS + 2) * 32;   // 448
-constexpr int WARP_MMA = NUM_EPI_WARPS + NUM_PROD_WARPS, WARP_BLOAD = WARP_MMA + 1;
+constexpr int CONS_THREADS = 256;        // two consumer warpgroups (warps 0-7) in every tensor-core kernel
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
@@ -53,28 +46,11 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
                  "l"(src), "r"(bytes), "r"(bar)
                  : "memory");
-}
-
-// multicast variant: the same bytes land at the same shared-memory offset of every CTA in `mask` and
-// complete_tx on the mbarrier at the same offset in each of them
-__device__ __forceinline__ void bulk_g2s_mc(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint16_t mask) {
-    asm volatile(
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
-        ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "h"(mask)
-        : "memory");
-}
-__device__ __forceinline__ void mma_commit_mc(uint32_t bar, uint16_t mask) {
-    asm volatile(
-        "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-        "h"(mask)
-        : "memory");
 }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
@@ -86,153 +62,112 @@ __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor layout):
-// start>>4 [0,14) | LBO>>4 [16,30) (=1, unused for swizzled K-major) | SBO>>4 [32,46) (=1024 B between
-// 8-row groups) | version=1 [46,48) | layout_type=2 (SWIZZLE_128B) [61,64)
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma: start>>4 [0,14) | LBO>>4 [16,30) (=1, unused for
+// swizzled K-major) | SBO>>4 [32,46) (=1024 B between 8-row groups) | layout type 1 = SWIZZLE_128B [62,64).
+// Operand tiles are 1024-byte aligned; a K step of 32 bytes inside the swizzle row adds 2 to the start field.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 
-// The MMA-issuing lane is an instruction-issue bottleneck long before the tensor pipe is (round-2 probe,
-// profiles/r2_mma_issue_probe.md: ~6-8 clk per SASS instruction in that single-thread stream, so a loop that rebuilds
-// three 64-bit descriptors per K step - ~20 instructions per UTCHMMA - runs at 100-130 clk per MMA against a 32-64
-// clk tensor floor).  Hence: the constant high word and the per-tile low word of a descriptor are split, a K=16 step
-// is "+2" on the low word (32 bytes >> 4; the 14-bit address field cannot carry, shared memory is < 256 KB), and the
-// issue loops are fully unrolled around these.
-constexpr uint32_t kDescHi = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);    // SBO | version 1 | SWIZZLE_128B
-__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
-constexpr uint32_t kDescK16 = 2u;      // low-word advance per K=16 step of fp16 operands (32 bytes)
-
-// whole-warp convergent election (CUTLASS' elect_one_sync): exactly one lane gets true, always the same one
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}\n" : "=r"(pred));
-    return pred != 0;
+// wgmma ordering: fence before the first MMA of a batch (the accumulators were written by ordinary instructions),
+// commit the batch as a group, wait until at most N groups are still in flight.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A=B=tf32, both K-major
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, uint32_t fmt) {
-    return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// D[64 x N] += A[64 x K] * B[K x N]^T, both operands K-major in shared memory, fp32 accumulators in registers:
+// PREC 0 = kind tf32 (K = 8 per instruction), PREC 1 = f16 (K = 16).  Thread t of the warpgroup holds rows
+// 16 (t / 32) + (t % 32) / 4 + 8 i and columns 8 j + 2 (t % 4) + e at d[4 j + 2 i + e].  scale_d = 0: D = A * B
+// (the accumulator's previous contents are ignored).
+template <int PREC, int N>
+__device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+template <>
+__device__ __forceinline__ void wgmma<1, 16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(scale_d) : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma<1, 32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(scale_d) : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma<1, 64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d) : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma<1, 128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d) : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma<0, 16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(scale_d) : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma<0, 32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(scale_d) : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma<0, 64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d) : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma<0, 128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d) : "memory");
 }
 
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accum)
-        : "memory");
-}
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accum)
-        : "memory");
-}
-// kind::f16 with descriptors given as low words (high word = kDescHi); ACCUM is a compile-time flag where known
-__device__ __forceinline__ void mma_f16_lo(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "mov.b64 da, {%1, %5};\n\t"
-        "mov.b64 db, {%2, %5};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accum), "r"(kDescHi)
-        : "memory");
-}
-// MODE 0 plain, 1 = fill collector b0 with B, 2 = last use of b0 (weight-stationary form, see mma_f16_ws)
-template <int MODE>
-__device__ __forceinline__ void mma_f16_ws_lo(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accum) {
-    if constexpr (MODE == 1)
-        asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, %4, 0;\n\tmov.b64 da, {%1, %5};\n\t"
-                     "mov.b64 db, {%2, %5};\n\t"
-                     "tcgen05.mma.ws.cta_group::1.kind::f16.collector::b0::fill [%0], da, db, %3, p;\n\t}\n" ::"r"(tmem_d),
-                     "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accum), "r"(kDescHi) : "memory");
-    else if constexpr (MODE == 2)
-        asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, %4, 0;\n\tmov.b64 da, {%1, %5};\n\t"
-                     "mov.b64 db, {%2, %5};\n\t"
-                     "tcgen05.mma.ws.cta_group::1.kind::f16.collector::b0::lastuse [%0], da, db, %3, p;\n\t}\n" ::"r"(tmem_d),
-                     "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accum), "r"(kDescHi) : "memory");
-    else
-        asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, %4, 0;\n\tmov.b64 da, {%1, %5};\n\t"
-                     "mov.b64 db, {%2, %5};\n\t"
-                     "tcgen05.mma.ws.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t}\n" ::"r"(tmem_d),
-                     "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accum), "r"(kDescHi) : "memory");
-}
-// A-collector forms: MODE 1 = keep A after this MMA (fill), 2 = take A from the collector (lastuse)
-template <int MODE>
-__device__ __forceinline__ void mma_f16_acoll_lo(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accum) {
-    if constexpr (MODE == 1)
-        asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, %4, 0;\n\tmov.b64 da, {%1, %5};\n\t"
-                     "mov.b64 db, {%2, %5};\n\t"
-                     "tcgen05.mma.cta_group::1.kind::f16.collector::a::fill [%0], da, db, %3, p;\n\t}\n" ::"r"(tmem_d),
-                     "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accum), "r"(kDescHi) : "memory");
-    else
-        asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, %4, 0;\n\tmov.b64 da, {%1, %5};\n\t"
-                     "mov.b64 db, {%2, %5};\n\t"
-                     "tcgen05.mma.cta_group::1.kind::f16.collector::a::lastuse [%0], da, db, %3, p;\n\t}\n" ::"r"(tmem_d),
-                     "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accum), "r"(kDescHi) : "memory");
-}
-// Same instruction with the A-operand collector: `keep` leaves A in the tensor core's collector buffer after this
-// MMA, `reuse` takes A from there instead of reading shared memory again (SASS: UTCHMMA ... A_KEEP / A_REUSE).
-__device__ __forceinline__ void mma_f16_akeep(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16.collector::a::fill [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accum)
-        : "memory");
-}
-__device__ __forceinline__ void mma_f16_areuse(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16.collector::a::lastuse [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accum)
-        : "memory");
-}
-// Weight-stationary form: the B operand can stay in collector buffer b0 (SASS: UTCHMMA.WS ... B_KEEP / B_REUSE).
-// mode 0 = plain, 1 = fill b0, 2 = last use of b0.
-template <int MODE>
-__device__ __forceinline__ void mma_f16_ws(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-    if constexpr (MODE == 1)
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                     "tcgen05.mma.ws.cta_group::1.kind::f16.collector::b0::fill [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-                     "l"(da), "l"(db), "r"(idesc), "r"(accum) : "memory");
-    else if constexpr (MODE == 2)
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                     "tcgen05.mma.ws.cta_group::1.kind::f16.collector::b0::lastuse [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-                     "l"(da), "l"(db), "r"(idesc), "r"(accum) : "memory");
-    else
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                     "tcgen05.mma.ws.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-                     "l"(da), "l"(db), "r"(idesc), "r"(accum) : "memory");
-}
-template <int PREC>
-__device__ __forceinline__ void mma_any(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-    if constexpr (PREC == 0) mma_tf32(tmem_d, da, db, idesc, accum); else mma_f16(tmem_d, da, db, idesc, accum);
-}
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// One 128-byte K chunk (four K steps) of the split product x*w ~= xh*wh + (xh*wl + xl*wh): the two small products
+// go to their own accumulator, which keeps the 2^-11-smaller terms out of the big one (tensor-core accumulation
+// truncates; fewer accumulate steps on the big sum), and the epilogue adds the two once in fp32 RN.
+// big_fresh: the chunk's first MMA overwrites `big` instead of adding to it (per-chunk partial sums).
+template <int PREC, int N>
+__device__ __forceinline__ void mma_chunk_x3(float (&big)[N / 2], float (&small)[N / 2], uint32_t a_hi, uint32_t a_lo,
+                                             uint32_t b_hi, uint32_t b_lo, bool big_fresh = false) {
+    const uint64_t dah = make_desc(a_hi), dal = make_desc(a_lo), dbh = make_desc(b_hi), dbl = make_desc(b_lo);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint64_t ko = 2ull * (uint64_t)k;
+        wgmma<PREC, N>(small, dal + ko, dbh + ko, 1u);
+        wgmma<PREC, N>(small, dah + ko, dbl + ko, 1u);
+        wgmma<PREC, N>(big, dah + ko, dbh + ko, (k == 0 && big_fresh) ? 0u : 1u);
+    }
 }
 
 // fp32 -> tf32 with round-to-nearest (the tensor core would otherwise just drop the 13 low bits, which
@@ -247,30 +182,8 @@ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
     lo = tf32_rn(x - hi);
 }
 
-template <int CW>
-__device__ __forceinline__ void tmem_ld(uint32_t (&v)[CW], uint32_t taddr) {
-    if constexpr (CW == 32) {
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-              "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-              "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr));
-    } else {
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-              "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-            : "r"(taddr));
-    }
-}
-
-// PREC 0 = 3xTF32 (kind::tf32, 32 channels per 128-byte row, K=8 per MMA),
-// PREC 1 = 3xFP16 (kind::f16, 64 channels per row, K=16 per MMA, twice the MMA rate and half the operand bytes).
+// PREC 0 = 3xTF32 (32 channels per 128-byte row, K=8 per MMA),
+// PREC 1 = 3xFP16 (64 channels per row, K=16 per MMA, twice the MMA rate and half the operand bytes).
 // FP16 split: hi = half_rn(x), lo = half_rn((x - hi) * 2048); the residual is scaled into the normal fp16 range,
 // the "small" accumulator therefore carries a factor 2048 that the epilogue removes.  22 significand bits survive
 // (vs 21 for the tf32 split); |x| must stay below 65504 (fp16 range) — activations of this network are O(1..100).
@@ -279,7 +192,6 @@ template <int PREC>
 struct Prec {
     static constexpr int BKC = PREC == 0 ? 32 : 64;   // input channels per pipeline chunk
     static constexpr int NF4 = BKC / 4;               // float4 loads per row per chunk
-    static constexpr uint32_t FMT = PREC == 0 ? 2u : 0u;   // UMMA operand format: TF32 = 2, F16 = 0
 };
 
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
@@ -303,10 +215,8 @@ __device__ __forceinline__ void split_f16x2(float x, float y, uint32_t& hi2, uin
 
 // Host: launch `kern`, optionally as a programmatic dependent of the previous kernel in the stream (every kernel launched
 // through here calls pdl_wait() before touching global data, so only its prologue overlaps the predecessor's tail).
-// Measured (round 2, B=1): +2 % with one step on the GPU at a time, -8 % with four captured steps in flight, where the
-// early-resident CTAs of the next layer sit on SMs another frame's kernels could have used.  So it is a per-capture
-// choice: sassd_set_pdl(1) while the latency graph is captured (detectors._GraphedStep), off otherwise; the environment
-// variable SASSD_PDL=0/1 is the default when sassd_set_pdl was never called (experiments).
+// A per-capture choice: sassd_set_pdl(1) while the latency graph is captured (detectors._GraphedStep), off otherwise;
+// the environment variable SASSD_PDL=0/1 is the default when sassd_set_pdl was never called.
 extern int g_sassd_pdl;      // -1: not set (voxelize.cu)
 inline bool pdl_enabled() {
     if (g_sassd_pdl >= 0) return g_sassd_pdl != 0;

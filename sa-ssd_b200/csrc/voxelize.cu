@@ -410,7 +410,7 @@ extern "C" int sassd_anchor_mask(const int32_t* coors, const int32_t* d_rows, in
 
 extern "C" int sassd_version(void) { return 100; }
 
-// launch hint of the tcgen05 kernels (tc_common.cuh: launch_pdl)
+// launch hint of the tensor-core kernels (tc_common.cuh: launch_pdl)
 namespace tc { int g_sassd_pdl = -1; }
 extern "C" int sassd_set_pdl(int on) {
     const int prev = tc::g_sassd_pdl;

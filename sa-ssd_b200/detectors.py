@@ -52,8 +52,8 @@ class SingleStageDetector(nn.Module):
         return hasattr(self, "rpn_head") and self.rpn_head is not None
 
     def set_precision(self, precision, sparse=None):
-        """ops.PREC_F16X3 (default) = tcgen05 tensor-core kernels on the fp32-accurate 3xFP16 operand split
-        (TMA-fed dense convs, cp.async-fed sparse convs); ops.PREC_TF32X3 = the 3xTF32 tcgen05 kernels;
+        """ops.PREC_F16X3 (default) = Hopper tensor-core (wgmma) kernels on the fp32-accurate 3xFP16 operand split
+        (TMA-fed dense convs, cp.async-fed sparse convs); ops.PREC_TF32X3 = the 3xTF32 tensor-core kernels;
         ops.PREC_FP32 = CUDA-core FFMA kernels (bisecting / accuracy yard-stick).  ``sparse`` optionally selects a
         different path for the 13 ruled sparse convs."""
         self.neck.set_precision(precision, sparse)

@@ -2,7 +2,7 @@
 backbone) + BEVNet (dense BEV convs) — mmdet/models/necks/cmn.py:12-29,102-119,138-282.
 
 Parameter names and shapes equal the reference's (SURVEY.md §8b) so that its
-checkpoints load; all arithmetic runs in the sm_100a kernels of csrc/gconv.cu
+checkpoints load; all arithmetic runs in the sm_90a kernels of csrc/gconv.cu
 (BatchNorm folded into each conv's epilogue, eval mode).  The training-only aux head
 (cmn.py:44-100,121-135) is out of scope: its Linear parameters exist for checkpoint
 compatibility, ``is_test=False`` raises.

@@ -1,7 +1,7 @@
 """Functional wrappers over the C ABI (include/sassd_b200.h) on torch CUDA tensors.
 
 torch is plumbing here (device memory, streams); every computation is a
-hand-written sm_100a kernel in csrc/.  All wrappers are asynchronous on the
+hand-written sm_90a kernel in csrc/.  All wrappers are asynchronous on the
 current torch stream and keep data-dependent sizes on the device (``d_rows``
 style int32 tensors) — nothing in this module synchronises.
 """
@@ -18,7 +18,7 @@ from .lib import (GCONV_CONV2D, GCONV_ROWS, GCONV_TABLE, PREC_F16X3, PREC_FP32, 
                   check)
 
 NMS_CAP = 4096
-# Product default: every conv on the tcgen05 kernels with the fp32-accurate 3xFP16 operand split (csrc/spconv_split.cu,
+# Product default: every conv on the tensor-core (wgmma) kernels with the fp32-accurate 3xFP16 operand split (csrc/spconv_split.cu,
 # csrc/conv2d_tma.cu).  PREC_FP32 (CUDA-core FFMA) and PREC_TF32X3 stay selectable per model
 # (SingleStageDetector.set_precision) for bisecting.
 DEFAULT_PRECISION = PREC_F16X3
@@ -41,7 +41,7 @@ def _ptr(t):
 
 def require_cuda():
     if not torch.cuda.is_available():
-        raise _lib.SassdError("sassd_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise _lib.SassdError("sassd_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
 
 
 def next_pow2(n):
@@ -412,8 +412,6 @@ class SplitMap:
 
 
 TILE_OCCUPANCY = os.environ.get("SASSD_TMA_OCC", "1") != "0"     # constant-region tile skipping in the BEV convs
-CONV2D_NSPLIT_MAX_TILES_STREAM = int(os.environ.get("SASSD_NSPLIT_STREAM_TILES", "296"))   # detect_stream slots: B = 1 only (+3 % e2e)
-CONV2D_NSPLIT_MAX_TILES = 1184   # B <= 4 at 200x176: measured +5 % (B=1), +15 % (B=4) on `value`, nothing beyond
 CONV2D_TILE_ORDER = 0       # 1 while a latency-oriented step is captured (computed tiles first, see sassd_b200.h)
 CONV2D_COUNTERS = None     # bench instrumentation: {label: int32[2] device tensor} += tiles computed, += tiles
 _TILE_FAR = 1 << 20
@@ -482,9 +480,7 @@ def conv2d_split(x, weight, scale, shift, relu, cout, out_split=True, out_f32=Fa
     d.batch, d.H, d.W, d.cin, d.cin_stored = B, H, W, cin, x.planes.shape[-1]
     d.cout, d.taps, d.relu = cout, taps, 1 if relu else 0
     d.tile_order = CONV2D_TILE_ORDER
-    # latency-oriented steps split the 3x3 256-channel layers of small maps into half-width units (sassd_b200.h)
-    tiles = B * ((H + 7) // 8) * ((W + 15) // 16)
-    d.n_split = 2 if (taps == 9 and cout > 128 and tiles <= (CONV2D_NSPLIT_MAX_TILES if CONV2D_TILE_ORDER else CONV2D_NSPLIT_MAX_TILES_STREAM)) else 0
+    d.n_split = 0        # the kernel picks its units (cout > 128: two 128-channel units per tile)
     osp = of = None
     if out_split:
         cs = (cout + 63) // 64 * 64

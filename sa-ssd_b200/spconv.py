@@ -4,7 +4,7 @@ SubMConv3d, SparseConv3d, SparseSequential.  spconv itself is third-party and no
 vendored by the reference; the semantics implemented here are those of SURVEY.md
 §A.2 (and are tested by definition against dense conv3d).
 
-Everything computes through the sm_100a kernels behind the C ABI
+Everything computes through the sm_90a kernels behind the C ABI
 (rulebook.cu + gconv.cu); there is no torch fallback.  Tensors carry a capacity
 and a device-side row count (``d_rows``) so that a chain of layers never
 synchronises; ``features`` / ``indices`` properties trim to the exact row count

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): every CUDA stage, called through the C ABI
+"""GPU parity tests (need an H100): every CUDA stage, called through the C ABI
 (ctypes), against the CPU oracle on the same seeded inputs and against the committed
 golden fixtures produced by the reference's own Python.
 
@@ -238,7 +238,7 @@ def test_sparse_conv_layers(dev, cin, cout, prec):
 
 
 def _make_model(dev, num_class=1, cfg_name="car_cfg.py", prec=None):
-    """prec None = the product default (3xFP16 tcgen05 kernels); "fp32" / "tf32x3" select the other paths."""
+    """prec None = the product default (3xFP16 tensor-core kernels); "fp32" / "tf32x3" select the other paths."""
     import sassd_b200 as S
     from sassd_b200 import checkpoint, ops
     cfg = S.Config.fromfile(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "configs", cfg_name))
@@ -335,42 +335,37 @@ def _random_boxes(n, seed, spread=20.0):
     return b7, s
 
 
-def _load_ref_nms():
-    from oracle import build as ob
-    path = ob.build_ref()
-    if path is None:
-        return None
-    lib = ctypes.CDLL(path)
-    fn = getattr(lib, "_Z11nmsLauncherPKfPyif")
-    fn.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_float]
-    fn.restype = None
-    return fn
+NMS_CASES = [(1, 0), (2, 1), (63, 2), (64, 3), (65, 4), (300, 5), (1500, 6)]
+NMS_THR = 0.1
 
 
-@pytest.mark.parametrize("n,seed", [(1, 0), (2, 1), (63, 2), (64, 3), (65, 4), (300, 5), (1500, 6)])
-def test_nms_mask_and_keep(dev, n, seed):
-    """Keep mask vs the CPU oracle; suppression bitmask vs the UNMODIFIED reference CUDA kernel
-    (oracle/_ref, built from /root/reference in the build container) bit for bit."""
+def _sorted_bev(n, seed):
+    """BEV boxes of _random_boxes(n, seed) in descending score order (the input of the NMS mask kernels)."""
+    from sassd_b200.single_stage_heads import boxes3d_to_bev_torch
+    b7, s = _random_boxes(n, seed)
+    order = torch.sort(torch.from_numpy(s), descending=True, stable=True)[1]
+    return boxes3d_to_bev_torch(torch.from_numpy(b7))[order].contiguous()
+
+
+@pytest.mark.parametrize("n,seed", NMS_CASES)
+def test_nms_mask_and_keep(dev, golden_dir, n, seed):
+    """Keep mask vs the CPU oracle; suppression bitmask vs the UNMODIFIED reference CUDA kernel bit for bit (its masks
+    for these inputs are stored in tests/golden/nms_ref.npz by tests/golden/make_golden_nms.py)."""
     from sassd_b200 import ops
     from sassd_b200.single_stage_heads import boxes3d_to_bev_torch, nms_gpu
     b7, s = _random_boxes(n, seed)
     bev = boxes3d_to_bev_torch(torch.from_numpy(b7))
-    order = torch.sort(torch.from_numpy(s), descending=True, stable=True)[1]
-    sorted_bev = bev[order].contiguous()
-    thr = 0.1
+    sorted_bev = _sorted_bev(n, seed)
+    thr = NMS_THR
     mask = ops.nms_mask(sorted_bev.to(dev), thr).cpu().numpy().view(np.uint64)
-    ref = _load_ref_nms()
     colb = (n + 63) // 64
     upper = np.zeros((n, colb), bool)
     for i in range(n):
         upper[i, i // 64:] = True
-    if ref is not None:
-        rmask = torch.zeros((n, colb), dtype=torch.int64, device=dev)
-        torch.cuda.synchronize()
-        ref(ctypes.c_void_p(sorted_bev.to(dev).data_ptr()), ctypes.c_void_p(rmask.data_ptr()), n, ctypes.c_float(thr))
-        torch.cuda.synchronize()
-        rm = rmask.cpu().numpy().view(np.uint64)
-        assert np.array_equal(mask[upper], rm[upper]), "suppression bitmask differs from the reference kernel"
+    ref = np.load(os.path.join(golden_dir, "nms_ref.npz"))
+    np.testing.assert_array_equal(sorted_bev.numpy(), ref["bev_%d_%d" % (n, seed)])    # the inputs the masks were made for
+    rm = ref["mask_%d_%d" % (n, seed)]
+    assert np.array_equal(mask[upper], rm[upper]), "suppression bitmask differs from the reference kernel"
     keep = nms_gpu(bev.to(dev), torch.from_numpy(s).to(dev), thr).cpu().numpy()
     okeep = O.nms_rotated(bev, torch.from_numpy(s), thr).numpy()
     iou = O.iou_matrix(sorted_bev.numpy())
@@ -574,7 +569,7 @@ def test_reference_signature_forward_test(dev, car_model):
 
 # ------------------------------------------------------------------ the other tensor-core split (3xTF32)
 def test_end_to_end_tf32x3_path(dev):
-    """The same raw-points -> detections comparison on the 3xTF32 tcgen05 kernels (selectable, not the default)."""
+    """The same raw-points -> detections comparison on the 3xTF32 tensor-core kernels (selectable, not the default)."""
     model, sd = _make_model(dev, prec="tf32x3")
     # the TF32 split keeps 21 significand bits per operand (fp16 split: 22): activation maps at 4e-4
     _check_against_oracle(model, sd, [synth_cloud(0), synth_cloud(9)], "tf32x3", min_total=10, map_tol=4e-4)
@@ -582,7 +577,7 @@ def test_end_to_end_tf32x3_path(dev):
 
 @pytest.mark.parametrize("cin,cout,taps", [(256, 256, 9), (320, 256, 9), (256, 28, 9), (28, 28, 1), (256, 20, 1)])
 def test_tensor_core_conv_matches_fp64(dev, cin, cout, taps):
-    """tcgen05 3xTF32 dense conv vs an fp64 reference: error must stay within 4x of the fp32 FFMA kernel's."""
+    """Tensor-core 3xTF32 dense conv vs an fp64 reference: error must stay within 4x of the fp32 FFMA kernel's."""
     from sassd_b200 import ops
     torch.manual_seed(cin + cout)
     B, H, W = 2, 24, 20
@@ -689,17 +684,14 @@ def test_density_sweep_endpoints(dev, car_model):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("stage,env", [("tma", {}), ("tma", {"SASSD_TMA_PAIR": "1"}), ("split", {})])
-def test_tcgen05_kernel_unit_checks(stage, env):
-    """tests/tools/tc_check.py compares the TMA dense conv (single-CTA and the opt-in CTA-pair kernel) and the
-    split-row sparse conv with fp64 references over the shape/edge cases of the pipeline; a fresh process because
-    the kernel selection is read from the environment once."""
+@pytest.mark.parametrize("stage", ["tma", "split"])
+def test_tensor_core_kernel_unit_checks(stage):
+    """tests/tools/tc_check.py compares the TMA dense conv and the split-row sparse conv with fp64 references over the
+    shape/edge cases of the pipeline, in a fresh process."""
     import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    e = dict(os.environ)
-    e.update(env)
-    r = subprocess.run([sys.executable, os.path.join(root, "tests", "tools", "tc_check.py"), stage], cwd=root, env=e,
+    r = subprocess.run([sys.executable, os.path.join(root, "tests", "tools", "tc_check.py"), stage], cwd=root,
                        capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
     assert "MISMATCH" not in r.stdout, r.stdout[-3000:]

@@ -96,10 +96,11 @@ def test_vxnet_tiny_end_to_end_vs_dense():
     c, f = _random_sparse(B, shape, 200, 4, 4)
     feats, c3, shape3 = O.vxnet_forward(sd, f, c, shape)
     assert shape3 == [1, 2, 2] and feats.shape[1] == 64
-    # dense emulation
-    x = _densify(c, f, B, shape)
+    # dense emulation, in float64: an exact yardstick (fp32 conv3d rounds differently from one CPU's kernels to the next)
+    x = _densify(c, f, B, shape).double()
     act = _densify(c, torch.ones(c.shape[0], 1), B, shape) > 0
     p = "neck.backbone."
+    sd = {k: (v.double() if v.is_floating_point() else v) for k, v in sd.items()}
 
     def bnrelu(x, name):
         return torch.relu(O.bn_eval(x, sd, p + name))

@@ -1,4 +1,4 @@
-"""GPU dev tool: check the tcgen05 (3xTF32) gathered-GEMM kernel against the FFMA path and fp64,
+"""GPU dev tool: check the tensor-core (3xTF32 / 3xFP16) gathered-GEMM kernels against the FFMA path and fp64,
 smallest cases first, printing diagnostics instead of asserting."""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -273,9 +273,9 @@ if stage in ("splitperf",):
         e1.record(); torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / 5
         pairs = int((nbr_t.cpu().numpy() >= 0).sum())
-        print("splitperf %s dbg=%s: %.3f ms  pair-model %.0f GB/s  (%.0f clk per executed chunk)" % (
-            tag, os.environ.get("SASSD_SPS_DBG", "0"), ms, pairs * (4 * cin + 4 * cout + 8) / ms / 1e6,
-            ms * 1e-3 * 1.9e9 / (n_chunks / 148)), flush=True)
+        print("splitperf %s: %.3f ms  pair-model %.0f GB/s  (%.0f clk per executed chunk)" % (
+            tag, ms, pairs * (4 * cin + 4 * cout + 8) / ms / 1e6,
+            ms * 1e-3 * 1.98e9 / (n_chunks / torch.cuda.get_device_properties(0).multi_processor_count)), flush=True)
 
     timed("all taps", nbr, None, 27 * (M / 128))
     # 30 % of the (tile, tap) combinations absent, like the level-2 SubM rulebook of a KITTI-shaped cloud
@@ -295,21 +295,3 @@ if stage in ("splitperf",):
         M = M_full
         d_rows = torch.tensor([M], dtype=torch.int32, device=dev)
 
-if stage in ("splittrace",):
-    # SASSD_SPS_TRACE=2 python tests/tools/tc_check.py splittrace <rows>: per-CTA clock sums of the second launch
-    rows = int(sys.argv[2]) if len(sys.argv) > 2 else 120000
-    cin = cout = 64
-    rs = np.random.RandomState(1)
-    x = torch.randn(rows, cin, device=dev)
-    w = torch.randn(27, cin, cout, device=dev) * 0.1
-    nb = np.where(rs.rand(rows, 27) < 0.35, np.clip(np.arange(rows)[:, None] + rs.randint(-300, 300, (rows, 27)), 0, rows - 1), -1).astype(np.int32)
-    gone = rs.rand((rows + 127) // 128, 27) < 0.3
-    nb[np.repeat(gone, 128, axis=0)[:rows]] = -1
-    nbr = torch.from_numpy(nb).to(dev)
-    tm = torch.from_numpy(tile_masks(nb, rows)).to(dev)
-    d_rows = torch.tensor([rows], dtype=torch.int32, device=dev)
-    planes = ops.features_to_split(x)
-    for _ in range(3):
-        ops.spconv_split(planes, w, None, None, True, cout, rows, nbr=nbr, d_rows=d_rows, tile_mask=tm)
-    torch.cuda.synchronize()
-    print("splittrace done", rows)
