@@ -211,6 +211,19 @@ int sassd_conv2d_f16x3_occ(const sassd_conv2d_desc* host_desc, const void* in_sp
                            const float* scale, const float* shift, float* out_f32, void* out_split,
                            const int32_t* tile_dist, int reach, const float* const_out, int32_t* counters,
                            sassd_stream_t stream);     /* counters: optional int32[2], += tiles computed, += tiles */
+/* Same, with a background for the border tiles.  A tile on the image border with tile_dist > reach (reach >= 2) sees
+ * only inactive cells and the zero padding, so its output does not depend on the frame: it equals, bit for bit, this
+ * function's output on an empty scene at the same pixels (one output element per lane, a fixed chunk order, no
+ * atomics).  bg_split [2][1][H][W][out_split_ch] / bg_f32 [1][H][W][out_f32_stride] hold that output - the layer run
+ * with batch 1 and no tile skipping on the previous layer's background (an all-zero map for the first conv) - and
+ * every frame's far border tiles copy it with 16-byte loads and stores, without loads of the input or MMAs.  Interior
+ * far tiles still store const_out.  The background must hold every output the call writes (SASSD_ERR_ARG
+ * otherwise); both NULL: sassd_conv2d_f16x3_occ, which computes the border tiles.  counters count computed tiles
+ * only. */
+int sassd_conv2d_f16x3_occ_bg(const sassd_conv2d_desc* host_desc, const void* in_split, const void* wpack,
+                              const float* scale, const float* shift, float* out_f32, void* out_split,
+                              const int32_t* tile_dist, int reach, const float* const_out, const void* bg_split,
+                              const float* bg_f32, int32_t* counters, sassd_stream_t stream);
 /* dense() of the last sparse tensor straight into a (pre-zeroed) split map [2,batch,H,W,D*C]. */
 int sassd_sparse_to_bev_split(const float* feat, const int32_t* coors, const int32_t* d_rows, int rows_cap, int C,
                               int D, int H, int W, int batch, void* bev_split, int32_t* tile_dist,

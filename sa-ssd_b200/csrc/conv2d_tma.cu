@@ -26,6 +26,7 @@ using namespace tc;
 constexpr int TILE_H = SASSD_CONV2D_TILE_H, TILE_W = SASSD_CONV2D_TILE_W;   // 8 x 16 = 128 output pixels per tile
 constexpr int BKC = 64;                         // channels per chunk (one 128-byte fp16 row)
 constexpr int kConstTile = 1 << 30;             // tile reference flag: the tile only stores the layer's constant vector
+constexpr int kBgTile = 1 << 29;                // tile reference flag: the tile copies the layer's background map
 constexpr int CONS_WARPS = CONS_THREADS / 32;   // 8
 constexpr int THREADS2 = CONS_THREADS + 32;     // + the TMA / bulk-copy issuing warp
 constexpr int W_LOAD = CONS_WARPS;
@@ -58,16 +59,60 @@ struct Conv2dArgs {
     const int* tile_dist; // optional: distance of each tile to the nearest active cell of the scattered map
     const float* cvec;    // output constant of the tiles that see a constant input (tile_dist > reach, not on the border)
     int reach;
-    int* counters;        // optional [2]: += tiles computed (not stored as a constant), += tiles (bench instrumentation)
+    int* counters;        // optional [2]: += tiles computed (not stored or copied), += tiles (bench instrumentation)
     int tile_order;       // 1: computed tiles first, 0: round-robin
     int nsplit;           // work units per tile: 1, or 2 = each unit computes BN of the 2*BN output channels (the weight
                           // pack is the 2*BN-wide one)
 };
 
-// True when tile (ty, tx) sees a constant input and its output is p.cvec (see sassd_conv2d_f16x3_occ in the header).
-__device__ __forceinline__ bool tile_is_constant(const Conv2dArgs& p, int tile, int ty, int tx, int tiles_y, int tiles_x) {
-    if (!p.tile_dist || __ldg(&p.tile_dist[tile]) <= p.reach) return false;
-    return p.reach < 2 || !(ty == 0 || ty == tiles_y - 1 || tx == 0 || tx == tiles_x - 1);
+// Optional: the layer's outputs on an empty scene, batch 1 (same H, W, strides), copied into the far border tiles.  A
+// kernel parameter of its own: grown by two pointers, Conv2dArgs tips the BN = 128 kernel over its 168 registers.
+struct Background {
+    const __half* split;
+    const float* f32;
+};
+
+// How tile (ty, tx) at distance `dist` from the active cells is produced (see sassd_conv2d_f16x3_occ_bg in the header):
+// 0 = computed; kConstTile = it sees a constant input and its output is p.cvec; kBgTile = it sees only inactive cells
+// and the zero padding, so its output is the background map's at the same pixels.
+__device__ __forceinline__ int tile_skip_flag(const Conv2dArgs& p, const Background& bg, int dist, int ty, int tx,
+                                              int tiles_y, int tiles_x) {
+    if (dist <= p.reach) return 0;
+    if (p.reach < 2 || !(ty == 0 || ty == tiles_y - 1 || tx == 0 || tx == tiles_x - 1)) return kConstTile;
+    return (bg.split || bg.f32) ? kBgTile : 0;      // the border sees the zero padding, which differs from cvec
+}
+
+// A unit of a background tile: channels [n_off, n_off + bn) of its pixels copied from the background map (batch 1) to
+// frame b, split planes and fp32 alike, with 16-byte loads and stores by the nthreads consumer threads.  The same
+// columns the register epilogue writes: those below out_split_ch / out_f32_stride.
+__device__ __forceinline__ void copy_background_unit(const Conv2dArgs& p, const Background& bg, int b, int ty, int tx,
+                                                     int n_off, int bn, int tid, int nthreads) {
+    const size_t hw = (size_t)p.H * p.W;
+    if (p.out_split) {
+        const int vpp = min(bn, p.out_split_ch - n_off) >> 3;            // 16-byte vectors per pixel and plane
+        const size_t bg_plane = hw * p.out_split_ch, plane = (size_t)p.batch * bg_plane;
+        for (int i = tid; i < TILE_H * TILE_W * vpp; i += nthreads) {
+            const int pix = i / vpp;
+            const int y = ty * TILE_H + pix / TILE_W, x = tx * TILE_W + pix % TILE_W;
+            if (y >= p.H || x >= p.W) continue;
+            const size_t src = ((size_t)y * p.W + x) * p.out_split_ch + n_off + 8 * (i % vpp);
+            const uint4 hi = __ldg((const uint4*)(bg.split + src));
+            const uint4 lo = __ldg((const uint4*)(bg.split + bg_plane + src));
+            __half* dst = p.out_split + (size_t)b * bg_plane + src;
+            *(uint4*)dst = hi;
+            *(uint4*)(dst + plane) = lo;
+        }
+    }
+    if (p.out_f32) {
+        const int vpp = min(bn, p.out_f32_stride - n_off) >> 2;
+        for (int i = tid; i < TILE_H * TILE_W * vpp; i += nthreads) {
+            const int pix = i / vpp;
+            const int y = ty * TILE_H + pix / TILE_W, x = tx * TILE_W + pix % TILE_W;
+            if (y >= p.H || x >= p.W) continue;
+            const size_t src = ((size_t)y * p.W + x) * p.out_f32_stride + n_off + 4 * (i % vpp);
+            *(float4*)(p.out_f32 + (size_t)b * hw * p.out_f32_stride + src) = __ldg((const float4*)(bg.f32 + src));
+        }
+    }
 }
 
 // A unit of a constant-region tile: every pixel gets the layer's constant vector (channels [n_off, n_off + ncols) of it).
@@ -102,7 +147,7 @@ __device__ __forceinline__ void store_constant_unit(const Conv2dArgs& p, int b, 
 
 template <int BN>
 __global__ void __launch_bounds__(THREADS2, 1)
-conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p) {
+conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, const Background bg) {
     using C = Cfg2<BN>;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -128,20 +173,20 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p) 
     __syncthreads();
     pdl_wait();                   // the producing layer has completed; nothing above touched global data
 
-    // With constant-region information most tiles only store a constant.  Static round-robin leaves some CTAs with
-    // two computed tiles and others with none; with tile_order = 1 (for maps of up to ORDER_CAP tiles) every CTA
-    // builds the same order - computed tiles first, constant tiles after - and all roles walk
-    // order[blockIdx.x + i * gridDim.x].  Round-robin is the default: with several steps in flight the SMs that
-    // only store constants are what the other frames' kernels run on.
+    // With constant-region information most tiles only store a constant or copy the background.  Static round-robin
+    // leaves some CTAs with two computed tiles and others with none; with tile_order = 1 (for maps of up to ORDER_CAP
+    // tiles) every CTA builds the same order - computed tiles first, stored and copied tiles after - and all roles
+    // walk order[blockIdx.x + i * gridDim.x].  Round-robin is the default: with several steps in flight the SMs that
+    // only store are what the other frames' kernels run on.
     uint16_t* order = (uint16_t*)(base_ptr + C::STAGES * C::STAGE_BYTES + 256);
     const bool small_map = p.tile_dist != nullptr && ntiles <= C::ORDER_CAP;
     const bool use_order = p.tile_order && small_map;
     // For maps of up to ORDER_CAP tiles warp 0 fetches every tile's distance in one batch of loads (one memory latency
-    // instead of one per tile and role) and keeps the verdicts as order[k] bit 15.
+    // instead of one per tile and role) and keeps the verdicts as order[k] bit 15 (constant) and bit 14 (background).
     if (small_map) {
         if (warp == 0) {
-            // verdicts of tiles lane, lane + 32, ... as bits of one word; the distances are fetched four at a time
-            uint32_t cst_bits = 0u;
+            // verdicts of tiles lane, lane + 32, ... as bits of two words; the distances are fetched four at a time
+            uint32_t cst_bits = 0u, bg_bits = 0u;
             int ty = (lane / tiles_x) % tiles_y, tx = lane % tiles_x;      // tile `lane`; advanced by 32 tiles per slot
 #pragma unroll 1
             for (int i0 = 0; i0 * 32 < ntiles; i0 += 4) {
@@ -154,39 +199,44 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p) 
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const int t = (i0 + e) * 32 + lane;
-                    const bool border = ty == 0 || ty == tiles_y - 1 || tx == 0 || tx == tiles_x - 1;   // sees the zero padding
-                    if (t < ntiles && dist[e] > p.reach && (p.reach < 2 || !border)) cst_bits |= 1u << (i0 + e);
+                    const int f = t < ntiles ? tile_skip_flag(p, bg, dist[e], ty, tx, tiles_y, tiles_x) : 0;
+                    if (f == kConstTile) cst_bits |= 1u << (i0 + e);
+                    if (f == kBgTile) bg_bits |= 1u << (i0 + e);
                     tx += 32;
                     while (tx >= tiles_x) { tx -= tiles_x; if (++ty == tiles_y) ty = 0; }
                 }
             }
+            auto word = [&](int t, int i) {
+                return (uint16_t)(t | (((cst_bits >> i) & 1u) ? 0x8000 : 0) | (((bg_bits >> i) & 1u) ? 0x4000 : 0));
+            };
             if (use_order) {
                 int n = 0;
                 for (int pass = 0; pass < 2; ++pass)
 #pragma unroll 1
                     for (int i = 0; i * 32 < ntiles; ++i) {
                         const int t = i * 32 + lane;
-                        const bool cst = (cst_bits >> i) & 1u;
-                        const bool take = t < ntiles && (cst == (pass == 1));
+                        const bool skip = ((cst_bits | bg_bits) >> i) & 1u;
+                        const bool take = t < ntiles && (skip == (pass == 1));
                         const uint32_t m = __ballot_sync(0xffffffffu, take);
-                        if (take) order[n + __popc(m & ((1u << lane) - 1u))] = (uint16_t)(t | (cst ? 0x8000 : 0));
+                        if (take) order[n + __popc(m & ((1u << lane) - 1u))] = word(t, i);
                         n += __popc(m);
                     }
             } else {
 #pragma unroll 1
                 for (int i = 0; i * 32 < ntiles; ++i) {
                     const int t = i * 32 + lane;
-                    if (t < ntiles) order[t] = (uint16_t)(t | (((cst_bits >> i) & 1u) ? 0x8000 : 0));
+                    if (t < ntiles) order[t] = word(t, i);
                 }
             }
         }
         __syncthreads();
     }
-    // tile_ref(k): the k-th tile in walking order, bit 30 set when it only stores the layer's constant
+    // tile_ref(k): the k-th tile in walking order, | kConstTile when it only stores the layer's constant, | kBgTile when
+    // it copies the background
     auto tile_ref = [&](int k) -> int {
-        if (small_map) { const int v = order[k]; return (v & 0x7fff) | ((v & 0x8000) << 15); }
+        if (small_map) { const int v = order[k]; return (v & 0x3fff) | ((v & 0xc000) << 15); }
         if (!p.tile_dist) return k;
-        return tile_is_constant(p, k, (k / tiles_x) % tiles_y, k % tiles_x, tiles_y, tiles_x) ? (k | kConstTile) : k;
+        return k | tile_skip_flag(p, bg, __ldg(&p.tile_dist[k]), (k / tiles_x) % tiles_y, k % tiles_x, tiles_y, tiles_x);
     };
 
     if (warp == W_LOAD) {
@@ -195,7 +245,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p) 
             uint32_t phase = 0;
             for (int k = blockIdx.x; k < nunits; k += gridDim.x) {
                 const int ref = tile_ref(k / nsplit), half = k % nsplit;
-                if (ref & kConstTile) continue;                                         // nothing to load
+                if (ref & (kConstTile | kBgTile)) continue;                             // nothing to load
                 const int tile = ref;
                 const int b = tile / (tiles_y * tiles_x);
                 const int ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
@@ -237,10 +287,11 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p) 
         int computed = 0;
         for (int k = blockIdx.x; k < nunits; k += gridDim.x) {
             const int ref = tile_ref(k / nsplit), n_off = (k % nsplit) * BN;
-            const int tile = ref & ~kConstTile;
+            const int tile = ref & ~(kConstTile | kBgTile);
             const bool const_tile = (ref & kConstTile) != 0;
             const int b = tile / (tiles_y * tiles_x);
             const int ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
+            if (ref & kBgTile) continue;                                    // copied after this loop
             if (const_tile) {                                               // no MMAs run for this tile
                 const int ncols = min(BN, p.out_split_ch - n_off);
                 if (p.out_split && !p.out_f32 && (ncols == 64 || ncols == 128 || ncols == 256)) {
@@ -309,6 +360,17 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p) 
                 }
             }
         }
+        // Background tiles in a pass of their own: interleaved with the MMA units, the copy's address arithmetic is
+        // hoisted across the accumulators and spills them.
+        if (bg.split || bg.f32) {
+            for (int k = blockIdx.x; k < nunits; k += gridDim.x) {
+                const int ref = tile_ref(k / nsplit);
+                if (!(ref & kBgTile)) continue;
+                const int tile = ref & ~kBgTile;
+                copy_background_unit(p, bg, tile / (tiles_y * tiles_x), (tile / tiles_x) % tiles_y, tile % tiles_x,
+                                     (k % nsplit) * BN, BN, threadIdx.x, CONS_THREADS);
+            }
+        }
         if (p.counters && threadIdx.x == 0) {
             if (computed) atomicAdd(&p.counters[0], computed);
             if (blockIdx.x == 0) atomicAdd(&p.counters[1], ntiles);
@@ -335,7 +397,7 @@ static EncodeTiledFn get_encode() {
 }
 
 template <int BN>
-static int launch2(const CUtensorMap& map, const Conv2dArgs& a, cudaStream_t stream) {
+static int launch2(const CUtensorMap& map, const Conv2dArgs& a, const Background& bg, cudaStream_t stream) {
     using C = Cfg2<BN>;
     auto kern = conv2d_tma_kernel<BN>;
     static bool configured = false;
@@ -346,7 +408,7 @@ static int launch2(const CUtensorMap& map, const Conv2dArgs& a, cudaStream_t str
     }
     const int units = a.batch * sassd_div_up(a.H, TILE_H) * sassd_div_up(a.W, TILE_W) * a.nsplit;
     const int grid = units < sassd_num_sms() ? units : sassd_num_sms();
-    if (launch_pdl(kern, dim3(grid), dim3(THREADS2), C::SMEM_BYTES, stream, map, a) != cudaSuccess) return SASSD_ERR_LAUNCH;
+    if (launch_pdl(kern, dim3(grid), dim3(THREADS2), C::SMEM_BYTES, stream, map, a, bg) != cudaSuccess) return SASSD_ERR_LAUNCH;
     return sassd_check_launch();
 }
 
@@ -355,14 +417,26 @@ static int launch2(const CUtensorMap& map, const Conv2dArgs& a, cudaStream_t str
 extern "C" int sassd_conv2d_f16x3(const sassd_conv2d_desc* d, const void* in_split, const void* wpack,
                                   const float* scale, const float* shift, float* out_f32, void* out_split,
                                   sassd_stream_t stream_) {
-    return sassd_conv2d_f16x3_occ(d, in_split, wpack, scale, shift, out_f32, out_split, nullptr, 0, nullptr, nullptr, stream_);
+    return sassd_conv2d_f16x3_occ_bg(d, in_split, wpack, scale, shift, out_f32, out_split, nullptr, 0, nullptr, nullptr,
+                                     nullptr, nullptr, stream_);
 }
 
 extern "C" int sassd_conv2d_f16x3_occ(const sassd_conv2d_desc* d, const void* in_split, const void* wpack,
                                       const float* scale, const float* shift, float* out_f32, void* out_split,
                                       const int32_t* tile_dist, int reach, const float* const_out, int32_t* counters,
                                       sassd_stream_t stream_) {
+    return sassd_conv2d_f16x3_occ_bg(d, in_split, wpack, scale, shift, out_f32, out_split, tile_dist, reach, const_out,
+                                     nullptr, nullptr, counters, stream_);
+}
+
+extern "C" int sassd_conv2d_f16x3_occ_bg(const sassd_conv2d_desc* d, const void* in_split, const void* wpack,
+                                         const float* scale, const float* shift, float* out_f32, void* out_split,
+                                         const int32_t* tile_dist, int reach, const float* const_out,
+                                         const void* bg_split, const float* bg_f32, int32_t* counters,
+                                         sassd_stream_t stream_) {
     if (tile_dist && (!const_out || reach < 0)) return SASSD_ERR_ARG;
+    // a background must hold every output the layer writes
+    if ((bg_split || bg_f32) && ((out_split && !bg_split) || (out_f32 && !bg_f32))) return SASSD_ERR_ARG;
     if (tile_dist) {
         // The constant-region rule is exact only while (a) the layer is within the range tile distances are recorded
         // for and (b) the zero-padding disturbance (reach-1 pixels deep) stays inside the outermost tile row / column,
@@ -399,13 +473,14 @@ extern "C" int sassd_conv2d_f16x3_occ(const sassd_conv2d_desc* d, const void* in
     a.tile_dist = tile_dist; a.reach = reach; a.cvec = const_out; a.counters = counters;
     a.tile_order = d->tile_order;
     a.nsplit = 1;
+    const Background bg = {out_split ? (const __half*)bg_split : nullptr, out_f32 ? bg_f32 : nullptr};
     cudaStream_t stream = (cudaStream_t)stream_;
-    if (d->cout <= 32) return launch2<32>(map, a, stream);
-    if (d->cout <= 64) return launch2<64>(map, a, stream);
-    if (d->cout <= 128) return launch2<128>(map, a, stream);
+    if (d->cout <= 32) return launch2<32>(map, a, bg, stream);
+    if (d->cout <= 64) return launch2<64>(map, a, bg, stream);
+    if (d->cout <= 128) return launch2<128>(map, a, bg, stream);
     // 128 < cout <= 256: two units per tile, each 128 output channels of the 256-wide weight pack
     a.nsplit = 2;
-    return launch2<128>(map, a, stream);
+    return launch2<128>(map, a, bg, stream);
 }
 
 // SparseConvTensor.dense() into the split BEV map: hi / lo*2048 fp16 planes [2,B,H,W,D*C] (channel d*C + c).

@@ -283,10 +283,12 @@ class _GraphedStep:
             torch.cuda.current_stream(dev).wait_stream(side)
             torch.cuda.synchronize(dev)
             self.graph = torch.cuda.CUDAGraph()
+            self.backgrounds = ops.BACKGROUND_PINS = []       # the captured kernels bake their addresses in
             with torch.cuda.graph(self.graph):
                 self.det, self.d_ndet, self.status, self.aux = model.forward_device(self.points, self.pt_off,
                                                                                     self.batch, self.maxpts)
         finally:
+            ops.BACKGROUND_PINS = None
             ops._WS = shared_ws
             ops.CONV2D_TILE_ORDER = order0
             if pdl0 is not None:

@@ -64,6 +64,7 @@ _SIGNATURES = {
     "sassd_gconv_pack": (c_int, [P, c_int, c_int, c_int, c_int, P, P]),
     "sassd_conv2d_f16x3": (c_int, [ctypes.POINTER(Conv2dDesc), P, P, P, P, P, P, P]),
     "sassd_conv2d_f16x3_occ": (c_int, [ctypes.POINTER(Conv2dDesc), P, P, P, P, P, P, P, c_int, P, P, P]),
+    "sassd_conv2d_f16x3_occ_bg": (c_int, [ctypes.POINTER(Conv2dDesc), P, P, P, P, P, P, P, c_int, P, P, P, P, P]),
     "sassd_rotate_overlap_eval": (c_int, [P, P, P, P, P, c_int, c_int, c_int, P, P]),
     "sassd_kitti_match": (c_int, [c_int, P, P, P, P, P, P, P, P, P, P, P, P, c_int, ctypes.c_double, c_int, c_int, P, P,
                                   P, P]),

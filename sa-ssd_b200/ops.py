@@ -5,6 +5,7 @@ hand-written sm_90a kernel in csrc/.  All wrappers are asynchronous on the
 current torch stream and keep data-dependent sizes on the device (``d_rows``
 style int32 tensors) — nothing in this module synchronises.
 """
+import collections
 import ctypes
 import os
 import math
@@ -52,7 +53,7 @@ def next_pow2(n):
 # kernels launched by each C-ABI entry point (memsets not counted)
 _KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
-            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
+            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
             "sassd_boxes_iou_bev": 1}
 LAUNCHES = 0          # running count of kernels launched through this module
@@ -378,13 +379,16 @@ class SplitMap:
     """Activation map as two fp16 planes [2, B, H, W, C_stored] (hi, lo*2048) — the operand format of
     sassd_conv2d_f16x3; ``channels`` of the C_stored are meaningful, the rest are zero."""
 
-    def __init__(self, planes, channels, tile_dist=None, reach=0, const=None):
+    def __init__(self, planes, channels, tile_dist=None, reach=0, const=None, background=None):
         # Maps that descend from a scattered sparse tensor are constant over large regions.  tile_dist: int32
         # [B * tiles_y * tiles_x], pixel distance of every conv tile to the nearest active cell of the scattered map;
-        # reach: number of 3x3 convs applied since; const: fp32 [channels] value of the constant region (None = 0).
-        # conv2d_split uses them to skip the tiles whose output is the layer's constant (see sassd_conv2d_f16x3_occ).
+        # reach: number of 3x3 convs applied since; const: fp32 [channels] value of the constant region (None = 0);
+        # background: SplitMap of batch 1, the same layers applied to an empty scene (None: all zero at reach 0,
+        # unknown beyond).  conv2d_split uses them to skip the tiles whose output is the layer's constant or, on the
+        # image border, the layer's background (see sassd_conv2d_f16x3_occ_bg).
         self.planes, self.channels = planes, channels
         self.tile_dist, self.reach, self.const = tile_dist, reach, const
+        self.background = background
 
     @property
     def shape(self):
@@ -463,6 +467,44 @@ def conv_constant(x_const, cin, weight, scale, shift, relu, cout):
     return ent[0]
 
 
+_BACKGROUNDS = collections.OrderedDict()
+# One background is a full map (36 MB for 256 channels on the 200x176 grid, ~0.3 GB for a detector's chain of layers):
+# the least recently used are dropped beyond this many bytes, which also bounds the maps a weight reload leaves stale.
+BACKGROUND_CACHE_BYTES = 4 << 30
+BACKGROUND_PINS = None     # a list while a CUDA graph is captured: the backgrounds its kernels read, kept by the graph
+
+
+def conv_background(x, weight, scale, shift, relu, cout, out_split, out_f32):
+    """The layer's outputs on an empty scene, batch 1: (SplitMap | None, fp32 map | None), computed in full by the very
+    kernel from x's background, or None when x's background is unknown.  The border tiles far from every active cell
+    copy it (sassd_conv2d_f16x3_occ_bg): their receptive field holds only inactive cells and the zero padding, so they
+    equal it bit for bit.  Cached per weights and input background (warm before CUDA-graph capture)."""
+    B, H, W, cin = x.shape
+    src = x.background
+    if src is None and x.reach > 0:
+        return None
+    key = (weight.data_ptr(), weight._version, None if scale is None else (scale.data_ptr(), scale._version),
+           None if shift is None else (shift.data_ptr(), shift._version), bool(relu), cout, cin, x.planes.shape[-1], H, W,
+           None if src is None else src.planes.data_ptr(), bool(out_split), bool(out_f32))
+    ent = _BACKGROUNDS.get(key)
+    if ent is None:
+        if src is None:
+            src_in = SplitMap(torch.zeros((2, 1, H, W, x.planes.shape[-1]), dtype=torch.float16, device=x.device), cin)
+        else:
+            src_in = src
+        bg = conv2d_split(src_in, weight, scale, shift, relu, cout, out_split=out_split, out_f32=out_f32)
+        nbytes = sum(t.numel() * t.element_size() for t in (bg[0] and bg[0].planes, bg[1]) if t is not None)
+        ent = (bg, nbytes, weight, scale, shift, src)       # keep the keys alive
+        _BACKGROUNDS[key] = ent
+        while len(_BACKGROUNDS) > 1 and sum(e[1] for e in _BACKGROUNDS.values()) > BACKGROUND_CACHE_BYTES:
+            _BACKGROUNDS.popitem(last=False)
+    else:
+        _BACKGROUNDS.move_to_end(key)
+    if BACKGROUND_PINS is not None:
+        BACKGROUND_PINS.append(ent[0])
+    return ent[0]
+
+
 def sparse_to_bev_split(feat, coors, d_rows, C, D, H, W, batch):
     planes = torch.zeros((2, batch, H, W, D * C), dtype=torch.float16, device=feat.device)
     dist = _tile_dist(batch, H, W, feat.device)
@@ -494,17 +536,20 @@ def conv2d_split(x, weight, scale, shift, relu, cout, out_split=True, out_f32=Fa
         d.out_f32_stride = stride
     label = "conv2d_tma[taps=%d %d->%d]" % (taps, cin, cout)
     dist = x.tile_dist if TILE_OCCUPANCY else None
-    reach, cvec = 0, None
+    reach, cvec, bg_sp, bg_f = 0, None, None, None
     if dist is not None:
         reach = x.reach + (1 if taps == 9 else 0)
         if not tile_skipping_valid(H, W, reach):
             dist = None        # the map is computed in full from here on (see tile_skipping_valid)
     if dist is not None:
         cvec = conv_constant(x.const, cin, weight, scale, shift, relu, cout)
-    _call("sassd_conv2d_f16x3_occ", label, ctypes.byref(d), _ptr(x.planes), _ptr(wp), _ptr(scale), _ptr(shift), _ptr(of),
-          _ptr(osp), _ptr(dist), reach, _ptr(cvec), _ptr(CONV2D_COUNTERS.get(label) if CONV2D_COUNTERS is not None else None),
-          _stream())
-    return (SplitMap(osp, cout, dist, reach, cvec) if osp is not None else None), of
+        bg = conv_background(x, weight, scale, shift, relu, cout, out_split, out_f32)
+        if bg is not None:
+            bg_sp, bg_f = bg
+    _call("sassd_conv2d_f16x3_occ_bg", label, ctypes.byref(d), _ptr(x.planes), _ptr(wp), _ptr(scale), _ptr(shift),
+          _ptr(of), _ptr(osp), _ptr(dist), reach, _ptr(cvec), _ptr(bg_sp.planes if bg_sp is not None else None),
+          _ptr(bg_f), _ptr(CONV2D_COUNTERS.get(label) if CONV2D_COUNTERS is not None else None), _stream())
+    return (SplitMap(osp, cout, dist, reach, cvec, bg_sp) if osp is not None else None), of
 
 
 # ---------------------------------------------------------------------------- sparse conv on split rows
