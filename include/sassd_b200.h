@@ -92,6 +92,26 @@ int sassd_voxel_mean(const float* voxels, const int32_t* num_points, const int32
                      int max_points, float* mean, sassd_stream_t stream);
 
 /* ------------------------------------------------------------------------
+ * Camera-frustum crop of full sweeps.  Replaces the offline reduced-cloud
+ * step, tools/create_data.py:107-140 -> remove_outside_points
+ * (mmdet/core/bbox3d/geometry.py:50-61), on the device.
+ *
+ * points [n_points_cap,4], frame b = rows [d_pt_off[b], d_pt_off[b+1]) as for
+ * sassd_voxelize; planes [batch][6][4] fp64 (n.x, n.y, n.z, d per face, the
+ * normals pointing into the frustum).  Point i of frame b is kept when
+ * s = ((x*n.x + y*n.y) + z*n.z) + d is < 0 for all 6 faces, evaluated in fp64
+ * in that order without contraction (points_in_convex_polygon_3d_jit,
+ * geometry.py:190-222: `s >= 0` rejects, so a NaN coordinate keeps the point).
+ * Kept rows are compacted in input order, frames concatenated:
+ * points_out [n_points_cap,4], d_pt_off_out [batch+1].  One pass, no host
+ * synchronisation: graph-capturable.  batch <= 256.
+ * ---------------------------------------------------------------------- */
+size_t sassd_frustum_crop_workspace_bytes(int n_points_cap, int batch);
+int sassd_frustum_crop(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch,
+                       const double* planes, float* points_out, int32_t* d_pt_off_out,
+                       void* ws, size_t ws_bytes, sassd_stream_t stream);
+
+/* ------------------------------------------------------------------------
  * anchors_mask.  Replaces mmdet/datasets/kitti.py:333-343 +
  * mmdet/core/bbox3d/geometry.py:675-709 (occupancy count, two cumsums,
  * integral-image lookup, `> threshold`).  rects [n_anchors,4] int32 are the

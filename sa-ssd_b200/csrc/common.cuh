@@ -37,6 +37,16 @@ static inline int sassd_grid(long long work, int block, int ctas_per_sm = 8) {
     return (int)(need < cap ? need : cap);
 }
 
+// Frame of point i of concatenated frames: the b with off[b] <= i < off[b+1] (off in shared memory, off[0] <= i).
+__device__ __forceinline__ int sassd_frame_of(const int* s_off, int batch, int i) {
+    int lo = 0, hi = batch;
+    while (hi - lo > 1) {
+        int mid = (lo + hi) >> 1;
+        if (s_off[mid] <= i) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
 // An active BEV cell (b, y, x) lowers tile_dist of every conv tile within SASSD_TILE_DIST_MAX pixels to its Chebyshev
 // distance from the tile rectangle (0 inside the tile).  sassd_conv2d_f16x3_occ compares it with the layer's reach.
 __device__ __forceinline__ void sassd_mark_conv2d_tiles(int* __restrict__ tile_dist, int b, int y, int x, int H, int W) {

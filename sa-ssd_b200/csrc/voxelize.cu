@@ -29,15 +29,6 @@ struct VoxConst {
     int max_points, max_voxels;
 };
 
-__device__ __forceinline__ int vox_frame_of(const int* s_off, int batch, int i) {
-    int lo = 0, hi = batch;  // find b with off[b] <= i < off[b+1]
-    while (hi - lo > 1) {
-        int mid = (lo + hi) >> 1;
-        if (s_off[mid] <= i) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 __global__ void __launch_bounds__(256)
 vox_insert_kernel(const float4* __restrict__ points, const int* __restrict__ pt_off, int batch, VoxConst P,
                   int slots, int* __restrict__ keys, int* __restrict__ first, int* __restrict__ head,
@@ -74,7 +65,7 @@ vox_insert_kernel(const float4* __restrict__ points, const int* __restrict__ pt_
             ok = (cx >= 0.f) && (cx < (float)P.grid[0]) && (cy >= 0.f) && (cy < (float)P.grid[1]) &&
                  (cz >= 0.f) && (cz < (float)P.grid[2]);
             if (ok) {
-                b = vox_frame_of(s_off, batch, i);
+                b = sassd_frame_of(s_off, batch, i);
                 cell = ((int)cz * P.grid[1] + (int)cy) * P.grid[0] + (int)cx;
             }
         }
@@ -185,7 +176,7 @@ vox_emit_kernel(const float4* __restrict__ points, const int* __restrict__ pt_of
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const int slot = __ldg(&pt_slot[i]);
         if (slot < 0 || __ldg(&first[slot]) != i) continue;
-        const int b = vox_frame_of(s_off, batch, i);
+        const int b = sassd_frame_of(s_off, batch, i);
         const int cut = __ldg(&frame_cut[b]);
         if (i >= cut) continue;  // opener at/after the cut: its voxel id was never assigned
         const int v = __ldg(&vid[slot]);

@@ -8,6 +8,8 @@ Two entry points:
   * ``forward_points(points)`` — the fused path from raw Velodyne points on the host:
     one H2D copy, voxelize + anchors_mask + backbone + neck + heads + PSWarp + NMS with
     every data-dependent size kept on the device, one D2H copy of the fixed-size result.
+    With ``frustum_planes`` the frames are full sweeps, cropped to the camera frustum on the
+    device first (the reference crops them offline into ``velodyne_reduced``).
 """
 import numpy as np
 import torch
@@ -39,6 +41,7 @@ class SingleStageDetector(nn.Module):
         self._pinned = None
         self._mask_stream = None
         self._graph = None
+        self._crop_graph = None
         self._graph_args = None
         self._stream_slots = None
         self._stream_key = None
@@ -65,6 +68,7 @@ class SingleStageDetector(nn.Module):
         """Captured steps bake in the device addresses of packed weights, folded BN vectors and layer constants and
         the kernel selection; anything that changes those must force a re-capture."""
         self._graph = None
+        self._crop_graph = None
         self._stream_slots = None
         self._stream_key = None
 
@@ -176,29 +180,38 @@ class SingleStageDetector(nn.Module):
     def enable_cuda_graph(self, batch, max_points_per_frame=32768):
         """Capture forward_device once for (batch, max_points_per_frame) and replay it per step: every
         data-dependent size already lives on the device, so the ~65 launches of a step become one graph
-        launch.  Steps whose shape does not fit fall back to the eager path."""
+        launch.  Steps whose shape does not fit fall back to the eager path.  Calls with ``frustum_planes`` replay a
+        second graph, captured on their first use, that runs the crop and the step; there ``max_points_per_frame`` bounds
+        the full sweeps (e.g. 131072)."""
         self._graph_args = (int(batch), int(max_points_per_frame))
         self._graph = _GraphedStep(self, batch, max_points_per_frame, latency=True)
         return self._graph
 
     def disable_cuda_graph(self):
         self._graph = None
+        self._crop_graph = None
         self._graph_args = None
 
-    def detect_stream(self, batches, batch, max_points_per_frame=32768, depth=4, concurrent=True):
+    def detect_stream(self, batches, batch, max_points_per_frame=32768, depth=4, concurrent=True, crop=False):
         """Throughput API: iterate over batches (each a list of ``batch`` raw point arrays) and yield their
         detections in order.  ``depth`` captured graphs with their own static buffers and scratch are used
         round-robin: while the GPU runs step i, the host stages and uploads step i+1 (copy stream) and unpacks
         step i-1.  With ``concurrent`` every slot replays on its own stream, so the low-occupancy phases of one
-        step (voxelize, rulebooks, the sparse layers, NMS) run beside the dense layers of its neighbour."""
+        step (voxelize, rulebooks, the sparse layers, NMS) run beside the dense layers of its neighbour.
+        With ``crop`` each item of ``batches`` is (points_list, planes [batch,6,4]) of full sweeps: every slot's graph
+        crops the frames to their camera frustums (forward_points' ``frustum_planes``) before the step, and
+        ``max_points_per_frame`` bounds the full sweeps."""
         ops.require_cuda()
-        key = (batch, max_points_per_frame, depth)
+        key = (batch, max_points_per_frame, depth, bool(crop))
         if self._stream_key != key or self._stream_slots is None:
-            self._stream_slots = [_GraphedStep(self, batch, max_points_per_frame) for _ in range(depth)]
+            self._stream_slots = [_GraphedStep(self, batch, max_points_per_frame, crop=crop) for _ in range(depth)]
             self._copy_stream = torch.cuda.Stream()
             self._stream_key = key
         slots, pending = self._stream_slots, []
-        for i, fb in enumerate(batches):
+        for i, item in enumerate(batches):
+            fb, planes = item if crop else (item, None)
+            if crop:
+                planes = _frame_planes(planes, len(fb))
             counts = [int(p.shape[0]) for p in fb]
             slot = slots[i % depth]
             if len(pending) == depth:                       # the slot we are about to reuse must be drained
@@ -207,32 +220,51 @@ class SingleStageDetector(nn.Module):
             if not slot.fits(len(fb), counts):
                 raise ValueError("batch does not fit the captured shape (batch %d, %d points/frame)" %
                                  (batch, max_points_per_frame))
-            slot.submit(fb, counts, self._copy_stream, own_stream=concurrent)
+            slot.submit(fb, counts, self._copy_stream, own_stream=concurrent, planes=planes)
             pending.append(slot)
         for slot in pending:
             bbs, scs, lbs = slot.collect()
             yield [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(bbs, scs, lbs)]
 
-    def forward_points(self, points_list, return_aux=False):
+    def forward_points(self, points_list, return_aux=False, frustum_planes=None):
         """Raw points in (list of [N_i,>=4] numpy arrays), detections out: per frame a dict of
-        boxes_lidar [D,7], scores [D], label_preds [D] (or None entries when nothing survives)."""
+        boxes_lidar [D,7], scores [D], label_preds [D] (or None entries when nothing survives).
+        ``frustum_planes``: one float64 [6,4] array per frame (frustum.camera_frustum_planes).  The frames are then
+        full sweeps; each is cropped to its camera frustum on the device, in point order (ops.frustum_crop), and the
+        step runs on what is left, as on the reference's offline-cropped ``velodyne_reduced`` clouds."""
         ops.require_cuda()
         if self.voxel_generator is None or self.anchor_set is None:
             raise RuntimeError("call attach_data_pipeline(voxel_generator, anchor_set) first")
         dev = next(self.parameters()).device
+        planes = None if frustum_planes is None else _frame_planes(frustum_planes, len(points_list))
         hp, ho, counts = self.stage_points(points_list)
-        if self._graph is None and self._graph_args is not None:     # dropped by a weight / precision change
-            self._graph = _GraphedStep(self, *self._graph_args, latency=True)
-        g = self._graph
+        if planes is None:
+            if self._graph is None and self._graph_args is not None:     # dropped by a weight / precision change
+                self._graph = _GraphedStep(self, *self._graph_args, latency=True)
+            g = self._graph
+        else:
+            if self._crop_graph is None and self._graph_args is not None:
+                self._crop_graph = _GraphedStep(self, *self._graph_args, latency=True, crop=True)
+            g = self._crop_graph
         if g is not None and not return_aux and g.fits(len(points_list), counts):
-            bbs, scs, lbs = g.run_host(hp, ho, sum(counts))
+            bbs, scs, lbs = g.run_host(hp, ho, sum(counts), planes)
             return [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(bbs, scs, lbs)]
         points = hp.to(dev, non_blocking=True)
         pt_off = ho.to(dev, non_blocking=True)
+        if planes is not None:
+            points, pt_off = ops.frustum_crop(points, pt_off, len(points_list), torch.from_numpy(planes).to(dev))
         det, d_ndet, status, aux = self.forward_device(points, pt_off, len(points_list), max(counts + [1]))
         bbs, scs, lbs = unpack_detections(det, d_ndet, status)
         out = [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(bbs, scs, lbs)]
         return (out, aux) if return_aux else out
+
+
+def _frame_planes(frustum_planes, batch):
+    """One [6,4] plane set per frame -> contiguous float64 [batch,6,4]."""
+    planes = np.ascontiguousarray(np.asarray(frustum_planes, dtype=np.float64))
+    if planes.shape != (batch, 6, 4):
+        raise ValueError("frustum_planes: expected %d arrays of shape [6,4], got shape %s" % (batch, planes.shape))
+    return planes
 
 
 def _pinned_pair(n_points, n_off):
@@ -257,15 +289,20 @@ def _stage_into(hp, ho, points_list, counts):
 class _GraphedStep:
     """One captured step of SingleStageDetector.forward_device with static input/output buffers."""
 
-    def __init__(self, model, batch, max_points_per_frame, latency=False):
+    def __init__(self, model, batch, max_points_per_frame, latency=False, crop=False):
         """latency=True: this step will run alone on the GPU (enable_cuda_graph / forward_points): the dense convs walk
         the computed tiles first so that the constant-region tiles shorten every layer; False (detect_stream slots,
-        several steps in flight): round-robin tiles, the SMs a layer leaves idle serve the other steps."""
+        several steps in flight): round-robin tiles, the SMs a layer leaves idle serve the other steps.
+        crop=True: the static points are full sweeps and the graph crops them to the frustums given by the static
+        planes [batch,6,4] (ops.frustum_crop) before the step; the cropped frames never exceed the full ones."""
         dev = next(model.parameters()).device
         self.model, self.batch, self.maxpts = model, int(batch), int(max_points_per_frame)
         self.cap = self.batch * self.maxpts
+        self.crop = bool(crop)
         self.points = torch.zeros((self.cap, 4), dtype=torch.float32, device=dev)
         self.pt_off = torch.zeros((self.batch + 1,), dtype=torch.int32, device=dev)
+        if self.crop:
+            self.planes = torch.zeros((self.batch, 6, 4), dtype=torch.float64, device=dev)
         # Scratch buffers private to this graph (the captured kernels bake their addresses in), so that several
         # captured steps can be in flight on different streams without sharing anything but read-only weights.
         self.ws = ops.Workspace()
@@ -279,14 +316,13 @@ class _GraphedStep:
             side.wait_stream(torch.cuda.current_stream(dev))
             with torch.cuda.stream(side):   # warm-up: workspaces, weight packs and folded BN get created eagerly
                 for _ in range(2):
-                    model.forward_device(self.points, self.pt_off, self.batch, self.maxpts)
+                    self._step()
             torch.cuda.current_stream(dev).wait_stream(side)
             torch.cuda.synchronize(dev)
             self.graph = torch.cuda.CUDAGraph()
             self.backgrounds = ops.BACKGROUND_PINS = []       # the captured kernels bake their addresses in
             with torch.cuda.graph(self.graph):
-                self.det, self.d_ndet, self.status, self.aux = model.forward_device(self.points, self.pt_off,
-                                                                                    self.batch, self.maxpts)
+                self.det, self.d_ndet, self.status, self.aux = self._step()
         finally:
             ops.BACKGROUND_PINS = None
             ops._WS = shared_ws
@@ -297,8 +333,16 @@ class _GraphedStep:
         self.h_nd = torch.empty(self.d_ndet.shape, dtype=torch.int32, pin_memory=True)
         self.h_status = torch.empty((1,), dtype=torch.int32, pin_memory=True)
         self.h_points, self.h_off = _pinned_pair(self.cap, self.batch + 1)
+        if self.crop:
+            self.h_planes = torch.empty((self.batch, 6, 4), dtype=torch.float64, pin_memory=True)
         self.done = torch.cuda.Event()
         self.loaded = torch.cuda.Event()
+
+    def _step(self):
+        points, pt_off = self.points, self.pt_off
+        if self.crop:
+            points, pt_off = ops.frustum_crop(points, pt_off, self.batch, self.planes)
+        return self.model.forward_device(points, pt_off, self.batch, self.maxpts)
 
     def fits(self, batch, counts):
         return batch == self.batch and max(counts + [0]) <= self.maxpts
@@ -312,10 +356,13 @@ class _GraphedStep:
         self.graph.replay()
         return self.det, self.d_ndet, self.status
 
-    def run_host(self, hp, ho, total):
+    def run_host(self, hp, ho, total, planes=None):
         """pinned host points in, numpy detections out: H2D, one graph launch, D2H, one stream sync."""
         self.points[:total].copy_(hp[:total], non_blocking=True)
         self.pt_off.copy_(ho, non_blocking=True)
+        if self.crop:
+            self.h_planes.numpy()[...] = planes
+            self.planes.copy_(self.h_planes, non_blocking=True)
         self.graph.replay()
         self.h_det.copy_(self.det, non_blocking=True)
         self.h_nd.copy_(self.d_ndet, non_blocking=True)
@@ -324,15 +371,19 @@ class _GraphedStep:
         return self.unpack()
 
     # ---- asynchronous use (SingleStageDetector.detect_stream): submit() ... collect()
-    def submit(self, points_list, counts, copy_stream, own_stream=False):
+    def submit(self, points_list, counts, copy_stream, own_stream=False, planes=None):
         """Stage into this slot's pinned buffer, H2D on the copy stream, then replay + D2H on the current stream or,
         with ``own_stream``, on this slot's stream so that consecutive steps overlap on the GPU."""
         _stage_into(self.h_points, self.h_off, points_list, counts)
+        if self.crop:
+            self.h_planes.numpy()[...] = planes
         total = sum(counts)
         cur = self.stream if own_stream else torch.cuda.current_stream()
         with torch.cuda.stream(copy_stream):
             self.points[:total].copy_(self.h_points[:total], non_blocking=True)
             self.pt_off.copy_(self.h_off, non_blocking=True)
+            if self.crop:
+                self.planes.copy_(self.h_planes, non_blocking=True)
             self.loaded.record(copy_stream)
         cur.wait_event(self.loaded)
         with torch.cuda.stream(cur):

@@ -48,6 +48,8 @@ _SIGNATURES = {
     "sassd_voxelize": (c_int, [P, P, c_int, c_int, ctypes.POINTER(VoxelParams), c_int, P, P, P, P, c_int, P, P, P,
                                c_size_t, P]),
     "sassd_voxel_mean": (c_int, [P, P, P, c_int, c_int, P, P]),
+    "sassd_frustum_crop_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "sassd_frustum_crop": (c_int, [P, P, c_int, c_int, P, P, P, P, c_size_t, P]),
     "sassd_anchor_mask_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "sassd_anchor_mask": (c_int, [P, P, c_int, c_int, c_int, c_int, P, c_int, c_int, P, P, c_size_t, P]),
     "sassd_hash_build": (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, P]),

@@ -51,7 +51,7 @@ def next_pow2(n):
 
 # --- launch accounting / optional per-call CUDA-event timing (bench.py) ---------------
 # kernels launched by each C-ABI entry point (memsets not counted)
-_KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
+_KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1,"sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
             "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
@@ -120,6 +120,22 @@ def voxelize(points, pt_off, batch, params, rows_cap, slots_per_frame, status, w
                               _ptr(voxels), _ptr(coors), _ptr(num), _ptr(mean), rows_cap, _ptr(frame_rows),
                               _ptr(status), _ptr(w), w.numel(), _stream())
     return voxels, coors, num, mean, frame_rows
+
+
+def frustum_crop(points, pt_off, batch, planes, ws=None):
+    """points [Ncap,4] f32, pt_off [batch+1] i32, planes [batch,6,4] f64 (device; frustum.camera_frustum_planes).
+    Returns (points_out [Ncap,4], pt_off_out [batch+1]): each frame's points inside its camera frustum, in input
+    order, frames concatenated.  Rows past pt_off_out[batch] are left unwritten."""
+    dev = points.device
+    n_cap = points.shape[0]
+    assert planes.dtype == torch.float64 and tuple(planes.shape) == (batch, 6, 4), "planes must be float64 [batch,6,4]"
+    out = torch.empty_like(points)
+    off = torch.empty((batch + 1,), dtype=torch.int32, device=dev)
+    nbytes = _L().sassd_frustum_crop_workspace_bytes(n_cap, batch)
+    w = (ws or _WS).get("frustum", nbytes, dev)
+    _call("sassd_frustum_crop", None, _ptr(points), _ptr(pt_off), n_cap, batch, _ptr(planes), _ptr(out), _ptr(off),
+          _ptr(w), w.numel(), _stream())
+    return out, off
 
 
 def voxel_mean(voxels, num_points, d_rows=None):
