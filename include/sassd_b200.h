@@ -208,7 +208,8 @@ typedef struct {
     int32_t out_f32_stride, out_split_ch;
     int32_t tile_order;            /* sassd_conv2d_f16x3_occ: 0 = tiles round-robin over the CTAs (best with several steps
                                       in flight), 1 = computed tiles first, constant tiles after (best for one step at a
-                                      time: no CTA gets two computed tiles while others only store constants) */
+                                      time: no CTA gets two computed tiles while others only store constants); honoured
+                                      for maps of up to 4608 tiles (16 frames of 200 x 176), round-robin above */
     int32_t n_split;               /* accepted for ABI compatibility and ignored: a work unit is a tile and at most 128 of
                                       its output channels (the register accumulators' budget), so cout > 128 always runs
                                       as two units per tile */

@@ -6,9 +6,12 @@
 // (LDG -> split -> STS), nine times per element for a 3x3 conv.  Here
 //   * activations live in HBM already split: two fp16 planes [2][B][H][W][C] (hi, lo*2048), written
 //     once by the epilogue of the producing layer (or by the sparse->BEV scatter);
-//   * a tile is an 8x16-pixel patch; for tap (dy,dx) and a 64-channel chunk the A operand is ONE
-//     cp.async.bulk.tensor.4d box {64 ch, 16 x, 8 y, 1} at (y0+dy, x0+dx) — TMA writes it 128B-swizzled
-//     straight into the wgmma operand layout and zero-fills out-of-image pixels (= the conv's zero padding);
+//   * a tile is an 8x16-pixel patch; a unit walks (tap column dx, 64-channel chunk) outer and the vertical taps dy
+//     inner.  Per (dx, chunk) the A operand is ONE cp.async.bulk.tensor.4d halo box {64 ch, 16 x, 10 y, 1} per plane
+//     at (y0-1, x0+dx) that all three dy taps read, at 2048-byte row offsets (a 1x1 conv: one column, an 8-row box) —
+//     TMA writes it 128B-swizzled straight into the wgmma operand layout and zero-fills out-of-image pixels (= the
+//     conv's zero padding);
+//   * two rings: A stages (40 KB, released after the box's last tap) and B stages (one (tap, chunk) of weights);
 //   * no producer warps: warp 8 lane 0 issues the TMA boxes (A hi, A lo) and the weight bulk copies, two consumer
 //     warpgroups (pixel rows 0-63 / 64-127 of the tile) issue the MMAs and store the outputs from registers.
 // A work unit is a tile and up to 128 of its output channels: the two register accumulators (big, small) of a
@@ -31,14 +34,24 @@ constexpr int CONS_WARPS = CONS_THREADS / 32;   // 8
 constexpr int THREADS2 = CONS_THREADS + 32;     // + the TMA / bulk-copy issuing warp
 constexpr int W_LOAD = CONS_WARPS;
 
+// The A operand of a (dx, chunk) step is one halo box per plane: TILE_H + 2 pixel rows (TILE_H for a 1x1 conv) of
+// TILE_W pixels; the three vertical taps read it at row offsets 0, 1, 2, i.e. 2048-byte (swizzle-phase preserving) steps.
+constexpr int A_ROWS = TILE_H + 2;
+constexpr int A_PLANE_BYTES = A_ROWS * TILE_W * 128;    // 20 KB (hi) ; same for lo, right after it
+constexpr int A_STAGE_BYTES = 2 * A_PLANE_BYTES;
+constexpr int A_STAGES = 2;
+
 template <int BN>
 struct Cfg2 {
     static constexpr int B_TILE_BYTES = BN * 128;
-    static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-    static constexpr int STAGES = (BN >= 128) ? 3 : (BN >= 64 ? 4 : 5);
-    // tile order (active tiles first) when the map carries constant-region information: uint16 per tile
-    static constexpr int ORDER_CAP = 832;
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256 + ORDER_CAP * 2;
+    static constexpr int B_STAGE_BYTES = 2 * B_TILE_BYTES;     // one (tap, chunk): hi | lo
+    static constexpr int B_STAGES = (BN >= 128) ? 4 : 6;
+    static constexpr int RING_BYTES = A_STAGES * A_STAGE_BYTES + B_STAGES * B_STAGE_BYTES;
+    // tile order (computed tiles first) when the map carries constant-region information: two verdict bits and a uint16
+    // per tile, up to 16 frames of the 200 x 176 BEV grid (4400 tiles); the word keeps the tile index in 14 bits
+    static constexpr int ORDER_CAP = 4608;
+    static constexpr int SMEM_BYTES = RING_BYTES + 1024 + 256 + ORDER_CAP / 4 + ORDER_CAP * 2;
+    static_assert(SMEM_BYTES <= 227 * 1024, "dynamic shared memory above the sm_90 limit");
 };
 
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
@@ -150,11 +163,17 @@ __global__ void __launch_bounds__(THREADS2, 1)
 conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, const Background bg) {
     using C = Cfg2<BN>;
     extern __shared__ uint8_t smem_raw[];
+    __shared__ int s_ncomp;       // computed tiles at the head of the tile order
+    __shared__ int s_walk[6];     // see next_unit
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    const uint32_t bar_base = base + C::STAGES * C::STAGE_BYTES;
-    auto full = [&](int s) { return bar_base + 8u * s; };
-    auto empty = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
+    // rings: A stages (halo boxes, hi | lo) at base, B stages (weights of one (tap, chunk), hi | lo) after them
+    const uint32_t b_ring = base + A_STAGES * A_STAGE_BYTES;
+    const uint32_t bar_base = base + C::RING_BYTES;
+    auto a_full = [&](int s) { return bar_base + 8u * s; };
+    auto a_empty = [&](int s) { return bar_base + 8u * (A_STAGES + s); };
+    auto b_full = [&](int s) { return bar_base + 8u * (2 * A_STAGES + s); };
+    auto b_empty = [&](int s) { return bar_base + 8u * (2 * A_STAGES + C::B_STAGES + s); };
 
     pdl_launch_dependents();      // the next layer may be scheduled as this grid's CTAs retire
     // warp index through a shuffle so that the compiler knows it is warp-uniform
@@ -164,73 +183,114 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
     const int nsplit = p.nsplit, nunits = ntiles * nsplit;      // work unit k: tile k / nsplit, output channels (k % nsplit) * BN ...
     const int kchunks = (p.cin + BKC - 1) / BKC;
     const int nchunks = p.taps * kchunks;
+    // A unit walks (dx, chunk) outer and dy inner: ncols = 3 (1) tap columns, each chunk's box serves nrows = 3 (1) taps
+    const int ncols = p.taps == 9 ? 3 : 1, nrows = ncols, halo = ncols / 2;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < C::STAGES; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 2); }
+        for (int s = 0; s < A_STAGES; ++s) { mbar_init(a_full(s), 1); mbar_init(a_empty(s), 2); }
+        for (int s = 0; s < C::B_STAGES; ++s) { mbar_init(b_full(s), 1); mbar_init(b_empty(s), 2); }
         fence_barrier_init();
         asm volatile("prefetch.tensormap [%0];" ::"l"(&amap) : "memory");
+        s_walk[0] = s_walk[1] = nunits;                 // round-robin; next_unit() with the tile order is set below
+        s_walk[2] = s_walk[4] = nunits + blockIdx.x;
+        s_walk[3] = 1;
+        s_walk[5] = blockIdx.x;
     }
     __syncthreads();
     pdl_wait();                   // the producing layer has completed; nothing above touched global data
 
     // With constant-region information most tiles only store a constant or copy the background.  Static round-robin
-    // leaves some CTAs with two computed tiles and others with none; with tile_order = 1 (for maps of up to ORDER_CAP
-    // tiles) every CTA builds the same order - computed tiles first, stored and copied tiles after - and all roles
-    // walk order[blockIdx.x + i * gridDim.x].  Round-robin is the default: with several steps in flight the SMs that
-    // only store are what the other frames' kernels run on.
-    uint16_t* order = (uint16_t*)(base_ptr + C::STAGES * C::STAGE_BYTES + 256);
+    // leaves some CTAs with two computed tiles and others with none (on the 11-tile-wide BEV grid a stride of 132 units
+    // is 6 tile rows: a CTA stays in one tile column); with tile_order = 1 (for maps of up to ORDER_CAP tiles, above it
+    // round-robin with per-tile distance loads) every CTA builds the same order - computed tiles first, stored and copied
+    // tiles after - and all roles walk it as next_unit() deals it.  Round-robin is the default: with several steps in
+    // flight the SMs that only store are what the other frames' kernels run on.
+    uint32_t* verdict = (uint32_t*)(base_ptr + C::RING_BYTES + 256);   // [2][ORDER_CAP / 32]: constant, background bits
+    uint16_t* order = (uint16_t*)(verdict + 2 * (C::ORDER_CAP / 32));
     const bool small_map = p.tile_dist != nullptr && ntiles <= C::ORDER_CAP;
     const bool use_order = p.tile_order && small_map;
-    // For maps of up to ORDER_CAP tiles warp 0 fetches every tile's distance in one batch of loads (one memory latency
-    // instead of one per tile and role) and keeps the verdicts as order[k] bit 15 (constant) and bit 14 (background).
+    // For maps of up to ORDER_CAP tiles the CTA fetches every tile's distance once (one memory latency per four 32-tile
+    // slots and warp instead of one per tile and role) and keeps the verdicts as order[k] bit 15 (constant) and bit 14
+    // (background).
     if (small_map) {
-        if (warp == 0) {
-            // verdicts of tiles lane, lane + 32, ... as bits of two words; the distances are fetched four at a time
-            uint32_t cst_bits = 0u, bg_bits = 0u;
-            int ty = (lane / tiles_x) % tiles_y, tx = lane % tiles_x;      // tile `lane`; advanced by 32 tiles per slot
+        const int nslots = (ntiles + 31) / 32;
 #pragma unroll 1
-            for (int i0 = 0; i0 * 32 < ntiles; i0 += 4) {
-                int dist[4];
+        for (int i0 = 4 * warp; i0 < nslots; i0 += 4 * (THREADS2 / 32)) {
+            int dist[4];
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const int t = (i0 + e) * 32 + lane;
-                    dist[e] = t < ntiles ? __ldg(&p.tile_dist[t]) : 0;
-                }
+            for (int e = 0; e < 4; ++e) {
+                const int t = (i0 + e) * 32 + lane;
+                dist[e] = t < ntiles ? __ldg(&p.tile_dist[t]) : 0;
+            }
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const int t = (i0 + e) * 32 + lane;
-                    const int f = t < ntiles ? tile_skip_flag(p, bg, dist[e], ty, tx, tiles_y, tiles_x) : 0;
-                    if (f == kConstTile) cst_bits |= 1u << (i0 + e);
-                    if (f == kBgTile) bg_bits |= 1u << (i0 + e);
-                    tx += 32;
-                    while (tx >= tiles_x) { tx -= tiles_x; if (++ty == tiles_y) ty = 0; }
+            for (int e = 0; e < 4; ++e) {
+                const int t = (i0 + e) * 32 + lane;
+                const int f = t < ntiles ? tile_skip_flag(p, bg, dist[e], (t / tiles_x) % tiles_y, t % tiles_x, tiles_y,
+                                                          tiles_x) : 0;
+                const uint32_t cst = __ballot_sync(0xffffffffu, f == kConstTile);
+                const uint32_t bgm = __ballot_sync(0xffffffffu, f == kBgTile);
+                if (lane == 0 && i0 + e < nslots) {
+                    verdict[i0 + e] = cst;
+                    verdict[C::ORDER_CAP / 32 + i0 + e] = bgm;
                 }
             }
-            auto word = [&](int t, int i) {
-                return (uint16_t)(t | (((cst_bits >> i) & 1u) ? 0x8000 : 0) | (((bg_bits >> i) & 1u) ? 0x4000 : 0));
+        }
+        __syncthreads();
+        if (warp == 0) {
+            auto word = [&](int t, uint32_t cst, uint32_t bgm) {
+                return (uint16_t)(t | (((cst >> lane) & 1u) ? 0x8000 : 0) | (((bgm >> lane) & 1u) ? 0x4000 : 0));
             };
             if (use_order) {
                 int n = 0;
-                for (int pass = 0; pass < 2; ++pass)
+                for (int pass = 0; pass < 2; ++pass) {
 #pragma unroll 1
-                    for (int i = 0; i * 32 < ntiles; ++i) {
+                    for (int i = 0; i < nslots; ++i) {
                         const int t = i * 32 + lane;
-                        const bool skip = ((cst_bits | bg_bits) >> i) & 1u;
+                        const uint32_t cst = verdict[i], bgm = verdict[C::ORDER_CAP / 32 + i];
+                        const bool skip = ((cst | bgm) >> lane) & 1u;
                         const bool take = t < ntiles && (skip == (pass == 1));
                         const uint32_t m = __ballot_sync(0xffffffffu, take);
-                        if (take) order[n + __popc(m & ((1u << lane) - 1u))] = word(t, i);
+                        if (take) order[n + __popc(m & ((1u << lane) - 1u))] = word(t, cst, bgm);
                         n += __popc(m);
                     }
+                    if (pass == 0 && lane == 0) s_ncomp = n;
+                }
+                if (lane == 0) {
+                    constexpr int kTailAbsorb = 8;
+                    const int G = gridDim.x, c = blockIdx.x;
+                    const int ucomp = s_ncomp * nsplit;
+                    const int heavy = ucomp % G, light = G - heavy;
+                    const int absorb = heavy ? min(nunits - ucomp, kTailAbsorb * light) : 0;
+                    const int s2 = ucomp + c - heavy, s3 = ucomp + absorb + c;      // this CTA's first unit of each tail part
+                    const int first_tail = (c >= heavy && s2 < ucomp + absorb) ? s2 : s3;
+                    s_walk[0] = ucomp;
+                    s_walk[1] = ucomp + absorb;
+                    s_walk[2] = first_tail;
+                    s_walk[3] = light;
+                    s_walk[4] = s3;
+                    s_walk[5] = c < ucomp ? c : first_tail;
+                }
             } else {
 #pragma unroll 1
-                for (int i = 0; i * 32 < ntiles; ++i) {
+                for (int i = 0; i < nslots; ++i) {
                     const int t = i * 32 + lane;
-                    if (t < ntiles) order[t] = word(t, i);
+                    if (t < ntiles) order[t] = word(t, verdict[i], verdict[C::ORDER_CAP / 32 + i]);
                 }
             }
         }
         __syncthreads();
     }
+    // The units a CTA walks: s_walk[5], then next_unit(k) while below nunits.  Without the tile order: c, c + G, ...
+    // (c = blockIdx.x, G = gridDim.x).  With it, the ucomp computed units go round-robin the same way, which leaves
+    // `heavy` = ucomp % G CTAs with one more of them than the others; the stored and copied units after them go first to
+    // the other CTAs, up to kTailAbsorb each (a store or copy takes a small fraction of a computed unit's time), and
+    // round-robin over every CTA beyond that.  So the CTAs that compute most do not also store.  The walk lives in
+    // shared memory: the BN = 128 consumers have no register to spare across their MMA loop.
+    auto next_unit = [&](int k) -> int {
+        if (k < s_walk[0]) { k += gridDim.x; return k < s_walk[0] ? k : s_walk[2]; }
+        if (k < s_walk[1]) { k += s_walk[3]; return k < s_walk[1] ? k : s_walk[4]; }
+        return k + gridDim.x;
+    };
     // tile_ref(k): the k-th tile in walking order, | kConstTile when it only stores the layer's constant, | kBgTile when
     // it copies the background
     auto tile_ref = [&](int k) -> int {
@@ -241,37 +301,45 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
 
     if (warp == W_LOAD) {
         if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int k = blockIdx.x; k < nunits; k += gridDim.x) {
+            int a_stage = 0, b_stage = 0;
+            uint32_t a_phase = 0, b_phase = 0;
+            // one box per plane and (dx, chunk): rows y0 - halo .. y0 + TILE_H - 1 + halo (the TMA box height of the map)
+            const uint32_t a_bytes = 2u * (TILE_H + 2 * halo) * TILE_W * 128;
+            for (int k = s_walk[5]; k < nunits; k = next_unit(k)) {
                 const int ref = tile_ref(k / nsplit), half = k % nsplit;
                 if (ref & (kConstTile | kBgTile)) continue;                             // nothing to load
                 const int tile = ref;
                 const int b = tile / (tiles_y * tiles_x);
                 const int ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
                 const int y0 = ty * TILE_H, x0 = tx * TILE_W;
-                for (int t = 0; t < p.taps; ++t) {
-                    const int dy = p.taps == 9 ? t / 3 - 1 : 0, dx = p.taps == 9 ? t % 3 - 1 : 0;
+                for (int col = 0; col < ncols; ++col) {
+                    const int dx = col - halo;
                     for (int kc = 0; kc < kchunks; ++kc) {
-                        mbar_wait(empty(stage), phase ^ 1u);
-                        const uint32_t a_hi = base + stage * C::STAGE_BYTES, a_lo = a_hi + A_TILE_BYTES;
-                        const uint32_t b_dst = a_hi + 2 * A_TILE_BYTES;
-                        mbar_expect_tx(full(stage), 2 * A_TILE_BYTES + 2 * C::B_TILE_BYTES);
+                        mbar_wait(a_empty(a_stage), a_phase ^ 1u);
+                        const uint32_t a_hi = base + a_stage * A_STAGE_BYTES;
+                        mbar_expect_tx(a_full(a_stage), a_bytes);
                         // coordinates innermost first: {channel, x, y, plane*B + b}; out-of-image pixels arrive as zeros
-                        tma_load_4d(a_hi, &amap, kc * BKC, x0 + dx, y0 + dy, b, full(stage));
-                        tma_load_4d(a_lo, &amap, kc * BKC, x0 + dx, y0 + dy, p.batch + b, full(stage));
-                        // pack: per (tap, chunk) [hi | lo], each nsplit * BN rows of 128 bytes; this unit's BN rows of each
-                        const uint8_t* src = (const uint8_t*)p.wpack +
-                                             (size_t)(t * kchunks + kc) * (size_t)(2 * nsplit) * C::B_TILE_BYTES +
-                                             (size_t)half * C::B_TILE_BYTES;
-                        constexpr uint32_t kPiece = (C::B_TILE_BYTES >= 8192) ? 8192u : (uint32_t)C::B_TILE_BYTES;
+                        tma_load_4d(a_hi, &amap, kc * BKC, x0 + dx, y0 - halo, b, a_full(a_stage));
+                        tma_load_4d(a_hi + A_PLANE_BYTES, &amap, kc * BKC, x0 + dx, y0 - halo, p.batch + b, a_full(a_stage));
+                        if (++a_stage == A_STAGES) { a_stage = 0; a_phase ^= 1u; }
+                        for (int row = 0; row < nrows; ++row) {
+                            const int t = row * ncols + col;                            // tap (dy + 1) * 3 + dx + 1
+                            mbar_wait(b_empty(b_stage), b_phase ^ 1u);
+                            const uint32_t b_dst = b_ring + b_stage * C::B_STAGE_BYTES;
+                            mbar_expect_tx(b_full(b_stage), C::B_STAGE_BYTES);
+                            // pack: per (tap, chunk) [hi | lo], each nsplit * BN rows of 128 bytes; this unit's BN rows
+                            const uint8_t* src = (const uint8_t*)p.wpack +
+                                                 (size_t)(t * kchunks + kc) * (size_t)(2 * nsplit) * C::B_TILE_BYTES +
+                                                 (size_t)half * C::B_TILE_BYTES;
+                            constexpr uint32_t kPiece = (C::B_TILE_BYTES >= 8192) ? 8192u : (uint32_t)C::B_TILE_BYTES;
 #pragma unroll 1
-                        for (int part = 0; part < 2; ++part)
+                            for (int part = 0; part < 2; ++part)
 #pragma unroll 1
-                            for (uint32_t o = 0; o < (uint32_t)C::B_TILE_BYTES; o += kPiece)
-                                bulk_g2s(b_dst + part * C::B_TILE_BYTES + o,
-                                         src + (size_t)part * nsplit * C::B_TILE_BYTES + o, kPiece, full(stage));
-                        if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
+                                for (uint32_t o = 0; o < (uint32_t)C::B_TILE_BYTES; o += kPiece)
+                                    bulk_g2s(b_dst + part * C::B_TILE_BYTES + o,
+                                             src + (size_t)part * nsplit * C::B_TILE_BYTES + o, kPiece, b_full(b_stage));
+                            if (++b_stage == C::B_STAGES) { b_stage = 0; b_phase ^= 1u; }
+                        }
                     }
                 }
             }
@@ -282,10 +350,10 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
         const int rl0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);        // tile rows rl0 and rl0 + 8 (= pixel py * 16 + px)
         const size_t plane = (size_t)p.batch * p.H * p.W * p.out_split_ch;
         float big[BN / 2], small[BN / 2];
-        int stage = 0;
-        uint32_t phase = 0;
+        int a_stage = 0, b_stage = 0;
+        uint32_t a_phase = 0, b_phase = 0;
         int computed = 0;
-        for (int k = blockIdx.x; k < nunits; k += gridDim.x) {
+        for (int k = s_walk[5]; k < nunits; k = next_unit(k)) {
             const int ref = tile_ref(k / nsplit), n_off = (k % nsplit) * BN;
             const int tile = ref & ~(kConstTile | kBgTile);
             const bool const_tile = (ref & kConstTile) != 0;
@@ -302,23 +370,39 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                 if (k % nsplit == 0) ++computed;
 #pragma unroll
                 for (int i = 0; i < BN / 2; ++i) { big[i] = 0.f; small[i] = 0.f; }
-                int prev = -1;
+                // stages the previous chunk's MMAs read: released once they are known complete (prev_a only after
+                // the last of the box's nrows taps)
+                int prev_b = -1, prev_a = -1, row = 0;
                 for (int ch = 0; ch < nchunks; ++ch) {
-                    mbar_wait(full(stage), phase);
-                    const uint32_t ah = base + stage * C::STAGE_BYTES + (uint32_t)wg * (A_TILE_BYTES / 2);
-                    const uint32_t bh = base + stage * C::STAGE_BYTES + 2 * A_TILE_BYTES;
+                    if (row == 0) mbar_wait(a_full(a_stage), a_phase);
+                    mbar_wait(b_full(b_stage), b_phase);
+                    // tap row `row` of this warpgroup's 4 pixel rows: box rows row + 4 wg .. row + 4 wg + 3
+                    const uint32_t ah = base + a_stage * A_STAGE_BYTES + (uint32_t)(row * TILE_W + wg * 64) * 128u;
+                    const uint32_t bh = b_ring + b_stage * C::B_STAGE_BYTES;
                     wgmma_fence();
-                    mma_chunk_x3<1, BN>(big, small, ah, ah + A_TILE_BYTES, bh, bh + C::B_TILE_BYTES);
+                    mma_chunk_x3<1, BN>(big, small, ah, ah + A_PLANE_BYTES, bh, bh + C::B_TILE_BYTES);
                     wgmma_commit();
-                    wgmma_wait<1>();            // the previous chunk's MMAs have read their stage
-                    if (prev >= 0 && t == 0) mbar_arrive(empty(prev));
-                    prev = stage;
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
+                    wgmma_wait<1>();            // the previous chunk's MMAs have read their stages
+                    if (t == 0) {
+                        if (prev_b >= 0) mbar_arrive(b_empty(prev_b));
+                        if (prev_a >= 0) mbar_arrive(a_empty(prev_a));
+                    }
+                    prev_b = b_stage;
+                    if (++b_stage == C::B_STAGES) { b_stage = 0; b_phase ^= 1u; }
+                    prev_a = -1;
+                    if (++row == nrows) {
+                        row = 0;
+                        prev_a = a_stage;
+                        if (++a_stage == A_STAGES) { a_stage = 0; a_phase ^= 1u; }
+                    }
                 }
                 wgmma_wait<0>();
                 fence_regs<BN / 2>(big);
                 fence_regs<BN / 2>(small);
-                if (prev >= 0 && t == 0) mbar_arrive(empty(prev));
+                if (t == 0) {
+                    if (prev_b >= 0) mbar_arrive(b_empty(prev_b));
+                    if (prev_a >= 0) mbar_arrive(a_empty(prev_a));
+                }
             }
             // epilogue from registers: folded BN + ReLU (or the layer constant), fp32 and / or split-plane stores
 #pragma unroll
@@ -363,7 +447,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
         // Background tiles in a pass of their own: interleaved with the MMA units, the copy's address arithmetic is
         // hoisted across the accumulators and spills them.
         if (bg.split || bg.f32) {
-            for (int k = blockIdx.x; k < nunits; k += gridDim.x) {
+            for (int k = s_walk[5]; k < nunits; k = next_unit(k)) {
                 const int ref = tile_ref(k / nsplit);
                 if (!(ref & kBgTile)) continue;
                 const int tile = ref & ~kBgTile;
@@ -460,7 +544,8 @@ extern "C" int sassd_conv2d_f16x3_occ_bg(const sassd_conv2d_desc* d, const void*
     cuuint64_t dims[4] = {(cuuint64_t)d->cin_stored, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)(2 * d->batch)};
     cuuint64_t strides[3] = {(cuuint64_t)d->cin_stored * 2, (cuuint64_t)d->W * d->cin_stored * 2,
                              (cuuint64_t)d->H * d->W * d->cin_stored * 2};
-    cuuint32_t box[4] = {(cuuint32_t)BKC, (cuuint32_t)TILE_W, (cuuint32_t)TILE_H, 1u};
+    // one box holds every row the tile's vertical taps read: the tile and a halo row above and below (3x3)
+    cuuint32_t box[4] = {(cuuint32_t)BKC, (cuuint32_t)TILE_W, (cuuint32_t)(d->taps == 9 ? A_ROWS : TILE_H), 1u};
     cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
     CUresult rc = enc(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(in_split), dims, strides, box, estr,
                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
