@@ -328,6 +328,25 @@ int sassd_rescore_nms(const float* boxes, const float* scores, const int32_t* la
                       float* det, int32_t* d_ndet, int det_cap, int32_t* d_status,
                       void* ws, size_t ws_bytes, sassd_stream_t stream);
 
+/* ------------------------------------------------------------------------
+ * KITTI result formatting of the NMS output, results.kitti_bbox2results
+ * (transforms.py:225-279) for a whole batch.  det [batch,det_cap,9] and
+ * d_ndet [batch] as written by sassd_rescore_nms; meta [batch][36] fp64 =
+ * P2 (12), Tr_velo_to_cam (12), R0_rect (9), img_h, img_w, pad
+ * (results.meta_block).  rows [batch,det_cap,14] fp64 = (alpha, bbox x1 y1 x2
+ * y2, dimensions l h w, location x y z, rotation_y, score, label) of the boxes
+ * whose image projection is not wholly outside the image, clipped to it, in
+ * detection order; n_out [batch] their number.  Rows past n_out[b] are left
+ * unwritten.  Arithmetic follows the host formatter's dtypes (fp32 yaw wrap,
+ * corners and alpha; fp64 transforms and projection); sinf / cosf / atan2f and
+ * the summation order of the host's matrix products differ, so the agreement
+ * is within stated bounds, not bitwise.  No host synchronisation.
+ * ---------------------------------------------------------------------- */
+#define SASSD_KITTI_META 36
+#define SASSD_KITTI_ROW 14
+int sassd_kitti_format(const float* det, const int32_t* d_ndet, int batch, int det_cap, const double* meta,
+                       double* rows, int32_t* n_out, sassd_stream_t stream);
+
 /* iou3d_cuda.nms_gpu alone (iou3d.cpp:73-120): boxes [n,5] already sorted by
  * score; mask [n, ceil(n/64)] u64 in the reference layout (only columns j > i
  * are filled; the reference also fills the unused lower triangle); keep [n]

@@ -9,7 +9,8 @@ Two entry points:
     one H2D copy, voxelize + anchors_mask + backbone + neck + heads + PSWarp + NMS with
     every data-dependent size kept on the device, one D2H copy of the fixed-size result.
     With ``frustum_planes`` the frames are full sweeps, cropped to the camera frustum on the
-    device first (the reference crops them offline into ``velodyne_reduced``).
+    device first (the reference crops them offline into ``velodyne_reduced``).  With ``metas``
+    the step also formats its detections as KITTI annotations on the device (ops.kitti_format).
 """
 import numpy as np
 import torch
@@ -17,6 +18,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import builder, ops
+from .results import annos_from_rows, meta_block
 from .single_stage_heads import unpack_detections
 
 
@@ -42,6 +44,7 @@ class SingleStageDetector(nn.Module):
         self._mask_stream = None
         self._graph = None
         self._crop_graph = None
+        self._kitti_graphs = {}           # crop -> captured step that also formats KITTI rows (forward_points metas=)
         self._graph_args = None
         self._stream_slots = None
         self._stream_key = None
@@ -69,6 +72,7 @@ class SingleStageDetector(nn.Module):
         the kernel selection; anything that changes those must force a re-capture."""
         self._graph = None
         self._crop_graph = None
+        self._kitti_graphs = {}
         self._stream_slots = None
         self._stream_key = None
 
@@ -182,7 +186,8 @@ class SingleStageDetector(nn.Module):
         data-dependent size already lives on the device, so the ~65 launches of a step become one graph
         launch.  Steps whose shape does not fit fall back to the eager path.  Calls with ``frustum_planes`` replay a
         second graph, captured on their first use, that runs the crop and the step; there ``max_points_per_frame`` bounds
-        the full sweeps (e.g. 131072)."""
+        the full sweeps (e.g. 131072).  Calls with ``metas`` replay a graph, again captured on first use, that ends with
+        the KITTI result formatter."""
         self._graph_args = (int(batch), int(max_points_per_frame))
         self._graph = _GraphedStep(self, batch, max_points_per_frame, latency=True)
         return self._graph
@@ -190,9 +195,11 @@ class SingleStageDetector(nn.Module):
     def disable_cuda_graph(self):
         self._graph = None
         self._crop_graph = None
+        self._kitti_graphs = {}
         self._graph_args = None
 
-    def detect_stream(self, batches, batch, max_points_per_frame=32768, depth=4, concurrent=True, crop=False):
+    def detect_stream(self, batches, batch, max_points_per_frame=32768, depth=4, concurrent=True, crop=False,
+                      kitti=False):
         """Throughput API: iterate over batches (each a list of ``batch`` raw point arrays) and yield their
         detections in order.  ``depth`` captured graphs with their own static buffers and scratch are used
         round-robin: while the GPU runs step i, the host stages and uploads step i+1 (copy stream) and unpacks
@@ -200,45 +207,70 @@ class SingleStageDetector(nn.Module):
         step (voxelize, rulebooks, the sparse layers, NMS) run beside the dense layers of its neighbour.
         With ``crop`` each item of ``batches`` is (points_list, planes [batch,6,4]) of full sweeps: every slot's graph
         crops the frames to their camera frustums (forward_points' ``frustum_planes``) before the step, and
-        ``max_points_per_frame`` bounds the full sweeps."""
+        ``max_points_per_frame`` bounds the full sweeps.
+        With ``kitti`` each item also carries the frames' ``img_meta``-style dicts (forward_points' ``metas``):
+        (points_list, planes, metas) with ``crop``, else (points_list, metas); every slot's graph ends with the KITTI
+        result formatter and each yield is the batch's annotation dicts (kitti_bbox2results' format)."""
         ops.require_cuda()
-        key = (batch, max_points_per_frame, depth, bool(crop))
+        if kitti and self.class_names is None:
+            raise ValueError("detect_stream(kitti=True) needs class_names")
+        key = (batch, max_points_per_frame, depth, bool(crop), bool(kitti))
         if self._stream_key != key or self._stream_slots is None:
-            self._stream_slots = [_GraphedStep(self, batch, max_points_per_frame, crop=crop) for _ in range(depth)]
+            self._stream_slots = [_GraphedStep(self, batch, max_points_per_frame, crop=crop, kitti=kitti)
+                                  for _ in range(depth)]
             self._copy_stream = torch.cuda.Stream()
             self._stream_key = key
         slots, pending = self._stream_slots, []
         for i, item in enumerate(batches):
-            fb, planes = item if crop else (item, None)
-            if crop:
-                planes = _frame_planes(planes, len(fb))
+            item = tuple(item) if (crop or kitti) else (item,)
+            fb = item[0]
+            planes = _frame_planes(item[1], len(fb)) if crop else None
+            metas = item[-1] if kitti else None
+            meta = _meta_blocks(metas, len(fb)) if kitti else None
             counts = [int(p.shape[0]) for p in fb]
             slot = slots[i % depth]
             if len(pending) == depth:                       # the slot we are about to reuse must be drained
-                bbs, scs, lbs = pending.pop(0).collect()
-                yield [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(bbs, scs, lbs)]
+                yield self._collected(*pending.pop(0))
             if not slot.fits(len(fb), counts):
                 raise ValueError("batch does not fit the captured shape (batch %d, %d points/frame)" %
                                  (batch, max_points_per_frame))
-            slot.submit(fb, counts, self._copy_stream, own_stream=concurrent, planes=planes)
-            pending.append(slot)
-        for slot in pending:
-            bbs, scs, lbs = slot.collect()
-            yield [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(bbs, scs, lbs)]
+            slot.submit(fb, counts, self._copy_stream, own_stream=concurrent, planes=planes, meta=meta)
+            pending.append((slot, metas))
+        for slot, metas in pending:
+            yield self._collected(slot, metas)
 
-    def forward_points(self, points_list, return_aux=False, frustum_planes=None):
+    def _collected(self, slot, metas):
+        """Wait for a slot's step and convert its host copy into the caller's per-frame results."""
+        out = slot.collect()
+        if slot.kitti:
+            return annos_from_rows(*out, self.class_names, [m["sample_idx"] for m in metas])
+        return [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(*out)]
+
+    def forward_points(self, points_list, return_aux=False, frustum_planes=None, metas=None):
         """Raw points in (list of [N_i,>=4] numpy arrays), detections out: per frame a dict of
         boxes_lidar [D,7], scores [D], label_preds [D] (or None entries when nothing survives).
         ``frustum_planes``: one float64 [6,4] array per frame (frustum.camera_frustum_planes).  The frames are then
         full sweeps; each is cropped to its camera frustum on the device, in point order (ops.frustum_crop), and the
-        step runs on what is left, as on the reference's offline-cropped ``velodyne_reduced`` clouds."""
+        step runs on what is left, as on the reference's offline-cropped ``velodyne_reduced`` clouds.
+        ``metas``: one ``img_meta``-style dict per frame ('calib' a results.Calibration, 'img_shape', 'sample_idx').
+        The detections are then formatted on the device (ops.kitti_format) and the call returns, like forward_test,
+        one KITTI annotation dict per frame; ``class_names`` must be set.  With ``return_aux`` the aux dict also holds
+        the unformatted detections (det, ndet)."""
         ops.require_cuda()
         if self.voxel_generator is None or self.anchor_set is None:
             raise RuntimeError("call attach_data_pipeline(voxel_generator, anchor_set) first")
+        if metas is not None and self.class_names is None:
+            raise ValueError("forward_points(metas=) needs class_names")
         dev = next(self.parameters()).device
         planes = None if frustum_planes is None else _frame_planes(frustum_planes, len(points_list))
+        meta = None if metas is None else _meta_blocks(metas, len(points_list))
         hp, ho, counts = self.stage_points(points_list)
-        if planes is None:
+        if meta is not None:
+            crop = planes is not None
+            if crop not in self._kitti_graphs and self._graph_args is not None:
+                self._kitti_graphs[crop] = _GraphedStep(self, *self._graph_args, latency=True, crop=crop, kitti=True)
+            g = self._kitti_graphs.get(crop)
+        elif planes is None:
             if self._graph is None and self._graph_args is not None:     # dropped by a weight / precision change
                 self._graph = _GraphedStep(self, *self._graph_args, latency=True)
             g = self._graph
@@ -247,13 +279,24 @@ class SingleStageDetector(nn.Module):
                 self._crop_graph = _GraphedStep(self, *self._graph_args, latency=True, crop=True)
             g = self._crop_graph
         if g is not None and not return_aux and g.fits(len(points_list), counts):
-            bbs, scs, lbs = g.run_host(hp, ho, sum(counts), planes)
-            return [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(bbs, scs, lbs)]
+            out = g.run_host(hp, ho, sum(counts), planes, meta)
+            if meta is not None:
+                return annos_from_rows(*out, self.class_names, [m["sample_idx"] for m in metas])
+            return [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(*out)]
         points = hp.to(dev, non_blocking=True)
         pt_off = ho.to(dev, non_blocking=True)
         if planes is not None:
             points, pt_off = ops.frustum_crop(points, pt_off, len(points_list), torch.from_numpy(planes).to(dev))
         det, d_ndet, status, aux = self.forward_device(points, pt_off, len(points_list), max(counts + [1]))
+        if meta is not None:
+            rows, n_out = ops.kitti_format(det, d_ndet, torch.from_numpy(meta).to(dev))
+            word = int(status.item())
+            if word:
+                raise ops._lib.SassdError("capacity overflow on device: %s" % ops._lib.decode_flags(word))
+            out = annos_from_rows(rows.cpu().numpy(), n_out.cpu().numpy(), self.class_names,
+                                  [m["sample_idx"] for m in metas])
+            aux.update(det=det, ndet=d_ndet)
+            return (out, aux) if return_aux else out
         bbs, scs, lbs = unpack_detections(det, d_ndet, status)
         out = [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(bbs, scs, lbs)]
         return (out, aux) if return_aux else out
@@ -265,6 +308,13 @@ def _frame_planes(frustum_planes, batch):
     if planes.shape != (batch, 6, 4):
         raise ValueError("frustum_planes: expected %d arrays of shape [6,4], got shape %s" % (batch, planes.shape))
     return planes
+
+
+def _meta_blocks(metas, batch):
+    """One ``img_meta``-style dict per frame -> contiguous float64 [batch,36] (results.meta_block)."""
+    if len(metas) != batch:
+        raise ValueError("metas: expected %d dicts, got %d" % (batch, len(metas)))
+    return np.stack([meta_block(m["calib"], m["img_shape"]) for m in metas])
 
 
 def _pinned_pair(n_points, n_off):
@@ -289,20 +339,24 @@ def _stage_into(hp, ho, points_list, counts):
 class _GraphedStep:
     """One captured step of SingleStageDetector.forward_device with static input/output buffers."""
 
-    def __init__(self, model, batch, max_points_per_frame, latency=False, crop=False):
+    def __init__(self, model, batch, max_points_per_frame, latency=False, crop=False, kitti=False):
         """latency=True: this step will run alone on the GPU (enable_cuda_graph / forward_points): the dense convs walk
         the computed tiles first so that the constant-region tiles shorten every layer; False (detect_stream slots,
         several steps in flight): round-robin tiles, the SMs a layer leaves idle serve the other steps.
         crop=True: the static points are full sweeps and the graph crops them to the frustums given by the static
-        planes [batch,6,4] (ops.frustum_crop) before the step; the cropped frames never exceed the full ones."""
+        planes [batch,6,4] (ops.frustum_crop) before the step; the cropped frames never exceed the full ones.
+        kitti=True: the graph ends with the KITTI result formatter (ops.kitti_format) on the static meta blocks
+        [batch,36]; the host copy is its rows and counts instead of the detections."""
         dev = next(model.parameters()).device
         self.model, self.batch, self.maxpts = model, int(batch), int(max_points_per_frame)
         self.cap = self.batch * self.maxpts
-        self.crop = bool(crop)
+        self.crop, self.kitti = bool(crop), bool(kitti)
         self.points = torch.zeros((self.cap, 4), dtype=torch.float32, device=dev)
         self.pt_off = torch.zeros((self.batch + 1,), dtype=torch.int32, device=dev)
         if self.crop:
             self.planes = torch.zeros((self.batch, 6, 4), dtype=torch.float64, device=dev)
+        if self.kitti:
+            self.meta = torch.zeros((self.batch, ops._lib.KITTI_META), dtype=torch.float64, device=dev)
         # Scratch buffers private to this graph (the captured kernels bake their addresses in), so that several
         # captured steps can be in flight on different streams without sharing anything but read-only weights.
         self.ws = ops.Workspace()
@@ -329,8 +383,13 @@ class _GraphedStep:
             ops.CONV2D_TILE_ORDER = order0
             if pdl0 is not None:
                 ops._lib.load().sassd_set_pdl(pdl0)
-        self.h_det = torch.empty(self.det.shape, dtype=torch.float32, pin_memory=True)
-        self.h_nd = torch.empty(self.d_ndet.shape, dtype=torch.int32, pin_memory=True)
+        if self.kitti:
+            self.h_rows = torch.empty(self.rows.shape, dtype=torch.float64, pin_memory=True)
+            self.h_nout = torch.empty(self.n_out.shape, dtype=torch.int32, pin_memory=True)
+            self.h_meta = torch.empty(self.meta.shape, dtype=torch.float64, pin_memory=True)
+        else:
+            self.h_det = torch.empty(self.det.shape, dtype=torch.float32, pin_memory=True)
+            self.h_nd = torch.empty(self.d_ndet.shape, dtype=torch.int32, pin_memory=True)
         self.h_status = torch.empty((1,), dtype=torch.int32, pin_memory=True)
         self.h_points, self.h_off = _pinned_pair(self.cap, self.batch + 1)
         if self.crop:
@@ -342,7 +401,10 @@ class _GraphedStep:
         points, pt_off = self.points, self.pt_off
         if self.crop:
             points, pt_off = ops.frustum_crop(points, pt_off, self.batch, self.planes)
-        return self.model.forward_device(points, pt_off, self.batch, self.maxpts)
+        det, d_ndet, status, aux = self.model.forward_device(points, pt_off, self.batch, self.maxpts)
+        if self.kitti:
+            self.rows, self.n_out = ops.kitti_format(det, d_ndet, self.meta)
+        return det, d_ndet, status, aux
 
     def fits(self, batch, counts):
         return batch == self.batch and max(counts + [0]) <= self.maxpts
@@ -356,27 +418,41 @@ class _GraphedStep:
         self.graph.replay()
         return self.det, self.d_ndet, self.status
 
-    def run_host(self, hp, ho, total, planes=None):
-        """pinned host points in, numpy detections out: H2D, one graph launch, D2H, one stream sync."""
+    def run_host(self, hp, ho, total, planes=None, meta=None):
+        """pinned host points in, numpy detections (or KITTI rows) out: H2D, one graph launch, D2H, one stream sync."""
         self.points[:total].copy_(hp[:total], non_blocking=True)
         self.pt_off.copy_(ho, non_blocking=True)
         if self.crop:
             self.h_planes.numpy()[...] = planes
             self.planes.copy_(self.h_planes, non_blocking=True)
+        if self.kitti:
+            self.h_meta.numpy()[...] = meta
+            self.meta.copy_(self.h_meta, non_blocking=True)
         self.graph.replay()
-        self.h_det.copy_(self.det, non_blocking=True)
-        self.h_nd.copy_(self.d_ndet, non_blocking=True)
-        self.h_status.copy_(self.status, non_blocking=True)
+        self._download()
         torch.cuda.current_stream().synchronize()
         return self.unpack()
 
+    def _download(self):
+        """D2H of the step's result on the current stream: the KITTI rows and counts of a formatting step, else the
+        detections and counts; and the status word."""
+        if self.kitti:
+            self.h_rows.copy_(self.rows, non_blocking=True)
+            self.h_nout.copy_(self.n_out, non_blocking=True)
+        else:
+            self.h_det.copy_(self.det, non_blocking=True)
+            self.h_nd.copy_(self.d_ndet, non_blocking=True)
+        self.h_status.copy_(self.status, non_blocking=True)
+
     # ---- asynchronous use (SingleStageDetector.detect_stream): submit() ... collect()
-    def submit(self, points_list, counts, copy_stream, own_stream=False, planes=None):
+    def submit(self, points_list, counts, copy_stream, own_stream=False, planes=None, meta=None):
         """Stage into this slot's pinned buffer, H2D on the copy stream, then replay + D2H on the current stream or,
         with ``own_stream``, on this slot's stream so that consecutive steps overlap on the GPU."""
         _stage_into(self.h_points, self.h_off, points_list, counts)
         if self.crop:
             self.h_planes.numpy()[...] = planes
+        if self.kitti:
+            self.h_meta.numpy()[...] = meta
         total = sum(counts)
         cur = self.stream if own_stream else torch.cuda.current_stream()
         with torch.cuda.stream(copy_stream):
@@ -384,13 +460,13 @@ class _GraphedStep:
             self.pt_off.copy_(self.h_off, non_blocking=True)
             if self.crop:
                 self.planes.copy_(self.h_planes, non_blocking=True)
+            if self.kitti:
+                self.meta.copy_(self.h_meta, non_blocking=True)
             self.loaded.record(copy_stream)
         cur.wait_event(self.loaded)
         with torch.cuda.stream(cur):
             self.graph.replay()
-            self.h_det.copy_(self.det, non_blocking=True)
-            self.h_nd.copy_(self.d_ndet, non_blocking=True)
-            self.h_status.copy_(self.status, non_blocking=True)
+            self._download()
             self.done.record(cur)
 
     def collect(self):
@@ -401,6 +477,8 @@ class _GraphedStep:
         word = int(self.h_status.numpy()[0])
         if word:
             raise ops._lib.SassdError("capacity overflow on device: %s" % ops._lib.decode_flags(word))
+        if self.kitti:      # (rows, n_out): results.annos_from_rows
+            return self.h_rows.numpy().copy(), self.h_nout.numpy().copy()
         det, n = self.h_det.numpy(), self.h_nd.numpy()
         bbs, scs, lbs = [], [], []
         for b in range(det.shape[0]):

@@ -1,0 +1,187 @@
+"""Reading a KITTI object split from disk for evaluation (host side of ``python -m sassd_b200.test``).
+
+Layout (the reference's ``data/kitti``): ``ImageSets/<split>.txt`` lists the frame ids; every frame's files are under
+``training/`` (``testing/`` has no labels):
+  * ``velodyne/%06d.bin`` full sweeps (cropped to the camera frustum on the device) or ``velodyne_reduced/%06d.bin``
+    (cropped offline), float32 (x, y, z, reflectance) rows;
+  * ``calib/%06d.txt`` (results.Calibration);
+  * ``image_2/%06d.png``, of which only the IHDR chunk is read: the reference decodes the whole image for its shape
+    alone (mmdet/datasets/kitti.py:270-272), and KITTI image sizes vary (375x1242, 370x1224, 376x1241, ...);
+  * ``label_2/%06d.txt``, read into ground-truth annotations with the semantics of the reference's
+    get_label_anno / get_label_annos (tools/kitti_common.py:560-601, 648-666).
+"""
+import os
+import struct
+from concurrent.futures import ThreadPoolExecutor
+
+import numpy as np
+
+from .frustum import camera_frustum_planes
+from .results import Calibration
+
+PNG_SIGNATURE = b"\x89PNG\r\n\x1a\n"
+_PNG_CHANNELS = {0: 1, 2: 3, 3: 3, 4: 2, 6: 4}      # IHDR colour type -> channels of the decoded image
+
+
+def read_split(root, split):
+    """Frame ids of ``ImageSets/<split>.txt`` (one integer per line), in file order."""
+    with open(os.path.join(root, "ImageSets", split + ".txt")) as fh:
+        return [int(line) for line in fh.read().split()]
+
+
+def png_shape(path):
+    """(height, width, channels) from a PNG's IHDR chunk; anything that is not a PNG is refused."""
+    with open(path, "rb") as fh:
+        head = fh.read(33)          # signature (8) + IHDR length (4), type (4), data (13) ...
+    if len(head) < 8 or head[:8] != PNG_SIGNATURE:
+        raise ValueError("%s: not a PNG file" % path)
+    if len(head) < 29:
+        raise ValueError("%s: truncated PNG header" % path)
+    length, ctype = struct.unpack(">I4s", head[8:16])
+    if ctype != b"IHDR" or length != 13:
+        raise ValueError("%s: PNG does not start with an IHDR chunk" % path)
+    width, height, _depth, colour = struct.unpack(">IIBB", head[16:26])
+    if width == 0 or height == 0 or colour not in _PNG_CHANNELS:
+        raise ValueError("%s: invalid PNG header" % path)
+    return int(height), int(width), _PNG_CHANNELS[colour]
+
+
+def read_points(path):
+    """float32 [N, 4] point cloud; a file whose size is not a multiple of 16 bytes is refused."""
+    size = os.path.getsize(path)
+    if size % 16:
+        raise ValueError("%s: %d bytes is not a whole number of (x, y, z, r) float32 rows" % (path, size))
+    return np.fromfile(path, dtype=np.float32).reshape(-1, 4)
+
+
+def read_label(path):
+    """One ``label_2`` file -> ground-truth annotation dict (get_label_anno's semantics).
+
+    Every line's name is kept, DontCare included; ``index`` numbers the objects that are not DontCare, which KITTI
+    lists first, and gives -1 to the rest; ``group_ids`` numbers every line.  The file's h, w, l dimensions become
+    l, h, w.  ``score`` is the 16th field when the first line has one, zeros otherwise."""
+    with open(path) as fh:
+        fields = [line.strip().split(" ") for line in fh.readlines()]
+    n = len(fields)
+    n_obj = sum(1 for f in fields if f[0] != "DontCare")
+    floats = lambda lo, hi: np.array([[float(v) for v in f[lo:hi]] for f in fields])    # noqa: E731
+    anno = {
+        "name": np.array([f[0] for f in fields]),
+        "truncated": np.array([float(f[1]) for f in fields]),
+        "occluded": np.array([int(float(f[2])) for f in fields]),
+        "alpha": np.array([float(f[3]) for f in fields]),
+        "bbox": floats(4, 8).reshape(-1, 4),
+        "dimensions": floats(8, 11).reshape(-1, 3)[:, [2, 0, 1]],
+        "location": floats(11, 14).reshape(-1, 3),
+        "rotation_y": np.array([float(f[14]) for f in fields]).reshape(-1),
+    }
+    if n and len(fields[0]) == 16:
+        anno["score"] = np.array([float(f[15]) for f in fields])
+    else:
+        anno["score"] = np.zeros((anno["bbox"].shape[0],))
+    anno["index"] = np.array(list(range(n_obj)) + [-1] * (n - n_obj), dtype=np.int32)
+    anno["group_ids"] = np.arange(n, dtype=np.int32)
+    return anno
+
+
+def read_labels(label_dir, ids):
+    """``label_dir/%06d.txt`` of every id -> annotation dicts with ``image_idx`` (get_label_annos)."""
+    annos = []
+    for idx in ids:
+        anno = read_label(os.path.join(label_dir, "%06d.txt" % idx))
+        anno["image_idx"] = np.array([idx] * anno["name"].shape[0], dtype=np.int64)
+        annos.append(anno)
+    return annos
+
+
+class PlaneCache:
+    """camera_frustum_planes per (calibration values, image height and width): a KITTI split has few distinct
+    calibrations (one per recording day), so the plane sets are computed once each."""
+
+    def __init__(self):
+        self._planes = {}
+
+    def __call__(self, calib, img_shape):
+        key = (calib.P2.tobytes(), calib.V2C.tobytes(), calib.R0.tobytes(), int(img_shape[0]), int(img_shape[1]))
+        p = self._planes.get(key)
+        if p is None:
+            p = self._planes[key] = camera_frustum_planes(calib, img_shape)
+        return p
+
+    def __len__(self):
+        return len(self._planes)
+
+
+def padded_batches(ids, batch):
+    """Frame ids -> lists of ``batch`` entries; the last list is padded with None (empty frames whose results the
+    caller drops)."""
+    out = [list(ids[i:i + batch]) for i in range(0, len(ids), batch)]
+    if out and len(out[-1]) < batch:
+        out[-1] += [None] * (batch - len(out[-1]))
+    return out
+
+
+class KittiSplit:
+    """Frames of one split: ``frame(idx)`` -> (points [N,4] f32, img_meta dict with calib, img_shape, sample_idx)."""
+
+    def __init__(self, root, split="val", lidar="velodyne"):
+        if lidar not in ("velodyne", "velodyne_reduced"):
+            raise ValueError("lidar must be velodyne or velodyne_reduced, not %r" % lidar)
+        self.root, self.split, self.lidar = root, split, lidar
+        self.ids = read_split(root, split)
+        self.dir = os.path.join(root, "training")
+        self.planes = PlaneCache()
+        self._pad_meta = None
+
+    def path(self, sub, idx, ext):
+        return os.path.join(self.dir, sub, "%06d.%s" % (idx, ext))
+
+    def meta(self, idx):
+        """img_meta-style dict of one frame: calib, img_shape (from the PNG header), sample_idx."""
+        return dict(calib=Calibration(self.path("calib", idx, "txt")),
+                    img_shape=png_shape(self.path("image_2", idx, "png")), sample_idx=idx)
+
+    def frame(self, idx):
+        return read_points(self.path(self.lidar, idx, "bin")), self.meta(idx)
+
+    def pad_frame(self):
+        """A padding frame: no points, the calibration and image shape of the split's first frame, sample_idx -1.
+        It does not depend on the batch it pads, which may hold no real frame at all (a rank's last batch under
+        torchrun, or every batch of a rank when the split has fewer frames than ranks)."""
+        if self._pad_meta is None:
+            self._pad_meta = dict(self.meta(self.ids[0]), sample_idx=-1)
+        return np.zeros((0, 4), np.float32), self._pad_meta
+
+    def gt_annos(self, ids=None):
+        return read_labels(os.path.join(self.dir, "label_2"), self.ids if ids is None else ids)
+
+
+class Prefetcher:
+    """Reads batches of frames ``depth`` batches ahead on a thread pool (np.fromfile releases the GIL) and yields
+    (ids, points_list, metas) in order.  ``wait`` accumulates the seconds the consumer spent blocked on reads."""
+
+    def __init__(self, split, batches, depth=4, workers=4):
+        self.split, self.batches, self.depth = split, batches, max(1, int(depth))
+        self.pool = ThreadPoolExecutor(max_workers=max(1, int(workers)))
+        self.wait = 0.0
+
+    def _submit(self, ids):
+        return [self.pool.submit(self.split.frame, i) if i is not None else None for i in ids]
+
+    def __iter__(self):
+        import time
+        try:
+            pending = [(ids, self._submit(ids)) for ids in self.batches[:self.depth]]
+            nxt = len(pending)
+            while pending:
+                ids, futs = pending.pop(0)
+                t0 = time.perf_counter()
+                frames = [f.result() if f is not None else None for f in futs]
+                self.wait += time.perf_counter() - t0
+                if nxt < len(self.batches):
+                    pending.append((self.batches[nxt], self._submit(self.batches[nxt])))
+                    nxt += 1
+                frames = [fr if fr is not None else self.split.pad_frame() for fr in frames]
+                yield ids, [p for p, _ in frames], [m for _, m in frames]
+        finally:
+            self.pool.shutdown(wait=True, cancel_futures=True)

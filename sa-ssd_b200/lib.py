@@ -36,6 +36,7 @@ PREC_FP32, PREC_TF32X3, PREC_F16X3 = 0, 1, 2
 CONV2D_TILE_H, CONV2D_TILE_W = 8, 16      # SASSD_CONV2D_TILE_H / _W of the header
 TILE_DIST_MAX = 9                         # SASSD_TILE_DIST_MAX
 SPCONV_TILE_ROWS = 128                    # SASSD_SPCONV_TILE_ROWS
+KITTI_META, KITTI_ROW = 36, 14            # SASSD_KITTI_META / SASSD_KITTI_ROW
 
 OK = 0
 ERRORS = {-1: "SASSD_ERR_ARG", -2: "SASSD_ERR_LAUNCH", -3: "SASSD_ERR_WORKSPACE", -4: "SASSD_ERR_UNSUPPORTED"}
@@ -84,6 +85,7 @@ _SIGNATURES = {
     "sassd_pswarp": (c_int, [P, c_int, c_int, c_int, c_int, P, P, c_int, c_float, c_float, c_float, P, P]),
     "sassd_rescore_nms_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "sassd_rescore_nms": (c_int, [P, P, P, P, c_int, c_int, c_float, c_float, c_int, P, P, c_int, P, P, c_size_t, P]),
+    "sassd_kitti_format": (c_int, [P, P, c_int, c_int, P, P, P, P]),
     "sassd_nms_workspace_bytes": (c_size_t, [c_int]),
     "sassd_nms_mask": (c_int, [P, c_int, c_float, P, P]),
     "sassd_nms_sorted": (c_int, [P, c_int, c_float, P, P, P, c_size_t, P]),

@@ -54,7 +54,7 @@ def next_pow2(n):
 _KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1,"sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
             "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
-            "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
+            "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
             "sassd_boxes_iou_bev": 1}
 LAUNCHES = 0          # running count of kernels launched through this module
 PROFILE = None        # set to a list to collect (name, label, start_event, end_event)
@@ -361,6 +361,21 @@ def rescore_nms(boxes, scores, labels, d_k, score_thr, iou_thr, det_cap, status,
                                  ctypes.c_float(score_thr), ctypes.c_float(iou_thr), NMS_CAP, _ptr(det), _ptr(d_ndet),
                                  det_cap, _ptr(status), _ptr(w), w.numel(), _stream())
     return det, d_ndet
+
+
+def kitti_format(det, d_ndet, meta):
+    """det [B,det_cap,9] f32, d_ndet [B] i32 (rescore_nms), meta [B,36] f64 (results.meta_block; device).
+    Returns (rows [B,det_cap,14] f64, n_out [B] i32): per frame the KITTI annotation rows of the detections whose image
+    projection is not wholly outside the image (results.annos_from_rows), in detection order.  Rows past n_out[b] are
+    left unwritten."""
+    dev = det.device
+    B, det_cap = det.shape[0], det.shape[1]
+    assert meta.dtype == torch.float64 and tuple(meta.shape) == (B, _lib.KITTI_META), "meta must be float64 [B,36]"
+    rows = torch.empty((B, det_cap, _lib.KITTI_ROW), dtype=torch.float64, device=dev)
+    n_out = torch.empty((B,), dtype=torch.int32, device=dev)
+    _call("sassd_kitti_format", None, _ptr(det), _ptr(d_ndet), B, det_cap, _ptr(meta), _ptr(rows), _ptr(n_out),
+          _stream())
+    return rows, n_out
 
 
 def nms_mask(boxes5, thr):

@@ -15,6 +15,8 @@ the reference and here (DESIGN.md §8: not on the device path).
 """
 import numpy as np
 
+from .lib import KITTI_META, KITTI_ROW      # the header's SASSD_KITTI_META / SASSD_KITTI_ROW
+
 _RESULT_KEYS = ('name', 'truncated', 'occluded', 'alpha', 'bbox',
                 'dimensions', 'location', 'rotation_y', 'score')
 
@@ -161,6 +163,59 @@ def kitti_bbox2results(boxes_lidar, scores, labels, meta, class_names=None):
 def kitti_bbox2results_batch(boxes_lidar, scores, labels, metas, class_names=None):
     """All frames of a batch (the loop of single_stage.py:127-131 over ``kitti_bbox2results``)."""
     return [kitti_bbox2results(b, s, l, m, class_names) for b, s, l, m in zip(boxes_lidar, scores, labels, metas)]
+
+
+def meta_block(calib, img_shape):
+    """Calibration + image (h, w, ...) -> the float64 [36] block the device formatter reads per frame
+    (ops.kitti_format): P2, Tr_velo_to_cam, R0_rect row-major, then img_h, img_w and one pad value."""
+    out = np.zeros(KITTI_META, np.float64)
+    out[0:12] = calib.P2.ravel()
+    out[12:24] = calib.V2C.ravel()
+    out[24:33] = calib.R0.ravel()
+    out[33], out[34] = float(img_shape[0]), float(img_shape[1])
+    return out
+
+
+def annos_from_rows(rows, n_out, class_names, sample_ids):
+    """Device formatter output (rows [B,cap,14] f64 = alpha, bbox (4), dimensions l h w, location (3), rotation_y,
+    score, label; n_out [B]) -> one annotation dict per frame, with the keys and dtypes of ``kitti_bbox2results``; a
+    frame without rows gets ``empty_result_anno()``."""
+    names_all = np.asarray(class_names)
+    out = []
+    for b in range(len(sample_ids)):
+        n = int(n_out[b])
+        if n == 0:
+            out.append(empty_result_anno())
+            continue
+        r = rows[b, :n]
+        names = names_all[r[:, 13].astype(np.int64)]
+        names = names.astype('<U%d' % int(np.char.str_len(names).max()))
+        out.append({
+            'name': names, 'truncated': np.zeros(n), 'occluded': np.zeros(n, np.int64),
+            'alpha': r[:, 0].astype(np.float32), 'bbox': r[:, 1:5].copy(),
+            'dimensions': r[:, 5:8].astype(np.float32), 'location': r[:, 8:11].astype(np.float32),
+            'rotation_y': r[:, 11].astype(np.float32), 'score': r[:, 12].astype(np.float32),
+            'image_idx': np.full(n, int(sample_ids[b]), np.int64),
+        })
+    return out
+
+
+def rows_from_annos(annos, class_names, cap):
+    """Inverse of ``annos_from_rows`` (exact: every field widens to float64): annotation dicts -> (rows [B,cap,14]
+    f64, n_out [B] int32), e.g. for one fixed-size exchange of a rank's results (dist.DetectionGather)."""
+    index = {n: i for i, n in enumerate(class_names)}
+    rows = np.zeros((len(annos), cap, KITTI_ROW), np.float64)
+    n_out = np.zeros(len(annos), np.int32)
+    for b, a in enumerate(annos):
+        n = len(a['name'])
+        if n > cap:
+            raise ValueError("frame %d: %d rows exceed the capacity %d" % (b, n, cap))
+        n_out[b] = n
+        if n:
+            rows[b, :n] = np.concatenate([a['alpha'][:, None], a['bbox'], a['dimensions'], a['location'],
+                                          a['rotation_y'][:, None], a['score'][:, None],
+                                          np.array([index[str(x)] for x in a['name']], np.float64)[:, None]], axis=1)
+    return rows, n_out
 
 
 _LINE_DEFAULTS = (('name', None), ('truncated', -1), ('occluded', -1), ('alpha', -10), ('bbox', None),

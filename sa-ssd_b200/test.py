@@ -1,0 +1,164 @@
+"""Evaluate a checkpoint on a KITTI split end to end (the reference's tools/test.py):
+
+    python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR [--split val] [--batch 16]
+                              [--lidar velodyne|velodyne_reduced] [--out DIR] [--workers N] [--json FILE]
+
+Frames are read from disk a few batches ahead (kitti_data.Prefetcher) and streamed through the captured step
+(SingleStageDetector.detect_stream): full sweeps (``--lidar velodyne``) are cropped to the camera frustum on the
+device, and every step ends with the KITTI result formatter on the device (ops.kitti_format).  The last batch is
+padded with empty frames whose results are dropped.  Prints the official AP table (kitti_eval), the frame rate (wall
+clock of the streamed detection, the evaluation excluded) and the time spent waiting on reads.
+
+Under torchrun, frame i of the split goes to rank i mod W; at the end every rank contributes one fixed-size block of
+KITTI rows and counts to a single all_gather_into_tensor (dist.DetectionGather) and rank 0 re-interleaves, writes and
+evaluates.
+"""
+import argparse
+import json
+import math
+import os
+import sys
+import time
+
+import numpy as np
+
+DEFAULT_MAX_POINTS = {"velodyne": 131072, "velodyne_reduced": 32768}
+
+
+def parse_args(argv=None):
+    p = argparse.ArgumentParser(prog="python -m sassd_b200.test", description=__doc__.split("\n\n")[0])
+    p.add_argument("config")
+    p.add_argument("checkpoint")
+    p.add_argument("--data-root", required=True, help="KITTI root holding ImageSets/ and training/")
+    p.add_argument("--split", default="val")
+    p.add_argument("--batch", type=int, default=16)
+    p.add_argument("--lidar", default="velodyne", choices=("velodyne", "velodyne_reduced"),
+                   help="full sweeps (cropped on the device) or the offline-cropped reduced clouds")
+    p.add_argument("--max-points", type=int, default=None,
+                   help="points per frame the captured step holds (default 131072 full, 32768 reduced)")
+    p.add_argument("--out", default=None, help="write one KITTI result file %%06d.txt per frame here")
+    p.add_argument("--workers", type=int, default=4, help="reader threads")
+    p.add_argument("--depth", type=int, default=4, help="batches read ahead")
+    p.add_argument("--json", default=None, help="write the AP arrays and rates here")
+    args = p.parse_args(argv)
+    if args.batch < 1:
+        p.error("--batch must be positive")
+    if args.max_points is None:
+        args.max_points = DEFAULT_MAX_POINTS[args.lidar]
+    return args
+
+
+def rank_batches(ids, rank, world, batch):
+    """This rank's frames (ids[rank::world]) as padded batches; every rank gets the same number of batches so that the
+    result blocks of the final exchange have one size."""
+    from .kitti_data import padded_batches
+    per_rank = math.ceil(len(ids) / world)
+    n_batches = max(1, math.ceil(per_rank / batch))
+    mine = list(ids[rank::world])
+    return padded_batches(mine + [None] * (n_batches * batch - len(mine)), batch)
+
+
+def gather_annos(annos_local, ids, class_names, cap, device):
+    """Every rank's per-frame annotation dicts (its frames j*W + rank, padding included) -> the annotations of the
+    split's frames ``ids``, in order, on every rank, through one all_gather of [rows | n_out]."""
+    import torch
+    from . import dist as D
+    from .results import annos_from_rows, rows_from_annos
+    rows, n_out = rows_from_annos(annos_local, class_names, cap)
+    g = D.DetectionGather(len(annos_local), cap, device, width=2 * rows.shape[2])
+    rows_all, n_all = g(torch.from_numpy(rows).to(device).view(torch.float32),
+                        torch.from_numpy(n_out).to(device))
+    rows_all, n_all = D.interleave(rows_all, n_all)
+    rows_all = rows_all.contiguous().view(torch.float64)[:len(ids)].cpu().numpy()
+    n_all = n_all[:len(ids)].cpu().numpy()
+    return annos_from_rows(rows_all, n_all, class_names, ids)
+
+
+def write_results(out_dir, ids, annos):
+    """One ``%06d.txt`` per frame, annos_to_kitti_label(with_score=True); a frame without detections gets an empty
+    file.  The annotations hold dimensions as l, h, w; KITTI files hold h, w, l (what kitti_data.read_label and the
+    official devkit read)."""
+    from .results import annos_to_kitti_label
+    os.makedirs(out_dir, exist_ok=True)
+    for idx, anno in zip(ids, annos):
+        lines = annos_to_kitti_label(dict(anno, dimensions=anno["dimensions"][:, [1, 2, 0]]), with_score=True)
+        with open(os.path.join(out_dir, "%06d.txt" % idx), "w") as fh:
+            fh.write("".join(l + "\n" for l in lines))
+
+
+def run(args, log=print):
+    """Returns the result dict (AP arrays as nested lists, rates) on rank 0, None on the other ranks."""
+    import torch
+    import sassd_b200 as S
+    from . import dist as D
+    from . import ops
+    from .checkpoint import load_params_from_file
+    from .kitti_data import KittiSplit, Prefetcher
+
+    split = KittiSplit(args.data_root, args.split, args.lidar)
+    if not split.ids:
+        raise ValueError("split %s of %s lists no frames" % (args.split, args.data_root))
+    cfg = S.Config.fromfile(args.config)
+    rank, world, local = D.init_from_env()
+    batches = rank_batches(split.ids, rank, world, args.batch)
+    ops.require_cuda()                  # first device use below
+    device = torch.device("cuda", local)
+    torch.cuda.set_device(device)
+    model, _, _ = S.build_from_config(cfg, device=device)
+    load_params_from_file(model, args.checkpoint)
+    crop = args.lidar == "velodyne"
+    class_names = model.class_names
+
+    def items(reader):
+        for ids, points, metas in reader:
+            if crop:
+                yield points, [split.planes(m["calib"], m["img_shape"]) for m in metas], metas
+            else:
+                yield points, metas
+
+    stream = lambda src: model.detect_stream(src, args.batch, args.max_points, depth=4, crop=crop,  # noqa: E731
+                                             kitti=True)
+    for _ in stream([]):                # capture the slots' graphs before the clock starts
+        pass
+    torch.cuda.synchronize(device)
+    reader = Prefetcher(split, batches, depth=args.depth, workers=args.workers)
+    t0 = time.perf_counter()
+    annos_local = [a for annos in stream(items(reader)) for a in annos]
+    torch.cuda.synchronize(device)
+    wall = time.perf_counter() - t0
+    n_local = sum(i is not None for ids in batches for i in ids)
+    wall = D.max_over_ranks(wall, device)
+
+    if world > 1:
+        dt_annos = gather_annos(annos_local, split.ids, class_names, model.extra_head.det_cap, device)
+    else:
+        dt_annos = [a for i, a in zip([i for ids in batches for i in ids], annos_local) if i is not None]
+    if rank != 0:
+        D.barrier()
+        return None
+    if args.out:
+        write_results(args.out, split.ids, dt_annos)
+    from .kitti_eval import official_eval
+    gt_annos = split.gt_annos()
+    text, ap = official_eval(gt_annos, dt_annos, class_names)
+    fps = len(split.ids) / wall
+    log(text, end="")
+    log("frames: %d (%d rank%s), %.1f frames/s, read wait %.3f s on rank 0 (%d of %d frames on rank 0)" % (
+        len(split.ids), world, "s" if world > 1 else "", fps, reader.wait, n_local, len(split.ids)))
+    result = dict(frames=len(split.ids), world=world, batch=args.batch, lidar=args.lidar, frames_per_s=fps,
+                  wall_s=wall, read_wait_s=reader.wait, text=text,
+                  ap={k: (None if v is None else np.asarray(v).tolist()) for k, v in ap.items()})
+    if args.json:
+        with open(args.json, "w") as fh:
+            json.dump(result, fh, indent=1)
+    D.barrier()
+    return result
+
+
+def main(argv=None):
+    return run(parse_args(argv))
+
+
+if __name__ == "__main__":
+    main(sys.argv[1:])
+    sys.exit(0)
