@@ -347,6 +347,48 @@ int sassd_rescore_nms(const float* boxes, const float* scores, const int32_t* la
 int sassd_kitti_format(const float* det, const int32_t* d_ndet, int batch, int det_cap, const double* meta,
                        double* rows, int32_t* n_out, sassd_stream_t stream);
 
+/* ------------------------------------------------------------------------
+ * Auxiliary point-wise head, SpMiddleFHD.forward(is_test=False)
+ * (cmn.py:121-135, :175-189): per voxel a foreground logit and a centre offset.
+ *
+ * sassd_three_nn: for every level-0 row r < *d_rows0 (mean [rows_cap0,4] =
+ * SimpleVoxel mean x,y,z,r; coors0 [rows_cap0,4] (b,z,y,x)) the three nearest
+ * centres of its own frame at each of the levels 1..3 (coorsL [capL,4], rows
+ * sorted by flattened (b,z,y,x), *d_rowsL of them).  Centres are tensor2points
+ * (transforms.py:218-223) with the reference's literal offset (0,-40,-3) and
+ * voxel sizes (.1,.1,.2), (.2,.2,.4), (.4,.4,.8).  idx / dist2 [rows_cap0,3,3]
+ * = (row, level, k): global row indices of the level and squared distances,
+ * bit-identical to pointnet2 three_nn (interpolate_gpu.cu:9-56); a frame with
+ * fewer than three centres gets idx 0 and dist2 +inf in the missing slots.
+ * points_mean [rows_cap0,4] (may be NULL) receives (b, x, y, z), cmn.py:104-106.
+ * Rows past *d_rows0 are left unwritten.
+ *
+ * sassd_point_aux_head: weights 1/(sqrt(dist2)+1e-8) normalised per level,
+ * three_interpolate of each level's features, point_fc (160->64, no bias, no
+ * activation), point_cls (64->1), point_reg (64->3), all fp32.  host_levels[3]
+ * describe the features of levels 1..3 (32, 64, 64 channels): fp32 rows, or
+ * split fp16 rows (hi plane, lo plane plane_stride elements further,
+ * x = hi + lo * 2^-11).  w_fc_t = point_fc.weight^T [160,64]; w_out [4,64] =
+ * point_cls.weight then point_reg.weight.  cls [rows_cap0], reg [rows_cap0,3].
+ * Neither function synchronises with the host.
+ * ---------------------------------------------------------------------- */
+typedef struct {
+    const void* rows;
+    int64_t plane_stride;   /* split rows: elements from the hi to the lo plane */
+    int32_t row_stride;     /* elements */
+    int32_t channels;
+    int32_t split;          /* 0: fp32 rows, 1: split fp16 rows */
+    int32_t pad;
+} sassd_point_levels;
+
+int sassd_three_nn(const float* mean, const int32_t* coors0, const int32_t* d_rows0, int rows_cap0,
+                   const int32_t* coors1, const int32_t* d_rows1, const int32_t* coors2, const int32_t* d_rows2,
+                   const int32_t* coors3, const int32_t* d_rows3, int32_t* idx, float* dist2, float* points_mean,
+                   sassd_stream_t stream);
+int sassd_point_aux_head(const int32_t* idx, const float* dist2, const int32_t* d_rows0, int rows_cap0,
+                         const sassd_point_levels* host_levels, const float* w_fc_t, const float* w_out, float* cls,
+                         float* reg, sassd_stream_t stream);
+
 /* iou3d_cuda.nms_gpu alone (iou3d.cpp:73-120): boxes [n,5] already sorted by
  * score; mask [n, ceil(n/64)] u64 in the reference layout (only columns j > i
  * are filled; the reference also fills the unused lower triangle); keep [n]

@@ -8,8 +8,10 @@ wrapper, tools/test.py:142-143) and are copied only where name and shape match.
 Parameter names (SURVEY.md §8b): ``neck.backbone.{conv0,down0,...}.{0,3,6}.weight``
 in spconv-v1 layout ``[kz,ky,kx,Cin,Cout]`` with BatchNorm1d at ``.{1,4,7}``;
 ``neck.fcn.conv{0..7}.weight`` / ``neck.fcn.bn{0..7}.*``; ``rpn_head.conv_{cls,box,
-dir_cls}.{weight,bias}``; ``extra_head.convs.{0,1,3}.*``.  The aux-head keys
-(``neck.point_fc/point_cls/point_reg``, cmn.py:27-29) are training-only and ignored.
+dir_cls}.{weight,bias}``; ``extra_head.convs.{0,1,3}.*``.  The aux-network keys
+(``neck.point_fc/point_cls/point_reg``, cmn.py:27-29) are loaded like the others and used by
+``SpMiddleFHD.forward(is_test=False)`` / ``forward_points(point_outputs=True)``;
+``make_synthetic_state_dict`` does not set them.
 """
 import math
 import os

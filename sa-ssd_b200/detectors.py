@@ -10,7 +10,8 @@ Two entry points:
     every data-dependent size kept on the device, one D2H copy of the fixed-size result.
     With ``frustum_planes`` the frames are full sweeps, cropped to the camera frustum on the
     device first (the reference crops them offline into ``velodyne_reduced``).  With ``metas``
-    the step also formats its detections as KITTI annotations on the device (ops.kitti_format).
+    the step also formats its detections as KITTI annotations on the device (ops.kitti_format).  With
+    ``point_outputs`` it also returns the auxiliary network's per-voxel foreground logits and centre offsets.
 """
 import numpy as np
 import torch
@@ -45,6 +46,7 @@ class SingleStageDetector(nn.Module):
         self._graph = None
         self._crop_graph = None
         self._kitti_graphs = {}           # crop -> captured step that also formats KITTI rows (forward_points metas=)
+        self._point_graphs = {}           # (crop, kitti) -> captured step that also runs the aux network (point_outputs)
         self._graph_args = None
         self._stream_slots = None
         self._stream_key = None
@@ -73,6 +75,7 @@ class SingleStageDetector(nn.Module):
         self._graph = None
         self._crop_graph = None
         self._kitti_graphs = {}
+        self._point_graphs = {}
         self._stream_slots = None
         self._stream_key = None
 
@@ -142,9 +145,11 @@ class SingleStageDetector(nn.Module):
         self.anchor_set = anchor_set.to(dev)
         return self
 
-    def forward_device(self, points, pt_off, batch, max_points_per_frame):
+    def forward_device(self, points, pt_off, batch, max_points_per_frame, point_outputs=False):
         """Everything on the device, no synchronisation.  points [Ncap,4], pt_off [batch+1] int32.
-        Returns (det [B,det_cap,9], d_ndet [B], status [1], aux dict)."""
+        Returns (det [B,det_cap,9], d_ndet [B], status [1], aux dict).  With ``point_outputs`` the aux dict also holds
+        the auxiliary network's points_mean [cap,4] (b, x, y, z), point_cls [cap] and point_reg [cap,3] (neck.point_head)
+        for the voxel rows (frame_rows)."""
         dev = points.device
         status = torch.zeros((1,), dtype=torch.int32, device=dev)
         vg, aset = self.voxel_generator, self.anchor_set
@@ -157,7 +162,8 @@ class SingleStageDetector(nn.Module):
         self._mask_stream.wait_stream(main)
         with torch.cuda.stream(self._mask_stream):
             mask = aset.mask_device(coors, d_rows, batch)
-        y, conv6, xs = self.neck.forward_nhwc(mean, coors, batch, d_rows=d_rows, status=status)
+        out = self.neck.forward_nhwc(mean, coors, batch, d_rows=d_rows, status=status, point_outputs=point_outputs)
+        y, conv6, xs = out[:3]
         main.wait_stream(self._mask_stream)
         head = self.rpn_head.forward_nhwc(y)
         anchors, _ = aset.device_tensors()
@@ -167,6 +173,8 @@ class SingleStageDetector(nn.Module):
         aux = dict(voxels=voxels, coors=coors, num_points=num, mean=mean, frame_rows=frame_rows, mask=mask, x=y,
                    conv6=conv6, head=head, guided=boxes, guided_labels=labels, guided_index=index, d_k=d_k,
                    ps_scores=scores, sparse=xs)
+        if point_outputs:
+            aux.update(out[3])
         return det, d_ndet, status, aux
 
     def stage_points(self, points_list):
@@ -187,7 +195,7 @@ class SingleStageDetector(nn.Module):
         launch.  Steps whose shape does not fit fall back to the eager path.  Calls with ``frustum_planes`` replay a
         second graph, captured on their first use, that runs the crop and the step; there ``max_points_per_frame`` bounds
         the full sweeps (e.g. 131072).  Calls with ``metas`` replay a graph, again captured on first use, that ends with
-        the KITTI result formatter."""
+        the KITTI result formatter, and calls with ``point_outputs`` one that also runs the auxiliary network."""
         self._graph_args = (int(batch), int(max_points_per_frame))
         self._graph = _GraphedStep(self, batch, max_points_per_frame, latency=True)
         return self._graph
@@ -196,6 +204,7 @@ class SingleStageDetector(nn.Module):
         self._graph = None
         self._crop_graph = None
         self._kitti_graphs = {}
+        self._point_graphs = {}
         self._graph_args = None
 
     def detect_stream(self, batches, batch, max_points_per_frame=32768, depth=4, concurrent=True, crop=False,
@@ -246,7 +255,7 @@ class SingleStageDetector(nn.Module):
             return annos_from_rows(*out, self.class_names, [m["sample_idx"] for m in metas])
         return [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(*out)]
 
-    def forward_points(self, points_list, return_aux=False, frustum_planes=None, metas=None):
+    def forward_points(self, points_list, return_aux=False, frustum_planes=None, metas=None, point_outputs=False):
         """Raw points in (list of [N_i,>=4] numpy arrays), detections out: per frame a dict of
         boxes_lidar [D,7], scores [D], label_preds [D] (or None entries when nothing survives).
         ``frustum_planes``: one float64 [6,4] array per frame (frustum.camera_frustum_planes).  The frames are then
@@ -255,7 +264,11 @@ class SingleStageDetector(nn.Module):
         ``metas``: one ``img_meta``-style dict per frame ('calib' a results.Calibration, 'img_shape', 'sample_idx').
         The detections are then formatted on the device (ops.kitti_format) and the call returns, like forward_test,
         one KITTI annotation dict per frame; ``class_names`` must be set.  With ``return_aux`` the aux dict also holds
-        the unformatted detections (det, ndet)."""
+        the unformatted detections (det, ndet).
+        ``point_outputs``: the step also runs SA-SSD's auxiliary network (neck.point_head) and the call returns
+        (results, points), results as without it and ``points`` one dict per frame of xyz [V,3] (the voxel means),
+        cls [V] (foreground logits) and reg [V,3] (offsets to the box centre), V the frame's voxels in voxel-row order.
+        With ``return_aux`` the aux dict comes third."""
         ops.require_cuda()
         if self.voxel_generator is None or self.anchor_set is None:
             raise RuntimeError("call attach_data_pipeline(voxel_generator, anchor_set) first")
@@ -265,7 +278,13 @@ class SingleStageDetector(nn.Module):
         planes = None if frustum_planes is None else _frame_planes(frustum_planes, len(points_list))
         meta = None if metas is None else _meta_blocks(metas, len(points_list))
         hp, ho, counts = self.stage_points(points_list)
-        if meta is not None:
+        if point_outputs:
+            key = (planes is not None, meta is not None)
+            if key not in self._point_graphs and self._graph_args is not None:
+                self._point_graphs[key] = _GraphedStep(self, *self._graph_args, latency=True, crop=key[0], kitti=key[1],
+                                                       point_outputs=True)
+            g = self._point_graphs.get(key)
+        elif meta is not None:
             crop = planes is not None
             if crop not in self._kitti_graphs and self._graph_args is not None:
                 self._kitti_graphs[crop] = _GraphedStep(self, *self._graph_args, latency=True, crop=crop, kitti=True)
@@ -281,13 +300,20 @@ class SingleStageDetector(nn.Module):
         if g is not None and not return_aux and g.fits(len(points_list), counts):
             out = g.run_host(hp, ho, sum(counts), planes, meta)
             if meta is not None:
-                return annos_from_rows(*out, self.class_names, [m["sample_idx"] for m in metas])
-            return [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(*out)]
+                res = annos_from_rows(*out, self.class_names, [m["sample_idx"] for m in metas])
+            else:
+                res = [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(*out)]
+            return (res, g.point_results()) if point_outputs else res
         points = hp.to(dev, non_blocking=True)
         pt_off = ho.to(dev, non_blocking=True)
         if planes is not None:
             points, pt_off = ops.frustum_crop(points, pt_off, len(points_list), torch.from_numpy(planes).to(dev))
-        det, d_ndet, status, aux = self.forward_device(points, pt_off, len(points_list), max(counts + [1]))
+        det, d_ndet, status, aux = self.forward_device(points, pt_off, len(points_list), max(counts + [1]),
+                                                       point_outputs=point_outputs)
+        pts = None
+        if point_outputs:
+            pts = _split_points(aux["points_mean"].cpu().numpy(), aux["point_cls"].cpu().numpy(),
+                                aux["point_reg"].cpu().numpy(), aux["frame_rows"].cpu().numpy())
         if meta is not None:
             rows, n_out = ops.kitti_format(det, d_ndet, torch.from_numpy(meta).to(dev))
             word = int(status.item())
@@ -296,10 +322,20 @@ class SingleStageDetector(nn.Module):
             out = annos_from_rows(rows.cpu().numpy(), n_out.cpu().numpy(), self.class_names,
                                   [m["sample_idx"] for m in metas])
             aux.update(det=det, ndet=d_ndet)
-            return (out, aux) if return_aux else out
-        bbs, scs, lbs = unpack_detections(det, d_ndet, status)
-        out = [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(bbs, scs, lbs)]
-        return (out, aux) if return_aux else out
+        else:
+            bbs, scs, lbs = unpack_detections(det, d_ndet, status)
+            out = [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(bbs, scs, lbs)]
+        ret = (out,) + ((pts,) if point_outputs else ()) + ((aux,) if return_aux else ())
+        return ret if len(ret) > 1 else out
+
+
+def _split_points(points_mean, cls, reg, frame_rows):
+    """Capacity-sized aux outputs (host) -> one dict per frame of its voxel rows: xyz [V,3], cls [V], reg [V,3]."""
+    out = []
+    for b in range(frame_rows.shape[0] - 1):
+        r0, r1 = int(frame_rows[b]), int(frame_rows[b + 1])
+        out.append(dict(xyz=points_mean[r0:r1, 1:4].copy(), cls=cls[r0:r1].copy(), reg=reg[r0:r1].copy()))
+    return out
 
 
 def _frame_planes(frustum_planes, batch):
@@ -339,18 +375,20 @@ def _stage_into(hp, ho, points_list, counts):
 class _GraphedStep:
     """One captured step of SingleStageDetector.forward_device with static input/output buffers."""
 
-    def __init__(self, model, batch, max_points_per_frame, latency=False, crop=False, kitti=False):
+    def __init__(self, model, batch, max_points_per_frame, latency=False, crop=False, kitti=False, point_outputs=False):
         """latency=True: this step will run alone on the GPU (enable_cuda_graph / forward_points): the dense convs walk
         the computed tiles first so that the constant-region tiles shorten every layer; False (detect_stream slots,
         several steps in flight): round-robin tiles, the SMs a layer leaves idle serve the other steps.
         crop=True: the static points are full sweeps and the graph crops them to the frustums given by the static
         planes [batch,6,4] (ops.frustum_crop) before the step; the cropped frames never exceed the full ones.
         kitti=True: the graph ends with the KITTI result formatter (ops.kitti_format) on the static meta blocks
-        [batch,36]; the host copy is its rows and counts instead of the detections."""
+        [batch,36]; the host copy is its rows and counts instead of the detections.
+        point_outputs=True: the step also runs the auxiliary network and copies its outputs and the frame row offsets to
+        the host (point_results)."""
         dev = next(model.parameters()).device
         self.model, self.batch, self.maxpts = model, int(batch), int(max_points_per_frame)
         self.cap = self.batch * self.maxpts
-        self.crop, self.kitti = bool(crop), bool(kitti)
+        self.crop, self.kitti, self.point_outputs = bool(crop), bool(kitti), bool(point_outputs)
         self.points = torch.zeros((self.cap, 4), dtype=torch.float32, device=dev)
         self.pt_off = torch.zeros((self.batch + 1,), dtype=torch.int32, device=dev)
         if self.crop:
@@ -390,6 +428,9 @@ class _GraphedStep:
         else:
             self.h_det = torch.empty(self.det.shape, dtype=torch.float32, pin_memory=True)
             self.h_nd = torch.empty(self.d_ndet.shape, dtype=torch.int32, pin_memory=True)
+        if self.point_outputs:
+            self.h_pts = {k: torch.empty(self.aux[k].shape, dtype=self.aux[k].dtype, pin_memory=True)
+                          for k in ("points_mean", "point_cls", "point_reg", "frame_rows")}
         self.h_status = torch.empty((1,), dtype=torch.int32, pin_memory=True)
         self.h_points, self.h_off = _pinned_pair(self.cap, self.batch + 1)
         if self.crop:
@@ -401,7 +442,8 @@ class _GraphedStep:
         points, pt_off = self.points, self.pt_off
         if self.crop:
             points, pt_off = ops.frustum_crop(points, pt_off, self.batch, self.planes)
-        det, d_ndet, status, aux = self.model.forward_device(points, pt_off, self.batch, self.maxpts)
+        det, d_ndet, status, aux = self.model.forward_device(points, pt_off, self.batch, self.maxpts,
+                                                             point_outputs=self.point_outputs)
         if self.kitti:
             self.rows, self.n_out = ops.kitti_format(det, d_ndet, self.meta)
         return det, d_ndet, status, aux
@@ -442,6 +484,9 @@ class _GraphedStep:
         else:
             self.h_det.copy_(self.det, non_blocking=True)
             self.h_nd.copy_(self.d_ndet, non_blocking=True)
+        if self.point_outputs:
+            for k, h in self.h_pts.items():
+                h.copy_(self.aux[k], non_blocking=True)
         self.h_status.copy_(self.status, non_blocking=True)
 
     # ---- asynchronous use (SingleStageDetector.detect_stream): submit() ... collect()
@@ -472,6 +517,12 @@ class _GraphedStep:
     def collect(self):
         self.done.synchronize()
         return self.unpack()
+
+    def point_results(self):
+        """The last run's aux outputs, per frame (forward_points(point_outputs=True))."""
+        h = self.h_pts
+        return _split_points(h["points_mean"].numpy(), h["point_cls"].numpy(), h["point_reg"].numpy(),
+                             h["frame_rows"].numpy())
 
     def unpack(self):
         word = int(self.h_status.numpy()[0])

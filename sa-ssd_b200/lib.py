@@ -31,12 +31,19 @@ class GConvDesc(ctypes.Structure):
                                               "rows_cap", "batch", "H", "W", "relu")]
 
 
+class PointLevels(ctypes.Structure):
+    _fields_ = [("rows", c_void_p), ("plane_stride", ctypes.c_int64), ("row_stride", ctypes.c_int32),
+                ("channels", ctypes.c_int32), ("split", ctypes.c_int32), ("pad", ctypes.c_int32)]
+
+
 GCONV_TABLE, GCONV_CONV2D, GCONV_ROWS = 0, 1, 2
 PREC_FP32, PREC_TF32X3, PREC_F16X3 = 0, 1, 2
 CONV2D_TILE_H, CONV2D_TILE_W = 8, 16      # SASSD_CONV2D_TILE_H / _W of the header
 TILE_DIST_MAX = 9                         # SASSD_TILE_DIST_MAX
 SPCONV_TILE_ROWS = 128                    # SASSD_SPCONV_TILE_ROWS
 KITTI_META, KITTI_ROW = 36, 14            # SASSD_KITTI_META / SASSD_KITTI_ROW
+POINT_LEVEL_CHANNELS = (32, 64, 64)       # sassd_point_aux_head: features of backbone levels 1..3 (conv1, conv2, conv3)
+POINT_FC_IN, POINT_FC_OUT = 160, 64       # point_fc: Linear(160, 64); point_cls / point_reg read its 64 outputs
 
 OK = 0
 ERRORS = {-1: "SASSD_ERR_ARG", -2: "SASSD_ERR_LAUNCH", -3: "SASSD_ERR_WORKSPACE", -4: "SASSD_ERR_UNSUPPORTED"}
@@ -86,6 +93,8 @@ _SIGNATURES = {
     "sassd_rescore_nms_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "sassd_rescore_nms": (c_int, [P, P, P, P, c_int, c_int, c_float, c_float, c_int, P, P, c_int, P, P, c_size_t, P]),
     "sassd_kitti_format": (c_int, [P, P, c_int, c_int, P, P, P, P]),
+    "sassd_three_nn": (c_int, [P, P, P, c_int, P, P, P, P, P, P, P, P, P, P]),
+    "sassd_point_aux_head": (c_int, [P, P, P, c_int, ctypes.POINTER(PointLevels), P, P, P, P, P]),
     "sassd_nms_workspace_bytes": (c_size_t, [c_int]),
     "sassd_nms_mask": (c_int, [P, c_int, c_float, P, P]),
     "sassd_nms_sorted": (c_int, [P, c_int, c_float, P, P, P, c_size_t, P]),

@@ -3,9 +3,10 @@ backbone) + BEVNet (dense BEV convs) — mmdet/models/necks/cmn.py:12-29,102-119
 
 Parameter names and shapes equal the reference's (SURVEY.md §8b) so that its
 checkpoints load; all arithmetic runs in the sm_90a kernels of csrc/gconv.cu
-(BatchNorm folded into each conv's epilogue, eval mode).  The training-only aux head
-(cmn.py:44-100,121-135) is out of scope: its Linear parameters exist for checkpoint
-compatibility, ``is_test=False`` raises.
+(BatchNorm folded into each conv's epilogue, eval mode).  The auxiliary point-wise network
+(cmn.py:121-135, :175-189) runs in eval mode: ``forward(..., is_test=False)`` returns the reference's
+``(x, conv6, (points_mean, point_cls, point_reg))`` through csrc/point_aux.cu.  Its loss and targets
+(cmn.py:44-100) serve training only and are not built; in training mode ``forward`` raises.
 """
 import torch
 from torch import nn
@@ -211,7 +212,7 @@ class SpMiddleFHD(nn.Module):
         self.sparse_shape = list(output_shape)
         self.backbone = VxNet(num_input_features)
         self.fcn = BEVNet(in_features=num_hidden_features, num_filters=256)
-        # training-only aux head (cmn.py:27-29): parameters kept so reference checkpoints load completely
+        # auxiliary point-wise network (cmn.py:27-29), run by forward_nhwc(point_outputs=True)
         self.point_fc = nn.Linear(160, 64, bias=False)
         self.point_cls = nn.Linear(64, 1, bias=False)
         self.point_reg = nn.Linear(64, 3, bias=False)
@@ -219,18 +220,52 @@ class SpMiddleFHD(nn.Module):
         self.dense_tma = True             # F16X3: keep the BEV maps as split fp16 planes and feed the convs by TMA
         self.overlap_rulebooks = True     # build the rulebook chain on a side stream, concurrently with the convs
         self._side = None
+        self._point_packed = None
+
+    def _point_weights(self):
+        """(point_fc.weight^T [160,64], [point_cls.weight; point_reg.weight] [4,64]) fp32, re-derived when a reload
+        changes the parameters (the same version check as BEVNet._weights)."""
+        ver = _versions(self.point_fc.weight, self.point_cls.weight, self.point_reg.weight)
+        c = self._point_packed
+        if c is None or c[0] != ver:
+            with torch.no_grad():
+                fc_t = self.point_fc.weight.detach().t().contiguous().float()
+                out = torch.cat([self.point_cls.weight.detach(), self.point_reg.weight.detach()], 0).contiguous().float()
+            c = self._point_packed = (ver, fc_t, out)
+        return c[1], c[2]
+
+    def point_head(self, mean, coors, d_rows, middle):
+        """The auxiliary network on the device (cmn.py:121-135): ``mean`` / ``coors`` [cap,4] are the voxel rows,
+        ``middle`` the outputs of conv1, conv2, conv3.  Returns dict(points_mean [cap,4] (b, x, y, z), point_cls [cap],
+        point_reg [cap,3], idx / dist2 [cap,3,3] of the three nearest centres per level); rows past d_rows are
+        unwritten.  point_reg is what the reference regresses, the offset from the point to its box centre
+        (points_op.cpp:107-144)."""
+        levels = [(m._indices, m.d_rows) for m in middle]
+        idx, dist2, pm = ops.three_nn(mean, coors, d_rows, levels, points_mean=True)
+        feats = []
+        for m, ch in zip(middle, ops._lib.POINT_LEVEL_CHANNELS):
+            if m._features is not None:
+                feats.append(ops.point_level(feat=m._features, channels=ch))
+            else:
+                feats.append(ops.point_level(split=m._split, channels=ch))
+        fc_t, w_out = self._point_weights()
+        cls, reg = ops.point_aux_head(idx, dist2, d_rows, feats, fc_t, w_out)
+        return dict(points_mean=pm, point_cls=cls, point_reg=reg, idx=idx, dist2=dist2, middle=middle)
 
     def set_precision(self, precision, sparse=None):
         """precision for the dense BEV convs; ``sparse`` (default: same) for the ruled sparse convs."""
         self.backbone.set_precision(precision if sparse is None else sparse)
         self.fcn.precision = precision
 
-    def forward_nhwc(self, voxel_features, coors, batch_size, d_rows=None, status=None):
-        """Device-side entry: capacity-sized inputs + row counter; returns NHWC (x, conv6) and the tensor."""
+    def forward_nhwc(self, voxel_features, coors, batch_size, d_rows=None, status=None, point_outputs=False):
+        """Device-side entry: capacity-sized inputs + row counter; returns NHWC (x, conv6) and the tensor.  With
+        ``point_outputs`` the auxiliary network runs after conv3, before the dense neck, and its outputs
+        (point_head) come fourth."""
         if self.training:
             raise NotImplementedError("sassd_b200 is inference-only: call .eval()")
         x = spconv.SparseConvTensor(voxel_features, coors, self.sparse_shape, batch_size, d_rows=d_rows, status=status)
         x.row_cap_factor = self.row_cap_factor
+        x0_mean, x0_coors, rows0 = x._features, x._indices, x.d_rows     # level 0: the voxel means (SimpleVoxel)
         if self.overlap_rulebooks:
             if self._side is None:
                 self._side = torch.cuda.Stream(device=x.device)
@@ -239,6 +274,9 @@ class SpMiddleFHD(nn.Module):
         x, middle = self.backbone(x)
         if self.overlap_rulebooks:
             torch.cuda.current_stream().wait_stream(self._side)   # join (also required to end a graph capture)
+        pts = None
+        if point_outputs:
+            pts = self.point_head(x0_mean, x0_coors, rows0, middle)
         C = x._channels
         D, H, W = x.spatial_shape
         if self.fcn.precision == ops.PREC_F16X3 and self.dense_tma:
@@ -252,12 +290,24 @@ class SpMiddleFHD(nn.Module):
             bev = torch.zeros((batch_size, H, W, D * C), dtype=torch.float32, device=feats.device)
             ops.sparse_to_bev(feats, x._indices, x.d_rows, C, D, H, W, bev)
         y, conv6 = self.fcn.forward_nhwc(bev, dc_order=(C, D))
+        if point_outputs:
+            return y, conv6, x, pts
         return y, conv6, x
 
     def forward(self, voxel_features, coors, batch_size, is_test=False, d_rows=None, status=None):
-        if not is_test:
-            raise NotImplementedError("the auxiliary training branch (cmn.py:121-135) is out of scope")
-        y, conv6, x = self.forward_nhwc(voxel_features, coors, batch_size, d_rows, status)
+        """cmn.py:102-135.  Returns (x, conv6), both [B, 256, H, W]; with ``is_test=False`` (eval mode only) also the
+        auxiliary outputs (points_mean [N,4] = (b, x, y, z), point_cls [N,1] foreground logits, point_reg [N,3]
+        offsets to the box centre), N the voxel rows.  The aux loss and its targets are not built, so training mode
+        raises."""
+        if not is_test and self.training:
+            raise NotImplementedError("the auxiliary training branch (cmn.py:44-100) is out of scope: call .eval()")
+        out = self.forward_nhwc(voxel_features, coors, batch_size, d_rows, status, point_outputs=not is_test)
+        y, conv6 = out[0], out[1]
         if isinstance(y, ops.SplitMap):
             y, conv6 = y.float(), conv6.float()
-        return y.permute(0, 3, 1, 2), conv6.permute(0, 3, 1, 2)
+        y, conv6 = y.permute(0, 3, 1, 2), conv6.permute(0, 3, 1, 2)
+        if is_test:
+            return y, conv6
+        pts = out[3]
+        n = voxel_features.shape[0] if d_rows is None else int(d_rows.reshape(-1)[0].item())
+        return y, conv6, (pts["points_mean"][:n], pts["point_cls"][:n].unsqueeze(1), pts["point_reg"][:n])

@@ -54,7 +54,7 @@ def next_pow2(n):
 _KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1,"sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
             "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
-            "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
+            "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
             "sassd_boxes_iou_bev": 1}
 LAUNCHES = 0          # running count of kernels launched through this module
 PROFILE = None        # set to a list to collect (name, label, start_event, end_event)
@@ -376,6 +376,55 @@ def kitti_format(det, d_ndet, meta):
     _call("sassd_kitti_format", None, _ptr(det), _ptr(d_ndet), B, det_cap, _ptr(meta), _ptr(rows), _ptr(n_out),
           _stream())
     return rows, n_out
+
+
+# ---------------------------------------------------------------------------- auxiliary point-wise head
+def three_nn(mean, coors0, d_rows0, levels, points_mean=False):
+    """mean [cap0,4] f32 (x, y, z, r of each voxel), coors0 [cap0,4] i32 (b,z,y,x), d_rows0 [1]; ``levels``: three
+    (coors [capL,4] i32, d_rows [1]) of backbone levels 1..3, rows sorted by flattened (b,z,y,x).  Returns
+    (idx [cap0,3,3] i32, dist2 [cap0,3,3] f32, points_mean [cap0,4] f32 or None): per voxel row, level and k the global
+    row of its k-th nearest centre of the same frame and the squared distance (pointnet2 three_nn, bit for bit;
+    missing slots idx 0, dist2 +inf); points_mean rows are (b, x, y, z).  Rows past d_rows0 are left unwritten."""
+    dev = mean.device
+    cap0 = mean.shape[0]
+    assert len(levels) == 3 and coors0.shape[0] == cap0 and tuple(mean.shape[1:]) == (4,) and mean.dtype == torch.float32
+    idx = torch.empty((cap0, 3, 3), dtype=torch.int32, device=dev)
+    dist2 = torch.empty((cap0, 3, 3), dtype=torch.float32, device=dev)
+    pm = torch.empty((cap0, 4), dtype=torch.float32, device=dev) if points_mean else None
+    (c1, n1), (c2, n2), (c3, n3) = levels
+    _call("sassd_three_nn", None, _ptr(mean), _ptr(coors0), _ptr(d_rows0), cap0, _ptr(c1), _ptr(n1), _ptr(c2),
+          _ptr(n2), _ptr(c3), _ptr(n3), _ptr(idx), _ptr(dist2), _ptr(pm), _stream())
+    return idx, dist2, pm
+
+
+def point_level(feat=None, split=None, channels=None):
+    """Feature rows of one backbone level for point_aux_head: fp32 ``feat`` [cap, >=C] or split fp16 rows ``split``
+    [2, cap, >=C] (features_to_split / spconv_split)."""
+    d = _lib.PointLevels()
+    if feat is not None:
+        assert feat.dtype == torch.float32 and feat.dim() == 2
+        d.rows, d.plane_stride, d.row_stride, d.split = _ptr(feat).value, 0, feat.stride(0), 0
+        d.channels = channels if channels is not None else feat.shape[1]
+    else:
+        assert split.dtype == torch.float16 and split.dim() == 3 and split.shape[0] == 2
+        d.rows, d.plane_stride, d.row_stride, d.split = _ptr(split).value, split.stride(0), split.stride(1), 1
+        d.channels = channels if channels is not None else split.shape[2]
+    return d
+
+
+def point_aux_head(idx, dist2, d_rows0, levels, w_fc_t, w_out):
+    """idx / dist2 from three_nn; ``levels``: three point_level() of levels 1..3 (32, 64, 64 channels); w_fc_t
+    [160,64] = point_fc.weight^T, w_out [4,64] = point_cls.weight then point_reg.weight (fp32, device).
+    Returns (cls [cap0] logits, reg [cap0,3]); rows past d_rows0 are left unwritten."""
+    dev = idx.device
+    cap0 = idx.shape[0]
+    assert tuple(w_fc_t.shape) == (_lib.POINT_FC_IN, _lib.POINT_FC_OUT) and tuple(w_out.shape) == (4, _lib.POINT_FC_OUT)
+    arr = (_lib.PointLevels * 3)(*levels)
+    cls = torch.empty((cap0,), dtype=torch.float32, device=dev)
+    reg = torch.empty((cap0, 3), dtype=torch.float32, device=dev)
+    _call("sassd_point_aux_head", None, _ptr(idx), _ptr(dist2), _ptr(d_rows0), cap0, arr, _ptr(w_fc_t), _ptr(w_out),
+          _ptr(cls), _ptr(reg), _stream())
+    return cls, reg
 
 
 def nms_mask(boxes5, thr):
