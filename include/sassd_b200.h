@@ -44,10 +44,13 @@ enum {
 enum { /* bits of *d_status */
     SASSD_FLAG_VOXEL_CAP = 1,   /* more voxel rows than the output capacity */
     SASSD_FLAG_ROWS_CAP = 2,    /* strided-conv output rows exceed capacity */
-    SASSD_FLAG_GUIDED_CAP = 4,  /* guided anchors per frame exceed capacity */
-    SASSD_FLAG_NMS_CAP = 8,     /* NMS candidates per frame exceed capacity */
+    SASSD_FLAG_GUIDED_CAP = 4,  /* guided anchors per frame exceed capacity: the first k_cap selected anchors in
+                                   anchor order are kept (sassd_decode_select) */
+    SASSD_FLAG_NMS_CAP = 8,     /* NMS candidates per frame exceed capacity: the NMS runs on the first 4096 score
+                                   passers in candidate order (sassd_rescore_nms) */
     SASSD_FLAG_HASH_FULL = 16,
-    SASSD_FLAG_DET_CAP = 32     /* boxes kept by the NMS exceed the detection capacity */
+    SASSD_FLAG_DET_CAP = 32     /* boxes kept by the NMS exceed the detection capacity: the first det_cap kept
+                                   boxes in score order are returned */
 };
 
 int sassd_version(void);
