@@ -12,7 +12,19 @@ model = dict(
     extra_head=dict(type='PSWarpHead', grid_offsets=(0., 40.), featmap_stride=.4, in_channels=256,
                     num_class=1, num_parts=28),
 )
-train_cfg = None
+# Target assignment of the losses (SingleStageDetector.forward_train / loss_points); inference reads none of it.
+train_cfg = dict(
+    rpn=dict(
+        assigner=dict(
+            Car=dict(pos_iou_thr=0.6, neg_iou_thr=0.45, min_pos_iou=0.45),
+            Pedestrian=dict(pos_iou_thr=0.5, neg_iou_thr=0.35, min_pos_iou=0.35),
+            Cyclist=dict(pos_iou_thr=0.5, neg_iou_thr=0.35, min_pos_iou=0.35),
+            ignore_iof_thr=-1, similarity_fn='NearestIouSimilarity'),
+        anchor_thr=0.1),
+    extra=dict(
+        assigner=dict(pos_iou_thr=0.7, neg_iou_thr=0.7, min_pos_iou=0.7, ignore_iof_thr=-1,
+                      similarity_fn='RotateIou3dSimilarity')),
+)
 test_cfg = dict(
     rpn=dict(nms_across_levels=False, nms_pre=2000, nms_post=100, nms_thr=0.7, min_bbox_size=0),
     extra=dict(score_thr=0.3, nms=dict(type='nms', iou_thr=0.1), max_per_img=100),

@@ -49,8 +49,10 @@ enum { /* bits of *d_status */
     SASSD_FLAG_NMS_CAP = 8,     /* NMS candidates per frame exceed capacity: the NMS runs on the first 4096 score
                                    passers in candidate order (sassd_rescore_nms) */
     SASSD_FLAG_HASH_FULL = 16,
-    SASSD_FLAG_DET_CAP = 32     /* boxes kept by the NMS exceed the detection capacity: the first det_cap kept
+    SASSD_FLAG_DET_CAP = 32,    /* boxes kept by the NMS exceed the detection capacity: the first det_cap kept
                                    boxes in score order are returned */
+    SASSD_FLAG_GT_CAP = 64      /* ground-truth boxes per frame exceed gt_cap: the first gt_cap boxes are used
+                                   (sassd_points_in_boxes, sassd_assign_*) */
 };
 
 int sassd_version(void);
@@ -391,6 +393,71 @@ int sassd_three_nn(const float* mean, const int32_t* coors0, const int32_t* d_ro
 int sassd_point_aux_head(const int32_t* idx, const float* dist2, const int32_t* d_rows0, int rows_cap0,
                          const sassd_point_levels* host_levels, const float* w_fc_t, const float* w_out, float* cls,
                          float* reg, sassd_stream_t stream);
+
+/* ------------------------------------------------------------------------
+ * Training targets and losses, forward only, for labelled frames
+ * (cmn.py:44-100, target_ops.py:139-277, ssd_rotate_head.py:237-305,450-485,
+ * losses.py:31-114).  Ground truth per frame: gt [batch,gt_cap,7] boxes
+ * (x, y, z_bottom, w, l, h, ry), d_ngt [batch] their number (more than
+ * gt_cap sets SASSD_FLAG_GT_CAP; the first gt_cap are used), gt_cap <=
+ * SASSD_GT_CAP_MAX.  A frame without GT is all background.  No host
+ * synchronisation; workspace: sassd_loss_workspace_bytes(batch, gt_cap).
+ * Loss sums are fp32 per element, fp64 across elements, reduced in a fixed
+ * order: the same inputs give the same bits.
+ *
+ * sassd_points_in_boxes: pts_in_boxes3d of each voxel row r < *d_rows
+ * (points_mean [rows_cap,4] = (b, x, y, z)) against its frame's boxes with
+ * the reference's C++ expression types.  labels [rows_cap] = 1 inside any
+ * box, offsets [rows_cap,3] = point - centre of the LAST containing box in
+ * box order (z centre = z_bottom + fourth value / 2, as points_op.cpp:139),
+ * 0 when none; *d_npos = number of labelled rows.
+ *
+ * sassd_assign_rpn: create_target_torch with NearestIouSimilarity per frame
+ * and class.  anchors [n_anchors,7] (shared) or [batch,n_anchors,7], classes
+ * concatenated (n_anchors / num_class each), mask [batch,n_anchors];
+ * gt_class [batch,gt_cap] = anchor class of each GT (-1: none), gt_label =
+ * the label a positive gets; host_pos_thr / host_neg_thr [num_class],
+ * num_class <= 8.  labels [batch,n_anchors] (-1 unmasked / ignored, 0
+ * background, > 0 positive), targets [batch,n_anchors,7] second_box_encode
+ * for the positives (0 elsewhere), ious (may be NULL) = anchor_to_gt_max
+ * (0 unmasked), d_npos [batch] positives per frame.
+ *
+ * sassd_assign_pswarp: the same rules with RotateIou3dSimilarity, every
+ * label 1 and no mask, over box slots [batch,n_box,7]: slots [0, head_cap)
+ * hold d_head[b] boxes (the GT rows of the guided list; d_head may be NULL
+ * when head_cap is 0) and slots [head_cap, n_box) hold d_k[b] boxes.
+ * labels [batch,n_box] (-1 in empty slots), ious, d_npos [batch].
+ *
+ * sassd_rpn_loss: out[3] = rpn_loc_loss, rpn_cls_loss, rpn_dir_loss
+ * (NormByNumPositives per frame, / batch, x2 and x0.2) from the head map of
+ * sassd_decode_select and the labels / targets / d_npos of sassd_assign_rpn.
+ * sassd_pswarp_loss: out[1] = loss_cls, focal loss over scores
+ * [batch,n_box] normalised by the positives of the whole batch, / batch.
+ * sassd_aux_loss: out[2] = aux_loss_cls, aux_loss_reg from point_cls
+ * [rows_cap], point_reg [rows_cap,3] and sassd_points_in_boxes' outputs.
+ * ---------------------------------------------------------------------- */
+#define SASSD_GT_CAP_MAX 256
+size_t sassd_loss_workspace_bytes(int batch, int gt_cap);
+int sassd_points_in_boxes(const float* points_mean, const int32_t* d_rows, int rows_cap, const float* gt,
+                          const int32_t* d_ngt, int batch, int gt_cap, int32_t* labels, float* offsets,
+                          int32_t* d_npos, int32_t* d_status, sassd_stream_t stream);
+int sassd_assign_rpn(const float* anchors, int anchors_per_frame, const uint8_t* mask, int n_anchors, int num_class,
+                     const float* gt, const int32_t* gt_class, const int32_t* gt_label, const int32_t* d_ngt,
+                     int batch, int gt_cap, const float* host_pos_thr, const float* host_neg_thr, int32_t* labels,
+                     float* targets, float* ious, int32_t* d_npos, int32_t* d_status, void* ws, size_t ws_bytes,
+                     sassd_stream_t stream);
+int sassd_assign_pswarp(const float* gt, const int32_t* d_ngt, int batch, int gt_cap, const float* boxes, int n_box,
+                        const int32_t* d_head, int head_cap, const int32_t* d_k, float pos_thr, float neg_thr,
+                        int32_t* labels, float* ious, int32_t* d_npos, int32_t* d_status, void* ws,
+                        size_t ws_bytes, sassd_stream_t stream);
+int sassd_rpn_loss(const float* head, int head_stride, int batch, int H, int W, int num_class, const float* anchors,
+                   int anchors_per_frame, int n_anchors, const int32_t* labels, const float* targets,
+                   const int32_t* d_npos, float* out, void* ws, size_t ws_bytes, sassd_stream_t stream);
+int sassd_pswarp_loss(const float* scores, const int32_t* labels, int batch, int n_box, const int32_t* d_npos,
+                      float* out, void* ws, size_t ws_bytes, sassd_stream_t stream);
+int sassd_aux_loss(const float* point_cls, const float* point_reg, const int32_t* labels, const float* offsets,
+                   const int32_t* d_rows, int rows_cap, int batch, const int32_t* d_npos, float* out, void* ws,
+                   size_t ws_bytes, sassd_stream_t stream);
 
 /* iou3d_cuda.nms_gpu alone (iou3d.cpp:73-120): boxes [n,5] already sorted by
  * score; mask [n, ceil(n/64)] u64 in the reference layout (only columns j > i

@@ -25,7 +25,7 @@ def build_from_config(cfg, device="cuda", data_key="val"):
     from . import anchors as A
     from . import voxel_generator as V
     from .builder import build_detector
-    model = build_detector(cfg.model, train_cfg=None, test_cfg=cfg.test_cfg).to(device)
+    model = build_detector(cfg.model, train_cfg=cfg.get("train_cfg"), test_cfg=cfg.test_cfg).to(device)
     d = cfg.data[data_key]
     vg = obj_from_dict(d["generator"], V, dict(device=device))
     gens = {k: obj_from_dict(v, A) for k, v in d["anchor_generator"].items()}

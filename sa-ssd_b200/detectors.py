@@ -12,6 +12,8 @@ Two entry points:
     device first (the reference crops them offline into ``velodyne_reduced``).  With ``metas``
     the step also formats its detections as KITTI annotations on the device (ops.kitti_format).  With
     ``point_outputs`` it also returns the auxiliary network's per-voxel foreground logits and centre offsets.
+  * ``forward(..., return_loss=True)`` / ``forward_train`` and ``loss_points`` — the training losses, forward only, in
+    eval() mode (csrc/targets.cu).
 """
 import numpy as np
 import torch
@@ -106,8 +108,43 @@ class SingleStageDetector(nn.Module):
 
     def forward(self, img=None, img_meta=None, return_loss=False, **kwargs):
         if return_loss:
-            raise NotImplementedError("training (forward_train, single_stage.py:75-108) is out of scope")
+            if self.training:
+                raise NotImplementedError("the losses are computed forward only, with BatchNorm's running statistics: "
+                                          "call .eval() first (training is not supported)")
+            return self.forward_train(img, img_meta, **kwargs)
         return self.forward_test(img, img_meta, **kwargs)
+
+    def forward_train(self, img, img_meta, **kwargs):
+        """single_stage.py:75-108 for a model in eval() mode: the loss dict (aux_loss_cls, aux_loss_reg, rpn_loc_loss,
+        rpn_cls_loss, rpn_dir_loss, loss_cls), each a [1] tensor, computed on the device without autograd.  kwargs as
+        the training dataset gives them: voxels, num_points, coordinates, anchors / anchors_mask (per-class dicts or
+        tensors), gt_bboxes (x, y, z_bottom, w, l, h, ry per frame), gt_labels, gt_types.  A frame without GT is all
+        background (aux labels 0, masked anchors 0, no GT rows in the guided boxes); the reference never sees one."""
+        ops.require_cuda()
+        if self.training:
+            raise NotImplementedError("forward_train runs in eval() mode only")
+        if self.train_cfg is None:
+            raise ValueError("forward_train needs train_cfg (build_from_config passes cfg.train_cfg)")
+        batch_size = len(img_meta)
+        dev = next(self.parameters()).device
+        ret = self.merge_second_batch({k: v for k, v in kwargs.items() if v is not None})
+        voxels = ret["voxels"].to(dev).float().contiguous()
+        coords = ret["coordinates"].to(dev).int().contiguous()
+        gt_bboxes = [torch.as_tensor(g).to(dev).float().reshape(-1, 7) for g in ret["gt_bboxes"]]
+        gt_labels = [torch.as_tensor(g).to(dev).long().reshape(-1) for g in ret["gt_labels"]]
+        anchors, anchors_mask = _on_device(ret["anchors"], dev), _on_device(ret["anchors_mask"], dev)
+        vx = self.backbone(voxels, ret["num_points"].to(dev))
+        x, conv6, point_misc = self.neck(vx, coords, batch_size, is_test=False)
+        losses = dict()
+        losses.update(self.neck.aux_loss(*point_misc, gt_bboxes=gt_bboxes))
+        rpn_outs = self.rpn_head(x)
+        losses.update(self.rpn_head.loss(*rpn_outs, gt_bboxes, gt_labels, ret.get("gt_types"), anchors, anchors_mask,
+                                         self.train_cfg.rpn))
+        guided_anchors, _ = self.rpn_head.get_guided_anchors(*rpn_outs, anchors, anchors_mask, gt_bboxes,
+                                                             gt_labels, thr=self.train_cfg.rpn.anchor_thr)
+        bbox_score = self.extra_head(conv6, guided_anchors)
+        losses.update(self.extra_head.loss(bbox_score, gt_bboxes, gt_labels, guided_anchors, self.train_cfg.extra))
+        return losses
 
     def forward_test(self, img, img_meta, **kwargs):
         """single_stage.py:110-131.  When every ``img_meta`` carries the KITTI calibration (``calib``) and the
@@ -145,9 +182,10 @@ class SingleStageDetector(nn.Module):
         self.anchor_set = anchor_set.to(dev)
         return self
 
-    def forward_device(self, points, pt_off, batch, max_points_per_frame, point_outputs=False):
+    def forward_device(self, points, pt_off, batch, max_points_per_frame, point_outputs=False, detections=True):
         """Everything on the device, no synchronisation.  points [Ncap,4], pt_off [batch+1] int32.
-        Returns (det [B,det_cap,9], d_ndet [B], status [1], aux dict).  With ``point_outputs`` the aux dict also holds
+        Returns (det [B,det_cap,9], d_ndet [B], status [1], aux dict); without ``detections`` the rescoring and NMS are
+        skipped and det, d_ndet are None (the loss path reads only the guided boxes and their scores).  With ``point_outputs`` the aux dict also holds
         the auxiliary network's points_mean [cap,4] (b, x, y, z), point_cls [cap] and point_reg [cap,3] (neck.point_head)
         for the voxel rows (frame_rows)."""
         dev = points.device
@@ -168,11 +206,14 @@ class SingleStageDetector(nn.Module):
         head = self.rpn_head.forward_nhwc(y)
         anchors, _ = aset.device_tensors()
         boxes, labels, index, d_k = self.rpn_head.guided_anchors_device(head, anchors, mask, self.guided_thr, status)
-        scores = self.extra_head.forward_device(conv6, boxes, d_k)
-        det, d_ndet = self.extra_head.rescore_device(boxes, scores, labels, d_k, self.test_cfg.extra, status)
+        ps_feat = self.extra_head.convs_nhwc(conv6)
+        scores = self.extra_head.sample(ps_feat, boxes, d_k)
+        det = d_ndet = None
+        if detections:
+            det, d_ndet = self.extra_head.rescore_device(boxes, scores, labels, d_k, self.test_cfg.extra, status)
         aux = dict(voxels=voxels, coors=coors, num_points=num, mean=mean, frame_rows=frame_rows, mask=mask, x=y,
                    conv6=conv6, head=head, guided=boxes, guided_labels=labels, guided_index=index, d_k=d_k,
-                   ps_scores=scores, sparse=xs)
+                   ps_feat=ps_feat, ps_scores=scores, sparse=xs)
         if point_outputs:
             aux.update(out[3])
         return det, d_ndet, status, aux
@@ -327,6 +368,89 @@ class SingleStageDetector(nn.Module):
             out = [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(bbs, scs, lbs)]
         ret = (out,) + ((pts,) if point_outputs else ()) + ((aux,) if return_aux else ())
         return ret if len(ret) > 1 else out
+
+
+    def loss_device(self, aux, batch, gt, gt_class, gt_label, d_ngt, n_gt_host, status):
+        """Targets and losses of one forward_device(point_outputs=True) step, on the device: returns the loss vector
+        [6] in ops.LOSS_KEYS order and a dict of the targets.  gt [B,gt_cap,7] etc. as stage_gt gives them;
+        ``n_gt_host`` the per-frame counts (the GT rows PSWarp scores)."""
+        dev = gt.device
+        gt_cap = gt.shape[1]
+        out = torch.zeros((len(ops.LOSS_KEYS),), dtype=torch.float32, device=dev)
+        cfg = self.train_cfg
+        d_rows = aux["frame_rows"][batch:batch + 1]
+        p_lab, p_off, p_npos = ops.points_in_boxes(aux["points_mean"], d_rows, gt, d_ngt, status)
+        ops.aux_loss(aux["point_cls"], aux["point_reg"], p_lab, p_off, d_rows, batch, p_npos, out[0:2])
+        anchors, _ = self.anchor_set.device_tensors()
+        names = list(self.class_names) if self.class_names is not None else [None]
+        pos, neg = self.rpn_head.thresholds(cfg.rpn, names)
+        r_lab, r_tgt, r_iou, _ = self.rpn_head.loss_device(aux["head"], anchors, aux["mask"], gt, gt_class, gt_label,
+                                                           d_ngt, pos, neg, out[2:5], status)
+        # PSWarp scores the GT rows the reference prepends to each frame's guided boxes (:364-367) in a slot segment of
+        # their own, so the guided capacity does not grow
+        d_head = torch.from_numpy(np.minimum(n_gt_host, gt_cap).astype(np.int32)).to(dev)
+        gt_scores = self.extra_head.sample(aux["ps_feat"], gt, d_head)
+        boxes = torch.cat([gt, aux["guided"]], 1).contiguous()
+        scores = torch.cat([gt_scores, aux["ps_scores"]], 1).contiguous()
+        e_lab, e_iou, _ = self.extra_head.loss_device(scores, boxes, aux["d_k"], gt, d_ngt, cfg.extra, out[5:6], status,
+                                                      d_head=d_head, head_cap=gt_cap)
+        return out, dict(point_labels=p_lab, point_offsets=p_off, rpn_labels=r_lab, rpn_targets=r_tgt, rpn_ious=r_iou,
+                         ps_boxes=boxes, ps_scores=scores, ps_labels=e_lab, ps_ious=e_iou)
+
+    def loss_points(self, points_list, gt_bboxes, gt_labels, frustum_planes=None, return_aux=False):
+        """The losses of forward(return_loss=True) from raw points: ``points_list`` as forward_points takes it, per frame
+        the GT boxes [G,7] (x, y, z_bottom, w, l, h, ry, lidar frame) and their labels (1-based over class_names; a box
+        counts for the anchors of class_names[label - 1]).  Runs forward_device(point_outputs=True) up to the guided boxes'
+        PSWarp scores (no rescoring or NMS), scores the GT boxes
+        on PSWarp's map, then every target and loss on the device; one device-to-host copy of the loss vector and the
+        status word.  Returns a dict of Python floats keyed like forward_train (with ``return_aux`` also the step's aux
+        dict and the targets).  The model must be in eval() mode; frames without GT are all background."""
+        ops.require_cuda()
+        if self.training:
+            raise NotImplementedError("loss_points runs in eval() mode only")
+        if self.voxel_generator is None or self.anchor_set is None:
+            raise RuntimeError("call attach_data_pipeline(voxel_generator, anchor_set) first")
+        if self.train_cfg is None:
+            raise ValueError("loss_points needs train_cfg (build_from_config passes cfg.train_cfg)")
+        from .single_stage_heads import stage_gt
+        B = len(points_list)
+        if len(gt_bboxes) != B or len(gt_labels) != B:
+            raise ValueError("loss_points: one GT box set and label set per frame")
+        dev = next(self.parameters()).device
+        planes = None if frustum_planes is None else _frame_planes(frustum_planes, B)
+        hp, ho, counts = self.stage_points(points_list)
+        labels = [np.asarray(l, np.int64).reshape(-1) for l in gt_labels]
+        gt_class = [(l - 1).astype(np.int32) for l in labels]
+        gt, gcls, glab, d_ngt = stage_gt(gt_bboxes, gt_class, labels, dev)
+        n_gt = np.array([np.asarray(g).reshape(-1, 7).shape[0] for g in gt_bboxes], np.int64)
+        points = hp.to(dev, non_blocking=True)
+        pt_off = ho.to(dev, non_blocking=True)
+        if planes is not None:
+            points, pt_off = ops.frustum_crop(points, pt_off, B, torch.from_numpy(planes).to(dev))
+        thr0, self.guided_thr = self.guided_thr, float(self.train_cfg.rpn.anchor_thr)
+        try:
+            _, _, status, aux = self.forward_device(points, pt_off, B, max(counts + [1]), point_outputs=True,
+                                                    detections=False)
+        finally:
+            self.guided_thr = thr0
+        out, targets = self.loss_device(aux, B, gt, gcls, glab, d_ngt, n_gt, status)
+        h = torch.empty((len(ops.LOSS_KEYS) + 1,), dtype=torch.float32, pin_memory=True)
+        h[:-1].copy_(out, non_blocking=True)
+        h[-1:].copy_(status.view(torch.float32), non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        word = int(h[-1:].view(torch.int32).item())
+        if word:
+            raise ops._lib.SassdError("capacity overflow on device: %s" % ops._lib.decode_flags(word))
+        res = {k: float(v) for k, v in zip(ops.LOSS_KEYS, h[:-1].tolist())}
+        if return_aux:
+            aux.update(targets)
+            return res, aux
+        return res
+
+
+def _on_device(v, dev):
+    """A tensor or a per-class dict of tensors, on ``dev``."""
+    return {k: t.to(dev) for k, t in v.items()} if isinstance(v, dict) else v.to(dev)
 
 
 def _split_points(points_mean, cls, reg, frame_rows):

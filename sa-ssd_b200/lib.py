@@ -44,10 +44,12 @@ SPCONV_TILE_ROWS = 128                    # SASSD_SPCONV_TILE_ROWS
 KITTI_META, KITTI_ROW = 36, 14            # SASSD_KITTI_META / SASSD_KITTI_ROW
 POINT_LEVEL_CHANNELS = (32, 64, 64)       # sassd_point_aux_head: features of backbone levels 1..3 (conv1, conv2, conv3)
 POINT_FC_IN, POINT_FC_OUT = 160, 64       # point_fc: Linear(160, 64); point_cls / point_reg read its 64 outputs
+GT_CAP_MAX = 256                          # SASSD_GT_CAP_MAX: ground-truth boxes per frame the loss kernels take
 
 OK = 0
 ERRORS = {-1: "SASSD_ERR_ARG", -2: "SASSD_ERR_LAUNCH", -3: "SASSD_ERR_WORKSPACE", -4: "SASSD_ERR_UNSUPPORTED"}
-FLAGS = {1: "VOXEL_CAP", 2: "ROWS_CAP", 4: "GUIDED_CAP", 8: "NMS_CAP", 16: "HASH_FULL", 32: "DET_CAP"}
+FLAGS = {1: "VOXEL_CAP", 2: "ROWS_CAP", 4: "GUIDED_CAP", 8: "NMS_CAP", 16: "HASH_FULL", 32: "DET_CAP",
+         64: "GT_CAP"}
 
 P = c_void_p
 _SIGNATURES = {
@@ -99,6 +101,15 @@ _SIGNATURES = {
     "sassd_nms_mask": (c_int, [P, c_int, c_float, P, P]),
     "sassd_nms_sorted": (c_int, [P, c_int, c_float, P, P, P, c_size_t, P]),
     "sassd_boxes_iou_bev": (c_int, [P, c_int, P, c_int, P, P]),
+    "sassd_loss_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "sassd_points_in_boxes": (c_int, [P, P, c_int, P, P, c_int, c_int, P, P, P, P, P]),
+    "sassd_assign_rpn": (c_int, [P, c_int, P, c_int, c_int, P, P, P, P, c_int, c_int, P, P, P, P, P, P, P, P, c_size_t,
+                                 P]),
+    "sassd_assign_pswarp": (c_int, [P, P, c_int, c_int, P, c_int, P, c_int, P, c_float, c_float, P, P, P, P, P, c_size_t,
+                                    P]),
+    "sassd_rpn_loss": (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, c_int, c_int, P, P, P, P, P, c_size_t, P]),
+    "sassd_pswarp_loss": (c_int, [P, P, c_int, c_int, P, P, P, c_size_t, P]),
+    "sassd_aux_loss": (c_int, [P, P, P, P, P, c_int, c_int, P, P, P, c_size_t, P]),
 }
 
 _LIB = None

@@ -252,6 +252,47 @@ class SpMiddleFHD(nn.Module):
         cls, reg = ops.point_aux_head(idx, dist2, d_rows, feats, fc_t, w_out)
         return dict(points_mean=pm, point_cls=cls, point_reg=reg, idx=idx, dist2=dist2, middle=middle)
 
+    def build_aux_target(self, nxyz, gt_boxes3d, enlarge=1.0):
+        """cmn.py:44-70 on the device: nxyz [N,4] (b, x, y, z) voxel means, frames in row order; gt_boxes3d one [G_b,7]
+        tensor per frame (x, y, z_bottom, w, l, h, ry).  Returns (pts_labels [N] uint8: inside any box of the point's
+        frame, center_offsets [N,3]: point minus the centre of the last box containing it, 0 when none), as
+        pts_in_boxes3d computes them (points_op.cpp:92-144, including its z centre from the box's fourth value).  A frame
+        without boxes is all background (the reference never sees one)."""
+        labels, offsets, _ = self._aux_targets(nxyz, gt_boxes3d, enlarge)
+        return labels.to(torch.uint8), offsets
+
+    def _aux_targets(self, nxyz, gt_boxes3d, enlarge=1.0):
+        from .single_stage_heads import stage_gt, _raise_on_flags
+        ops.require_cuda()
+        dev = nxyz.device if nxyz.is_cuda else torch.device("cuda")
+        boxes = []
+        for g in gt_boxes3d:
+            g = torch.as_tensor(g, dtype=torch.float32).reshape(-1, 7).clone()
+            g[:, 3:6] *= enlarge
+            boxes.append(g)
+        gt, _, _, d_ngt = stage_gt(boxes, None, None, dev)
+        pm = nxyz.to(dev).float().contiguous()
+        n = pm.shape[0]
+        if n == 0:
+            return torch.zeros(0, dtype=torch.int32, device=dev), torch.zeros((0, 3), device=dev), None
+        status = torch.zeros((1,), dtype=torch.int32, device=dev)
+        d_rows = torch.tensor([n], dtype=torch.int32, device=dev)
+        labels, offsets, d_npos = ops.points_in_boxes(pm, d_rows, gt, d_ngt, status)
+        _raise_on_flags(status)
+        return labels, offsets, (d_rows, d_npos)
+
+    def aux_loss(self, points, point_cls, point_reg, gt_bboxes):
+        """cmn.py:72-100: dict(aux_loss_cls, aux_loss_reg), each a [1] tensor, from the auxiliary outputs of
+        forward(is_test=False) and one GT tensor per frame."""
+        labels, offsets, rows = self._aux_targets(points, gt_bboxes)
+        dev = labels.device
+        out = torch.zeros((2,), dtype=torch.float32, device=dev)
+        if rows is not None:
+            d_rows, d_npos = rows
+            ops.aux_loss(point_cls.reshape(-1).float().contiguous(), point_reg.float().contiguous(), labels, offsets,
+                         d_rows, len(gt_bboxes), d_npos, out)
+        return dict(aux_loss_cls=out[0:1], aux_loss_reg=out[1:2])
+
     def set_precision(self, precision, sparse=None):
         """precision for the dense BEV convs; ``sparse`` (default: same) for the ruled sparse convs."""
         self.backbone.set_precision(precision if sparse is None else sparse)
@@ -297,8 +338,8 @@ class SpMiddleFHD(nn.Module):
     def forward(self, voxel_features, coors, batch_size, is_test=False, d_rows=None, status=None):
         """cmn.py:102-135.  Returns (x, conv6), both [B, 256, H, W]; with ``is_test=False`` (eval mode only) also the
         auxiliary outputs (points_mean [N,4] = (b, x, y, z), point_cls [N,1] foreground logits, point_reg [N,3]
-        offsets to the box centre), N the voxel rows.  The aux loss and its targets are not built, so training mode
-        raises."""
+        offsets to the box centre), N the voxel rows (aux_loss takes them).  Training mode raises: BatchNorm batch
+        statistics are not built."""
         if not is_test and self.training:
             raise NotImplementedError("the auxiliary training branch (cmn.py:44-100) is out of scope: call .eval()")
         out = self.forward_nhwc(voxel_features, coors, batch_size, d_rows, status, point_outputs=not is_test)

@@ -55,7 +55,8 @@ _KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
             "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
-            "sassd_boxes_iou_bev": 1}
+            "sassd_boxes_iou_bev": 1, "sassd_points_in_boxes": 2, "sassd_assign_rpn": 3, "sassd_assign_pswarp": 3,
+            "sassd_rpn_loss": 2, "sassd_pswarp_loss": 2, "sassd_aux_loss": 2}
 LAUNCHES = 0          # running count of kernels launched through this module
 PROFILE = None        # set to a list to collect (name, label, start_event, end_event)
 
@@ -452,6 +453,91 @@ def boxes_iou_bev(a, b):
     out = torch.empty((a.shape[0], b.shape[0]), dtype=torch.float32, device=a.device)
     _call("sassd_boxes_iou_bev", None, _ptr(a), a.shape[0], _ptr(b), b.shape[0], _ptr(out), _stream())
     return out
+
+
+# ---------------------------------------------------------------------------- training targets and losses
+# Output vector of loss_vector(): the keys of SingleStageDetector.forward_train, in this order.
+LOSS_KEYS = ("aux_loss_cls", "aux_loss_reg", "rpn_loc_loss", "rpn_cls_loss", "rpn_dir_loss", "loss_cls")
+
+
+def _loss_ws(batch, gt_cap, device, ws=None):
+    nbytes = _L().sassd_loss_workspace_bytes(batch, gt_cap)
+    return (ws or _WS).get("loss", nbytes, device)
+
+
+def points_in_boxes(points_mean, d_rows, gt, d_ngt, status, ws=None):
+    """points_mean [cap,4] (b, x, y, z), d_rows [1]; gt [B,gt_cap,7] (x, y, z_bottom, w, l, h, ry), d_ngt [B] i32.
+    Returns (labels [cap] i32, offsets [cap,3], d_npos [1]): pts_in_boxes3d per frame (build_aux_target).  Rows past
+    d_rows are left unwritten."""
+    dev = points_mean.device
+    cap = points_mean.shape[0]
+    B, gt_cap = gt.shape[0], gt.shape[1]
+    labels = torch.empty((cap,), dtype=torch.int32, device=dev)
+    offsets = torch.empty((cap, 3), dtype=torch.float32, device=dev)
+    d_npos = torch.empty((1,), dtype=torch.int32, device=dev)
+    _call("sassd_points_in_boxes", None, _ptr(points_mean), _ptr(d_rows), cap, _ptr(gt), _ptr(d_ngt), B, gt_cap,
+          _ptr(labels), _ptr(offsets), _ptr(d_npos), _ptr(status), _stream())
+    return labels, offsets, d_npos
+
+
+def assign_rpn(anchors, mask, num_class, gt, gt_class, gt_label, d_ngt, pos_thr, neg_thr, status, ws=None):
+    """anchors [Na,7] (shared) or [B,Na,7], classes concatenated; mask [B,Na] u8; gt [B,gt_cap,7], gt_class /
+    gt_label [B,gt_cap] i32, d_ngt [B]; pos_thr / neg_thr one per class.  Returns (labels [B,Na] i32, targets
+    [B,Na,7], ious [B,Na], d_npos [B])."""
+    dev = gt.device
+    B, gt_cap = gt.shape[0], gt.shape[1]
+    na = anchors.shape[-2]
+    labels = torch.empty((B, na), dtype=torch.int32, device=dev)
+    targets = torch.empty((B, na, 7), dtype=torch.float32, device=dev)
+    ious = torch.empty((B, na), dtype=torch.float32, device=dev)
+    d_npos = torch.empty((B,), dtype=torch.int32, device=dev)
+    pos = (ctypes.c_float * num_class)(*[float(v) for v in pos_thr])
+    neg = (ctypes.c_float * num_class)(*[float(v) for v in neg_thr])
+    w = _loss_ws(B, gt_cap, dev, ws)
+    _call("sassd_assign_rpn", None, _ptr(anchors), 1 if anchors.dim() == 3 else 0, _ptr(mask), na, num_class, _ptr(gt),
+          _ptr(gt_class), _ptr(gt_label), _ptr(d_ngt), B, gt_cap, pos, neg, _ptr(labels), _ptr(targets), _ptr(ious),
+          _ptr(d_npos), _ptr(status), _ptr(w), w.numel(), _stream())
+    return labels, targets, ious, d_npos
+
+
+def assign_pswarp(gt, d_ngt, boxes, d_k, pos_thr, neg_thr, status, d_head=None, head_cap=0, ws=None):
+    """gt [B,gt_cap,7], d_ngt [B]; boxes [B,n,7]: slots [0, head_cap) hold d_head[b] boxes, slots [head_cap, n) hold
+    d_k[b] boxes.  Returns (labels [B,n] i32 (-1 in empty slots), ious [B,n], d_npos [B])."""
+    dev = gt.device
+    B, gt_cap = gt.shape[0], gt.shape[1]
+    n = boxes.shape[1]
+    labels = torch.empty((B, n), dtype=torch.int32, device=dev)
+    ious = torch.empty((B, n), dtype=torch.float32, device=dev)
+    d_npos = torch.empty((B,), dtype=torch.int32, device=dev)
+    w = _loss_ws(B, gt_cap, dev, ws)
+    _call("sassd_assign_pswarp", None, _ptr(gt), _ptr(d_ngt), B, gt_cap, _ptr(boxes), n, _ptr(d_head), head_cap,
+          _ptr(d_k), ctypes.c_float(pos_thr), ctypes.c_float(neg_thr), _ptr(labels), _ptr(ious), _ptr(d_npos),
+          _ptr(status), _ptr(w), w.numel(), _stream())
+    return labels, ious, d_npos
+
+
+def rpn_loss(head, num_class, anchors, labels, targets, d_npos, out, ws=None):
+    """head [B,H,W,stride] (SSDRotateHead.forward_nhwc); writes out[0:3] = rpn_loc_loss, rpn_cls_loss, rpn_dir_loss."""
+    B, H, W, stride = head.shape
+    w = _loss_ws(B, 1, head.device, ws)
+    _call("sassd_rpn_loss", None, _ptr(head), stride, B, H, W, num_class, _ptr(anchors), 1 if anchors.dim() == 3 else 0,
+          anchors.shape[-2], _ptr(labels), _ptr(targets), _ptr(d_npos), _ptr(out), _ptr(w), w.numel(), _stream())
+
+
+def pswarp_loss(scores, labels, d_npos, out, ws=None):
+    """scores / labels [B,n]; writes out[0] = loss_cls."""
+    B, n = scores.shape
+    w = _loss_ws(B, 1, scores.device, ws)
+    _call("sassd_pswarp_loss", None, _ptr(scores), _ptr(labels), B, n, _ptr(d_npos), _ptr(out), _ptr(w), w.numel(),
+          _stream())
+
+
+def aux_loss(point_cls, point_reg, labels, offsets, d_rows, batch, d_npos, out, ws=None):
+    """writes out[0:2] = aux_loss_cls, aux_loss_reg."""
+    cap = point_cls.shape[0]
+    w = _loss_ws(batch, 1, point_cls.device, ws)
+    _call("sassd_aux_loss", None, _ptr(point_cls), _ptr(point_reg), _ptr(labels), _ptr(offsets), _ptr(d_rows), cap,
+          batch, _ptr(d_npos), _ptr(out), _ptr(w), w.numel(), _stream())
 
 
 # ---------------------------------------------------------------------------- TMA dense conv on split maps

@@ -3,7 +3,8 @@ PSWarpHead (mmdet/models/single_stage_heads/ssd_rotate_head.py:95-125,218-235,
 307-372,416-447,487-533) plus the NMS wrappers they call
 (mmdet/core/post_processing/bbox_nms.py:4-27, mmdet/ops/iou3d/iou3d_utils.py:47-60,114-128).
 
-Inference methods only; ``loss`` / target assignment are training code and out of scope.
+The losses (``SSDRotateHead.loss``, ``PSWarpHead.loss``) and their target assignment run forward only, on the
+device (csrc/targets.cu), for a model in eval() mode.
 """
 
 import numpy as np
@@ -22,6 +23,35 @@ def _pad_lists(tensors, k_cap, width, dtype, device):
         if t is not None and len(t):
             out[b, : len(t)] = t.to(device=device, dtype=dtype)
     return out
+
+
+def stage_gt(gt_bboxes, gt_class, gt_labels, device):
+    """Per-frame ground truth -> the loss kernels' padded layout: gt [B,gt_cap,7] f32, gt_class / gt_label [B,gt_cap]
+    i32 and d_ngt [B] i32.  gt_cap is the batch's largest count, at most the kernels' capacity SASSD_GT_CAP_MAX; d_ngt
+    holds the true counts, so a frame with more boxes sets SASSD_FLAG_GT_CAP on the device and the caller raises.
+    ``gt_class`` (anchor class index per box, -1 none) and ``gt_labels`` default to 0 and 1."""
+    B = len(gt_bboxes)
+    gt_bboxes = [(g.detach().cpu().numpy() if torch.is_tensor(g) else np.asarray(g)).reshape(-1, 7) for g in gt_bboxes]
+    gt_cap = min(max([1] + [g.shape[0] for g in gt_bboxes]), ops._lib.GT_CAP_MAX)
+    gt = np.zeros((B, gt_cap, 7), np.float32)
+    cls = np.zeros((B, gt_cap), np.int32)
+    lab = np.ones((B, gt_cap), np.int32)
+    n = np.zeros((B,), np.int32)
+    for b, g in enumerate(gt_bboxes):
+        n[b] = g.shape[0]
+        k = min(g.shape[0], gt_cap)
+        gt[b, :k] = g[:k]
+        if gt_class is not None:
+            cls[b, :k] = np.asarray(gt_class[b]).reshape(-1)[:k]
+        if gt_labels is not None:
+            lv = gt_labels[b]
+            lab[b, :k] = (lv.detach().cpu().numpy() if torch.is_tensor(lv) else np.asarray(lv)).reshape(-1)[:k]
+    t = lambda a: torch.from_numpy(a).to(device)
+    return t(gt), t(cls), t(lab), t(n)
+
+
+def _as_class_dict(v):
+    return v if isinstance(v, dict) else {None: v}
 
 
 class SSDRotateHead(nn.Module):
@@ -100,11 +130,56 @@ class SSDRotateHead(nn.Module):
         return ops.decode_select(head, self._num_class, anchors.contiguous().float(),
                                  anchors_mask.to(torch.uint8).contiguous(), float(thr), self.k_cap, status)
 
+    def thresholds(self, cfg, names):
+        """(pos, neg) IoU thresholds per anchor class from train_cfg.rpn (``names``: the anchor classes in order; None =
+        the single class of the config)."""
+        a = cfg.assigner
+        if names == [None]:
+            keys = [k for k, v in a.items() if isinstance(v, dict)]
+            names = keys[:1]
+        return [float(a[k]["pos_iou_thr"]) for k in names], [float(a[k]["neg_iou_thr"]) for k in names]
+
+    def loss_device(self, head, anchors, mask, gt, gt_class, gt_label, d_ngt, pos_thr, neg_thr, out, status):
+        """No-sync path: targets (create_target_torch with NearestIouSimilarity, per frame and class) and the three
+        RPN losses into out[0:3].  anchors [Na,7] or [B,Na,7], classes concatenated; mask [B,Na] u8.  Returns (labels,
+        targets, ious, d_npos)."""
+        anchors = anchors.contiguous().float()
+        res = ops.assign_rpn(anchors, mask.to(torch.uint8).contiguous(), self._num_class, gt, gt_class, gt_label, d_ngt,
+                             pos_thr, neg_thr, status)
+        ops.rpn_loss(head, self._num_class, anchors, res[0], res[1], res[3], out)
+        return res
+
+    def loss(self, box_preds, cls_preds, dir_cls_preds, gt_bboxes, gt_labels, gt_types, anchors, anchors_mask, cfg):
+        """ssd_rotate_head.py:261-305: dict(rpn_loc_loss, rpn_cls_loss, rpn_dir_loss), each a [1] tensor.  ``anchors``
+        / ``anchors_mask``: per-class dicts of [B,Na_c,7] / [B,Na_c] (the training dataset's), or one tensor for a
+        single class.  ``gt_types``: per frame the class name of each box; a box counts for the anchors of its class.
+        Thresholds from ``cfg`` (train_cfg.rpn).  A frame without boxes of a class has every masked anchor of that
+        class as background."""
+        ops.require_cuda()
+        anchors, anchors_mask = _as_class_dict(anchors), _as_class_dict(anchors_mask)
+        names = list(anchors.keys())
+        head = self._as_head_map(box_preds, cls_preds, dir_cls_preds)
+        dev, B = head.device, head.shape[0]
+        a = torch.cat([anchors[k].to(dev).float().reshape(B, -1, 7) for k in names], 1).contiguous()
+        m = torch.cat([anchors_mask[k].to(dev).reshape(B, -1).to(torch.uint8) for k in names], 1).contiguous()
+        if names == [None] or gt_types is None:
+            gt_class = [np.zeros(len(g), np.int32) for g in gt_bboxes]
+        else:
+            index = {k: i for i, k in enumerate(names)}
+            gt_class = [np.array([index.get(str(t), -1) for t in np.asarray(ts).reshape(-1)], np.int32)
+                        for ts in gt_types]
+        gt, gcls, glab, d_ngt = stage_gt(gt_bboxes, gt_class, gt_labels, dev)
+        pos, neg = self.thresholds(cfg, names)
+        status = torch.zeros((1,), dtype=torch.int32, device=dev)
+        out = torch.zeros((3,), dtype=torch.float32, device=dev)
+        self.loss_device(head, a, m, gt, gcls, glab, d_ngt, pos, neg, out, status)
+        _raise_on_flags(status)
+        return dict(rpn_loc_loss=out[0:1], rpn_cls_loss=out[1:2], rpn_dir_loss=out[2:3])
+
     def get_guided_anchors(self, box_preds, cls_preds, dir_cls_preds, anchors, anchors_mask, gt_bboxes, gt_labels,
                            thr=.1):
-        """Reference signature (ssd_rotate_head.py:307-372); inference only (gt_* must be None)."""
-        if gt_bboxes is not None or gt_labels is not None:
-            raise NotImplementedError("ground-truth injection is a training feature")
+        """Reference signature (ssd_rotate_head.py:307-372).  With ``gt_bboxes`` / ``gt_labels`` (training) each frame's
+        boxes and labels are prepended to its selected boxes and labels (:364-367)."""
         if isinstance(anchors, dict):
             anchors = torch.cat([v for v in anchors.values()], 1)
         if isinstance(anchors_mask, dict):
@@ -115,7 +190,13 @@ class SSDRotateHead(nn.Module):
                                                                thr, status)
         ks = d_k.tolist()
         _raise_on_flags(status)
-        return ([boxes[b, :k] for b, k in enumerate(ks)], [labels[b, :k].long() for b, k in enumerate(ks)])
+        guided, lbls = [boxes[b, :k] for b, k in enumerate(ks)], [labels[b, :k].long() for b, k in enumerate(ks)]
+        if gt_bboxes is not None:
+            dev = head.device
+            guided = [torch.cat([torch.as_tensor(g).to(dev).float().reshape(-1, 7), x], 0)
+                      for g, x in zip(gt_bboxes, guided)]
+            lbls = [torch.cat([torch.as_tensor(l).to(dev).long().reshape(-1), x], 0) for l, x in zip(gt_labels, lbls)]
+        return guided, lbls
 
 
 def _raise_on_flags(status):
@@ -199,8 +280,41 @@ class PSWarpHead(nn.Module):
         return conv2d_nhwc(y, w1, None, None, False, c, self.precision)
 
     def forward_device(self, conv6_nhwc, boxes, d_k):
-        feat = self.convs_nhwc(conv6_nhwc)
+        return self.sample(self.convs_nhwc(conv6_nhwc), boxes, d_k)
+
+    def sample(self, feat, boxes, d_k):
+        """Scores of boxes [B,k_cap,7] (d_k [B] of them per frame) on the part-score map of convs_nhwc."""
         return ops.pswarp(feat, boxes, d_k, self.grid_offsets[0], self.grid_offsets[1], self.spatial_scale)
+
+    def loss_device(self, scores, boxes, d_k, gt, d_ngt, cfg, out, status, d_head=None, head_cap=0):
+        """No-sync path: targets (create_target_torch with RotateIou3dSimilarity) of box slots [B,n,7] (slots below
+        ``head_cap`` hold d_head[b] boxes, the rest d_k[b]; ops.assign_pswarp) and the focal loss of their scores
+        [B,n] into out[0].  Returns (labels, ious, d_npos)."""
+        a = cfg.assigner
+        res = ops.assign_pswarp(gt, d_ngt, boxes, d_k, float(a.pos_iou_thr), float(a.neg_iou_thr), status,
+                                d_head=d_head, head_cap=head_cap)
+        ops.pswarp_loss(scores.contiguous(), res[0], res[2], out)
+        return res
+
+    def loss(self, cls_preds, gt_bboxes, gt_labels, anchors, cfg):
+        """ssd_rotate_head.py:450-485: dict(loss_cls=[1] tensor).  ``cls_preds``: forward(is_test=False)'s scores of
+        the guided boxes ``anchors`` (one [K_b,7] tensor per frame, GT rows first as get_guided_anchors prepends them),
+        concatenated; thresholds from ``cfg`` (train_cfg.extra).  The focal loss is normalised by the positives of the
+        whole batch."""
+        ops.require_cuda()
+        dev = cls_preds.device
+        B = len(anchors)
+        ks = [len(g) for g in anchors]
+        k_cap = max(1, max(ks))
+        boxes = _pad_lists([g.view(-1, 7) for g in anchors], k_cap, 7, torch.float32, dev)
+        scores = _pad_lists(list(torch.split(cls_preds.reshape(-1), ks)), k_cap, 0, torch.float32, dev)
+        d_k = torch.tensor(ks, dtype=torch.int32, device=dev)
+        gt, _, _, d_ngt = stage_gt(gt_bboxes, None, None, dev)
+        status = torch.zeros((1,), dtype=torch.int32, device=dev)
+        out = torch.zeros((1,), dtype=torch.float32, device=dev)
+        self.loss_device(scores, boxes, d_k, gt, d_ngt, cfg, out, status)
+        _raise_on_flags(status)
+        return dict(loss_cls=out)
 
     def forward(self, x, guided_anchors, is_test=False):
         """Reference signature (ssd_rotate_head.py:431-447): x [B,256,H,W], list of [K_b,7]."""
