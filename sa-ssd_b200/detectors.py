@@ -22,7 +22,7 @@ from torch import nn
 
 from . import builder, ops
 from .results import annos_from_rows, meta_block
-from .single_stage_heads import unpack_detections
+from .single_stage_heads import split_detections, unpack_detections
 
 
 class SingleStageDetector(nn.Module):
@@ -45,10 +45,7 @@ class SingleStageDetector(nn.Module):
         self.anchor_set = None
         self._pinned = None
         self._mask_stream = None
-        self._graph = None
-        self._crop_graph = None
-        self._kitti_graphs = {}           # crop -> captured step that also formats KITTI rows (forward_points metas=)
-        self._point_graphs = {}           # (crop, kitti) -> captured step that also runs the aux network (point_outputs)
+        self._graphs = {}                 # (crop, kitti, point_outputs) -> captured single step (enable_cuda_graph)
         self._graph_args = None
         self._stream_slots = None
         self._stream_key = None
@@ -69,24 +66,17 @@ class SingleStageDetector(nn.Module):
         self.neck.set_precision(precision, sparse)
         self.rpn_head.precision = precision
         self.extra_head.precision = precision
-        self._drop_captured_graphs()
-
-    def _drop_captured_graphs(self):
-        """Captured steps bake in the device addresses of packed weights, folded BN vectors and layer constants and
-        the kernel selection; anything that changes those must force a re-capture."""
-        self._graph = None
-        self._crop_graph = None
-        self._kitti_graphs = {}
-        self._point_graphs = {}
-        self._stream_slots = None
-        self._stream_key = None
+        self.refresh_packed_weights()
 
     def refresh_packed_weights(self):
-        """Called after parameters were (re)loaded (checkpoint.load_state_dict_into).  Packed / folded tensors are
-        version-checked on eager use, but a CUDA-graph replay never re-checks: drop every captured step (the
-        single-step graph of enable_cuda_graph and the detect_stream slots) so the next call re-captures with the
-        new weights."""
-        self._drop_captured_graphs()
+        """Called after parameters were (re)loaded (checkpoint.load_state_dict_into) or the precision changed.
+        Captured steps bake in the device addresses of packed weights, folded BN vectors and layer constants and the
+        kernel selection; eager use version-checks the packed / folded tensors, but a CUDA-graph replay never
+        re-checks: drop every captured step (the single-step graphs of enable_cuda_graph and the detect_stream slots)
+        so the next call re-captures."""
+        self._graphs = {}
+        self._stream_slots = None
+        self._stream_key = None
 
     # ------------------------------------------------------------------ reference-signature path
     def merge_second_batch(self, batch_args):
@@ -182,12 +172,14 @@ class SingleStageDetector(nn.Module):
         self.anchor_set = anchor_set.to(dev)
         return self
 
-    def forward_device(self, points, pt_off, batch, max_points_per_frame, point_outputs=False, detections=True):
+    def forward_device(self, points, pt_off, batch, max_points_per_frame, point_outputs=False, detections=True,
+                       guided_thr=None):
         """Everything on the device, no synchronisation.  points [Ncap,4], pt_off [batch+1] int32.
         Returns (det [B,det_cap,9], d_ndet [B], status [1], aux dict); without ``detections`` the rescoring and NMS are
         skipped and det, d_ndet are None (the loss path reads only the guided boxes and their scores).  With ``point_outputs`` the aux dict also holds
         the auxiliary network's points_mean [cap,4] (b, x, y, z), point_cls [cap] and point_reg [cap,3] (neck.point_head)
-        for the voxel rows (frame_rows)."""
+        for the voxel rows (frame_rows).  ``guided_thr``: the guided anchors' score threshold (default self.guided_thr;
+        the losses use train_cfg.rpn.anchor_thr)."""
         dev = points.device
         status = torch.zeros((1,), dtype=torch.int32, device=dev)
         vg, aset = self.voxel_generator, self.anchor_set
@@ -205,7 +197,8 @@ class SingleStageDetector(nn.Module):
         main.wait_stream(self._mask_stream)
         head = self.rpn_head.forward_nhwc(y)
         anchors, _ = aset.device_tensors()
-        boxes, labels, index, d_k = self.rpn_head.guided_anchors_device(head, anchors, mask, self.guided_thr, status)
+        thr = self.guided_thr if guided_thr is None else guided_thr
+        boxes, labels, index, d_k = self.rpn_head.guided_anchors_device(head, anchors, mask, thr, status)
         ps_feat = self.extra_head.convs_nhwc(conv6)
         scores = self.extra_head.sample(ps_feat, boxes, d_k)
         det = d_ndet = None
@@ -233,20 +226,27 @@ class SingleStageDetector(nn.Module):
     def enable_cuda_graph(self, batch, max_points_per_frame=32768):
         """Capture forward_device once for (batch, max_points_per_frame) and replay it per step: every
         data-dependent size already lives on the device, so the ~65 launches of a step become one graph
-        launch.  Steps whose shape does not fit fall back to the eager path.  Calls with ``frustum_planes`` replay a
-        second graph, captured on their first use, that runs the crop and the step; there ``max_points_per_frame`` bounds
-        the full sweeps (e.g. 131072).  Calls with ``metas`` replay a graph, again captured on first use, that ends with
-        the KITTI result formatter, and calls with ``point_outputs`` one that also runs the auxiliary network."""
+        launch.  Steps whose shape does not fit fall back to the eager path.  forward_points replays one graph per kind
+        of call: with or without ``frustum_planes`` (the graph crops the full sweeps first, and ``max_points_per_frame``
+        bounds them, e.g. 131072), ``metas`` (it ends with the KITTI result formatter) and ``point_outputs`` (it also
+        runs the auxiliary network).  The plain kind is captured here and returned, the others on their first use; a
+        new call replaces every graph captured for an earlier shape."""
         self._graph_args = (int(batch), int(max_points_per_frame))
-        self._graph = _GraphedStep(self, batch, max_points_per_frame, latency=True)
-        return self._graph
+        self._graphs = {}
+        return self._graph_for(False, False, False)
 
     def disable_cuda_graph(self):
-        self._graph = None
-        self._crop_graph = None
-        self._kitti_graphs = {}
-        self._point_graphs = {}
+        self._graphs = {}
         self._graph_args = None
+
+    def _graph_for(self, crop, kitti, point_outputs):
+        """The captured single step of this kind at enable_cuda_graph's shape, captured on first use; None while the
+        graphs are disabled."""
+        key = (crop, kitti, point_outputs)
+        if key not in self._graphs and self._graph_args is not None:
+            self._graphs[key] = _GraphedStep(self, *self._graph_args, latency=True, crop=crop, kitti=kitti,
+                                             point_outputs=point_outputs)
+        return self._graphs.get(key)
 
     def detect_stream(self, batches, batch, max_points_per_frame=32768, depth=4, concurrent=True, crop=False,
                       kitti=False):
@@ -291,8 +291,12 @@ class SingleStageDetector(nn.Module):
 
     def _collected(self, slot, metas):
         """Wait for a slot's step and convert its host copy into the caller's per-frame results."""
-        out = slot.collect()
-        if slot.kitti:
+        return self._frame_results(slot.collect(), metas)
+
+    def _frame_results(self, out, metas):
+        """A step's host outputs -> the caller's per-frame results: with ``metas`` KITTI annotation dicts of the
+        formatter's (rows, n_out), else detection dicts of split_detections' (boxes, scores, labels)."""
+        if metas is not None:
             return annos_from_rows(*out, self.class_names, [m["sample_idx"] for m in metas])
         return [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(*out)]
 
@@ -315,59 +319,28 @@ class SingleStageDetector(nn.Module):
             raise RuntimeError("call attach_data_pipeline(voxel_generator, anchor_set) first")
         if metas is not None and self.class_names is None:
             raise ValueError("forward_points(metas=) needs class_names")
-        dev = next(self.parameters()).device
-        planes = None if frustum_planes is None else _frame_planes(frustum_planes, len(points_list))
-        meta = None if metas is None else _meta_blocks(metas, len(points_list))
+        B = len(points_list)
+        planes = None if frustum_planes is None else _frame_planes(frustum_planes, B)
+        meta = None if metas is None else _meta_blocks(metas, B)
         hp, ho, counts = self.stage_points(points_list)
-        if point_outputs:
-            key = (planes is not None, meta is not None)
-            if key not in self._point_graphs and self._graph_args is not None:
-                self._point_graphs[key] = _GraphedStep(self, *self._graph_args, latency=True, crop=key[0], kitti=key[1],
-                                                       point_outputs=True)
-            g = self._point_graphs.get(key)
-        elif meta is not None:
-            crop = planes is not None
-            if crop not in self._kitti_graphs and self._graph_args is not None:
-                self._kitti_graphs[crop] = _GraphedStep(self, *self._graph_args, latency=True, crop=crop, kitti=True)
-            g = self._kitti_graphs.get(crop)
-        elif planes is None:
-            if self._graph is None and self._graph_args is not None:     # dropped by a weight / precision change
-                self._graph = _GraphedStep(self, *self._graph_args, latency=True)
-            g = self._graph
-        else:
-            if self._crop_graph is None and self._graph_args is not None:
-                self._crop_graph = _GraphedStep(self, *self._graph_args, latency=True, crop=True)
-            g = self._crop_graph
-        if g is not None and not return_aux and g.fits(len(points_list), counts):
-            out = g.run_host(hp, ho, sum(counts), planes, meta)
-            if meta is not None:
-                res = annos_from_rows(*out, self.class_names, [m["sample_idx"] for m in metas])
-            else:
-                res = [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(*out)]
+        g = self._graph_for(planes is not None, meta is not None, bool(point_outputs))
+        if g is not None and not return_aux and g.fits(B, counts):
+            res = self._frame_results(g.run_host(hp, ho, sum(counts), planes, meta), metas)
             return (res, g.point_results()) if point_outputs else res
-        points = hp.to(dev, non_blocking=True)
-        pt_off = ho.to(dev, non_blocking=True)
-        if planes is not None:
-            points, pt_off = ops.frustum_crop(points, pt_off, len(points_list), torch.from_numpy(planes).to(dev))
-        det, d_ndet, status, aux = self.forward_device(points, pt_off, len(points_list), max(counts + [1]),
-                                                       point_outputs=point_outputs)
-        pts = None
-        if point_outputs:
-            pts = _split_points(aux["points_mean"].cpu().numpy(), aux["point_cls"].cpu().numpy(),
-                                aux["point_reg"].cpu().numpy(), aux["frame_rows"].cpu().numpy())
+        dev = next(self.parameters()).device
+        det, d_ndet, status, aux = _run_step(self, hp.to(dev, non_blocking=True), ho.to(dev, non_blocking=True), B,
+                                             max(counts + [1]), _to_device(planes, dev), _to_device(meta, dev),
+                                             point_outputs=point_outputs)
         if meta is not None:
-            rows, n_out = ops.kitti_format(det, d_ndet, torch.from_numpy(meta).to(dev))
-            word = int(status.item())
-            if word:
-                raise ops._lib.SassdError("capacity overflow on device: %s" % ops._lib.decode_flags(word))
-            out = annos_from_rows(rows.cpu().numpy(), n_out.cpu().numpy(), self.class_names,
-                                  [m["sample_idx"] for m in metas])
+            ops._lib.raise_on_status(status)
+            out = aux["rows"].cpu().numpy(), aux["n_out"].cpu().numpy()
             aux.update(det=det, ndet=d_ndet)
         else:
-            bbs, scs, lbs = unpack_detections(det, d_ndet, status)
-            out = [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(bbs, scs, lbs)]
-        ret = (out,) + ((pts,) if point_outputs else ()) + ((aux,) if return_aux else ())
-        return ret if len(ret) > 1 else out
+            out = unpack_detections(det, d_ndet, status)
+        res = self._frame_results(out, metas)
+        pts = _split_points(*(aux[k].cpu().numpy() for k in _POINT_KEYS)) if point_outputs else None
+        ret = (res,) + ((pts,) if point_outputs else ()) + ((aux,) if return_aux else ())
+        return ret if len(ret) > 1 else res
 
 
     def loss_device(self, aux, batch, gt, gt_class, gt_label, d_ngt, n_gt_host, status):
@@ -423,24 +396,15 @@ class SingleStageDetector(nn.Module):
         gt_class = [(l - 1).astype(np.int32) for l in labels]
         gt, gcls, glab, d_ngt = stage_gt(gt_bboxes, gt_class, labels, dev)
         n_gt = np.array([np.asarray(g).reshape(-1, 7).shape[0] for g in gt_bboxes], np.int64)
-        points = hp.to(dev, non_blocking=True)
-        pt_off = ho.to(dev, non_blocking=True)
-        if planes is not None:
-            points, pt_off = ops.frustum_crop(points, pt_off, B, torch.from_numpy(planes).to(dev))
-        thr0, self.guided_thr = self.guided_thr, float(self.train_cfg.rpn.anchor_thr)
-        try:
-            _, _, status, aux = self.forward_device(points, pt_off, B, max(counts + [1]), point_outputs=True,
-                                                    detections=False)
-        finally:
-            self.guided_thr = thr0
+        _, _, status, aux = _run_step(self, hp.to(dev, non_blocking=True), ho.to(dev, non_blocking=True), B,
+                                      max(counts + [1]), _to_device(planes, dev), point_outputs=True, detections=False,
+                                      guided_thr=float(self.train_cfg.rpn.anchor_thr))
         out, targets = self.loss_device(aux, B, gt, gcls, glab, d_ngt, n_gt, status)
         h = torch.empty((len(ops.LOSS_KEYS) + 1,), dtype=torch.float32, pin_memory=True)
         h[:-1].copy_(out, non_blocking=True)
         h[-1:].copy_(status.view(torch.float32), non_blocking=True)
         torch.cuda.current_stream().synchronize()
-        word = int(h[-1:].view(torch.int32).item())
-        if word:
-            raise ops._lib.SassdError("capacity overflow on device: %s" % ops._lib.decode_flags(word))
+        ops._lib.raise_on_status(h[-1:].view(torch.int32))
         res = {k: float(v) for k, v in zip(ops.LOSS_KEYS, h[:-1].tolist())}
         if return_aux:
             aux.update(targets)
@@ -451,6 +415,9 @@ class SingleStageDetector(nn.Module):
 def _on_device(v, dev):
     """A tensor or a per-class dict of tensors, on ``dev``."""
     return {k: t.to(dev) for k, t in v.items()} if isinstance(v, dict) else v.to(dev)
+
+
+_POINT_KEYS = ("points_mean", "point_cls", "point_reg", "frame_rows")     # the aux outputs _split_points takes
 
 
 def _split_points(points_mean, cls, reg, frame_rows):
@@ -477,6 +444,26 @@ def _meta_blocks(metas, batch):
     return np.stack([meta_block(m["calib"], m["img_shape"]) for m in metas])
 
 
+def _to_device(a, dev):
+    """A host numpy array (or None) -> a tensor on ``dev``."""
+    return None if a is None else torch.from_numpy(a).to(dev)
+
+
+def _run_step(model, points, pt_off, batch, maxpts, planes=None, meta=None, point_outputs=False, detections=True,
+              guided_thr=None):
+    """One detector step on the device, no synchronisation; the eager calls and every captured graph build their step
+    here.  With ``planes`` [batch,6,4] the frames are full sweeps, cropped to their camera frustums first
+    (ops.frustum_crop); then forward_device; with ``meta`` [batch,36] the detections are formatted as KITTI rows
+    (ops.kitti_format) into aux["rows"] / aux["n_out"].  Returns forward_device's (det, d_ndet, status, aux)."""
+    if planes is not None:
+        points, pt_off = ops.frustum_crop(points, pt_off, batch, planes)
+    det, d_ndet, status, aux = model.forward_device(points, pt_off, batch, maxpts, point_outputs=point_outputs,
+                                                    detections=detections, guided_thr=guided_thr)
+    if meta is not None:
+        aux["rows"], aux["n_out"] = ops.kitti_format(det, d_ndet, meta)
+    return det, d_ndet, status, aux
+
+
 def _pinned_pair(n_points, n_off):
     return (torch.empty((n_points, 4), dtype=torch.float32, pin_memory=True),
             torch.empty((n_off,), dtype=torch.int32, pin_memory=True))
@@ -497,7 +484,7 @@ def _stage_into(hp, ho, points_list, counts):
 
 
 class _GraphedStep:
-    """One captured step of SingleStageDetector.forward_device with static input/output buffers."""
+    """One captured detector step (_run_step) with static input/output buffers."""
 
     def __init__(self, model, batch, max_points_per_frame, latency=False, crop=False, kitti=False, point_outputs=False):
         """latency=True: this step will run alone on the GPU (enable_cuda_graph / forward_points): the dense convs walk
@@ -515,6 +502,7 @@ class _GraphedStep:
         self.crop, self.kitti, self.point_outputs = bool(crop), bool(kitti), bool(point_outputs)
         self.points = torch.zeros((self.cap, 4), dtype=torch.float32, device=dev)
         self.pt_off = torch.zeros((self.batch + 1,), dtype=torch.int32, device=dev)
+        self.planes = self.meta = None
         if self.crop:
             self.planes = torch.zeros((self.batch, 6, 4), dtype=torch.float64, device=dev)
         if self.kitti:
@@ -546,15 +534,15 @@ class _GraphedStep:
             if pdl0 is not None:
                 ops._lib.load().sassd_set_pdl(pdl0)
         if self.kitti:
-            self.h_rows = torch.empty(self.rows.shape, dtype=torch.float64, pin_memory=True)
-            self.h_nout = torch.empty(self.n_out.shape, dtype=torch.int32, pin_memory=True)
+            self.h_rows = torch.empty(self.aux["rows"].shape, dtype=torch.float64, pin_memory=True)
+            self.h_nout = torch.empty(self.aux["n_out"].shape, dtype=torch.int32, pin_memory=True)
             self.h_meta = torch.empty(self.meta.shape, dtype=torch.float64, pin_memory=True)
         else:
             self.h_det = torch.empty(self.det.shape, dtype=torch.float32, pin_memory=True)
             self.h_nd = torch.empty(self.d_ndet.shape, dtype=torch.int32, pin_memory=True)
         if self.point_outputs:
             self.h_pts = {k: torch.empty(self.aux[k].shape, dtype=self.aux[k].dtype, pin_memory=True)
-                          for k in ("points_mean", "point_cls", "point_reg", "frame_rows")}
+                          for k in _POINT_KEYS}
         self.h_status = torch.empty((1,), dtype=torch.int32, pin_memory=True)
         self.h_points, self.h_off = _pinned_pair(self.cap, self.batch + 1)
         if self.crop:
@@ -563,14 +551,8 @@ class _GraphedStep:
         self.loaded = torch.cuda.Event()
 
     def _step(self):
-        points, pt_off = self.points, self.pt_off
-        if self.crop:
-            points, pt_off = ops.frustum_crop(points, pt_off, self.batch, self.planes)
-        det, d_ndet, status, aux = self.model.forward_device(points, pt_off, self.batch, self.maxpts,
-                                                             point_outputs=self.point_outputs)
-        if self.kitti:
-            self.rows, self.n_out = ops.kitti_format(det, d_ndet, self.meta)
-        return det, d_ndet, status, aux
+        return _run_step(self.model, self.points, self.pt_off, self.batch, self.maxpts, self.planes, self.meta,
+                         point_outputs=self.point_outputs)
 
     def fits(self, batch, counts):
         return batch == self.batch and max(counts + [0]) <= self.maxpts
@@ -586,6 +568,15 @@ class _GraphedStep:
 
     def run_host(self, hp, ho, total, planes=None, meta=None):
         """pinned host points in, numpy detections (or KITTI rows) out: H2D, one graph launch, D2H, one stream sync."""
+        self._upload(hp, ho, total, planes, meta)
+        self.graph.replay()
+        self._download()
+        torch.cuda.current_stream().synchronize()
+        return self.unpack()
+
+    def _upload(self, hp, ho, total, planes, meta):
+        """H2D of a step's inputs into the static buffers on the current stream: ``total`` points of the pinned ``hp``,
+        the pinned offsets ``ho`` and, for a crop / formatting step, the numpy planes / meta blocks."""
         self.points[:total].copy_(hp[:total], non_blocking=True)
         self.pt_off.copy_(ho, non_blocking=True)
         if self.crop:
@@ -594,17 +585,13 @@ class _GraphedStep:
         if self.kitti:
             self.h_meta.numpy()[...] = meta
             self.meta.copy_(self.h_meta, non_blocking=True)
-        self.graph.replay()
-        self._download()
-        torch.cuda.current_stream().synchronize()
-        return self.unpack()
 
     def _download(self):
         """D2H of the step's result on the current stream: the KITTI rows and counts of a formatting step, else the
         detections and counts; and the status word."""
         if self.kitti:
-            self.h_rows.copy_(self.rows, non_blocking=True)
-            self.h_nout.copy_(self.n_out, non_blocking=True)
+            self.h_rows.copy_(self.aux["rows"], non_blocking=True)
+            self.h_nout.copy_(self.aux["n_out"], non_blocking=True)
         else:
             self.h_det.copy_(self.det, non_blocking=True)
             self.h_nd.copy_(self.d_ndet, non_blocking=True)
@@ -618,19 +605,9 @@ class _GraphedStep:
         """Stage into this slot's pinned buffer, H2D on the copy stream, then replay + D2H on the current stream or,
         with ``own_stream``, on this slot's stream so that consecutive steps overlap on the GPU."""
         _stage_into(self.h_points, self.h_off, points_list, counts)
-        if self.crop:
-            self.h_planes.numpy()[...] = planes
-        if self.kitti:
-            self.h_meta.numpy()[...] = meta
-        total = sum(counts)
         cur = self.stream if own_stream else torch.cuda.current_stream()
         with torch.cuda.stream(copy_stream):
-            self.points[:total].copy_(self.h_points[:total], non_blocking=True)
-            self.pt_off.copy_(self.h_off, non_blocking=True)
-            if self.crop:
-                self.planes.copy_(self.h_planes, non_blocking=True)
-            if self.kitti:
-                self.meta.copy_(self.h_meta, non_blocking=True)
+            self._upload(self.h_points, self.h_off, sum(counts), planes, meta)
             self.loaded.record(copy_stream)
         cur.wait_event(self.loaded)
         with torch.cuda.stream(cur):
@@ -644,23 +621,10 @@ class _GraphedStep:
 
     def point_results(self):
         """The last run's aux outputs, per frame (forward_points(point_outputs=True))."""
-        h = self.h_pts
-        return _split_points(h["points_mean"].numpy(), h["point_cls"].numpy(), h["point_reg"].numpy(),
-                             h["frame_rows"].numpy())
+        return _split_points(*(self.h_pts[k].numpy() for k in _POINT_KEYS))
 
     def unpack(self):
-        word = int(self.h_status.numpy()[0])
-        if word:
-            raise ops._lib.SassdError("capacity overflow on device: %s" % ops._lib.decode_flags(word))
+        ops._lib.raise_on_status(self.h_status.numpy()[0])
         if self.kitti:      # (rows, n_out): results.annos_from_rows
             return self.h_rows.numpy().copy(), self.h_nout.numpy().copy()
-        det, n = self.h_det.numpy(), self.h_nd.numpy()
-        bbs, scs, lbs = [], [], []
-        for b in range(det.shape[0]):
-            k = int(n[b])
-            if k == 0:
-                bbs.append(None); scs.append(None); lbs.append(None)
-                continue
-            bbs.append(det[b, :k, :7].copy()); scs.append(det[b, :k, 7].copy())
-            lbs.append(det[b, :k, 8].astype(np.int64))
-        return bbs, scs, lbs
+        return split_detections(self.h_det.numpy(), self.h_nd.numpy())

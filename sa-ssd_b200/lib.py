@@ -152,3 +152,11 @@ def check(rc, what):
 
 def decode_flags(word):
     return [name for bit, name in FLAGS.items() if word & bit]
+
+
+def raise_on_status(word):
+    """Raise SassdError naming the capacities that overflowed if the status word ``d_status`` of a step has a
+    SASSD_FLAG_* bit set.  ``word`` is an int or a one-element tensor (a device tensor is read with a sync)."""
+    word = int(word)
+    if word:
+        raise SassdError("capacity overflow on device: %s" % decode_flags(word))

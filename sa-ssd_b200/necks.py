@@ -262,7 +262,7 @@ class SpMiddleFHD(nn.Module):
         return labels.to(torch.uint8), offsets
 
     def _aux_targets(self, nxyz, gt_boxes3d, enlarge=1.0):
-        from .single_stage_heads import stage_gt, _raise_on_flags
+        from .single_stage_heads import stage_gt
         ops.require_cuda()
         dev = nxyz.device if nxyz.is_cuda else torch.device("cuda")
         boxes = []
@@ -278,7 +278,7 @@ class SpMiddleFHD(nn.Module):
         status = torch.zeros((1,), dtype=torch.int32, device=dev)
         d_rows = torch.tensor([n], dtype=torch.int32, device=dev)
         labels, offsets, d_npos = ops.points_in_boxes(pm, d_rows, gt, d_ngt, status)
-        _raise_on_flags(status)
+        ops._lib.raise_on_status(status)
         return labels, offsets, (d_rows, d_npos)
 
     def aux_loss(self, points, point_cls, point_reg, gt_bboxes):

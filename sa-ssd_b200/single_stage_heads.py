@@ -173,7 +173,7 @@ class SSDRotateHead(nn.Module):
         status = torch.zeros((1,), dtype=torch.int32, device=dev)
         out = torch.zeros((3,), dtype=torch.float32, device=dev)
         self.loss_device(head, a, m, gt, gcls, glab, d_ngt, pos, neg, out, status)
-        _raise_on_flags(status)
+        ops._lib.raise_on_status(status)
         return dict(rpn_loc_loss=out[0:1], rpn_cls_loss=out[1:2], rpn_dir_loss=out[2:3])
 
     def get_guided_anchors(self, box_preds, cls_preds, dir_cls_preds, anchors, anchors_mask, gt_bboxes, gt_labels,
@@ -189,7 +189,7 @@ class SSDRotateHead(nn.Module):
         boxes, labels, index, d_k = self.guided_anchors_device(head, anchors, anchors_mask.view(head.shape[0], -1),
                                                                thr, status)
         ks = d_k.tolist()
-        _raise_on_flags(status)
+        ops._lib.raise_on_status(status)
         guided, lbls = [boxes[b, :k] for b, k in enumerate(ks)], [labels[b, :k].long() for b, k in enumerate(ks)]
         if gt_bboxes is not None:
             dev = head.device
@@ -197,12 +197,6 @@ class SSDRotateHead(nn.Module):
                       for g, x in zip(gt_bboxes, guided)]
             lbls = [torch.cat([torch.as_tensor(l).to(dev).long().reshape(-1), x], 0) for l, x in zip(gt_labels, lbls)]
         return guided, lbls
-
-
-def _raise_on_flags(status):
-    word = int(status.item())
-    if word:
-        raise ops._lib.SassdError("capacity overflow on device: %s" % ops._lib.decode_flags(word))
 
 
 def boxes3d_to_bev_torch(boxes3d):
@@ -313,7 +307,7 @@ class PSWarpHead(nn.Module):
         status = torch.zeros((1,), dtype=torch.int32, device=dev)
         out = torch.zeros((1,), dtype=torch.float32, device=dev)
         self.loss_device(scores, boxes, d_k, gt, d_ngt, cfg, out, status)
-        _raise_on_flags(status)
+        ops._lib.raise_on_status(status)
         return dict(loss_cls=out)
 
     def forward(self, x, guided_anchors, is_test=False):
@@ -353,17 +347,22 @@ class PSWarpHead(nn.Module):
 
 
 def unpack_detections(det, d_ndet, status=None):
-    """[B,cap,9] + counts -> the reference's three lists (numpy [D,7], [D], [D] or None)."""
+    """Device [B,cap,9] + counts (+ the status word, checked) -> split_detections' three lists."""
     det_c = det.cpu().numpy()
     n = d_ndet.cpu().numpy()
     if status is not None:
-        _raise_on_flags(status)
+        ops._lib.raise_on_status(status)
+    return split_detections(det_c, n)
+
+
+def split_detections(det, n):
+    """Host [B,cap,9] rows + counts [B] -> the reference's three lists (numpy [D,7], [D], [D] or None)."""
     bbs, scs, lbs = [], [], []
-    for b in range(det_c.shape[0]):
+    for b in range(det.shape[0]):
         k = int(n[b])
         if k == 0:
             bbs.append(None); scs.append(None); lbs.append(None)
             continue
-        bbs.append(det_c[b, :k, :7].copy()); scs.append(det_c[b, :k, 7].copy())
-        lbs.append(det_c[b, :k, 8].astype(np.int64))
+        bbs.append(det[b, :k, :7].copy()); scs.append(det[b, :k, 7].copy())
+        lbs.append(det[b, :k, 8].astype(np.int64))
     return bbs, scs, lbs

@@ -116,9 +116,7 @@ class SparseConvTensor:
         return bev.view(self.batch_size, H, W, D, C).permute(0, 4, 3, 1, 2).contiguous()
 
     def check_status(self):
-        word = int(self.status.item())
-        if word:
-            raise ops._lib.SassdError("device status flags: %s" % ops._lib.decode_flags(word))
+        ops._lib.raise_on_status(self.status)
 
 
 class _SparseConvBase(nn.Module):

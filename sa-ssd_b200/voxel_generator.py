@@ -58,7 +58,5 @@ class VoxelGenerator:
         status = torch.zeros((1,), dtype=torch.int32, device=dev)
         voxels, coors, num, _, frame_rows = self.generate_device(d_pts, pt_off, 1, n, status)
         m = int(frame_rows[1].item())
-        word = int(status.item())
-        if word:
-            raise ops._lib.SassdError("voxelizer status flags: %s" % ops._lib.decode_flags(word))
+        ops._lib.raise_on_status(status)
         return (voxels[:m].cpu().numpy(), coors[:m, 1:].contiguous().cpu().numpy(), num[:m].cpu().numpy())

@@ -263,7 +263,7 @@ def _same(got, exp):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("prec", ["f16x3", "fp32"])
-def test_cropped_full_sweeps_detect_like_the_reference_reduced_clouds(gold, prec):
+def test_cropped_full_sweeps_detect_like_the_reduced_clouds_eager_captured_and_streamed(gold, prec):
     from sassd_b200 import ops
     model = _model(ops.PREC_F16X3 if prec == "f16x3" else ops.PREC_FP32)
     full, planes, reduced = _e2e_batches(gold)
@@ -276,7 +276,7 @@ def test_cropped_full_sweeps_detect_like_the_reference_reduced_clouds(gold, prec
     model.enable_cuda_graph(2, 131072)
     for f, p, r in zip(full, planes, reduced):
         _same(model.forward_points(f, frustum_planes=p), model.forward_points(r))
-    assert model._graph is not None and model._crop_graph is not None
+    assert set(model._graphs) == {(False, False, False), (True, False, False)}
     model.disable_cuda_graph()
     # detect_stream: crop slots against plain slots fed the reduced clouds
     order = [0, 1, 1, 0, 1]

@@ -198,7 +198,7 @@ def _host_of(dets, metas):
 
 
 @pytest.mark.gpu
-def test_forward_points_and_detect_stream_format_like_the_host(golden_dir):
+def test_forward_points_graphs_and_detect_stream_format_like_the_host(golden_dir):
     from sassd_b200.single_stage_heads import unpack_detections
     model = _model()
     model.class_names = NAMES
@@ -217,7 +217,7 @@ def test_forward_points_and_detect_stream_format_like_the_host(golden_dir):
         plain = model.forward_points(pts[2:], **kw)
         got = model.forward_points(pts[2:], metas=metas[2:], **kw)
         n += sum(same_annos(g, h, "graph %s" % list(kw)) for g, h in zip(got, _host_of(plain, metas[2:])))
-    assert set(model._kitti_graphs) == {False, True}
+    assert {k for k in model._graphs if k[1]} == {(False, True, False), (True, True, False)}
     model.disable_cuda_graph()
     # detect_stream: formatting crop slots against plain crop slots + host formatting
     order = [(0, 1), (2, 3), (1, 2)]

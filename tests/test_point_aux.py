@@ -385,7 +385,7 @@ def test_neck_is_test_false_and_unchanged_detections():
 
 
 @pytest.mark.gpu
-def test_forward_points_with_crop_metas_and_graph(golden_dir):
+def test_forward_points_with_crop_metas_and_graph_table(golden_dir):
     import sys
     sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
     from test_kitti_format import _sweeps_and_metas
@@ -408,12 +408,12 @@ def test_forward_points_with_crop_metas_and_graph(golden_dir):
         for e, g in zip(eager[1], graph[1]):
             for k in ("xyz", "cls", "reg"):
                 assert np.array_equal(e[k], g[k]), (kw, k)
-    assert len(model._point_graphs) == 3
+    assert {k for k in model._graphs if k[2]} == {(False, False, True), (True, False, True), (False, True, True)}
     before = model.forward_points(pts, point_outputs=True)[1]
     from sassd_b200 import checkpoint
     w = model.neck.point_fc.weight.detach().cpu() * 2.0
     checkpoint.load_state_dict_into(model, {"neck.point_fc.weight": w})
-    assert not model._point_graphs
+    assert not model._graphs
     after = model.forward_points(pts, point_outputs=True)[1]
     for a, b in zip(before, after):
         assert np.array_equal(a["xyz"], b["xyz"])
