@@ -272,9 +272,11 @@ int sassd_spconv_pack(const float* weight, int taps, int cin, int cin_stored, in
 /* tile_mask (optional, taps <= 27): int32 per SASSD_SPCONV_TILE_ROWS-row tile of the OUTPUT rows, bit t set when some
  * row of the tile has a neighbour at tap t (written by sassd_rulebook_subm / sassd_rulebook_conv_nbr); K chunks whose
  * taps are all absent are skipped (an absent pair contributes exactly zero, so the result is unchanged).
- * ws (optional, sassd_spconv_workspace_bytes()): scratch for the tap split - when the layer has at most half as many
- * tiles as CTAs, the two CTAs of a cluster share one tile's chunks and the peer's fp32 partial sums travel through
- * it.  counters (optional, int32[2], caller-zeroed): += executed (tile, chunk) pairs, += tiles (instrumentation). */
+ * ws (optional, sassd_spconv_workspace_bytes(), zero-filled before its first use, not shared by calls that may run at
+ * the same time): with it, a layer that has at most as many tiles as CTAs, and whose longest tile would otherwise
+ * dominate, deals its tiles' active K chunks evenly over all CTAs; the fp32 partial sums of tiles cut between CTAs and the counters that pick the CTA finishing each tile live
+ * in it, and every call leaves the counters zero again.  Without it, one CTA per tile.
+ * counters (optional, int32[2], caller-zeroed): += executed (tile, chunk) pairs, += tiles (instrumentation). */
 #define SASSD_SPCONV_TILE_ROWS 128
 size_t sassd_spconv_workspace_bytes(void);
 int sassd_spconv_f16x3(const sassd_spconv_desc* host_desc, const void* in_split, const void* wpack, const float* scale,

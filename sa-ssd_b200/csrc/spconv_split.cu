@@ -2,7 +2,7 @@
 // mmdet/models/necks/cmn.py:145-173,192-231) on the Hopper tensor cores (wgmma) with FP16x3 and the features kept in
 // "split rows": two fp16 planes [2][rows_cap][C] (hi = half(x), lo = half((x - hi) * 2048)), C a multiple of 8.
 //
-// Structure (one CTA = one 128-row output tile at a time, output-stationary, no atomics, deterministic):
+// Structure (output-stationary 128-row tiles, one CTA per SM, deterministic):
 //   * 8 producer warps only *issue* 16-byte cp.async gathers (zero fill for missing neighbours) straight into the
 //     128B-swizzled operand tiles plus an asynchronous mbarrier arrive; nobody waits for data.  Lane 0 of the first
 //     producer warp also streams the weight blocks and the tile's [128,27] neighbour indices with cp.async.bulk.
@@ -13,9 +13,15 @@
 //   * tap skipping: the rulebook kernel records, per 128-row tile, which of the 27 taps have a neighbour
 //     at all (tile_mask); chunks whose taps are all absent are skipped by every role - reference semantics only need
 //     the listed pairs (spconv's indice_pairs), an absent pair contributes exactly zero.
-//   * small layers (2 * tiles <= CTAs, i.e. one frame at a time): the two CTAs of a cluster split the active chunks
-//     of ONE tile (split-K over taps); each hands the fp32 partial sums of the rows it does not finalise to its peer
-//     through an L2-resident scratch row block and a remote mbarrier arrive (release/acquire at cluster scope).
+//   * large layers (tiles > CTAs, several frames): rounds of one whole tile per CTA.
+//   * small layers (tiles <= CTAs, one frame at a time) whose longest tile runs DEAL_MIN_GAIN chunks more than an
+//     even share: the CHUNK DEAL (other small layers: one tile per CTA).  The active chunks of all tiles, concatenated
+//     in tile order, are cut into one contiguous range per CTA, so every SM runs the same number of chunks (+-1)
+//     instead of every layer taking as long as its busiest tile.  A range holds whole tiles and at most two pieces of
+//     tiles it shares with its neighbours (its first and its last).  Each piece of a shared tile stores its fp32
+//     partial sums to a workspace slot and counts itself on an atomic counter; the piece that completes the count
+//     sums all pieces in piece order (bit-identical whichever CTA finishes last) and runs the epilogue.  No CTA ever
+//     waits for another, so the kernel is safe however many of its CTAs are resident (concurrent streams, PDL).
 #include "tc_common.cuh"
 
 namespace sps {
@@ -26,8 +32,11 @@ constexpr int BKC = 64;                 // channels per chunk
 constexpr int PROD_WARPS = 8;
 constexpr int THREADS3 = CONS_THREADS + PROD_WARPS * 32;   // 512: 16 warps split evenly over the register file
 constexpr int W_PROD = CONS_THREADS / 32;
-constexpr int CLUSTER = 2;              // CTAs per cluster (tap split for small layers)
-constexpr int SPLIT_TILES_MAX = 74;     // tiles of the scratch block (one per cluster: up to 148 CTAs per grid)
+constexpr int MAX_CTAS = 148;           // grid bound: deal table entries, workspace slots and counters
+// Chunks the deal must save on the layer's longest chain.  A hand-over costs about as much as several chunks at one
+// frame's layer sizes: on the bench's B=1 frames (H100 SXM, 700 W) the captured step was fastest at 14 of the
+// thresholds 0 - 18 tried; in practice the deal then serves the 64-channel layers that hold a 27-chunk tile.
+constexpr int DEAL_MIN_GAIN = 14;
 
 template <int BN>
 struct Cfg3 {
@@ -35,7 +44,10 @@ struct Cfg3 {
     static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
     static constexpr int STAGES = 4;
     static constexpr int NBR_TILE_BYTES = BM * 27 * 4;                    // one tile's rows of the [rows, 27] table
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * NBR_TILE_BYTES + 1024 + 512 + 256;
+    static constexpr int BAR_BYTES = 768;                                 // the mbarriers
+    // deal table: chunk prefix per tile [MAX_CTAS + 1], block-scan scratch [33], last-piece flags [2], longest tile
+    static constexpr int DEAL_INTS = MAX_CTAS + 1 + 33 + 2 + 1;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * NBR_TILE_BYTES + 1024 + BAR_BYTES + DEAL_INTS * 4;
 };
 
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
@@ -47,25 +59,15 @@ __device__ __forceinline__ void st_shared_zero16(uint32_t dst) {
 __device__ __forceinline__ void cp_async_arrive_noinc(uint32_t bar) {   // arrive when this thread's prior cp.async land
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
-// arrive (release, cluster scope) on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t rank) {
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
-        "}\n" ::"r"(bar), "r"(rank) : "memory");
+// barrier `id` (1, 2) over the 128 threads of one consumer warpgroup
+__device__ __forceinline__ void warpgroup_sync(int id) {
+    asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory");
 }
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {    // acquire at cluster scope
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "WAITC_LOOP:\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra.uni WAITC_DONE;\n\t"
-        "bra.uni WAITC_LOOP;\n\t"
-        "WAITC_DONE:\n\t"
-        "}\n" ::"r"(bar), "r"(parity) : "memory");
+// atomic add with release (the stores that precede it, through a barrier, included) and acquire semantics, gpu scope
+__device__ __forceinline__ int atomic_add_acq_rel(int* p, int v) {
+    int old;
+    asm volatile("atom.acq_rel.gpu.global.add.s32 %0, [%1], %2;" : "=r"(old) : "l"(p), "r"(v) : "memory");
+    return old;
 }
 
 struct Args {
@@ -80,36 +82,39 @@ struct Args {
     __half* out_split;      // [2][rows_cap][out_ch] or null
     size_t out_plane;
     float* out_f32;         // [rows_cap][out_f32_stride] or null
-    float* scratch;         // [SPLIT_TILES_MAX][128][BN] fp32 partial sums of the peer CTA (null: no tap split)
+    float* parts;           // [2 * MAX_CTAS][128][BN] fp32 partial sums of shared tiles, slot = (CTA, first / last
+                            // tile of its range)
+    int* arrivals;          // [MAX_CTAS][2] pieces of a shared tile done, per consumer warpgroup; zero between launches
+                            // (null: no chunk deal)
     int* counters;          // optional [2]: executed (tile, chunk) pairs, tiles (bench instrumentation)
     int cin, cout, taps, rows_cap, relu, out_ch, out_f32_stride;
 };
 
-// The chunks of one tile this CTA executes, identical in every role: chunk g is active when one of its taps is in the
-// tile's mask; with a tap split the active chunks are dealt out alternately to the two CTAs of the cluster.
-struct ChunkSet {
-    uint32_t mask;     // bit g = chunk g is executed by this CTA
-    __device__ __forceinline__ ChunkSet(uint32_t tap_mask, int tpg, int nchunks, int part, int nparts) {
-        uint32_t act = tap_mask;
-        if (tpg > 1) {
-            const uint32_t group = (1u << tpg) - 1u;
-            act = 0u;
-            for (int g = 0; g < nchunks; ++g)
-                if ((tap_mask >> (g * tpg)) & group) act |= 1u << g;
+// Chunk g of a tile is active when one of its `tpg` taps is in the tile's tap mask.
+__device__ __forceinline__ uint32_t active_chunks(uint32_t tap_mask, int tpg, int nchunks) {
+    if (tpg == 1) return tap_mask;
+    const uint32_t group = (1u << tpg) - 1u;
+    uint32_t act = 0u;
+    for (int g = 0; g < nchunks; ++g)
+        if ((tap_mask >> (g * tpg)) & group) act |= 1u << g;
+    return act;
+}
+
+// The active chunks of ranks [lo, hi) in the tile's walk order (chunk rot first, wrapping at nchunks).
+__device__ __forceinline__ uint32_t chunk_range(uint32_t act, int rot, int nchunks, int lo, int hi) {
+    uint32_t m = 0u;
+    for (int gi = 0, r = 0; gi < nchunks; ++gi) {
+        const int g = gi + rot < nchunks ? gi + rot : gi + rot - nchunks;
+        if ((act >> g) & 1u) {
+            if (r >= lo && r < hi) m |= 1u << g;
+            ++r;
         }
-        if (nparts == 1) { mask = act; return; }
-        uint32_t m = 0u, rest = act;          // deal the active chunks out alternately (nparts == 2)
-        for (int j = 0; rest; ++j) {
-            const uint32_t low = rest & (0u - rest);
-            if ((j & 1) == part) m |= low;
-            rest ^= low;
-        }
-        mask = m;
     }
-};
+    return m;
+}
 
 template <int TABLE, int BN>
-__global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) spconv_split_kernel(const Args p) {
+__global__ void __launch_bounds__(THREADS3, 1) spconv_split_kernel(const Args p) {
     using C = Cfg3<BN>;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -123,7 +128,10 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
     auto empty = [&](int s) { return bar_base + 8u * (3 * C::STAGES + s); };
     auto nbr_full = [&](int b) { return bar_base + 8u * (4 * C::STAGES + 4 + b); };
     auto nbr_empty = [&](int b) { return bar_base + 8u * (4 * C::STAGES + 6 + b); };
-    const uint32_t peer_done = bar_base + 8u * (4 * C::STAGES + 8);               // the peer's partial sums of my rows are in L2
+    int* deal_pre = (int*)(base_ptr + C::STAGES * C::STAGE_BYTES + 2 * C::NBR_TILE_BYTES + C::BAR_BYTES);
+    int* scan_smem = deal_pre + MAX_CTAS + 1;
+    int* last_flag = scan_smem + 33;
+    int* longest = last_flag + 2;             // the most active chunks of any tile
 
     pdl_launch_dependents();      // the next layer may be scheduled as this grid's CTAs retire
     // warp index through a shuffle: the compiler then knows it is warp-uniform
@@ -145,46 +153,81 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
             mbar_init(empty(s), 2);                      // one arrive per consumer warpgroup
         }
         for (int b = 0; b < 2; ++b) { mbar_init(nbr_full(b), 1); mbar_init(nbr_empty(b), PROD_WARPS); }
-        mbar_init(peer_done, 128);                       // the peer's giver warpgroup
         fence_barrier_init();
+        *longest = 0;
     }
-    __syncthreads();
-    cluster_sync_all();           // the peer's barriers exist before anyone arrives on them remotely
     pdl_wait();                   // producing layer / rulebook complete; nothing above touched global data
     const int M = p.d_rows ? min(__ldg(p.d_rows), p.rows_cap) : p.rows_cap;
     const int ntiles = (M + BM - 1) / BM;
-    // Work decomposition, uniform over the grid: R full rounds of one tile per CTA, then the remaining `rem` tiles.  A
-    // layer that has at most half as many tiles as there are CTAs (one frame at a time) runs as a TAP SPLIT: cluster q
-    // owns tile q and its two CTAs share that tile's chunks, so a 45-tile layer occupies 90 SMs with half the chunk
-    // chain each.  Splitting only the last partial round of a large layer does not pay: the hand-over at the very end
-    // of the kernel overlaps nothing.  Hence R == 0.
-    const uint32_t crank = cluster_ctarank();
     const int G = (int)gridDim.x;
-    const int R = ntiles / G, rem = ntiles - R * G;
-    const bool tail_split = TABLE && p.scratch && nchunks > 1 && R == 0 && rem > 0 && 2 * rem <= G &&
-                            rem <= SPLIT_TILES_MAX;
-    const int n_items = R + ((tail_split ? (int)(blockIdx.x >> 1) < rem : (int)blockIdx.x < rem) ? 1 : 0);
-    struct Item { int tile, part, nparts; };
-    auto item_at = [&](int i) {
-        Item it;
-        if (i < R) { it.tile = (int)blockIdx.x + i * G; it.part = 0; it.nparts = 1; }
-        else if (tail_split) { it.tile = R * G + (int)(blockIdx.x >> 1); it.part = (int)crank; it.nparts = 2; }
-        else { it.tile = R * G + (int)blockIdx.x; it.part = 0; it.nparts = 1; }
-        return it;
-    };
-    auto chunks_of = [&](const Item& it) {
+    auto active_of = [&](int tile) {
         uint32_t tm = all_taps;
         if (TABLE && p.tile_mask) {
-            tm = (uint32_t)__ldg(&p.tile_mask[it.tile]) & all_taps;
+            tm = (uint32_t)__ldg(&p.tile_mask[tile]) & all_taps;
             if (!tm) tm = 1u;       // a tile without any pair still has to produce act(shift): run one (all-zero) chunk
         }
-        return ChunkSet(tm, tpg, nchunks, it.part, it.nparts).mask;
+        return active_chunks(tm, tpg, nchunks);
     };
     // Every CTA streams the same weight chunks.  If they all walked the taps in the same order they would ask the
     // same few L2 lines for the same 16 KB at the same time; each tile therefore starts at a different tap
     // (rotation by a tile-dependent offset, identical in all roles; the sum over taps is order-independent up to fp32
     // rounding and deterministic per tile).
     auto rot_of = [&](int tile) { return (int)(((unsigned)tile * 11u) % (unsigned)nchunks); };
+    // Work decomposition, uniform over the grid.  Chunk deal (tiles <= CTAs): deal_pre[t] = active chunks of the tiles
+    // before t, S = all of them; CTA c < D = min(G, S) takes chunks [c S / D, (c + 1) S / D) of that list (at least
+    // one each, so every CTA that owns part of a tile has work in it).  Otherwise rounds of one tile per CTA.
+    const bool may_deal = TABLE && p.arrivals && ntiles > 0 && ntiles <= G;
+    if (may_deal) {               // block-uniform
+        const int t = (int)threadIdx.x, cnt = t < ntiles ? __popc(active_of(t)) : 0;
+        int total;
+        const int pre = sassd_block_exscan(cnt, scan_smem, &total);
+        if (t < ntiles) deal_pre[t] = pre;
+        if (t == 0) deal_pre[ntiles] = total;
+        const int wmax = __reduce_max_sync(0xffffffffu, cnt);
+        if (lane == 0) atomicMax(longest, wmax);
+    }
+    __syncthreads();              // barrier init and deal table visible to every thread
+    // The deal costs most CTAs a partial-sum hand-over.  It is taken when it shortens the layer's chain (one CTA per
+    // tile: the longest tile; dealt: ceil(S / G)) by at least DEAL_MIN_GAIN chunks.
+    const bool deal = may_deal && *longest - (deal_pre[ntiles] + G - 1) / G >= DEAL_MIN_GAIN;
+    const int S = deal ? deal_pre[ntiles] : 1, D = min(G, S);
+    const bool dealt = deal && (int)blockIdx.x < D;
+    const int s0 = dealt ? (int)blockIdx.x * S / D : 0;
+    const int s1 = dealt ? ((int)blockIdx.x + 1) * S / D : 0;
+    auto tile_of = [&](int k) {   // the tile holding chunk k of the list: the last t with deal_pre[t] <= k
+        int lo = 0, hi = ntiles - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (deal_pre[mid] <= k) lo = mid; else hi = mid - 1;
+        }
+        return lo;
+    };
+    auto owner_of = [&](int k) { return ((k + 1) * D - 1) / S; };     // the CTA whose range holds chunk k
+    const int t_first = s1 > s0 ? tile_of(s0) : 0;
+    const int R = ntiles / G;
+    const int n_items = deal ? (s1 > s0 ? tile_of(s1 - 1) - t_first + 1 : 0)
+                             : R + ((int)blockIdx.x < ntiles - R * G ? 1 : 0);
+    struct Item { int tile, lo, hi; };      // ranks [lo, hi) of the tile's active chunks in its walk order
+    auto item_at = [&](int i) {
+        Item it;
+        if (deal) {
+            it.tile = t_first + i;
+            const int b = deal_pre[it.tile];
+            it.lo = max(s0 - b, 0);
+            it.hi = min(s1, deal_pre[it.tile + 1]) - b;
+        } else {
+            it.tile = (int)blockIdx.x + i * G;
+            it.lo = 0;
+            it.hi = 32;
+        }
+        return it;
+    };
+    // the chunks of the item this CTA executes, identical in every role
+    auto chunks_of = [&](const Item& it) {
+        const uint32_t act = active_of(it.tile);
+        if (it.lo == 0 && it.hi >= __popc(act)) return act;
+        return chunk_range(act, rot_of(it.tile), nchunks, it.lo, it.hi);
+    };
 
     if (warp >= W_PROD) {
         // ===================== A producers: cp.async gather of split rows =====================
@@ -306,8 +349,7 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
         int executed = 0, tiles_done = 0;
         for (int ii = 0; ii < n_items; ++ii) {
             const Item item = item_at(ii);
-            const int tile = item.tile, part = item.part;
-            const bool split = item.nparts == 2;
+            const int tile = item.tile;
             const uint32_t cmask = chunks_of(item);
 #pragma unroll
             for (int i = 0; i < BN / 2; ++i) { big[i] = 0.f; small[i] = 0.f; }
@@ -337,18 +379,47 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
             fence_regs<BN / 2>(big);
             fence_regs<BN / 2>(small);
             if (prev >= 0 && t == 0) mbar_arrive(empty(prev));
-            if (part == 0) ++tiles_done;
-            // Tap split: the two CTAs hold partial sums of the SAME 128 rows.  Each finalises half of them - CTA 0
-            // rows 0..63 (warpgroup 0), CTA 1 rows 64..127 (warpgroup 1) - and its other warpgroup ("giver") hands
-            // the partial sums of the rows it does not own to the peer: fp32 values in an L2-resident scratch block
-            // at the positions of the (identical) register layout, then a remote mbarrier arrive (release / acquire
-            // at cluster scope).  Half the bytes cross, in both directions at once, and the epilogue work is shared.
-            const bool giver = split && wg != part;
-            const int rl0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);    // tile rows rl0 and rl0 + 8
-            float* prow = split ? p.scratch + (size_t)(tile - R * G) * BM * BN : nullptr;
-            if (split && !giver) {              // keeper: the peer's partial sums of my rows must be visible
-                mbar_wait_cluster(peer_done, 0u);
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) big[i] = __fadd_rn(big[i], small[i] * (1.f / kF16LoScale));
+            if (deal && (item.lo > 0 || item.hi < deal_pre[tile + 1] - deal_pre[tile])) {
+                // A tile shared by pieces of several CTAs: the CTAs owner_of(b) .. owner_of(e - 1) in that order.  A
+                // piece is the first tile of its CTA's range (slot 2c) unless it is the first piece and its CTA's range
+                // began in an earlier tile (slot 2c + 1, its last tile).  Each warpgroup reduces its own 64 rows.
+                const int b = deal_pre[tile], e = deal_pre[tile + 1];
+                const int first = owner_of(b), nparts = owner_of(e - 1) - first + 1;
+                const int part = (int)blockIdx.x - first;
+                auto slot = [&](int j) {                    // this thread's partial sums of piece j: float2 k at [128 k]
+                    const int c = first + j, s = 2 * c + ((j == 0 && c * S / D < b) ? 1 : 0);
+                    return (float2*)(p.parts + ((size_t)s * BM + wg * 64) * BN) + t;
+                };
+                float2* mine = slot(part);
+#pragma unroll
+                for (int k = 0; k < BN / 4; ++k) __stcg(mine + 128 * k, make_float2(big[2 * k], big[2 * k + 1]));
+                // The warpgroup's stores precede the count (barrier, then a release); a finishing piece reads the
+                // others' sums after its count (acquire, then barrier).
+                warpgroup_sync(1 + wg);
+                if (t == 0) {
+                    int* arrived = p.arrivals + 2 * tile + wg;
+                    const bool last = atomic_add_acq_rel(arrived, 1) == nparts - 1;
+                    if (last) *arrived = 0;                 // every piece has counted: ready for the next launch
+                    last_flag[wg] = last;
+                }
+                warpgroup_sync(1 + wg);
+                if (!last_flag[wg]) continue;               // another CTA finishes these rows
+                for (int j = 0; j < nparts; ++j) {          // fixed order: the same bits whoever finishes
+                    const float2* q = slot(j);
+#pragma unroll
+                    for (int k = 0; k < BN / 4; ++k) {
+                        const float2 v = j == part ? make_float2(big[2 * k], big[2 * k + 1]) : __ldcg(q + 128 * k);
+                        small[2 * k] = j == 0 ? v.x : __fadd_rn(small[2 * k], v.x);
+                        small[2 * k + 1] = j == 0 ? v.y : __fadd_rn(small[2 * k + 1], v.y);
+                    }
+                }
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) big[i] = small[i];
             }
+            ++tiles_done;                 // thread 0 (warpgroup 0) counts each tile once: in the CTA that finishes it
+            const int rl0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);    // tile rows rl0 and rl0 + 8
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
                 const int n = 8 * j + 2 * (t & 3);
@@ -358,21 +429,9 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
                 const float shl1 = (p.shift && n + 1 < p.cout) ? __ldg(&p.shift[n + 1]) : 0.f;
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
-                    const int rl = rl0 + 8 * i, m = tile * BM + rl;
-                    float a0 = __fadd_rn(big[4 * j + 2 * i], small[4 * j + 2 * i] * (1.f / kF16LoScale));
-                    float a1 = __fadd_rn(big[4 * j + 2 * i + 1], small[4 * j + 2 * i + 1] * (1.f / kF16LoScale));
-                    float2* q = split ? (float2*)(prow + (size_t)rl * BN + n) : nullptr;
-                    if (giver) {                    // hand the partial sums over, no epilogue for these rows here
-                        *q = make_float2(a0, a1);
-                        continue;
-                    }
-                    if (split) {
-                        const float2 pq = __ldcg(q);    // L2
-                        a0 = __fadd_rn(a0, pq.x);
-                        a1 = __fadd_rn(a1, pq.y);
-                    }
+                    const int m = tile * BM + rl0 + 8 * i;
                     // columns >= cout: zero weights, scale 1, shift 0 -> exactly 0
-                    float o0 = fmaf(a0, scl0, shl0), o1 = fmaf(a1, scl1, shl1);
+                    float o0 = fmaf(big[4 * j + 2 * i], scl0, shl0), o1 = fmaf(big[4 * j + 2 * i + 1], scl1, shl1);
                     if (p.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
                     if (m < M) {
                         if (p.out_f32 && n < p.out_f32_stride)
@@ -387,7 +446,6 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
                     }
                 }
             }
-            if (giver) mbar_arrive_remote(peer_done, (uint32_t)(part ^ 1));    // every thread releases its own stores
         }
         if (p.counters && threadIdx.x == 0 && executed) {
             atomicAdd(&p.counters[0], executed);
@@ -396,42 +454,30 @@ __global__ void __cluster_dims__(CLUSTER, 1, 1) __launch_bounds__(THREADS3, 1) s
     }
 
     __syncthreads();
-    cluster_sync_all();           // no CTA of the cluster exits while its peer may still arrive on its barriers
 }
 
+// max_work: CTAs the layer can keep busy at most (its tiles; with the chunk deal, its tiles' chunks)
 template <int TABLE, int BN>
-static int launch3(const Args& a, cudaStream_t stream) {
+static int launch3(const Args& a, int max_work, cudaStream_t stream) {
     using C = Cfg3<BN>;
     auto kern = spconv_split_kernel<TABLE, BN>;
-    // Persistent CTAs in clusters of two, one CTA per SM (~200 KB of shared memory): the grid must not exceed what is
-    // co-resident - GPCs with an odd number of free SMs cannot host a last cluster, and a cluster left over for a
-    // second wave would double the kernel's time.
-    static int max_ctas = 0;
-    if (!max_ctas) {
+    static bool smem_set = false;
+    if (!smem_set) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) != cudaSuccess)
             return SASSD_ERR_LAUNCH;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(CLUSTER * sassd_div_up(sassd_num_sms(), CLUSTER)); cfg.blockDim = dim3(THREADS3);
-        cfg.dynamicSmemBytes = C::SMEM_BYTES;
-        int clusters = 0;
-        if (cudaOccupancyMaxActiveClusters(&clusters, kern, &cfg) != cudaSuccess || clusters < 1) {
-            cudaGetLastError();
-            clusters = sassd_num_sms() / (2 * CLUSTER);
-        }
-        max_ctas = CLUSTER * (clusters < SPLIT_TILES_MAX ? clusters : SPLIT_TILES_MAX);
+        smem_set = true;
     }
-    // one CTA per tile up to the resident CTAs; with a tap split two CTAs per tile; always whole clusters
-    int grid = CLUSTER * sassd_div_up(a.rows_cap, BM);
-    if (grid > max_ctas) grid = max_ctas;
+    // persistent CTAs, one per SM (~220 KB of shared memory each)
+    const int grid = min(max_work, min(sassd_num_sms(), MAX_CTAS));
     if (launch_pdl(kern, dim3(grid), dim3(THREADS3), C::SMEM_BYTES, stream, a) != cudaSuccess) return SASSD_ERR_LAUNCH;
     return sassd_check_launch();
 }
 
 template <int TABLE>
-static int dispatch3(const Args& a, cudaStream_t s) {
-    if (a.cout <= 16) return launch3<TABLE, 16>(a, s);
-    if (a.cout <= 32) return launch3<TABLE, 32>(a, s);
-    if (a.cout <= 64) return launch3<TABLE, 64>(a, s);
+static int dispatch3(const Args& a, int max_work, cudaStream_t s) {
+    if (a.cout <= 16) return launch3<TABLE, 16>(a, max_work, s);
+    if (a.cout <= 32) return launch3<TABLE, 32>(a, max_work, s);
+    if (a.cout <= 64) return launch3<TABLE, 64>(a, max_work, s);
     return SASSD_ERR_UNSUPPORTED;
 }
 
@@ -478,9 +524,12 @@ extern "C" int sassd_spconv_pack(const float* weight, int taps, int cin, int cin
     return sassd_check_launch();
 }
 
+// chunk deal: fp32 partial sums, two slots (first / last tile) of 128 rows x 64 columns per CTA, then the per-tile,
+// per-warpgroup piece counters
+static size_t spconv_parts_bytes() { return (size_t)2 * sps::MAX_CTAS * sps::BM * 64 * sizeof(float); }
+
 extern "C" size_t sassd_spconv_workspace_bytes(void) {
-    // fp32 partial sums of the peer CTA for the tap split: SPLIT_TILES_MAX tiles x 128 rows x 64 columns
-    return (size_t)sps::SPLIT_TILES_MAX * sps::BM * 64 * sizeof(float);
+    return spconv_parts_bytes() + (size_t)sps::MAX_CTAS * 2 * sizeof(int32_t);
 }
 
 extern "C" int sassd_spconv_f16x3(const sassd_spconv_desc* d, const void* in_split, const void* wpack,
@@ -500,10 +549,14 @@ extern "C" int sassd_spconv_f16x3(const sassd_spconv_desc* d, const void* in_spl
     a.in = (const __half*)in_split; a.in_plane = (size_t)d->in_rows_cap * d->cin;
     a.wpack = wpack; a.scale = scale; a.shift = shift; a.nbr = nbr; a.tile_mask = tile_mask; a.d_rows = d_rows;
     a.out_split = (__half*)out_split; a.out_plane = (size_t)d->rows_cap * d->out_ch; a.out_f32 = out_f32;
-    a.scratch = (float*)ws; a.counters = counters;
+    a.parts = (float*)ws;
+    a.arrivals = ws ? (int*)((char*)ws + spconv_parts_bytes()) : nullptr;
+    a.counters = counters;
     a.cin = d->cin; a.cout = d->cout; a.taps = d->taps; a.rows_cap = d->rows_cap; a.relu = d->relu;
     a.out_ch = d->out_ch; a.out_f32_stride = d->out_f32_stride;
-    return d->taps > 1 ? sps::dispatch3<1>(a, (cudaStream_t)stream_) : sps::dispatch3<0>(a, (cudaStream_t)stream_);
+    const int tiles = sassd_div_up(d->rows_cap, sps::BM), tpg = spconv_tpg(d->cin);
+    if (d->taps == 1) return sps::dispatch3<0>(a, tiles, (cudaStream_t)stream_);
+    return sps::dispatch3<1>(a, ws ? tiles * ((d->taps + tpg - 1) / tpg) : tiles, (cudaStream_t)stream_);
 }
 
 // fp32 rows [rows, cin] -> split rows [2][rows_cap][cs] (cs >= cin, multiple of 8; padding channels zero)

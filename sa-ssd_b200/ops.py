@@ -82,10 +82,11 @@ class Workspace:
     def __init__(self):
         self._bufs = {}
 
-    def get(self, key, nbytes, device):
+    def get(self, key, nbytes, device, zeroed=False):
+        """zeroed: a new buffer starts zero-filled (for kernels that keep counters in it and leave them zero)."""
         buf = self._bufs.get(key)
         if buf is None or buf.numel() < nbytes or buf.device != device:
-            buf = torch.empty(max(int(nbytes), 256), dtype=torch.uint8, device=device)
+            buf = (torch.zeros if zeroed else torch.empty)(max(int(nbytes), 256), dtype=torch.uint8, device=device)
             self._bufs[key] = buf
         return buf
 
@@ -735,7 +736,7 @@ def split_rows_float(planes, channels):
 
 SPCONV_COUNTERS = None     # bench instrumentation: int32[2] device tensor -> += executed (tile, chunk) pairs, += tiles
 SPCONV_TAP_SKIP = os.environ.get("SASSD_SPS_SKIP", "1") != "0"      # use the rulebook's tile masks
-SPCONV_TAP_SPLIT = os.environ.get("SASSD_SPS_SPLIT", "1") != "0"    # cluster tap split for layers with few tiles
+SPCONV_TAP_SPLIT = os.environ.get("SASSD_SPS_SPLIT", "1") != "0"    # chunk deal over all SMs for layers with few tiles
 
 
 def spconv_split(planes, weight, scale, shift, relu, cout, rows_cap, nbr=None, d_rows=None, want_f32=False,
@@ -756,7 +757,7 @@ def spconv_split(planes, weight, scale, shift, relu, cout, rows_cap, nbr=None, d
     label = "spconv_split[taps=%d %d->%d]" % (taps, weight.shape[1], cout)
     w = None
     if SPCONV_TAP_SPLIT and taps > 1:
-        w = (ws or _WS).get("spconv_split", _L().sassd_spconv_workspace_bytes(), planes.device)
+        w = (ws or _WS).get("spconv_split", _L().sassd_spconv_workspace_bytes(), planes.device, zeroed=True)
     _call("sassd_spconv_f16x3", label, ctypes.byref(d), _ptr(planes), _ptr(wp), _ptr(scale), _ptr(shift), _ptr(nbr),
           _ptr(tile_mask if SPCONV_TAP_SKIP else None), _ptr(d_rows), _ptr(out), _ptr(of), _ptr(w),
           0 if w is None else w.numel(), _ptr(SPCONV_COUNTERS), _stream())
