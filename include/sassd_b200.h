@@ -117,6 +117,26 @@ int sassd_frustum_crop(const float* points, const int32_t* d_pt_off, int n_point
                        void* ws, size_t ws_bytes, sassd_stream_t stream);
 
 /* ------------------------------------------------------------------------
+ * Image-FOV crop of full sweeps: the reference's raw-drive dataset
+ * (KittiVideo, mmdet/datasets/kitti.py:394) crops every sweep with
+ * get_lidar_in_image_fov(points, calib, 0, 0, w, h, clip_distance=0.1)
+ * (mmdet/datasets/kitti_utils.py:252-263).
+ *
+ * points / d_pt_off as for sassd_frustum_crop; meta [batch][SASSD_KITTI_META]
+ * fp64 is the per-frame block of sassd_kitti_format (P2, Tr_velo_to_cam,
+ * R0_rect, img_h, img_w).  Per point, in fp64 from the widened x, y, z:
+ * ref = [x,y,z,1] V2C^T, rect = ref R0^T, uvw = [rect,1] P2^T, every dot
+ * product a sequential FMA chain from k = 0; u = uvw0/uvw2, v = uvw1/uvw2
+ * (IEEE division).  Kept when u < img_w && u >= 0 && v < img_h && v >= 0
+ * && x > clip_x (fp32 comparison); a NaN coordinate drops the point.
+ * Compaction, outputs, workspace (sassd_frustum_crop_workspace_bytes),
+ * argument checks and error codes are those of sassd_frustum_crop.
+ * ---------------------------------------------------------------------- */
+int sassd_image_fov_crop(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch,
+                         const double* meta, float clip_x, float* points_out, int32_t* d_pt_off_out,
+                         void* ws, size_t ws_bytes, sassd_stream_t stream);
+
+/* ------------------------------------------------------------------------
  * anchors_mask.  Replaces mmdet/datasets/kitti.py:333-343 +
  * mmdet/core/bbox3d/geometry.py:675-709 (occupancy count, two cumsums,
  * integral-image lookup, `> threshold`).  rects [n_anchors,4] int32 are the

@@ -1,10 +1,20 @@
-// Camera-frustum crop of full LiDAR sweeps: the device side of the reference's offline reduced-cloud step
-// (tools/create_data.py:107-140 -> remove_outside_points, mmdet/core/bbox3d/geometry.py:50-61).
+// Crops of full LiDAR sweeps, compacted in point order: the camera-frustum crop is the device side of the reference's
+// offline reduced-cloud step (tools/create_data.py:107-140 -> remove_outside_points, mmdet/core/bbox3d/geometry.py:50-61);
+// the image-FOV crop is what its raw-drive dataset applies to every sweep (KittiVideo, mmdet/datasets/kitti.py:394 ->
+// get_lidar_in_image_fov, mmdet/datasets/kitti_utils.py:252-263).  One compaction kernel, templated on the keep test.
 //
-// Keep test: points_in_convex_polygon_3d_jit (geometry.py:190-222) for one polygon of 6 faces.  The fp32 coordinates
+// Frustum keep test: points_in_convex_polygon_3d_jit (geometry.py:190-222) for one polygon of 6 faces.  The fp32 coordinates
 // are widened to fp64 and s = ((x*n0 + y*n1) + z*n2) + d is evaluated in exactly that order, every operation rounded on
 // its own (__dmul_rn / __dadd_rn, no FMA contraction), so the selection is the reference's bit for bit.  `s >= 0`
 // rejects, so a NaN coordinate keeps the point, as there.
+//
+// Image-FOV keep test: the point projected into image 2 through the frame's meta block (results.meta_block: P2,
+// Tr_velo_to_cam, R0_rect, img_h, img_w).  x, y, z are widened to fp64; ref = [x,y,z,1] V2C^T, rect = ref R0^T,
+// uvw = [rect,1] P2^T, each dot product a sequential FMA chain from k = 0, fma(a3,b3, fma(a2,b2, fma(a1,b1, a0*b0))),
+// which is the order numpy's fp64 matmul takes for these shapes (oracle/image_fov.py restates it; the fixture's
+// generator checks the two agree on every row).  u = uvw0/uvw2 and v = uvw1/uvw2 are IEEE divisions; the point is kept
+// when u < w && u >= 0 && v < h && v >= 0 && x > clip_x, the last comparison in fp32 as numpy makes it on the float32
+// cloud.  A NaN coordinate fails every comparison and drops the point; uvw2 <= 0 divides as IEEE says.
 //
 // One pass over the concatenated frames: FC_CHUNK points per CTA as FC_ROWS rows of FC_THREADS consecutive points
 // (one point per thread and row: coalesced 16-byte loads), warp ballots ranked by a scan of the chunk's (row, warp)
@@ -33,10 +43,41 @@ __device__ __forceinline__ bool fc_inside(float4 p, const double* __restrict__ p
     return in;
 }
 
+struct FrustumKeep {
+    const double* __restrict__ planes;    // [batch][6][4]
+    __device__ __forceinline__ bool operator()(float4 p, int frame) const { return fc_inside(p, planes + (size_t)frame * 24); }
+};
+
+// a0*b[0] + a1*b[1] + a2*b[2] (+ b[3] when `affine`): a sequential FMA chain from k = 0
+template <bool affine>
+__device__ __forceinline__ double fov_dot(double a0, double a1, double a2, const double* __restrict__ b) {
+    double acc = __fma_rn(a2, __ldg(&b[2]), __fma_rn(a1, __ldg(&b[1]), __dmul_rn(a0, __ldg(&b[0]))));
+    if (affine) acc = __fma_rn(1.0, __ldg(&b[3]), acc);
+    return acc;
+}
+
+struct ImageFovKeep {
+    const double* __restrict__ meta;      // [batch][SASSD_KITTI_META]: P2 (12), Tr_velo_to_cam (12), R0_rect (9), h, w
+    float clip_x;
+    __device__ __forceinline__ bool operator()(float4 p, int frame) const {
+        const double* m = meta + (size_t)frame * SASSD_KITTI_META;
+        const double x = p.x, y = p.y, z = p.z;
+        const double r0 = fov_dot<true>(x, y, z, m + 12), r1 = fov_dot<true>(x, y, z, m + 16),
+                     r2 = fov_dot<true>(x, y, z, m + 20);
+        const double c0 = fov_dot<false>(r0, r1, r2, m + 24), c1 = fov_dot<false>(r0, r1, r2, m + 27),
+                     c2 = fov_dot<false>(r0, r1, r2, m + 30);
+        const double w0 = fov_dot<true>(c0, c1, c2, m), w1 = fov_dot<true>(c0, c1, c2, m + 4),
+                     w2 = fov_dot<true>(c0, c1, c2, m + 8);
+        const double u = __ddiv_rn(w0, w2), v = __ddiv_rn(w1, w2);
+        const double h = __ldg(&m[33]), w = __ldg(&m[34]);
+        return u < w && u >= 0.0 && v < h && v >= 0.0 && p.x > clip_x;
+    }
+};
+
+template <class Keep>
 __global__ void __launch_bounds__(FC_THREADS)
-frustum_crop_kernel(const float4* __restrict__ points, const int* __restrict__ pt_off, int n_cap, int batch,
-                    const double* __restrict__ planes, float4* __restrict__ out, int* __restrict__ off_out,
-                    unsigned long long* __restrict__ desc) {
+crop_kernel(const float4* __restrict__ points, const int* __restrict__ pt_off, int n_cap, int batch, Keep inside,
+            float4* __restrict__ out, int* __restrict__ off_out, unsigned long long* __restrict__ desc) {
     __shared__ int s_off[FC_MAX_BATCH + 1];
     __shared__ unsigned s_ball[FC_ROWS * FC_WARPS];   // (row, warp) order = point order
     __shared__ int s_ex[FC_ROWS * FC_WARPS];
@@ -60,7 +101,7 @@ frustum_crop_kernel(const float4* __restrict__ points, const int* __restrict__ p
 #pragma unroll
     for (int j = 0; j < FC_ROWS; ++j) {
         const int i = c0 + j * FC_THREADS + (int)threadIdx.x;
-        if (i < n && fc_inside(p[j], planes + (size_t)sassd_frame_of(s_off, batch, i) * 24)) keep |= 1u << j;
+        if (i < n && inside(p[j], sassd_frame_of(s_off, batch, i))) keep |= 1u << j;
     }
 #pragma unroll
     for (int j = 0; j < FC_ROWS; ++j) {
@@ -119,17 +160,33 @@ extern "C" size_t sassd_frustum_crop_workspace_bytes(int n_points_cap, int batch
     return (size_t)fc_chunks(n_points_cap) * sizeof(unsigned long long);
 }
 
-extern "C" int sassd_frustum_crop(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch,
-                                  const double* planes, float* points_out, int32_t* d_pt_off_out, void* ws,
-                                  size_t ws_bytes, sassd_stream_t stream_) {
+// argument checks shared by both crops; then the descriptor reset and the one launch
+template <class Keep>
+static int crop_launch(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch, const double* params,
+                       Keep inside, float* points_out, int32_t* d_pt_off_out, void* ws, size_t ws_bytes,
+                       sassd_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
-    if (!points || !d_pt_off || !planes || !points_out || !d_pt_off_out || !ws) return SASSD_ERR_ARG;
+    if (!points || !d_pt_off || !params || !points_out || !d_pt_off_out || !ws) return SASSD_ERR_ARG;
     if (batch < 1 || batch > FC_MAX_BATCH || n_points_cap < 0) return SASSD_ERR_ARG;
     if (points == points_out) return SASSD_ERR_ARG;     // a chunk's output rows may hold a later chunk's input rows
     if (ws_bytes < sassd_frustum_crop_workspace_bytes(n_points_cap, batch)) return SASSD_ERR_WORKSPACE;
     const int chunks = fc_chunks(n_points_cap);
     cudaMemsetAsync(ws, 0, (size_t)chunks * sizeof(unsigned long long), stream);   // descriptors: nothing published
-    frustum_crop_kernel<<<chunks, FC_THREADS, 0, stream>>>((const float4*)points, d_pt_off, n_points_cap, batch, planes,
-                                                           (float4*)points_out, d_pt_off_out, (unsigned long long*)ws);
+    crop_kernel<<<chunks, FC_THREADS, 0, stream>>>((const float4*)points, d_pt_off, n_points_cap, batch, inside,
+                                                   (float4*)points_out, d_pt_off_out, (unsigned long long*)ws);
     return sassd_check_launch();
+}
+
+extern "C" int sassd_frustum_crop(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch,
+                                  const double* planes, float* points_out, int32_t* d_pt_off_out, void* ws,
+                                  size_t ws_bytes, sassd_stream_t stream) {
+    return crop_launch(points, d_pt_off, n_points_cap, batch, planes, FrustumKeep{planes}, points_out, d_pt_off_out, ws,
+                       ws_bytes, stream);
+}
+
+extern "C" int sassd_image_fov_crop(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch,
+                                    const double* meta, float clip_x, float* points_out, int32_t* d_pt_off_out,
+                                    void* ws, size_t ws_bytes, sassd_stream_t stream) {
+    return crop_launch(points, d_pt_off, n_points_cap, batch, meta, ImageFovKeep{meta, clip_x}, points_out,
+                       d_pt_off_out, ws, ws_bytes, stream);
 }

@@ -9,7 +9,8 @@ Two entry points:
     one H2D copy, voxelize + anchors_mask + backbone + neck + heads + PSWarp + NMS with
     every data-dependent size kept on the device, one D2H copy of the fixed-size result.
     With ``frustum_planes`` the frames are full sweeps, cropped to the camera frustum on the
-    device first (the reference crops them offline into ``velodyne_reduced``).  With ``metas``
+    device first (the reference crops them offline into ``velodyne_reduced``); with ``image_fov`` they are raw-drive
+    sweeps, cropped on the device to the points that project into the image (the reference's KittiVideo).  With ``metas``
     the step also formats its detections as KITTI annotations on the device (ops.kitti_format).  With
     ``point_outputs`` it also returns the auxiliary network's per-voxel foreground logits and centre offsets.
   * ``forward(..., return_loss=True)`` / ``forward_train`` and ``loss_points`` — the training losses, forward only, in
@@ -23,6 +24,10 @@ from torch import nn
 from . import builder, ops
 from .results import annos_from_rows, meta_block
 from .single_stage_heads import split_detections, unpack_detections
+
+# The crop a step runs before voxelizing: the first element of a captured-graph key.  0 and 1 equal False and True, so
+# a key reads (crop, kitti, point_outputs) with the frustum crop as True.
+CROP_NONE, CROP_FRUSTUM, CROP_IMAGE_FOV = 0, 1, 2
 
 
 class SingleStageDetector(nn.Module):
@@ -45,7 +50,7 @@ class SingleStageDetector(nn.Module):
         self.anchor_set = None
         self._pinned = None
         self._mask_stream = None
-        self._graphs = {}                 # (crop, kitti, point_outputs) -> captured single step (enable_cuda_graph)
+        self._graphs = {}                 # (crop kind, kitti, point_outputs) -> captured step (enable_cuda_graph)
         self._graph_args = None
         self._stream_slots = None
         self._stream_key = None
@@ -227,13 +232,13 @@ class SingleStageDetector(nn.Module):
         """Capture forward_device once for (batch, max_points_per_frame) and replay it per step: every
         data-dependent size already lives on the device, so the ~65 launches of a step become one graph
         launch.  Steps whose shape does not fit fall back to the eager path.  forward_points replays one graph per kind
-        of call: with or without ``frustum_planes`` (the graph crops the full sweeps first, and ``max_points_per_frame``
-        bounds them, e.g. 131072), ``metas`` (it ends with the KITTI result formatter) and ``point_outputs`` (it also
-        runs the auxiliary network).  The plain kind is captured here and returned, the others on their first use; a
+        of call: with ``frustum_planes``, with ``image_fov`` or without a crop (a cropping graph crops the full sweeps
+        first, and ``max_points_per_frame`` bounds them, e.g. 131072), ``metas`` (it ends with the KITTI result
+        formatter) and ``point_outputs`` (it also runs the auxiliary network).  The plain kind is captured here and returned, the others on their first use; a
         new call replaces every graph captured for an earlier shape."""
         self._graph_args = (int(batch), int(max_points_per_frame))
         self._graphs = {}
-        return self._graph_for(False, False, False)
+        return self._graph_for(CROP_NONE, False, False)
 
     def disable_cuda_graph(self):
         self._graphs = {}
@@ -242,14 +247,14 @@ class SingleStageDetector(nn.Module):
     def _graph_for(self, crop, kitti, point_outputs):
         """The captured single step of this kind at enable_cuda_graph's shape, captured on first use; None while the
         graphs are disabled."""
-        key = (crop, kitti, point_outputs)
+        key = (int(crop), kitti, point_outputs)
         if key not in self._graphs and self._graph_args is not None:
             self._graphs[key] = _GraphedStep(self, *self._graph_args, latency=True, crop=crop, kitti=kitti,
                                              point_outputs=point_outputs)
         return self._graphs.get(key)
 
     def detect_stream(self, batches, batch, max_points_per_frame=32768, depth=4, concurrent=True, crop=False,
-                      kitti=False):
+                      kitti=False, image_fov=False):
         """Throughput API: iterate over batches (each a list of ``batch`` raw point arrays) and yield their
         detections in order.  ``depth`` captured graphs with their own static buffers and scratch are used
         round-robin: while the GPU runs step i, the host stages and uploads step i+1 (copy stream) and unpacks
@@ -260,13 +265,17 @@ class SingleStageDetector(nn.Module):
         ``max_points_per_frame`` bounds the full sweeps.
         With ``kitti`` each item also carries the frames' ``img_meta``-style dicts (forward_points' ``metas``):
         (points_list, planes, metas) with ``crop``, else (points_list, metas); every slot's graph ends with the KITTI
-        result formatter and each yield is the batch's annotation dicts (kitti_bbox2results' format)."""
+        result formatter and each yield is the batch's annotation dicts (kitti_bbox2results' format).
+        With ``image_fov`` (needs ``kitti``, excludes ``crop``) the items are (points_list, metas) of raw-drive sweeps:
+        every slot's graph first crops each frame to the points that project into its image (forward_points'
+        ``image_fov``)."""
         ops.require_cuda()
         if kitti and self.class_names is None:
             raise ValueError("detect_stream(kitti=True) needs class_names")
-        key = (batch, max_points_per_frame, depth, bool(crop), bool(kitti))
+        kind = _crop_kind(bool(crop), image_fov, kitti)
+        key = (batch, max_points_per_frame, depth, kind, bool(kitti))
         if self._stream_key != key or self._stream_slots is None:
-            self._stream_slots = [_GraphedStep(self, batch, max_points_per_frame, crop=crop, kitti=kitti)
+            self._stream_slots = [_GraphedStep(self, batch, max_points_per_frame, crop=kind, kitti=kitti)
                                   for _ in range(depth)]
             self._copy_stream = torch.cuda.Stream()
             self._stream_key = key
@@ -300,7 +309,8 @@ class SingleStageDetector(nn.Module):
             return annos_from_rows(*out, self.class_names, [m["sample_idx"] for m in metas])
         return [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(*out)]
 
-    def forward_points(self, points_list, return_aux=False, frustum_planes=None, metas=None, point_outputs=False):
+    def forward_points(self, points_list, return_aux=False, frustum_planes=None, metas=None, point_outputs=False,
+                       image_fov=False):
         """Raw points in (list of [N_i,>=4] numpy arrays), detections out: per frame a dict of
         boxes_lidar [D,7], scores [D], label_preds [D] (or None entries when nothing survives).
         ``frustum_planes``: one float64 [6,4] array per frame (frustum.camera_frustum_planes).  The frames are then
@@ -313,24 +323,29 @@ class SingleStageDetector(nn.Module):
         ``point_outputs``: the step also runs SA-SSD's auxiliary network (neck.point_head) and the call returns
         (results, points), results as without it and ``points`` one dict per frame of xyz [V,3] (the voxel means),
         cls [V] (foreground logits) and reg [V,3] (offsets to the box centre), V the frame's voxels in voxel-row order.
-        With ``return_aux`` the aux dict comes third."""
+        With ``return_aux`` the aux dict comes third.
+        ``image_fov``: the frames are raw-drive sweeps; each is cropped on the device, in point order, to the points
+        that project into its image and lie in front of x = 0.1 m (ops.image_fov_crop), as the reference's KittiVideo
+        crops them (get_lidar_in_image_fov).  Needs ``metas``, whose calibration and image shape define the crop, and
+        excludes ``frustum_planes``."""
         ops.require_cuda()
         if self.voxel_generator is None or self.anchor_set is None:
             raise RuntimeError("call attach_data_pipeline(voxel_generator, anchor_set) first")
         if metas is not None and self.class_names is None:
             raise ValueError("forward_points(metas=) needs class_names")
+        kind = _crop_kind(frustum_planes is not None, image_fov, metas is not None)
         B = len(points_list)
         planes = None if frustum_planes is None else _frame_planes(frustum_planes, B)
         meta = None if metas is None else _meta_blocks(metas, B)
         hp, ho, counts = self.stage_points(points_list)
-        g = self._graph_for(planes is not None, meta is not None, bool(point_outputs))
+        g = self._graph_for(kind, meta is not None, bool(point_outputs))
         if g is not None and not return_aux and g.fits(B, counts):
             res = self._frame_results(g.run_host(hp, ho, sum(counts), planes, meta), metas)
             return (res, g.point_results()) if point_outputs else res
         dev = next(self.parameters()).device
         det, d_ndet, status, aux = _run_step(self, hp.to(dev, non_blocking=True), ho.to(dev, non_blocking=True), B,
                                              max(counts + [1]), _to_device(planes, dev), _to_device(meta, dev),
-                                             point_outputs=point_outputs)
+                                             point_outputs=point_outputs, image_fov=kind == CROP_IMAGE_FOV)
         if meta is not None:
             ops._lib.raise_on_status(status)
             out = aux["rows"].cpu().numpy(), aux["n_out"].cpu().numpy()
@@ -429,6 +444,16 @@ def _split_points(points_mean, cls, reg, frame_rows):
     return out
 
 
+def _crop_kind(frustum, image_fov, kitti):
+    """The crop kind of a step from its arguments; the image-FOV crop reads the frames' meta blocks, so it needs them."""
+    if image_fov and frustum:
+        raise ValueError("image_fov and a frustum crop exclude each other: a frame is cropped once")
+    if image_fov and not kitti:
+        raise ValueError("image_fov needs metas (kitti=True for detect_stream): the crop reads each frame's calibration "
+                         "and image shape")
+    return CROP_IMAGE_FOV if image_fov else CROP_FRUSTUM if frustum else CROP_NONE
+
+
 def _frame_planes(frustum_planes, batch):
     """One [6,4] plane set per frame -> contiguous float64 [batch,6,4]."""
     planes = np.ascontiguousarray(np.asarray(frustum_planes, dtype=np.float64))
@@ -450,13 +475,16 @@ def _to_device(a, dev):
 
 
 def _run_step(model, points, pt_off, batch, maxpts, planes=None, meta=None, point_outputs=False, detections=True,
-              guided_thr=None):
+              guided_thr=None, image_fov=False):
     """One detector step on the device, no synchronisation; the eager calls and every captured graph build their step
     here.  With ``planes`` [batch,6,4] the frames are full sweeps, cropped to their camera frustums first
-    (ops.frustum_crop); then forward_device; with ``meta`` [batch,36] the detections are formatted as KITTI rows
-    (ops.kitti_format) into aux["rows"] / aux["n_out"].  Returns forward_device's (det, d_ndet, status, aux)."""
+    (ops.frustum_crop); with ``image_fov`` they are cropped to their images through ``meta`` (ops.image_fov_crop); then
+    forward_device; with ``meta`` [batch,36] the detections are formatted as KITTI rows (ops.kitti_format) into
+    aux["rows"] / aux["n_out"].  Returns forward_device's (det, d_ndet, status, aux)."""
     if planes is not None:
         points, pt_off = ops.frustum_crop(points, pt_off, batch, planes)
+    elif image_fov:
+        points, pt_off = ops.image_fov_crop(points, pt_off, batch, meta)
     det, d_ndet, status, aux = model.forward_device(points, pt_off, batch, maxpts, point_outputs=point_outputs,
                                                     detections=detections, guided_thr=guided_thr)
     if meta is not None:
@@ -490,8 +518,10 @@ class _GraphedStep:
         """latency=True: this step will run alone on the GPU (enable_cuda_graph / forward_points): the dense convs walk
         the computed tiles first so that the constant-region tiles shorten every layer; False (detect_stream slots,
         several steps in flight): round-robin tiles, the SMs a layer leaves idle serve the other steps.
-        crop=True: the static points are full sweeps and the graph crops them to the frustums given by the static
-        planes [batch,6,4] (ops.frustum_crop) before the step; the cropped frames never exceed the full ones.
+        crop: the crop kind.  CROP_FRUSTUM (or True): the static points are full sweeps and the graph crops them to the
+        frustums given by the static planes [batch,6,4] (ops.frustum_crop) before the step; CROP_IMAGE_FOV (needs
+        ``kitti``): the graph crops them to the images of the static meta blocks (ops.image_fov_crop).  The cropped
+        frames never exceed the full ones.
         kitti=True: the graph ends with the KITTI result formatter (ops.kitti_format) on the static meta blocks
         [batch,36]; the host copy is its rows and counts instead of the detections.
         point_outputs=True: the step also runs the auxiliary network and copies its outputs and the frame row offsets to
@@ -499,11 +529,12 @@ class _GraphedStep:
         dev = next(model.parameters()).device
         self.model, self.batch, self.maxpts = model, int(batch), int(max_points_per_frame)
         self.cap = self.batch * self.maxpts
-        self.crop, self.kitti, self.point_outputs = bool(crop), bool(kitti), bool(point_outputs)
+        self.crop, self.kitti, self.point_outputs = int(crop), bool(kitti), bool(point_outputs)
+        _crop_kind(self.crop == CROP_FRUSTUM, self.crop == CROP_IMAGE_FOV, self.kitti)
         self.points = torch.zeros((self.cap, 4), dtype=torch.float32, device=dev)
         self.pt_off = torch.zeros((self.batch + 1,), dtype=torch.int32, device=dev)
         self.planes = self.meta = None
-        if self.crop:
+        if self.crop == CROP_FRUSTUM:
             self.planes = torch.zeros((self.batch, 6, 4), dtype=torch.float64, device=dev)
         if self.kitti:
             self.meta = torch.zeros((self.batch, ops._lib.KITTI_META), dtype=torch.float64, device=dev)
@@ -545,14 +576,14 @@ class _GraphedStep:
                           for k in _POINT_KEYS}
         self.h_status = torch.empty((1,), dtype=torch.int32, pin_memory=True)
         self.h_points, self.h_off = _pinned_pair(self.cap, self.batch + 1)
-        if self.crop:
+        if self.crop == CROP_FRUSTUM:
             self.h_planes = torch.empty((self.batch, 6, 4), dtype=torch.float64, pin_memory=True)
         self.done = torch.cuda.Event()
         self.loaded = torch.cuda.Event()
 
     def _step(self):
         return _run_step(self.model, self.points, self.pt_off, self.batch, self.maxpts, self.planes, self.meta,
-                         point_outputs=self.point_outputs)
+                         point_outputs=self.point_outputs, image_fov=self.crop == CROP_IMAGE_FOV)
 
     def fits(self, batch, counts):
         return batch == self.batch and max(counts + [0]) <= self.maxpts
@@ -579,7 +610,7 @@ class _GraphedStep:
         the pinned offsets ``ho`` and, for a crop / formatting step, the numpy planes / meta blocks."""
         self.points[:total].copy_(hp[:total], non_blocking=True)
         self.pt_off.copy_(ho, non_blocking=True)
-        if self.crop:
+        if self.crop == CROP_FRUSTUM:
             self.h_planes.numpy()[...] = planes
             self.planes.copy_(self.h_planes, non_blocking=True)
         if self.kitti:

@@ -1,7 +1,7 @@
-"""Reading a KITTI object split from disk for evaluation (host side of ``python -m sassd_b200.test``).
+"""Reading KITTI data from disk for detection and evaluation (host side of ``python -m sassd_b200.test``).
 
-Layout (the reference's ``data/kitti``): ``ImageSets/<split>.txt`` lists the frame ids; every frame's files are under
-``training/`` (``testing/`` has no labels):
+Object splits (KittiSplit; the reference's ``data/kitti``): ``ImageSets/<split>.txt`` lists the frame ids; every
+frame's files are under ``training/``, or ``testing/`` for the split ``test`` (which has no labels):
   * ``velodyne/%06d.bin`` full sweeps (cropped to the camera frustum on the device) or ``velodyne_reduced/%06d.bin``
     (cropped offline), float32 (x, y, z, reflectance) rows;
   * ``calib/%06d.txt`` (results.Calibration);
@@ -9,6 +9,11 @@ Layout (the reference's ``data/kitti``): ``ImageSets/<split>.txt`` lists the fra
     alone (mmdet/datasets/kitti.py:270-272), and KITTI image sizes vary (375x1242, 370x1224, 376x1241, ...);
   * ``label_2/%06d.txt``, read into ground-truth annotations with the semantics of the reference's
     get_label_anno / get_label_annos (tools/kitti_common.py:560-601, 648-666).
+
+Raw drives (KittiDrive; the reference's KittiVideo, mmdet/datasets/kitti.py:356-399): a ``*_sync`` directory with
+``image_02/data/%010d.png`` and ``velodyne_points/data/%010d.bin`` per frame, and one calibration for the drive from
+``calib_cam_to_cam.txt`` and ``calib_velo_to_cam.txt`` in the recording day's directory (results.Calibration.from_video).
+No labels.
 """
 import os
 import struct
@@ -121,15 +126,31 @@ def padded_batches(ids, batch):
     return out
 
 
-class KittiSplit:
-    """Frames of one split: ``frame(idx)`` -> (points [N,4] f32, img_meta dict with calib, img_shape, sample_idx)."""
+class _Frames:
+    """What Prefetcher reads: ``ids``, ``frame(idx)`` -> (points [N,4] f32, img_meta dict with calib, img_shape,
+    sample_idx) and ``pad_frame()``.  ``result_name`` formats a frame id as its result file's name."""
+    result_name = "%06d.txt"
+    labelled = True
+
+    def pad_frame(self):
+        """A padding frame: no points, the calibration and image shape of the first frame, sample_idx -1.
+        It does not depend on the batch it pads, which may hold no real frame at all (a rank's last batch under
+        torchrun, or every batch of a rank when there are fewer frames than ranks)."""
+        if self._pad_meta is None:
+            self._pad_meta = dict(self.meta(self.ids[0]), sample_idx=-1)
+        return np.zeros((0, 4), np.float32), self._pad_meta
+
+
+class KittiSplit(_Frames):
+    """Frames of one object split (``test`` reads ``testing/``, every other split ``training/``)."""
 
     def __init__(self, root, split="val", lidar="velodyne"):
         if lidar not in ("velodyne", "velodyne_reduced"):
             raise ValueError("lidar must be velodyne or velodyne_reduced, not %r" % lidar)
         self.root, self.split, self.lidar = root, split, lidar
         self.ids = read_split(root, split)
-        self.dir = os.path.join(root, "training")
+        self.labelled = split != "test"
+        self.dir = os.path.join(root, "training" if self.labelled else "testing")
         self.planes = PlaneCache()
         self._pad_meta = None
 
@@ -144,16 +165,57 @@ class KittiSplit:
     def frame(self, idx):
         return read_points(self.path(self.lidar, idx, "bin")), self.meta(idx)
 
-    def pad_frame(self):
-        """A padding frame: no points, the calibration and image shape of the split's first frame, sample_idx -1.
-        It does not depend on the batch it pads, which may hold no real frame at all (a rank's last batch under
-        torchrun, or every batch of a rank when the split has fewer frames than ranks)."""
-        if self._pad_meta is None:
-            self._pad_meta = dict(self.meta(self.ids[0]), sample_idx=-1)
-        return np.zeros((0, 4), np.float32), self._pad_meta
-
     def gt_annos(self, ids=None):
+        if not self.labelled:
+            raise ValueError("the test split has no labels")
         return read_labels(os.path.join(self.dir, "label_2"), self.ids if ids is None else ids)
+
+
+def _stems(path, ext):
+    """The frame ids of the ``%010d<ext>`` files of a raw-drive data directory; any other name is refused."""
+    ids = []
+    for name in os.listdir(path):
+        stem, e = os.path.splitext(name)
+        if e != ext:
+            continue
+        if not (len(stem) == 10 and stem.isdigit()):
+            raise ValueError("%s: %s is not a %%010d%s frame file" % (path, name, ext))
+        ids.append(int(stem))
+    return sorted(ids)
+
+
+class KittiDrive(_Frames):
+    """Frames of one raw KITTI drive (``.../2011_09_26/2011_09_26_drive_0001_sync``), for detection with the image-FOV
+    crop.  ``calib_dir`` holds the day's calib_cam_to_cam.txt and calib_velo_to_cam.txt (default: the drive's parent
+    directory, the raw data's layout).  The frames are the images' stems; the sweeps must have the same stems (the
+    reference pairs the two sorted listings by position and would silently misalign a drive with a missing file)."""
+    result_name = "%010d.txt"
+    labelled = False
+
+    def __init__(self, drive_dir, calib_dir=None):
+        self.root = drive_dir
+        if calib_dir is None:
+            calib_dir = os.path.dirname(os.path.abspath(drive_dir).rstrip(os.sep))
+        for name in ("calib_cam_to_cam.txt", "calib_velo_to_cam.txt"):
+            if not os.path.isfile(os.path.join(calib_dir, name)):
+                raise FileNotFoundError("raw-drive calibration %s not found in %s (pass calib_dir)" % (name, calib_dir))
+        self.calib = Calibration.from_video(calib_dir)
+        self.img_dir = os.path.join(drive_dir, "image_02", "data")
+        self.lidar_dir = os.path.join(drive_dir, "velodyne_points", "data")
+        self.ids = _stems(self.img_dir, ".png")
+        sweeps = _stems(self.lidar_dir, ".bin")
+        if sweeps != self.ids:
+            only_img, only_lidar = sorted(set(self.ids) - set(sweeps)), sorted(set(sweeps) - set(self.ids))
+            raise ValueError("%s: image_02 and velodyne_points frames differ (images only: %s; sweeps only: %s)" % (
+                drive_dir, only_img[:5], only_lidar[:5]))
+        self._pad_meta = None
+
+    def meta(self, idx):
+        return dict(calib=self.calib, img_shape=png_shape(os.path.join(self.img_dir, "%010d.png" % idx)),
+                    sample_idx=idx)
+
+    def frame(self, idx):
+        return read_points(os.path.join(self.lidar_dir, "%010d.bin" % idx)), self.meta(idx)
 
 
 class Prefetcher:

@@ -51,7 +51,7 @@ def next_pow2(n):
 
 # --- launch accounting / optional per-call CUDA-event timing (bench.py) ---------------
 # kernels launched by each C-ABI entry point (memsets not counted)
-_KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1,"sassd_anchor_mask": 4, "sassd_hash_build": 1,
+_KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
             "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
@@ -137,6 +137,27 @@ def frustum_crop(points, pt_off, batch, planes, ws=None):
     w = (ws or _WS).get("frustum", nbytes, dev)
     _call("sassd_frustum_crop", None, _ptr(points), _ptr(pt_off), n_cap, batch, _ptr(planes), _ptr(out), _ptr(off),
           _ptr(w), w.numel(), _stream())
+    return out, off
+
+
+IMAGE_FOV_CLIP_X = 0.1      # the reference's clip distance for raw drives (mmdet/datasets/kitti.py:394)
+
+
+def image_fov_crop(points, pt_off, batch, meta, clip_x=IMAGE_FOV_CLIP_X, ws=None):
+    """points [Ncap,4] f32, pt_off [batch+1] i32, meta [batch,36] f64 (device; results.meta_block).  Returns
+    (points_out [Ncap,4], pt_off_out [batch+1]): each frame's points that project into its image (0 <= u < img_w,
+    0 <= v < img_h) and lie in front of x = clip_x (compared in fp32), in input order, frames concatenated; the
+    reference's get_lidar_in_image_fov.  Rows past pt_off_out[batch] are left unwritten."""
+    dev = points.device
+    n_cap = points.shape[0]
+    assert meta.dtype == torch.float64 and tuple(meta.shape) == (batch, _lib.KITTI_META), \
+        "meta must be float64 [batch,%d]" % _lib.KITTI_META
+    out = torch.empty_like(points)
+    off = torch.empty((batch + 1,), dtype=torch.int32, device=dev)
+    nbytes = _L().sassd_frustum_crop_workspace_bytes(n_cap, batch)
+    w = (ws or _WS).get("frustum", nbytes, dev)      # the same look-back descriptors as the frustum crop
+    _call("sassd_image_fov_crop", None, _ptr(points), _ptr(pt_off), n_cap, batch, _ptr(meta), float(clip_x), _ptr(out),
+          _ptr(off), _ptr(w), w.numel(), _stream())
     return out, off
 
 

@@ -6,13 +6,16 @@ evaluation code:
 
 * `kitti_bbox2results`  <- mmdet/core/bbox/transforms.py:225-279
 * `Calibration`         <- mmdet/datasets/kitti_utils.py:49-107 (the fields the
-  formatter reads: P2, V2C, R0), `read_calib_file` :109-125
+  formatter reads: P2, V2C, R0), `read_calib_file` :109-125,
+  `Calibration.from_video` <- `read_calib_from_video` :128-144
 * `empty_result_anno`   <- tools/kitti_common.py:632-646
 * `kitti_result_line`, `annos_to_kitti_label` <- tools/kitti_common.py:413-471 (label / result file lines)
 
 This is float64 numpy on a few dozen boxes per frame; it stays on the host in
 the reference and here (DESIGN.md §8: not on the device path).
 """
+import os
+
 import numpy as np
 
 from .lib import KITTI_META, KITTI_ROW      # the header's SASSD_KITTI_META / SASSD_KITTI_ROW
@@ -44,6 +47,21 @@ class Calibration:
         self.f_u, self.f_v = self.P2[0, 0], self.P2[1, 1]
         self.b_x = self.P2[0, 3] / (-self.f_u)
         self.b_y = self.P2[1, 3] / (-self.f_v)
+
+    @classmethod
+    def from_video(cls, calib_dir):
+        """The calibration of a raw KITTI drive (the reference's ``Calibration(calib_dir, from_video=True)``):
+        ``calib_cam_to_cam.txt`` gives P2 = P_rect_02 and R0 = R_rect_00, ``calib_velo_to_cam.txt`` gives
+        Tr_velo_to_cam = [R | T].  Date lines are skipped."""
+        cam = cls.read_calib_file(os.path.join(calib_dir, 'calib_cam_to_cam.txt'))
+        velo = cls.read_calib_file(os.path.join(calib_dir, 'calib_velo_to_cam.txt'))
+        tr = np.zeros((3, 4))
+        tr[:, :3] = np.reshape(velo['R'], (3, 3))
+        tr[:, 3] = velo['T']
+        calib = {'P2': cam['P_rect_02'], 'Tr_velo_to_cam': tr, 'R0_rect': cam['R_rect_00']}
+        if 'P_rect_03' in cam:
+            calib['P3'] = cam['P_rect_03']
+        return cls(calib)
 
     @staticmethod
     def read_calib_file(path):

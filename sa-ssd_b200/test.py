@@ -1,13 +1,20 @@
-"""Evaluate a checkpoint on a KITTI split end to end (the reference's tools/test.py):
+"""Evaluate a checkpoint on a KITTI split end to end (the reference's tools/test.py), or detect on unlabelled data:
 
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR [--split val] [--batch 16]
                               [--lidar velodyne|velodyne_reduced] [--out DIR] [--workers N] [--json FILE]
+    python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR --split test --out DIR [...]
+    python -m sassd_b200.test CONFIG CHECKPOINT --drive DRIVE_DIR [--calib-dir DIR] --out DIR [...]
 
 Frames are read from disk a few batches ahead (kitti_data.Prefetcher) and streamed through the captured step
 (SingleStageDetector.detect_stream): full sweeps (``--lidar velodyne``) are cropped to the camera frustum on the
 device, and every step ends with the KITTI result formatter on the device (ops.kitti_format).  The last batch is
 padded with empty frames whose results are dropped.  Prints the official AP table (kitti_eval), the frame rate (wall
 clock of the streamed detection, the evaluation excluded) and the time spent waiting on reads.
+
+The test split (``testing/``) and raw drives (kitti_data.KittiDrive) have no labels: the driver writes the result
+files (``--out`` is required) and prints the frame rate and read wait only.  A raw drive's full sweeps are cropped on
+the device to the points that project into image 2 (ops.image_fov_crop, the reference's KittiVideo), and its result
+files are named by the frames' stems, ``%010d.txt``.
 
 Under torchrun, frame i of the split goes to rank i mod W; at the end every rank contributes one fixed-size block of
 KITTI rows and counts to a single all_gather_into_tensor (dist.DetectionGather) and rank 0 re-interleaves, writes and
@@ -29,20 +36,34 @@ def parse_args(argv=None):
     p = argparse.ArgumentParser(prog="python -m sassd_b200.test", description=__doc__.split("\n\n")[0])
     p.add_argument("config")
     p.add_argument("checkpoint")
-    p.add_argument("--data-root", required=True, help="KITTI root holding ImageSets/ and training/")
+    src = p.add_mutually_exclusive_group(required=True)
+    src.add_argument("--data-root", help="KITTI root holding ImageSets/ and training/ (testing/ for --split test)")
+    src.add_argument("--drive", help="a raw KITTI drive directory (*_sync) holding image_02/ and velodyne_points/")
+    p.add_argument("--calib-dir", default=None,
+                   help="with --drive: the directory of calib_cam_to_cam.txt / calib_velo_to_cam.txt "
+                        "(default: the drive's parent)")
     p.add_argument("--split", default="val")
     p.add_argument("--batch", type=int, default=16)
-    p.add_argument("--lidar", default="velodyne", choices=("velodyne", "velodyne_reduced"),
-                   help="full sweeps (cropped on the device) or the offline-cropped reduced clouds")
+    p.add_argument("--lidar", default=None, choices=("velodyne", "velodyne_reduced"),
+                   help="full sweeps (cropped on the device) or the offline-cropped reduced clouds (default velodyne)")
     p.add_argument("--max-points", type=int, default=None,
                    help="points per frame the captured step holds (default 131072 full, 32768 reduced)")
-    p.add_argument("--out", default=None, help="write one KITTI result file %%06d.txt per frame here")
+    p.add_argument("--out", default=None, help="write one KITTI result file %%06d.txt (drives: %%010d.txt) per frame "
+                                               "here; required without labels (--split test, --drive)")
     p.add_argument("--workers", type=int, default=4, help="reader threads")
     p.add_argument("--depth", type=int, default=4, help="batches read ahead")
     p.add_argument("--json", default=None, help="write the AP arrays and rates here")
     args = p.parse_args(argv)
     if args.batch < 1:
         p.error("--batch must be positive")
+    if args.drive:
+        if args.lidar == "velodyne_reduced":
+            p.error("--drive reads full sweeps: --lidar velodyne_reduced does not apply")
+    elif args.calib_dir is not None:
+        p.error("--calib-dir goes with --drive")
+    args.lidar = args.lidar or "velodyne"
+    if (args.drive or args.split == "test") and not args.out:
+        p.error("%s has no labels to evaluate against: --out is required" % ("--drive" if args.drive else "--split test"))
     if args.max_points is None:
         args.max_points = DEFAULT_MAX_POINTS[args.lidar]
     return args
@@ -74,30 +95,36 @@ def gather_annos(annos_local, ids, class_names, cap, device):
     return annos_from_rows(rows_all, n_all, class_names, ids)
 
 
-def write_results(out_dir, ids, annos):
-    """One ``%06d.txt`` per frame, annos_to_kitti_label(with_score=True); a frame without detections gets an empty
-    file.  The annotations hold dimensions as l, h, w; KITTI files hold h, w, l (what kitti_data.read_label and the
+def write_results(out_dir, ids, annos, name="%06d.txt"):
+    """One file per frame (``name`` % id), annos_to_kitti_label(with_score=True); a frame without detections gets an
+    empty file.  The annotations hold dimensions as l, h, w; KITTI files hold h, w, l (what kitti_data.read_label and the
     official devkit read)."""
     from .results import annos_to_kitti_label
     os.makedirs(out_dir, exist_ok=True)
     for idx, anno in zip(ids, annos):
         lines = annos_to_kitti_label(dict(anno, dimensions=anno["dimensions"][:, [1, 2, 0]]), with_score=True)
-        with open(os.path.join(out_dir, "%06d.txt" % idx), "w") as fh:
+        with open(os.path.join(out_dir, name % idx), "w") as fh:
             fh.write("".join(l + "\n" for l in lines))
 
 
 def run(args, log=print):
-    """Returns the result dict (AP arrays as nested lists, rates) on rank 0, None on the other ranks."""
+    """Returns the result dict (AP arrays as nested lists and rates; rates only without labels) on rank 0, None on the
+    other ranks."""
     import torch
     import sassd_b200 as S
     from . import dist as D
     from . import ops
     from .checkpoint import load_params_from_file
-    from .kitti_data import KittiSplit, Prefetcher
+    from .kitti_data import KittiDrive, KittiSplit, Prefetcher
 
-    split = KittiSplit(args.data_root, args.split, args.lidar)
-    if not split.ids:
-        raise ValueError("split %s of %s lists no frames" % (args.split, args.data_root))
+    if args.drive:
+        split = KittiDrive(args.drive, args.calib_dir)
+        if not split.ids:
+            raise ValueError("drive %s has no frames" % args.drive)
+    else:
+        split = KittiSplit(args.data_root, args.split, args.lidar)
+        if not split.ids:
+            raise ValueError("split %s of %s lists no frames" % (args.split, args.data_root))
     cfg = S.Config.fromfile(args.config)
     rank, world, local = D.init_from_env()
     batches = rank_batches(split.ids, rank, world, args.batch)
@@ -106,7 +133,8 @@ def run(args, log=print):
     torch.cuda.set_device(device)
     model, _, _ = S.build_from_config(cfg, device=device)
     load_params_from_file(model, args.checkpoint)
-    crop = args.lidar == "velodyne"
+    fov = bool(args.drive)
+    crop = args.lidar == "velodyne" and not fov
     class_names = model.class_names
 
     def items(reader):
@@ -117,7 +145,7 @@ def run(args, log=print):
                 yield points, metas
 
     stream = lambda src: model.detect_stream(src, args.batch, args.max_points, depth=4, crop=crop,  # noqa: E731
-                                             kitti=True)
+                                             kitti=True, image_fov=fov)
     for _ in stream([]):                # capture the slots' graphs before the clock starts
         pass
     torch.cuda.synchronize(device)
@@ -137,22 +165,32 @@ def run(args, log=print):
         D.barrier()
         return None
     if args.out:
-        write_results(args.out, split.ids, dt_annos)
+        write_results(args.out, split.ids, dt_annos, split.result_name)
+    fps = len(split.ids) / wall
+    rate = "frames: %d (%d rank%s), %.1f frames/s, read wait %.3f s on rank 0 (%d of %d frames on rank 0)" % (
+        len(split.ids), world, "s" if world > 1 else "", fps, reader.wait, n_local, len(split.ids))
+    result = dict(frames=len(split.ids), world=world, batch=args.batch, lidar=args.lidar, frames_per_s=fps,
+                  wall_s=wall, read_wait_s=reader.wait)
+    if not split.labelled:
+        log(rate)
+        _write_json(args.json, result)
+        D.barrier()
+        return result
     from .kitti_eval import official_eval
     gt_annos = split.gt_annos()
     text, ap = official_eval(gt_annos, dt_annos, class_names)
-    fps = len(split.ids) / wall
     log(text, end="")
-    log("frames: %d (%d rank%s), %.1f frames/s, read wait %.3f s on rank 0 (%d of %d frames on rank 0)" % (
-        len(split.ids), world, "s" if world > 1 else "", fps, reader.wait, n_local, len(split.ids)))
-    result = dict(frames=len(split.ids), world=world, batch=args.batch, lidar=args.lidar, frames_per_s=fps,
-                  wall_s=wall, read_wait_s=reader.wait, text=text,
-                  ap={k: (None if v is None else np.asarray(v).tolist()) for k, v in ap.items()})
-    if args.json:
-        with open(args.json, "w") as fh:
-            json.dump(result, fh, indent=1)
+    log(rate)
+    result.update(text=text, ap={k: (None if v is None else np.asarray(v).tolist()) for k, v in ap.items()})
+    _write_json(args.json, result)
     D.barrier()
     return result
+
+
+def _write_json(path, result):
+    if path:
+        with open(path, "w") as fh:
+            json.dump(result, fh, indent=1)
 
 
 def main(argv=None):
