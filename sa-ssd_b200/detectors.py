@@ -14,7 +14,8 @@ Two entry points:
     the step also formats its detections as KITTI annotations on the device (ops.kitti_format).  With
     ``point_outputs`` it also returns the auxiliary network's per-voxel foreground logits and centre offsets.
   * ``forward(..., return_loss=True)`` / ``forward_train`` and ``loss_points`` — the training losses, forward only, in
-    eval() mode (csrc/targets.cu).
+    eval() mode (csrc/targets.cu).  ``forward_points(..., gt_bboxes=, gt_labels=)`` and ``detect_stream(losses=True)``
+    compute them in the detection step itself (validation losses beside the detections, eager or captured).
 """
 import numpy as np
 import torch
@@ -23,10 +24,11 @@ from torch import nn
 
 from . import builder, ops
 from .results import annos_from_rows, meta_block
-from .single_stage_heads import split_detections, unpack_detections
+from .single_stage_heads import gt_arrays, split_detections, stage_gt, unpack_detections
 
 # The crop a step runs before voxelizing: the first element of a captured-graph key.  0 and 1 equal False and True, so
-# a key reads (crop, kitti, point_outputs) with the frustum crop as True.
+# a key reads (crop, kitti, point_outputs) with the frustum crop as True.  A step that also computes the losses has a
+# fourth element, True; the other kinds keep their three-element keys.
 CROP_NONE, CROP_FRUSTUM, CROP_IMAGE_FOV = 0, 1, 2
 
 
@@ -50,7 +52,7 @@ class SingleStageDetector(nn.Module):
         self.anchor_set = None
         self._pinned = None
         self._mask_stream = None
-        self._graphs = {}                 # (crop kind, kitti, point_outputs) -> captured step (enable_cuda_graph)
+        self._graphs = {}                 # (crop kind, kitti, point_outputs[, losses]) -> captured step (enable_cuda_graph)
         self._graph_args = None
         self._stream_slots = None
         self._stream_key = None
@@ -234,7 +236,8 @@ class SingleStageDetector(nn.Module):
         launch.  Steps whose shape does not fit fall back to the eager path.  forward_points replays one graph per kind
         of call: with ``frustum_planes``, with ``image_fov`` or without a crop (a cropping graph crops the full sweeps
         first, and ``max_points_per_frame`` bounds them, e.g. 131072), ``metas`` (it ends with the KITTI result
-        formatter) and ``point_outputs`` (it also runs the auxiliary network).  The plain kind is captured here and returned, the others on their first use; a
+        formatter), ``point_outputs`` (it also runs the auxiliary network) and ``gt_bboxes`` (it also computes the
+        losses).  The plain kind is captured here and returned, the others on their first use; a
         new call replaces every graph captured for an earlier shape."""
         self._graph_args = (int(batch), int(max_points_per_frame))
         self._graphs = {}
@@ -244,17 +247,39 @@ class SingleStageDetector(nn.Module):
         self._graphs = {}
         self._graph_args = None
 
-    def _graph_for(self, crop, kitti, point_outputs):
+    def _graph_for(self, crop, kitti, point_outputs, losses=False):
         """The captured single step of this kind at enable_cuda_graph's shape, captured on first use; None while the
         graphs are disabled."""
-        key = (int(crop), kitti, point_outputs)
+        key = (int(crop), kitti, point_outputs) + ((True,) if losses else ())
         if key not in self._graphs and self._graph_args is not None:
             self._graphs[key] = _GraphedStep(self, *self._graph_args, latency=True, crop=crop, kitti=kitti,
-                                             point_outputs=point_outputs)
+                                             point_outputs=point_outputs, losses=losses)
         return self._graphs.get(key)
 
+    def _require_loss_step(self):
+        """A detection step that also computes the losses needs train_cfg, eval() mode and one guided-anchor selection
+        for both: train_cfg.rpn.anchor_thr must equal the test threshold (both shipped configs set 0.1)."""
+        if self.training:
+            raise NotImplementedError("the losses are computed in eval() mode only")
+        if self.train_cfg is None:
+            raise ValueError("the losses need train_cfg (build_from_config passes cfg.train_cfg)")
+        thr = float(self.train_cfg.rpn.anchor_thr)
+        if thr != self.guided_thr:
+            raise ValueError("train_cfg.rpn.anchor_thr = %r differs from the test threshold %r: the losses and the "
+                             "detections select different guided anchors, so one step cannot give both (use "
+                             "loss_points)" % (thr, self.guided_thr))
+
+    @staticmethod
+    def _gt_inputs(gt_bboxes, gt_labels, batch):
+        """Per-frame GT boxes and 1-based labels -> gt_arrays' (boxes, anchor classes = labels - 1, labels)."""
+        if len(gt_bboxes) != batch or len(gt_labels) != batch:
+            raise ValueError("one GT box set and label set per frame: %d frames, %d box sets, %d label sets" %
+                             (batch, len(gt_bboxes), len(gt_labels)))
+        labels = [np.asarray(l, np.int64).reshape(-1) for l in gt_labels]
+        return gt_bboxes, [(l - 1).astype(np.int32) for l in labels], labels
+
     def detect_stream(self, batches, batch, max_points_per_frame=32768, depth=4, concurrent=True, crop=False,
-                      kitti=False, image_fov=False):
+                      kitti=False, image_fov=False, losses=False):
         """Throughput API: iterate over batches (each a list of ``batch`` raw point arrays) and yield their
         detections in order.  ``depth`` captured graphs with their own static buffers and scratch are used
         round-robin: while the GPU runs step i, the host stages and uploads step i+1 (copy stream) and unpacks
@@ -268,20 +293,29 @@ class SingleStageDetector(nn.Module):
         result formatter and each yield is the batch's annotation dicts (kitti_bbox2results' format).
         With ``image_fov`` (needs ``kitti``, excludes ``crop``) the items are (points_list, metas) of raw-drive sweeps:
         every slot's graph first crops each frame to the points that project into its image (forward_points'
-        ``image_fov``)."""
+        ``image_fov``).
+        With ``losses`` each item ends with the batch's ground truth, (gt_bboxes, gt_labels) as forward_points takes
+        them: every slot's graph also computes the losses, and each yield is (results, losses), ``losses`` the batch's
+        dict of floats (loss_points')."""
         ops.require_cuda()
         if kitti and self.class_names is None:
             raise ValueError("detect_stream(kitti=True) needs class_names")
         kind = _crop_kind(bool(crop), image_fov, kitti)
-        key = (batch, max_points_per_frame, depth, kind, bool(kitti))
+        losses = bool(losses)
+        if losses:
+            self._require_loss_step()
+        key = (batch, max_points_per_frame, depth, kind, bool(kitti), losses)
         if self._stream_key != key or self._stream_slots is None:
-            self._stream_slots = [_GraphedStep(self, batch, max_points_per_frame, crop=kind, kitti=kitti)
+            self._stream_slots = [_GraphedStep(self, batch, max_points_per_frame, crop=kind, kitti=kitti, losses=losses)
                                   for _ in range(depth)]
             self._copy_stream = torch.cuda.Stream()
             self._stream_key = key
         slots, pending = self._stream_slots, []
         for i, item in enumerate(batches):
-            item = tuple(item) if (crop or kitti) else (item,)
+            item = tuple(item) if (crop or kitti or losses) else (item,)
+            gt = None
+            if losses:
+                gt, item = self._gt_inputs(*item[-1], len(item[0])), item[:-1]
             fb = item[0]
             planes = _frame_planes(item[1], len(fb)) if crop else None
             metas = item[-1] if kitti else None
@@ -293,14 +327,15 @@ class SingleStageDetector(nn.Module):
             if not slot.fits(len(fb), counts):
                 raise ValueError("batch does not fit the captured shape (batch %d, %d points/frame)" %
                                  (batch, max_points_per_frame))
-            slot.submit(fb, counts, self._copy_stream, own_stream=concurrent, planes=planes, meta=meta)
+            slot.submit(fb, counts, self._copy_stream, own_stream=concurrent, planes=planes, meta=meta, gt=gt)
             pending.append((slot, metas))
         for slot, metas in pending:
             yield self._collected(slot, metas)
 
     def _collected(self, slot, metas):
-        """Wait for a slot's step and convert its host copy into the caller's per-frame results."""
-        return self._frame_results(slot.collect(), metas)
+        """Wait for a slot's step and convert its host copy into the caller's per-frame results (and its losses)."""
+        res = self._frame_results(slot.collect(), metas)
+        return (res, slot.loss_results()) if slot.losses else res
 
     def _frame_results(self, out, metas):
         """A step's host outputs -> the caller's per-frame results: with ``metas`` KITTI annotation dicts of the
@@ -310,7 +345,7 @@ class SingleStageDetector(nn.Module):
         return [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(*out)]
 
     def forward_points(self, points_list, return_aux=False, frustum_planes=None, metas=None, point_outputs=False,
-                       image_fov=False):
+                       image_fov=False, gt_bboxes=None, gt_labels=None):
         """Raw points in (list of [N_i,>=4] numpy arrays), detections out: per frame a dict of
         boxes_lidar [D,7], scores [D], label_preds [D] (or None entries when nothing survives).
         ``frustum_planes``: one float64 [6,4] array per frame (frustum.camera_frustum_planes).  The frames are then
@@ -327,7 +362,13 @@ class SingleStageDetector(nn.Module):
         ``image_fov``: the frames are raw-drive sweeps; each is cropped on the device, in point order, to the points
         that project into its image and lie in front of x = 0.1 m (ops.image_fov_crop), as the reference's KittiVideo
         crops them (get_lidar_in_image_fov).  Needs ``metas``, whose calibration and image shape define the crop, and
-        excludes ``frustum_planes``."""
+        excludes ``frustum_planes``.
+        ``gt_bboxes`` / ``gt_labels``: per frame the GT boxes [G,7] and 1-based labels as loss_points takes them.  The
+        same step then also computes SA-SSD's losses (loss_device, after the detections and before the formatter) and
+        the call returns (results, losses), ``results`` exactly as without GT and ``losses`` loss_points' dict of
+        floats for these frames; with ``point_outputs`` the points come before the losses, with ``return_aux`` the aux
+        dict last.  Needs train_cfg with rpn.anchor_thr equal to the test threshold (one guided-anchor selection
+        serves both); a frame with more than SASSD_GT_CAP_MAX boxes raises."""
         ops.require_cuda()
         if self.voxel_generator is None or self.anchor_set is None:
             raise RuntimeError("call attach_data_pipeline(voxel_generator, anchor_set) first")
@@ -335,17 +376,26 @@ class SingleStageDetector(nn.Module):
             raise ValueError("forward_points(metas=) needs class_names")
         kind = _crop_kind(frustum_planes is not None, image_fov, metas is not None)
         B = len(points_list)
+        losses = gt_bboxes is not None or gt_labels is not None
+        gt_in = None
+        if losses:
+            self._require_loss_step()
+            if gt_bboxes is None or gt_labels is None:
+                raise ValueError("forward_points: gt_bboxes and gt_labels go together")
+            gt_in = self._gt_inputs(gt_bboxes, gt_labels, B)
         planes = None if frustum_planes is None else _frame_planes(frustum_planes, B)
         meta = None if metas is None else _meta_blocks(metas, B)
         hp, ho, counts = self.stage_points(points_list)
-        g = self._graph_for(kind, meta is not None, bool(point_outputs))
+        g = self._graph_for(kind, meta is not None, bool(point_outputs), losses)
         if g is not None and not return_aux and g.fits(B, counts):
-            res = self._frame_results(g.run_host(hp, ho, sum(counts), planes, meta), metas)
-            return (res, g.point_results()) if point_outputs else res
+            res = self._frame_results(g.run_host(hp, ho, sum(counts), planes, meta, gt_in), metas)
+            ret = (res,) + ((g.point_results(),) if point_outputs else ()) + ((g.loss_results(),) if losses else ())
+            return ret if len(ret) > 1 else res
         dev = next(self.parameters()).device
+        gt = stage_gt(*gt_in, dev) if losses else None
         det, d_ndet, status, aux = _run_step(self, hp.to(dev, non_blocking=True), ho.to(dev, non_blocking=True), B,
                                              max(counts + [1]), _to_device(planes, dev), _to_device(meta, dev),
-                                             point_outputs=point_outputs, image_fov=kind == CROP_IMAGE_FOV)
+                                             point_outputs=point_outputs, image_fov=kind == CROP_IMAGE_FOV, gt=gt)
         if meta is not None:
             ops._lib.raise_on_status(status)
             out = aux["rows"].cpu().numpy(), aux["n_out"].cpu().numpy()
@@ -354,14 +404,15 @@ class SingleStageDetector(nn.Module):
             out = unpack_detections(det, d_ndet, status)
         res = self._frame_results(out, metas)
         pts = _split_points(*(aux[k].cpu().numpy() for k in _POINT_KEYS)) if point_outputs else None
-        ret = (res,) + ((pts,) if point_outputs else ()) + ((aux,) if return_aux else ())
+        loss = _loss_dict(aux["losses"].cpu()) if losses else None
+        ret = (res,) + ((pts,) if point_outputs else ()) + ((loss,) if losses else ()) + ((aux,) if return_aux else ())
         return ret if len(ret) > 1 else res
-
 
     def loss_device(self, aux, batch, gt, gt_class, gt_label, d_ngt, n_gt_host, status):
         """Targets and losses of one forward_device(point_outputs=True) step, on the device: returns the loss vector
-        [6] in ops.LOSS_KEYS order and a dict of the targets.  gt [B,gt_cap,7] etc. as stage_gt gives them;
-        ``n_gt_host`` the per-frame counts (the GT rows PSWarp scores)."""
+        [6] in ops.LOSS_KEYS order and a dict of the targets.  gt [B,gt_cap,7] etc. as stage_gt gives them.  Nothing
+        here reads the host: PSWarp scores min(d_ngt[b], gt_cap) GT rows of each frame, the cap applied by the pswarp
+        and assign_pswarp kernels, so the step can be captured; ``n_gt_host`` is not read."""
         dev = gt.device
         gt_cap = gt.shape[1]
         out = torch.zeros((len(ops.LOSS_KEYS),), dtype=torch.float32, device=dev)
@@ -376,12 +427,11 @@ class SingleStageDetector(nn.Module):
                                                            d_ngt, pos, neg, out[2:5], status)
         # PSWarp scores the GT rows the reference prepends to each frame's guided boxes (:364-367) in a slot segment of
         # their own, so the guided capacity does not grow
-        d_head = torch.from_numpy(np.minimum(n_gt_host, gt_cap).astype(np.int32)).to(dev)
-        gt_scores = self.extra_head.sample(aux["ps_feat"], gt, d_head)
+        gt_scores = self.extra_head.sample(aux["ps_feat"], gt, d_ngt)
         boxes = torch.cat([gt, aux["guided"]], 1).contiguous()
         scores = torch.cat([gt_scores, aux["ps_scores"]], 1).contiguous()
         e_lab, e_iou, _ = self.extra_head.loss_device(scores, boxes, aux["d_k"], gt, d_ngt, cfg.extra, out[5:6], status,
-                                                      d_head=d_head, head_cap=gt_cap)
+                                                      d_head=d_ngt, head_cap=gt_cap)
         return out, dict(point_labels=p_lab, point_offsets=p_off, rpn_labels=r_lab, rpn_targets=r_tgt, rpn_ious=r_iou,
                          ps_boxes=boxes, ps_scores=scores, ps_labels=e_lab, ps_ious=e_iou)
 
@@ -400,27 +450,21 @@ class SingleStageDetector(nn.Module):
             raise RuntimeError("call attach_data_pipeline(voxel_generator, anchor_set) first")
         if self.train_cfg is None:
             raise ValueError("loss_points needs train_cfg (build_from_config passes cfg.train_cfg)")
-        from .single_stage_heads import stage_gt
         B = len(points_list)
-        if len(gt_bboxes) != B or len(gt_labels) != B:
-            raise ValueError("loss_points: one GT box set and label set per frame")
+        gt_in = self._gt_inputs(gt_bboxes, gt_labels, B)
         dev = next(self.parameters()).device
         planes = None if frustum_planes is None else _frame_planes(frustum_planes, B)
         hp, ho, counts = self.stage_points(points_list)
-        labels = [np.asarray(l, np.int64).reshape(-1) for l in gt_labels]
-        gt_class = [(l - 1).astype(np.int32) for l in labels]
-        gt, gcls, glab, d_ngt = stage_gt(gt_bboxes, gt_class, labels, dev)
-        n_gt = np.array([np.asarray(g).reshape(-1, 7).shape[0] for g in gt_bboxes], np.int64)
         _, _, status, aux = _run_step(self, hp.to(dev, non_blocking=True), ho.to(dev, non_blocking=True), B,
-                                      max(counts + [1]), _to_device(planes, dev), point_outputs=True, detections=False,
-                                      guided_thr=float(self.train_cfg.rpn.anchor_thr))
-        out, targets = self.loss_device(aux, B, gt, gcls, glab, d_ngt, n_gt, status)
+                                      max(counts + [1]), _to_device(planes, dev), detections=False,
+                                      guided_thr=float(self.train_cfg.rpn.anchor_thr), gt=stage_gt(*gt_in, dev))
         h = torch.empty((len(ops.LOSS_KEYS) + 1,), dtype=torch.float32, pin_memory=True)
-        h[:-1].copy_(out, non_blocking=True)
+        h[:-1].copy_(aux["losses"], non_blocking=True)
         h[-1:].copy_(status.view(torch.float32), non_blocking=True)
         torch.cuda.current_stream().synchronize()
         ops._lib.raise_on_status(h[-1:].view(torch.int32))
-        res = {k: float(v) for k, v in zip(ops.LOSS_KEYS, h[:-1].tolist())}
+        res = _loss_dict(h[:-1])
+        targets = aux.pop("targets")
         if return_aux:
             aux.update(targets)
             return res, aux
@@ -474,19 +518,29 @@ def _to_device(a, dev):
     return None if a is None else torch.from_numpy(a).to(dev)
 
 
+def _loss_dict(h):
+    """A host loss vector [6] (ops.LOSS_KEYS order) -> dict of Python floats."""
+    return {k: float(v) for k, v in zip(ops.LOSS_KEYS, h.tolist())}
+
+
 def _run_step(model, points, pt_off, batch, maxpts, planes=None, meta=None, point_outputs=False, detections=True,
-              guided_thr=None, image_fov=False):
+              guided_thr=None, image_fov=False, gt=None):
     """One detector step on the device, no synchronisation; the eager calls and every captured graph build their step
     here.  With ``planes`` [batch,6,4] the frames are full sweeps, cropped to their camera frustums first
     (ops.frustum_crop); with ``image_fov`` they are cropped to their images through ``meta`` (ops.image_fov_crop); then
-    forward_device; with ``meta`` [batch,36] the detections are formatted as KITTI rows (ops.kitti_format) into
-    aux["rows"] / aux["n_out"].  Returns forward_device's (det, d_ndet, status, aux)."""
+    forward_device; with ``gt`` (stage_gt's device tensors) the auxiliary network runs too and loss_device puts the
+    loss vector [6] in aux["losses"] and its targets in aux["targets"]; with ``meta`` [batch,36] the detections are
+    formatted as KITTI rows (ops.kitti_format) into aux["rows"] / aux["n_out"].  Returns forward_device's (det, d_ndet,
+    status, aux)."""
     if planes is not None:
         points, pt_off = ops.frustum_crop(points, pt_off, batch, planes)
     elif image_fov:
         points, pt_off = ops.image_fov_crop(points, pt_off, batch, meta)
-    det, d_ndet, status, aux = model.forward_device(points, pt_off, batch, maxpts, point_outputs=point_outputs,
+    det, d_ndet, status, aux = model.forward_device(points, pt_off, batch, maxpts,
+                                                    point_outputs=point_outputs or gt is not None,
                                                     detections=detections, guided_thr=guided_thr)
+    if gt is not None:
+        aux["losses"], aux["targets"] = model.loss_device(aux, batch, *gt, None, status)
     if meta is not None:
         aux["rows"], aux["n_out"] = ops.kitti_format(det, d_ndet, meta)
     return det, d_ndet, status, aux
@@ -514,7 +568,8 @@ def _stage_into(hp, ho, points_list, counts):
 class _GraphedStep:
     """One captured detector step (_run_step) with static input/output buffers."""
 
-    def __init__(self, model, batch, max_points_per_frame, latency=False, crop=False, kitti=False, point_outputs=False):
+    def __init__(self, model, batch, max_points_per_frame, latency=False, crop=False, kitti=False, point_outputs=False,
+                 losses=False):
         """latency=True: this step will run alone on the GPU (enable_cuda_graph / forward_points): the dense convs walk
         the computed tiles first so that the constant-region tiles shorten every layer; False (detect_stream slots,
         several steps in flight): round-robin tiles, the SMs a layer leaves idle serve the other steps.
@@ -525,19 +580,28 @@ class _GraphedStep:
         kitti=True: the graph ends with the KITTI result formatter (ops.kitti_format) on the static meta blocks
         [batch,36]; the host copy is its rows and counts instead of the detections.
         point_outputs=True: the step also runs the auxiliary network and copies its outputs and the frame row offsets to
-        the host (point_results)."""
+        the host (point_results).
+        losses=True: the step also computes the losses of the GT in the static buffers gt [batch,SASSD_GT_CAP_MAX,7],
+        its classes, labels and per-frame counts (the true counts: a frame with more boxes raises), and copies the loss
+        vector to the host with the detections (loss_results)."""
         dev = next(model.parameters()).device
         self.model, self.batch, self.maxpts = model, int(batch), int(max_points_per_frame)
         self.cap = self.batch * self.maxpts
         self.crop, self.kitti, self.point_outputs = int(crop), bool(kitti), bool(point_outputs)
+        self.losses = bool(losses)
         _crop_kind(self.crop == CROP_FRUSTUM, self.crop == CROP_IMAGE_FOV, self.kitti)
         self.points = torch.zeros((self.cap, 4), dtype=torch.float32, device=dev)
         self.pt_off = torch.zeros((self.batch + 1,), dtype=torch.int32, device=dev)
-        self.planes = self.meta = None
+        self.planes = self.meta = self.gt = None
         if self.crop == CROP_FRUSTUM:
             self.planes = torch.zeros((self.batch, 6, 4), dtype=torch.float64, device=dev)
         if self.kitti:
             self.meta = torch.zeros((self.batch, ops._lib.KITTI_META), dtype=torch.float64, device=dev)
+        if self.losses:
+            self.h_gt = tuple(torch.from_numpy(a).pin_memory()
+                              for a in gt_arrays([np.zeros((0, 7), np.float32)] * self.batch, None, None,
+                                                 ops._lib.GT_CAP_MAX))
+            self.gt = tuple(h.to(dev) for h in self.h_gt)
         # Scratch buffers private to this graph (the captured kernels bake their addresses in), so that several
         # captured steps can be in flight on different streams without sharing anything but read-only weights.
         self.ws = ops.Workspace()
@@ -574,6 +638,8 @@ class _GraphedStep:
         if self.point_outputs:
             self.h_pts = {k: torch.empty(self.aux[k].shape, dtype=self.aux[k].dtype, pin_memory=True)
                           for k in _POINT_KEYS}
+        if self.losses:
+            self.h_loss = torch.empty((len(ops.LOSS_KEYS),), dtype=torch.float32, pin_memory=True)
         self.h_status = torch.empty((1,), dtype=torch.int32, pin_memory=True)
         self.h_points, self.h_off = _pinned_pair(self.cap, self.batch + 1)
         if self.crop == CROP_FRUSTUM:
@@ -583,7 +649,7 @@ class _GraphedStep:
 
     def _step(self):
         return _run_step(self.model, self.points, self.pt_off, self.batch, self.maxpts, self.planes, self.meta,
-                         point_outputs=self.point_outputs, image_fov=self.crop == CROP_IMAGE_FOV)
+                         point_outputs=self.point_outputs, image_fov=self.crop == CROP_IMAGE_FOV, gt=self.gt)
 
     def fits(self, batch, counts):
         return batch == self.batch and max(counts + [0]) <= self.maxpts
@@ -597,17 +663,18 @@ class _GraphedStep:
         self.graph.replay()
         return self.det, self.d_ndet, self.status
 
-    def run_host(self, hp, ho, total, planes=None, meta=None):
+    def run_host(self, hp, ho, total, planes=None, meta=None, gt=None):
         """pinned host points in, numpy detections (or KITTI rows) out: H2D, one graph launch, D2H, one stream sync."""
-        self._upload(hp, ho, total, planes, meta)
+        self._upload(hp, ho, total, planes, meta, gt)
         self.graph.replay()
         self._download()
         torch.cuda.current_stream().synchronize()
         return self.unpack()
 
-    def _upload(self, hp, ho, total, planes, meta):
+    def _upload(self, hp, ho, total, planes, meta, gt=None):
         """H2D of a step's inputs into the static buffers on the current stream: ``total`` points of the pinned ``hp``,
-        the pinned offsets ``ho`` and, for a crop / formatting step, the numpy planes / meta blocks."""
+        the pinned offsets ``ho`` and, for a crop / formatting / loss step, the numpy planes / meta blocks / gt_arrays'
+        inputs."""
         self.points[:total].copy_(hp[:total], non_blocking=True)
         self.pt_off.copy_(ho, non_blocking=True)
         if self.crop == CROP_FRUSTUM:
@@ -616,10 +683,14 @@ class _GraphedStep:
         if self.kitti:
             self.h_meta.numpy()[...] = meta
             self.meta.copy_(self.h_meta, non_blocking=True)
+        if self.losses:
+            for h, d, a in zip(self.h_gt, self.gt, gt_arrays(*gt, gt_cap=ops._lib.GT_CAP_MAX)):
+                h.numpy()[...] = a
+                d.copy_(h, non_blocking=True)
 
     def _download(self):
         """D2H of the step's result on the current stream: the KITTI rows and counts of a formatting step, else the
-        detections and counts; and the status word."""
+        detections and counts; the loss vector of a loss step; and the status word."""
         if self.kitti:
             self.h_rows.copy_(self.aux["rows"], non_blocking=True)
             self.h_nout.copy_(self.aux["n_out"], non_blocking=True)
@@ -629,16 +700,18 @@ class _GraphedStep:
         if self.point_outputs:
             for k, h in self.h_pts.items():
                 h.copy_(self.aux[k], non_blocking=True)
+        if self.losses:
+            self.h_loss.copy_(self.aux["losses"], non_blocking=True)
         self.h_status.copy_(self.status, non_blocking=True)
 
     # ---- asynchronous use (SingleStageDetector.detect_stream): submit() ... collect()
-    def submit(self, points_list, counts, copy_stream, own_stream=False, planes=None, meta=None):
+    def submit(self, points_list, counts, copy_stream, own_stream=False, planes=None, meta=None, gt=None):
         """Stage into this slot's pinned buffer, H2D on the copy stream, then replay + D2H on the current stream or,
         with ``own_stream``, on this slot's stream so that consecutive steps overlap on the GPU."""
         _stage_into(self.h_points, self.h_off, points_list, counts)
         cur = self.stream if own_stream else torch.cuda.current_stream()
         with torch.cuda.stream(copy_stream):
-            self._upload(self.h_points, self.h_off, sum(counts), planes, meta)
+            self._upload(self.h_points, self.h_off, sum(counts), planes, meta, gt)
             self.loaded.record(copy_stream)
         cur.wait_event(self.loaded)
         with torch.cuda.stream(cur):
@@ -653,6 +726,11 @@ class _GraphedStep:
     def point_results(self):
         """The last run's aux outputs, per frame (forward_points(point_outputs=True))."""
         return _split_points(*(self.h_pts[k].numpy() for k in _POINT_KEYS))
+
+    def loss_results(self):
+        """The last run's losses (forward_points with GT, detect_stream(losses=True)); read after unpack, which checks
+        the status word."""
+        return _loss_dict(self.h_loss)
 
     def unpack(self):
         ops._lib.raise_on_status(self.h_status.numpy()[0])

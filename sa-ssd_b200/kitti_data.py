@@ -22,7 +22,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 
 from .frustum import camera_frustum_planes
-from .results import Calibration
+from .results import Calibration, project_rect_to_velo
 
 PNG_SIGNATURE = b"\x89PNG\r\n\x1a\n"
 _PNG_CHANNELS = {0: 1, 2: 3, 3: 3, 4: 2, 6: 4}      # IHDR colour type -> channels of the decoded image
@@ -89,6 +89,29 @@ def read_label(path):
     return anno
 
 
+def gt_from_anno(anno, calib, class_names):
+    """One frame's read_label annotation -> the ground truth of the reference's labelled test path
+    (prepare_test_img(with_label=True), kitti.py:276-293): (boxes [G,7] float32 as (x, y, z_bottom, w, l, h, ry) in the
+    lidar frame, labels [G] int64, 1-based over ``class_names``).  DontCare rows are dropped, box3d is built in float32
+    (kitti_utils.py:36-37), its centre goes through project_rect_to_velo in float64 and is stored back into float32,
+    Van counts as Car, and only ``class_names`` are kept, in file order.  A frame with no box left gives [0,7] and [0]
+    (the reference's empty array there is 1-D and fails to index)."""
+    names = np.asarray(anno["name"]).reshape(-1)
+    keep = names != "DontCare"
+    box3d = np.concatenate([np.asarray(anno["location"]).reshape(-1, 3),
+                            np.asarray(anno["dimensions"]).reshape(-1, 3)[:, [2, 0, 1]],     # l, h, w -> w, l, h
+                            np.asarray(anno["rotation_y"]).reshape(-1, 1)], 1)[keep].astype(np.float32)
+    if len(box3d):
+        box3d[:, :3] = project_rect_to_velo(box3d[:, :3], calib)
+    types = ["Car" if n == "Van" else str(n) for n in names[keep]]
+    selected = [i for i, n in enumerate(types) if n in class_names]
+    labels = np.array([list(class_names).index(types[i]) + 1 for i in selected], dtype=np.int64)
+    return box3d[selected].reshape(-1, 7), labels
+
+
+_NO_GT = (np.zeros((0, 7), np.float32), np.zeros((0,), np.int64))
+
+
 def read_labels(label_dir, ids):
     """``label_dir/%06d.txt`` of every id -> annotation dicts with ``image_idx`` (get_label_annos)."""
     annos = []
@@ -131,25 +154,32 @@ class _Frames:
     sample_idx) and ``pad_frame()``.  ``result_name`` formats a frame id as its result file's name."""
     result_name = "%06d.txt"
     labelled = True
+    gt_classes = None
 
     def pad_frame(self):
-        """A padding frame: no points, the calibration and image shape of the first frame, sample_idx -1.
+        """A padding frame: no points, the calibration and image shape of the first frame, sample_idx -1 (and no GT
+        when the frames carry it).
         It does not depend on the batch it pads, which may hold no real frame at all (a rank's last batch under
         torchrun, or every batch of a rank when there are fewer frames than ranks)."""
         if self._pad_meta is None:
             self._pad_meta = dict(self.meta(self.ids[0]), sample_idx=-1)
-        return np.zeros((0, 4), np.float32), self._pad_meta
+        return (np.zeros((0, 4), np.float32), self._pad_meta) + ((_NO_GT,) if self.gt_classes is not None else ())
 
 
 class KittiSplit(_Frames):
-    """Frames of one object split (``test`` reads ``testing/``, every other split ``training/``)."""
+    """Frames of one object split (``test`` reads ``testing/``, every other split ``training/``).  With ``gt_classes``
+    (a labelled split only) every frame also carries its ground truth, gt_from_anno's (boxes, labels) over those
+    classes, and Prefetcher yields the batches' GT lists after their metas."""
 
-    def __init__(self, root, split="val", lidar="velodyne"):
+    def __init__(self, root, split="val", lidar="velodyne", gt_classes=None):
         if lidar not in ("velodyne", "velodyne_reduced"):
             raise ValueError("lidar must be velodyne or velodyne_reduced, not %r" % lidar)
         self.root, self.split, self.lidar = root, split, lidar
         self.ids = read_split(root, split)
         self.labelled = split != "test"
+        if gt_classes is not None and not self.labelled:
+            raise ValueError("the test split has no labels to give as ground truth")
+        self.gt_classes = None if gt_classes is None else list(gt_classes)
         self.dir = os.path.join(root, "training" if self.labelled else "testing")
         self.planes = PlaneCache()
         self._pad_meta = None
@@ -163,7 +193,11 @@ class KittiSplit(_Frames):
                     img_shape=png_shape(self.path("image_2", idx, "png")), sample_idx=idx)
 
     def frame(self, idx):
-        return read_points(self.path(self.lidar, idx, "bin")), self.meta(idx)
+        meta = self.meta(idx)
+        if self.gt_classes is None:
+            return read_points(self.path(self.lidar, idx, "bin")), meta
+        gt = gt_from_anno(read_label(self.path("label_2", idx, "txt")), meta["calib"], self.gt_classes)
+        return read_points(self.path(self.lidar, idx, "bin")), meta, gt
 
     def gt_annos(self, ids=None):
         if not self.labelled:
@@ -220,7 +254,8 @@ class KittiDrive(_Frames):
 
 class Prefetcher:
     """Reads batches of frames ``depth`` batches ahead on a thread pool (np.fromfile releases the GIL) and yields
-    (ids, points_list, metas) in order.  ``wait`` accumulates the seconds the consumer spent blocked on reads."""
+    (ids, points_list, metas) in order, or (ids, points_list, metas, gts) when the split's frames carry their ground
+    truth (KittiSplit's ``gt_classes``).  ``wait`` accumulates the seconds the consumer spent blocked on reads."""
 
     def __init__(self, split, batches, depth=4, workers=4):
         self.split, self.batches, self.depth = split, batches, max(1, int(depth))
@@ -244,6 +279,6 @@ class Prefetcher:
                     pending.append((self.batches[nxt], self._submit(self.batches[nxt])))
                     nxt += 1
                 frames = [fr if fr is not None else self.split.pad_frame() for fr in frames]
-                yield ids, [p for p, _ in frames], [m for _, m in frames]
+                yield (ids,) + tuple(list(parts) for parts in zip(*frames))
         finally:
             self.pool.shutdown(wait=True, cancel_futures=True)

@@ -251,8 +251,19 @@ def get_mAP(prec):
     return sum(prec[..., i] for i in range(0, prec.shape[-1], 4)) / 11 * 100
 
 
-def official_eval(gt_annos, dt_annos, current_classes, difficultys=(0, 1, 2), overlap_fn=None):
-    """-> (text, dict(bbox, bev, d3, aos) of AP arrays [class, difficulty, min_overlap])."""
+def get_mAP_R40(prec):
+    """AP at 40 recall positions over the same 41 samples: recall 1/40 ... 1, recall 0 dropped (the KITTI benchmark's
+    AP since 2019, which the reference's readme quotes)."""
+    return sum(prec[..., i] for i in range(1, prec.shape[-1])) / 40 * 100
+
+
+def official_eval(gt_annos, dt_annos, current_classes, difficultys=(0, 1, 2), overlap_fn=None, recall_positions=11):
+    """-> (text, dict(bbox, bev, d3, aos) of AP arrays [class, difficulty, min_overlap]).  ``recall_positions``: 11
+    (get_mAP, the reference's table) or 40 (get_mAP_R40; the text's headings then read AP_R40)."""
+    if recall_positions not in (11, 40):
+        raise ValueError("recall_positions must be 11 or 40, not %r" % (recall_positions,))
+    get_mAP_n = get_mAP if recall_positions == 11 else get_mAP_R40
+    tag = "AP" if recall_positions == 11 else "AP_R40"
     if not isinstance(current_classes, (list, tuple)):
         current_classes = [current_classes]
     name_to_class = {v: k for k, v in CLASS_TO_NAME.items()}
@@ -265,13 +276,13 @@ def official_eval(gt_annos, dt_annos, current_classes, difficultys=(0, 1, 2), ov
             break
     diffs = list(difficultys)
     r0 = eval_class(gt_annos, dt_annos, classes, diffs, 0, min_overlaps, compute_aos, overlap_fn)
-    ap = dict(bbox=get_mAP(r0["precision"]), aos=get_mAP(r0["orientation"]) if compute_aos else None,
-              bev=get_mAP(eval_class(gt_annos, dt_annos, classes, diffs, 1, min_overlaps, False, overlap_fn)["precision"]),
-              d3=get_mAP(eval_class(gt_annos, dt_annos, classes, diffs, 2, min_overlaps, False, overlap_fn)["precision"]))
+    ap = dict(bbox=get_mAP_n(r0["precision"]), aos=get_mAP_n(r0["orientation"]) if compute_aos else None,
+              bev=get_mAP_n(eval_class(gt_annos, dt_annos, classes, diffs, 1, min_overlaps, False, overlap_fn)["precision"]),
+              d3=get_mAP_n(eval_class(gt_annos, dt_annos, classes, diffs, 2, min_overlaps, False, overlap_fn)["precision"]))
     lines = []
     for j, cls in enumerate(classes):
         for i in range(min_overlaps.shape[0]):
-            lines.append("%s AP@%.2f, %.2f, %.2f:" % ((CLASS_TO_NAME[cls],) + tuple(min_overlaps[i, :, j])))
+            lines.append("%s %s@%.2f, %.2f, %.2f:" % ((CLASS_TO_NAME[cls], tag) + tuple(min_overlaps[i, :, j])))
             for key, label in (("bbox", "bbox AP"), ("bev", "bev  AP"), ("d3", "3d   AP")):
                 lines.append("%s:%.2f, %.2f, %.2f" % (label, ap[key][j, 0, i], ap[key][j, 1, i], ap[key][j, 2, i]))
             if compute_aos:

@@ -88,6 +88,11 @@ def project_velo_to_rect(pts_velo, calib):
     return (_homogeneous(pts_velo) @ calib.V2C.T) @ calib.R0.T
 
 
+def project_rect_to_velo(pts_rect, calib):
+    """kitti_utils.py:173-191 (rect -> ref through inv(R0), ref -> velo through C2V), float64."""
+    return _homogeneous(pts_rect @ np.linalg.inv(calib.R0).T) @ calib.C2V.T
+
+
 def project_rect_to_image(pts_rect, calib):
     """kitti_utils.py:194-202."""
     uvw = _homogeneous(pts_rect) @ calib.P2.T

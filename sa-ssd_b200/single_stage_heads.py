@@ -30,9 +30,17 @@ def stage_gt(gt_bboxes, gt_class, gt_labels, device):
     i32 and d_ngt [B] i32.  gt_cap is the batch's largest count, at most the kernels' capacity SASSD_GT_CAP_MAX; d_ngt
     holds the true counts, so a frame with more boxes sets SASSD_FLAG_GT_CAP on the device and the caller raises.
     ``gt_class`` (anchor class index per box, -1 none) and ``gt_labels`` default to 0 and 1."""
+    t = lambda a: torch.from_numpy(a).to(device)       # noqa: E731
+    return tuple(t(a) for a in gt_arrays(gt_bboxes, gt_class, gt_labels))
+
+
+def gt_arrays(gt_bboxes, gt_class, gt_labels, gt_cap=None):
+    """stage_gt's layout on the host: numpy (gt, gt_class, gt_label, n).  ``gt_cap`` defaults to the batch's largest
+    count; a captured step passes its fixed SASSD_GT_CAP_MAX."""
     B = len(gt_bboxes)
     gt_bboxes = [(g.detach().cpu().numpy() if torch.is_tensor(g) else np.asarray(g)).reshape(-1, 7) for g in gt_bboxes]
-    gt_cap = min(max([1] + [g.shape[0] for g in gt_bboxes]), ops._lib.GT_CAP_MAX)
+    if gt_cap is None:
+        gt_cap = min(max([1] + [g.shape[0] for g in gt_bboxes]), ops._lib.GT_CAP_MAX)
     gt = np.zeros((B, gt_cap, 7), np.float32)
     cls = np.zeros((B, gt_cap), np.int32)
     lab = np.ones((B, gt_cap), np.int32)
@@ -46,8 +54,7 @@ def stage_gt(gt_bboxes, gt_class, gt_labels, device):
         if gt_labels is not None:
             lv = gt_labels[b]
             lab[b, :k] = (lv.detach().cpu().numpy() if torch.is_tensor(lv) else np.asarray(lv)).reshape(-1)[:k]
-    t = lambda a: torch.from_numpy(a).to(device)
-    return t(gt), t(cls), t(lab), t(n)
+    return gt, cls, lab, n
 
 
 def _as_class_dict(v):

@@ -2,6 +2,7 @@
 
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR [--split val] [--batch 16]
                               [--lidar velodyne|velodyne_reduced] [--out DIR] [--workers N] [--json FILE]
+                              [--losses] [--r40]
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR --split test --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --drive DRIVE_DIR [--calib-dir DIR] --out DIR [...]
 
@@ -9,7 +10,14 @@ Frames are read from disk a few batches ahead (kitti_data.Prefetcher) and stream
 (SingleStageDetector.detect_stream): full sweeps (``--lidar velodyne``) are cropped to the camera frustum on the
 device, and every step ends with the KITTI result formatter on the device (ops.kitti_format).  The last batch is
 padded with empty frames whose results are dropped.  Prints the official AP table (kitti_eval), the frame rate (wall
-clock of the streamed detection, the evaluation excluded) and the time spent waiting on reads.
+clock of the streamed detection, the evaluation excluded) and the time spent waiting on reads.  ``--r40`` also prints
+the table at 40 recall positions (kitti_eval.official_eval(recall_positions=40)).
+
+``--losses`` (labelled splits): every frame also carries its ground truth (kitti_data.gt_from_anno) and the captured
+step computes SA-SSD's six losses beside the detections (detect_stream(losses=True)); the result files and AP tables
+are those of a run without it.  The driver prints each loss's mean over the batches that hold a real frame.  A
+batch's losses are normalised per batch (by its frame count and positives), so the values depend on ``--batch``, as
+the reference's depend on imgs_per_gpu; the last batch's padding frames count as frames without GT.
 
 The test split (``testing/``) and raw drives (kitti_data.KittiDrive) have no labels: the driver writes the result
 files (``--out`` is required) and prints the frame rate and read wait only.  A raw drive's full sweeps are cropped on
@@ -18,7 +26,7 @@ files are named by the frames' stems, ``%010d.txt``.
 
 Under torchrun, frame i of the split goes to rank i mod W; at the end every rank contributes one fixed-size block of
 KITTI rows and counts to a single all_gather_into_tensor (dist.DetectionGather) and rank 0 re-interleaves, writes and
-evaluates.
+evaluates; with ``--losses`` one more all_gather brings every rank's per-batch loss vectors to rank 0.
 """
 import argparse
 import json
@@ -53,9 +61,17 @@ def parse_args(argv=None):
     p.add_argument("--workers", type=int, default=4, help="reader threads")
     p.add_argument("--depth", type=int, default=4, help="batches read ahead")
     p.add_argument("--json", default=None, help="write the AP arrays and rates here")
+    p.add_argument("--losses", action="store_true",
+                   help="also compute SA-SSD's losses against the split's labels in the detection step and print "
+                        "their means over the batches")
+    p.add_argument("--r40", action="store_true", help="also print the AP table at 40 recall positions")
     args = p.parse_args(argv)
     if args.batch < 1:
         p.error("--batch must be positive")
+    if args.losses and (args.drive or args.split == "test"):
+        p.error("--losses needs a labelled split: %s has no labels" % ("--drive" if args.drive else "--split test"))
+    if args.r40 and (args.drive or args.split == "test"):
+        p.error("--r40 needs a labelled split: %s has no labels" % ("--drive" if args.drive else "--split test"))
     if args.drive:
         if args.lidar == "velodyne_reduced":
             p.error("--drive reads full sweeps: --lidar velodyne_reduced does not apply")
@@ -93,6 +109,19 @@ def gather_annos(annos_local, ids, class_names, cap, device):
     rows_all = rows_all.contiguous().view(torch.float64)[:len(ids)].cpu().numpy()
     n_all = n_all[:len(ids)].cpu().numpy()
     return annos_from_rows(rows_all, n_all, class_names, ids)
+
+
+def gather_losses(losses_local, n_real, device):
+    """Every rank's per-batch loss vectors (ops.LOSS_KEYS order) and real-frame counts -> the vectors of the batches
+    that hold a real frame, on every rank, in (batch, rank) order, through one all_gather (dist.DetectionGather)."""
+    import torch
+    from . import dist as D
+    from . import ops
+    width = len(ops.LOSS_KEYS)
+    g = D.DetectionGather(len(n_real), 1, device, width=width)
+    vec = torch.tensor(losses_local, dtype=torch.float32).reshape(len(n_real), 1, width)
+    vec_all, n_all = D.interleave(*g(vec.to(device), torch.tensor(n_real, dtype=torch.int32).to(device)))
+    return [v[0].tolist() for v, n in zip(vec_all.cpu(), n_all.cpu().tolist()) if n > 0]
 
 
 def write_results(out_dir, ids, annos, name="%06d.txt"):
@@ -136,22 +165,29 @@ def run(args, log=print):
     fov = bool(args.drive)
     crop = args.lidar == "velodyne" and not fov
     class_names = model.class_names
+    if args.losses:                     # from here on every frame carries its GT over the model's classes
+        split = KittiSplit(args.data_root, args.split, args.lidar, gt_classes=class_names)
 
     def items(reader):
-        for ids, points, metas in reader:
-            if crop:
-                yield points, [split.planes(m["calib"], m["img_shape"]) for m in metas], metas
-            else:
-                yield points, metas
+        for ids, points, metas, *gts in reader:
+            item = (points, [split.planes(m["calib"], m["img_shape"]) for m in metas], metas) if crop else (points, metas)
+            if args.losses:
+                item += (([b for b, _ in gts[0]], [l for _, l in gts[0]]),)
+            yield item
 
     stream = lambda src: model.detect_stream(src, args.batch, args.max_points, depth=4, crop=crop,  # noqa: E731
-                                             kitti=True, image_fov=fov)
+                                             kitti=True, image_fov=fov, losses=args.losses)
     for _ in stream([]):                # capture the slots' graphs before the clock starts
         pass
     torch.cuda.synchronize(device)
     reader = Prefetcher(split, batches, depth=args.depth, workers=args.workers)
     t0 = time.perf_counter()
-    annos_local = [a for annos in stream(items(reader)) for a in annos]
+    annos_local, losses_local = [], []
+    for out in stream(items(reader)):
+        if args.losses:
+            out, losses = out
+            losses_local.append([losses[k] for k in ops.LOSS_KEYS])
+        annos_local += out
     torch.cuda.synchronize(device)
     wall = time.perf_counter() - t0
     n_local = sum(i is not None for ids in batches for i in ids)
@@ -161,6 +197,8 @@ def run(args, log=print):
         dt_annos = gather_annos(annos_local, split.ids, class_names, model.extra_head.det_cap, device)
     else:
         dt_annos = [a for i, a in zip([i for ids in batches for i in ids], annos_local) if i is not None]
+    if args.losses:
+        per_batch = gather_losses(losses_local, [sum(i is not None for i in ids) for ids in batches], device)
     if rank != 0:
         D.barrier()
         return None
@@ -180,8 +218,19 @@ def run(args, log=print):
     gt_annos = split.gt_annos()
     text, ap = official_eval(gt_annos, dt_annos, class_names)
     log(text, end="")
+    as_lists = lambda ap: {k: (None if v is None else np.asarray(v).tolist()) for k, v in ap.items()}  # noqa: E731
+    result.update(text=text, ap=as_lists(ap))
+    if args.r40:
+        text40, ap40 = official_eval(gt_annos, dt_annos, class_names, recall_positions=40)
+        log(text40, end="")
+        result.update(text_r40=text40, ap_r40=as_lists(ap40))
+    if args.losses:
+        means = np.mean(np.asarray(per_batch, np.float64), axis=0)
+        log("losses: mean over %d batches of %d frames (per-batch values depend on --batch): %s" % (
+            len(per_batch), args.batch, ", ".join("%s %.6f" % (k, v) for k, v in zip(ops.LOSS_KEYS, means))))
+        result.update(losses=dict(zip(ops.LOSS_KEYS, means.tolist())),
+                      losses_per_batch=[dict(zip(ops.LOSS_KEYS, v)) for v in per_batch])
     log(rate)
-    result.update(text=text, ap={k: (None if v is None else np.asarray(v).tolist()) for k, v in ap.items()})
     _write_json(args.json, result)
     D.barrier()
     return result
