@@ -51,8 +51,10 @@ enum { /* bits of *d_status */
     SASSD_FLAG_HASH_FULL = 16,
     SASSD_FLAG_DET_CAP = 32,    /* boxes kept by the NMS exceed the detection capacity: the first det_cap kept
                                    boxes in score order are returned */
-    SASSD_FLAG_GT_CAP = 64      /* ground-truth boxes per frame exceed gt_cap: the first gt_cap boxes are used
-                                   (sassd_points_in_boxes, sassd_assign_*) */
+    SASSD_FLAG_GT_CAP = 64,     /* ground-truth boxes per frame exceed gt_cap: the first gt_cap boxes are used
+                                   (sassd_points_in_boxes, sassd_assign_*, sassd_points_in_rbboxes) */
+    SASSD_FLAG_GATHER_CAP = 128 /* gathered rows exceed gather_cap: rows past it are not written
+                                   (sassd_points_in_rbboxes) */
 };
 
 int sassd_version(void);
@@ -135,6 +137,36 @@ int sassd_frustum_crop(const float* points, const int32_t* d_pt_off, int n_point
 int sassd_image_fov_crop(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch,
                          const double* meta, float clip_x, float* points_out, int32_t* d_pt_off_out,
                          void* ws, size_t ws_bytes, sassd_stream_t stream);
+
+/* ------------------------------------------------------------------------
+ * Points in rotated boxes, gathered per box: the reference's ground-truth
+ * database and num_points_in_gt (tools/create_data.py:16-45, 233-240 ->
+ * points_in_rbbox, mmdet/core/bbox3d/geometry.py:63-74, 190-226).
+ *
+ * points / d_pt_off as for sassd_frustum_crop (the cropped frames);
+ * planes [batch][box_cap][6][4] fp64 (n.x, n.y, n.z, d, inward normals),
+ * centres [batch][box_cap][3] fp64 (box x, y, z, LiDAR frame), d_nbox [batch]:
+ * slots j < d_nbox[b] of frame b are boxes.  Point i of frame b is in box j
+ * under sassd_frustum_crop's test (fp64, no contraction, `s >= 0` rejects:
+ * a NaN coordinate is in every box, a box of zero size holds nothing); a point
+ * may be in several boxes.  Outputs:
+ *   counts [batch][box_cap]       members per slot (0 for empty slots),
+ *   seg_off [batch*box_cap + 1]   exclusive offsets of the slots' rows,
+ *   gathered [gather_cap][4]      box (b, j)'s members in input order, each
+ *                                 x, y, z as (float)((double)p - centre) and
+ *                                 the reflectance unchanged (a NaN keeps its bits).
+ * More rows than gather_cap: the rest are not written and
+ * SASSD_FLAG_GATHER_CAP is set (counts and seg_off stay exact); d_nbox[b] >
+ * box_cap sets SASSD_FLAG_GT_CAP and uses the first box_cap boxes.  gathered
+ * may be NULL when gather_cap is 0 (counts only).  box_cap <= SASSD_GT_CAP_MAX,
+ * batch <= 256.  No host synchronisation, no allocation: graph-capturable.
+ * Argument checks and error codes as for sassd_frustum_crop.
+ * ---------------------------------------------------------------------- */
+size_t sassd_points_in_rbboxes_workspace_bytes(int n_points_cap, int batch, int box_cap);
+int sassd_points_in_rbboxes(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch,
+                            const double* planes, const double* centres, const int32_t* d_nbox, int box_cap,
+                            int32_t* counts, int32_t* seg_off, float* gathered, int gather_cap,
+                            int32_t* d_status, void* ws, size_t ws_bytes, sassd_stream_t stream);
 
 /* ------------------------------------------------------------------------
  * anchors_mask.  Replaces mmdet/datasets/kitti.py:333-343 +

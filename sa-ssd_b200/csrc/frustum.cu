@@ -190,3 +190,145 @@ extern "C" int sassd_image_fov_crop(const float* points, const int32_t* d_pt_off
     return crop_launch(points, d_pt_off, n_points_cap, batch, meta, ImageFovKeep{meta, clip_x}, points_out,
                        d_pt_off_out, ws, ws_bytes, stream);
 }
+
+// ------------------------------------------------------------------------------------------------------------------
+// Points in rotated boxes, gathered per box: the reference's ground-truth database step (tools/create_data.py:233-240 ->
+// points_in_rbbox, geometry.py:63-74, then gt_points[:, :3] -= box[:3]) and its num_points_in_gt (create_data.py:16-45).
+// The membership test is fc_inside, the frustum crop's, applied to each box's 6 planes.
+//
+// One CTA per (frame, box slot) q = b * box_cap + j scans frame b twice: once to count its members, then - after the
+// count's exclusive prefix over q is known from a decoupled look-back (sassd_lookback, one descriptor per q) - to write
+// them in input order at seg_off[q] + rank, ranked like crop_kernel's rows.  The second scan stops after the box's last
+// member.  A gathered row is (float)((double)p - c) per coordinate, numpy's float32 -= float64; a NaN coordinate keeps
+// its bits (quieted), as the host's double round trip does.  Slots j >= nbox[b] count nothing.
+__device__ __forceinline__ float rb_shift(float v, double c) {
+    return isnan(v) ? __int_as_float(__float_as_int(v) | 0x00400000) : __double2float_rn(__dsub_rn((double)v, c));
+}
+
+__global__ void __launch_bounds__(FC_THREADS)
+rbbox_gather_kernel(const float4* __restrict__ points, const int* __restrict__ pt_off, int n_cap,
+                    const double* __restrict__ planes, const double* __restrict__ centres, const int* __restrict__ nbox,
+                    int box_cap, int* __restrict__ counts, int* __restrict__ seg_off, float4* __restrict__ gathered,
+                    int gather_cap, int* __restrict__ status, unsigned long long* __restrict__ desc) {
+    __shared__ unsigned s_ball[FC_ROWS * FC_WARPS];
+    __shared__ int s_ex[FC_ROWS * FC_WARPS];
+    __shared__ int s_red[FC_WARPS];
+    __shared__ int s_base, s_total, s_chunk;
+    const int q = blockIdx.x, b = q / box_cap, j = q - b * box_cap;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int lo = min(max(__ldg(&pt_off[b]), 0), n_cap);
+    const int hi = max(min(max(__ldg(&pt_off[b + 1]), 0), n_cap), lo);
+    const int nb = __ldg(&nbox[b]);
+    if (j == 0 && threadIdx.x == 0 && nb > box_cap) atomicOr(status, SASSD_FLAG_GT_CAP);
+    const bool active = j < nb;
+    const double* pl = planes + (size_t)q * 24;
+
+    int cnt = 0;
+    if (active)
+        for (int c0 = lo; c0 < hi; c0 += FC_CHUNK) {
+            float4 p[FC_ROWS];
+#pragma unroll
+            for (int r = 0; r < FC_ROWS; ++r) {
+                const int i = c0 + r * FC_THREADS + (int)threadIdx.x;
+                if (i < hi) p[r] = __ldg(&points[i]);
+            }
+#pragma unroll
+            for (int r = 0; r < FC_ROWS; ++r)
+                if (c0 + r * FC_THREADS + (int)threadIdx.x < hi && fc_inside(p[r], pl)) ++cnt;
+        }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if (lane == 0) s_red[warp] = cnt;
+    __syncthreads();
+    if (warp == 0) {
+        int total = lane < FC_WARPS ? s_red[lane] : 0;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+        volatile unsigned long long* vd = desc;
+        if (q > 0 && lane == 0) vd[q] = (SASSD_SCAN_AGG << 32) | (unsigned)total;
+        const int base = sassd_lookback(vd, q, lane);
+        if (lane == 0) {
+            vd[q] = (SASSD_SCAN_PREFIX << 32) | (unsigned)(base + total);
+            counts[q] = total;
+            seg_off[q] = base;
+            if (q == (int)gridDim.x - 1) {
+                seg_off[q + 1] = base + total;
+                if (base + total > gather_cap) atomicOr(status, SASSD_FLAG_GATHER_CAP);
+            }
+            s_base = base;
+            s_total = total;
+        }
+    }
+    __syncthreads();
+    const int base = s_base, end = min(base + s_total, gather_cap);
+    if (!gathered || base >= end) return;
+    const double cx = __ldg(&centres[3 * (size_t)q]), cy = __ldg(&centres[3 * (size_t)q + 1]),
+                 cz = __ldg(&centres[3 * (size_t)q + 2]);
+    const unsigned lt = (1u << lane) - 1u;
+    int run = base;
+    for (int c0 = lo; c0 < hi && run < end; c0 += FC_CHUNK) {
+        float4 p[FC_ROWS];
+        unsigned keep = 0;
+#pragma unroll
+        for (int r = 0; r < FC_ROWS; ++r) {
+            const int i = c0 + r * FC_THREADS + (int)threadIdx.x;
+            if (i < hi) p[r] = __ldg(&points[i]);
+        }
+#pragma unroll
+        for (int r = 0; r < FC_ROWS; ++r)
+            if (c0 + r * FC_THREADS + (int)threadIdx.x < hi && fc_inside(p[r], pl)) keep |= 1u << r;
+#pragma unroll
+        for (int r = 0; r < FC_ROWS; ++r) {
+            const unsigned bal = __ballot_sync(0xffffffffu, (keep >> r) & 1u);
+            if (lane == 0) s_ball[r * FC_WARPS + warp] = bal;
+        }
+        __syncthreads();
+        if (warp == 0) {
+            const int a = __popc(s_ball[2 * lane]), c = __popc(s_ball[2 * lane + 1]);
+            int inc = a + c;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const int t = __shfl_up_sync(0xffffffffu, inc, d);
+                if (lane >= d) inc += t;
+            }
+            s_ex[2 * lane] = inc - a - c;
+            s_ex[2 * lane + 1] = inc - c;
+            if (lane == 31) s_chunk = inc;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int r = 0; r < FC_ROWS; ++r)
+            if ((keep >> r) & 1u) {
+                const int k = r * FC_WARPS + warp;
+                const int o = run + s_ex[k] + __popc(s_ball[k] & lt);
+                if (o < end) gathered[o] = make_float4(rb_shift(p[r].x, cx), rb_shift(p[r].y, cy), rb_shift(p[r].z, cz), p[r].w);
+            }
+        run += s_chunk;
+        __syncthreads();    // s_ball / s_ex / s_chunk are rewritten by the next chunk
+    }
+}
+
+extern "C" size_t sassd_points_in_rbboxes_workspace_bytes(int n_points_cap, int batch, int box_cap) {
+    (void)n_points_cap;   // one look-back descriptor per (frame, box slot)
+    return (size_t)(batch > 0 ? batch : 0) * (size_t)(box_cap > 0 ? box_cap : 0) * sizeof(unsigned long long);
+}
+
+extern "C" int sassd_points_in_rbboxes(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch,
+                                       const double* planes, const double* centres, const int32_t* d_nbox, int box_cap,
+                                       int32_t* counts, int32_t* seg_off, float* gathered, int gather_cap,
+                                       int32_t* d_status, void* ws, size_t ws_bytes, sassd_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (!points || !d_pt_off || !planes || !centres || !d_nbox || !counts || !seg_off || !d_status || !ws)
+        return SASSD_ERR_ARG;
+    if (batch < 1 || batch > FC_MAX_BATCH || n_points_cap < 0) return SASSD_ERR_ARG;
+    if (box_cap < 1 || box_cap > SASSD_GT_CAP_MAX || gather_cap < 0 || (!gathered && gather_cap > 0))
+        return SASSD_ERR_ARG;
+    if (gathered == points) return SASSD_ERR_ARG;
+    if (ws_bytes < sassd_points_in_rbboxes_workspace_bytes(n_points_cap, batch, box_cap)) return SASSD_ERR_WORKSPACE;
+    const int segs = batch * box_cap;
+    cudaMemsetAsync(ws, 0, (size_t)segs * sizeof(unsigned long long), stream);   // descriptors: nothing published
+    rbbox_gather_kernel<<<segs, FC_THREADS, 0, stream>>>((const float4*)points, d_pt_off, n_points_cap, planes, centres,
+                                                         d_nbox, box_cap, counts, seg_off, (float4*)gathered,
+                                                         gather_cap, d_status, (unsigned long long*)ws);
+    return sassd_check_launch();
+}

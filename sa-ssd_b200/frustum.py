@@ -45,10 +45,16 @@ def frustum_corners(calib, img_shape):
     return (np.concatenate([cam.T, np.ones((8, 1))], axis=1) @ rect_to_velo.T)[:, :3]
 
 
+def corner_planes(corners):
+    """Corners [..., 8, 3] in the reference's layout (near/bottom face 0-3, far/top face 4-7) -> float64 [..., 6, 4]:
+    one plane per face from its first three corners, n = (c0 - c1) x (c1 - c2), d = -n.c0, normals pointing inside."""
+    c = corners[..., _FACES, :]                                               # [..., 6, 4, 3]
+    n = np.cross(c[..., 0, :] - c[..., 1, :], c[..., 1, :] - c[..., 2, :])
+    d = -(n * c[..., 0, :]).sum(axis=-1)
+    return np.concatenate([n, d[..., None]], axis=-1)
+
+
 def camera_frustum_planes(calib, img_shape):
     """results.Calibration + image (h, w) -> float64 [6, 4]: (n.x, n.y, n.z, d) per face, normals pointing inside.
     One frame's entry of the ``frustum_planes`` argument of SingleStageDetector.forward_points / detect_stream."""
-    c = frustum_corners(calib, img_shape)[_FACES]                             # [6, 4, 3]
-    n = np.cross(c[:, 0] - c[:, 1], c[:, 1] - c[:, 2])
-    d = -(n * c[:, 0]).sum(axis=1)
-    return np.concatenate([n, d[:, None]], axis=1)
+    return corner_planes(frustum_corners(calib, img_shape))

@@ -51,7 +51,7 @@ def next_pow2(n):
 
 # --- launch accounting / optional per-call CUDA-event timing (bench.py) ---------------
 # kernels launched by each C-ABI entry point (memsets not counted)
-_KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
+_KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_points_in_rbboxes": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
             "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
@@ -159,6 +159,34 @@ def image_fov_crop(points, pt_off, batch, meta, clip_x=IMAGE_FOV_CLIP_X, ws=None
     _call("sassd_image_fov_crop", None, _ptr(points), _ptr(pt_off), n_cap, batch, _ptr(meta), float(clip_x), _ptr(out),
           _ptr(off), _ptr(w), w.numel(), _stream())
     return out, off
+
+
+def points_in_rbboxes(points, pt_off, batch, planes, centres, nbox, gather_cap, status=None, ws=None):
+    """points [Ncap,4] f32, pt_off [batch+1] i32 (device; frustum_crop's outputs), planes [batch,box_cap,6,4] f64,
+    centres [batch,box_cap,3] f64, nbox [batch] i32 (device; create_data.box_planes).  Returns (counts
+    [batch,box_cap] i32, seg_off [batch*box_cap+1] i32, gathered [gather_cap,4] f32, status [1] i32): the members of
+    box (b, j) are gathered[seg_off[b*box_cap+j]:][:counts[b,j]] in input order, x, y, z relative to the box centre
+    (the reference's points_in_rbbox and gt database rows).  Raise on ``status`` (lib.raise_on_status) after the
+    caller's sync: GATHER_CAP when more than gather_cap rows were due, GT_CAP when nbox exceeds box_cap."""
+    dev = points.device
+    n_cap = points.shape[0]
+    box_cap = planes.shape[1] if planes.dim() == 4 else -1
+    assert planes.dtype == torch.float64 and tuple(planes.shape) == (batch, box_cap, 6, 4), \
+        "planes must be float64 [batch,box_cap,6,4]"
+    assert centres.dtype == torch.float64 and tuple(centres.shape) == (batch, box_cap, 3), \
+        "centres must be float64 [batch,box_cap,3]"
+    assert nbox.dtype == torch.int32 and tuple(nbox.shape) == (batch,), "nbox must be int32 [batch]"
+    if status is None:
+        status = torch.zeros((1,), dtype=torch.int32, device=dev)
+    counts = torch.empty((batch, box_cap), dtype=torch.int32, device=dev)
+    seg_off = torch.empty((batch * box_cap + 1,), dtype=torch.int32, device=dev)
+    gathered = torch.empty((max(int(gather_cap), 1), 4), dtype=torch.float32, device=dev)
+    nbytes = _L().sassd_points_in_rbboxes_workspace_bytes(n_cap, batch, box_cap)
+    w = (ws or _WS).get("rbboxes", nbytes, dev)
+    _call("sassd_points_in_rbboxes", None, _ptr(points), _ptr(pt_off), n_cap, batch, _ptr(planes), _ptr(centres),
+          _ptr(nbox), box_cap, _ptr(counts), _ptr(seg_off), _ptr(gathered), int(gather_cap), _ptr(status), _ptr(w),
+          w.numel(), _stream())
+    return counts, seg_off, gathered, status
 
 
 def voxel_mean(voxels, num_points, d_rows=None):
