@@ -1,6 +1,6 @@
 # Single-class (Car) SA-SSD inference config in the reference's config dialect
 # (same keys/values as the reference's configs/car_cfg.py for model, test_cfg and the
-# data-side voxel/anchor generators; the dataset's training sections are omitted).  The
+# data-side voxel/anchor generators; of the training data section only the augmentor).  The
 # reference's own file also loads unchanged through sassd_b200.Config.fromfile.
 model = dict(
     type='SingleStageDetector',
@@ -34,6 +34,14 @@ _generator = dict(type='VoxelGenerator', voxel_size=[0.05, 0.05, 0.1],
 _anchor = dict(type='AnchorGeneratorStride', anchor_strides=[0.4, 0.4, 1.0],
                anchor_offsets=[0.2, -39.8, -1.78], rotations=[0, 1.57])
 data = dict(
+    # Training-time augmentation (sassd_b200.augment): the reference's data.train.augmentor; `--data-root` replaces
+    # root_path and info_path with paths under that root.
+    train=dict(class_names=['Car'], generator=_generator,
+               augmentor=dict(type='PointAugmentor', root_path='data/kitti/',
+                              info_path='data/kitti/kitti_dbinfos_train.pkl', sample_classes=['Car'],
+                              min_num_points=[5], sample_max_num=[15], removed_difficulties=[-1],
+                              global_rot_range=[-0.78539816, 0.78539816], gt_rot_range=[-0.78539816, 0.78539816],
+                              center_noise_std=[1., 1., .5], scale_range=[0.95, 1.05])),
     val=dict(class_names=['Car'], generator=_generator,
              anchor_generator=dict(Car=dict(_anchor, sizes=[1.6, 3.9, 1.56])),
              anchor_area_threshold=1, out_size_factor=8, test_mode=True),

@@ -1,5 +1,6 @@
 # Three-class (Car / Pedestrian / Cyclist) SA-SSD inference config; differs from car_cfg.py
-# only in num_class, the class list and the two extra anchor sets (reference configs/multi_cfg.py).
+# only in num_class, the class lists, the two extra anchor sets and the augmentor's per-class sampling
+# (reference configs/multi_cfg.py).
 model = dict(
     type='SingleStageDetector',
     backbone=dict(type='SimpleVoxel', num_input_features=4, use_norm=True, num_filters=[32, 64],
@@ -34,6 +35,14 @@ _generator = dict(type='VoxelGenerator', voxel_size=[0.05, 0.05, 0.1],
 _anchor = dict(type='AnchorGeneratorStride', anchor_strides=[0.4, 0.4, 1.0],
                anchor_offsets=[0.2, -39.8, -1.78], rotations=[0, 1.57])
 data = dict(
+    # Training-time augmentation (sassd_b200.augment): the reference's data.train.augmentor; `--data-root` replaces
+    # root_path and info_path with paths under that root.
+    train=dict(class_names=['Car', 'Pedestrian', 'Cyclist'], generator=_generator,
+               augmentor=dict(type='PointAugmentor', root_path='data/kitti/',
+                              info_path='data/kitti/kitti_dbinfos_train.pkl', sample_classes=['Car', 'Pedestrian', 'Cyclist'],
+                              min_num_points=[5, 5, 5], sample_max_num=[15, 10, 10], removed_difficulties=[-1],
+                              global_rot_range=[-0.78539816, 0.78539816], gt_rot_range=[-0.78539816, 0.78539816],
+                              center_noise_std=[1., 1., .5], scale_range=[0.95, 1.05])),
     val=dict(class_names=['Car', 'Pedestrian', 'Cyclist'], generator=_generator,
              anchor_generator=dict(Car=dict(_anchor, sizes=[1.6, 3.9, 1.56]),
                                    Pedestrian=dict(_anchor, sizes=[0.6, 0.8, 1.73]),

@@ -53,8 +53,10 @@ enum { /* bits of *d_status */
                                    boxes in score order are returned */
     SASSD_FLAG_GT_CAP = 64,     /* ground-truth boxes per frame exceed gt_cap: the first gt_cap boxes are used
                                    (sassd_points_in_boxes, sassd_assign_*, sassd_points_in_rbboxes) */
-    SASSD_FLAG_GATHER_CAP = 128 /* gathered rows exceed gather_cap: rows past it are not written
+    SASSD_FLAG_GATHER_CAP = 128, /* gathered rows exceed gather_cap: rows past it are not written
                                    (sassd_points_in_rbboxes) */
+    SASSD_FLAG_POINTS_CAP = 256 /* augmented rows exceed out_cap: rows past it are not written
+                                   (sassd_augment_assemble) */
 };
 
 int sassd_version(void);
@@ -540,6 +542,48 @@ int sassd_kitti_match(int nframes, const double* overlaps, const int64_t* ov_off
                       const double* dt_score, const double* dt_bbox, const double* dc_bbox, const int32_t* ign_gt,
                       const int32_t* ign_dt, int metric, double min_overlap, int compute_aos, int nthresh,
                       const double* thresholds, double* pr, double* tp_scores, int64_t* n_tp_scores);
+
+/* ------------------------------------------------------------------------
+ * Training-time augmentation (the reference's PointAugmentor as
+ * prepare_train_img applies it, mmdet/core/point_cloud/point_augmentor.py,
+ * mmdet/datasets/kitti.py:181-209).  The host draws every random number and
+ * computes the box geometry; boxes of frame b are [d_box_off[b], d_box_off[b+1]).
+ *
+ * sassd_augment_drop_points: sassd_frustum_crop's compaction, keeping the
+ * points of frame b outside every box of frame b, under the reference's plane
+ * test in fp32 (planes [boxes][6][4] fp32, `s >= 0` rejects).  Workspace:
+ * sassd_frustum_crop_workspace_bytes.
+ *
+ * sassd_augment_noise_search: noise_per_box, one CTA per frame.  boxes
+ * [boxes][5] fp32 (x, y, w, l, ry), box_trig [boxes][2] (cosf, sinf of ry),
+ * try_trig [boxes][tries][2] (cos, sin of each try's rotation, rounded to
+ * fp32), loc [boxes][tries][3] fp64 location noise.  sel[k] = the smallest
+ * try whose BEV box collides with no other box's current corners (a box fully
+ * inside another collides), or -1.  Boxes of a frame past SASSD_GT_CAP_MAX
+ * get -1 and set SASSD_FLAG_GT_CAP.  tries <= 128.
+ *
+ * sassd_augment_assemble: per frame, the database rows of its sampled
+ * records (records s in [d_srow_off..] order: rows db[d_srec_db[s] ..] of
+ * count d_srec_off[s+1] - d_srec_off[s], each x, y, z plus srec_ctr[s] fp64)
+ * followed by the rows sassd_augment_drop_points kept; each row then takes
+ * the transform of the first box whose fp32 planes contain it (centres
+ * [boxes][3] fp32, its try sel[k]), the frame's flip, rotation and scale
+ * (frame_tf [batch][6]: flip, R00, R01, R10, R11, scale).  More than out_cap
+ * rows: the rest are not written and SASSD_FLAG_POINTS_CAP is set
+ * (d_pt_off_out stays exact).  batch <= 256.
+ * ---------------------------------------------------------------------- */
+int sassd_augment_drop_points(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch,
+                              const float* planes, const int32_t* d_box_off, float* points_out,
+                              int32_t* d_pt_off_out, void* ws, size_t ws_bytes, sassd_stream_t stream);
+int sassd_augment_noise_search(const float* boxes, const float* box_trig, const int32_t* d_box_off, int batch,
+                               int tries, const float* try_trig, const double* loc, int32_t* sel,
+                               int32_t* d_status, sassd_stream_t stream);
+int sassd_augment_assemble(const float* kept, const int32_t* d_kept_off, int batch, const int32_t* d_srow_off,
+                           const int32_t* d_srec_off, int n_rec, const int32_t* d_srec_db, const double* srec_ctr,
+                           const float* db, const int32_t* d_box_off, const float* planes, const float* centres,
+                           const int32_t* sel, int tries, const float* try_trig, const double* loc,
+                           const float* frame_tf, int out_cap, float* points_out, int32_t* d_pt_off_out,
+                           int32_t* d_status, sassd_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -64,6 +64,28 @@ __device__ __forceinline__ void sassd_mark_conv2d_tiles(int* __restrict__ tile_d
         }
 }
 
+// The reference's convex-polygon test (points_in_convex_polygon_3d_jit) for one polygon of 6 planes pl[k] = (n, d):
+// s = ((x*n0 + y*n1) + z*n2) + d in exactly that order, every operation rounded on its own (no FMA contraction), and
+// `s >= 0` rejects, so a NaN coordinate is inside.  T = double widens the fp32 point (the frustum crop and the
+// database gather, whose planes are fp64); T = float evaluates in fp32, as the reference does for float32 boxes.
+__device__ __forceinline__ double fc_mul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double fc_add(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ float fc_mul(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float fc_add(float a, float b) { return __fadd_rn(a, b); }
+template <class T>
+__device__ __forceinline__ bool fc_inside(float4 p, const T* __restrict__ pl) {
+    const T x = p.x, y = p.y, z = p.z;
+    bool in = true;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+        const T s = fc_add(fc_add(fc_add(fc_mul(x, __ldg(&pl[4 * k])), fc_mul(y, __ldg(&pl[4 * k + 1]))),
+                                  fc_mul(z, __ldg(&pl[4 * k + 2]))),
+                           __ldg(&pl[4 * k + 3]));
+        in &= !(s >= T(0));
+    }
+    return in;
+}
+
 // Decoupled look-back for single-pass scans over chunks: a chunk's descriptor is {flag << 32 | value}, flag 0 = not
 // published yet, AGG = the chunk's own total, PREFIX = inclusive prefix up to and including the chunk.
 #define SASSD_SCAN_AGG 1ull

@@ -30,19 +30,6 @@
 #define FC_CHUNK (FC_THREADS * FC_ROWS)
 static_assert(FC_ROWS * FC_WARPS == 64, "the chunk scan gives two (row, warp) counts to each lane of warp 0");
 
-__device__ __forceinline__ bool fc_inside(float4 p, const double* __restrict__ pl) {
-    const double x = p.x, y = p.y, z = p.z;
-    bool in = true;
-#pragma unroll
-    for (int k = 0; k < 6; ++k) {
-        const double s = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(x, __ldg(&pl[4 * k])), __dmul_rn(y, __ldg(&pl[4 * k + 1]))),
-                                             __dmul_rn(z, __ldg(&pl[4 * k + 2]))),
-                                   __ldg(&pl[4 * k + 3]));
-        in &= !(s >= 0.0);
-    }
-    return in;
-}
-
 struct FrustumKeep {
     const double* __restrict__ planes;    // [batch][6][4]
     __device__ __forceinline__ bool operator()(float4 p, int frame) const { return fc_inside(p, planes + (size_t)frame * 24); }
@@ -162,7 +149,7 @@ extern "C" size_t sassd_frustum_crop_workspace_bytes(int n_points_cap, int batch
 
 // argument checks shared by both crops; then the descriptor reset and the one launch
 template <class Keep>
-static int crop_launch(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch, const double* params,
+static int crop_launch(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch, const void* params,
                        Keep inside, float* points_out, int32_t* d_pt_off_out, void* ws, size_t ws_bytes,
                        sassd_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -188,6 +175,27 @@ extern "C" int sassd_image_fov_crop(const float* points, const int32_t* d_pt_off
                                     const double* meta, float clip_x, float* points_out, int32_t* d_pt_off_out,
                                     void* ws, size_t ws_bytes, sassd_stream_t stream) {
     return crop_launch(points, d_pt_off, n_points_cap, batch, meta, ImageFovKeep{meta, clip_x}, points_out,
+                       d_pt_off_out, ws, ws_bytes, stream);
+}
+
+// Keep test of the augmentation's scene crop (the reference's prepare_train_img, mmdet/datasets/kitti.py:187-189): a
+// point survives unless it is inside one of its frame's sampled boxes, under the fp32 plane test of float32 boxes.
+struct OutsideBoxesKeep {
+    const float* __restrict__ planes;     // [total boxes][6][4] fp32
+    const int* __restrict__ box_off;      // [batch + 1]: frame b's boxes are [box_off[b], box_off[b + 1])
+    __device__ __forceinline__ bool operator()(float4 p, int frame) const {
+        const int lo = __ldg(&box_off[frame]), hi = __ldg(&box_off[frame + 1]);
+        for (int j = lo; j < hi; ++j)
+            if (fc_inside(p, planes + (size_t)j * 24)) return false;
+        return true;
+    }
+};
+
+extern "C" int sassd_augment_drop_points(const float* points, const int32_t* d_pt_off, int n_points_cap, int batch,
+                                         const float* planes, const int32_t* d_box_off, float* points_out,
+                                         int32_t* d_pt_off_out, void* ws, size_t ws_bytes, sassd_stream_t stream) {
+    if (!d_box_off) return SASSD_ERR_ARG;
+    return crop_launch(points, d_pt_off, n_points_cap, batch, planes, OutsideBoxesKeep{planes, d_box_off}, points_out,
                        d_pt_off_out, ws, ws_bytes, stream);
 }
 

@@ -46,8 +46,10 @@ def frustum_corners(calib, img_shape):
 
 
 def corner_planes(corners):
-    """Corners [..., 8, 3] in the reference's layout (near/bottom face 0-3, far/top face 4-7) -> float64 [..., 6, 4]:
-    one plane per face from its first three corners, n = (c0 - c1) x (c1 - c2), d = -n.c0, normals pointing inside."""
+    """Corners [..., 8, 3] in the reference's layout (near/bottom face 0-3, far/top face 4-7) -> planes [..., 6, 4] in
+    the corners' dtype: one plane per face from its first three corners, n = (c0 - c1) x (c1 - c2), d = -n.c0, normals
+    pointing inside.  Nothing is widened: float32 corners give the reference's float32 planes (augment.box_planes32),
+    as its np.cross and einsum on float32 surfaces do."""
     c = corners[..., _FACES, :]                                               # [..., 6, 4, 3]
     n = np.cross(c[..., 0, :] - c[..., 1, :], c[..., 1, :] - c[..., 2, :])
     d = -(n * c[..., 0, :]).sum(axis=-1)

@@ -89,13 +89,10 @@ def read_label(path):
     return anno
 
 
-def gt_from_anno(anno, calib, class_names):
-    """One frame's read_label annotation -> the ground truth of the reference's labelled test path
-    (prepare_test_img(with_label=True), kitti.py:276-293): (boxes [G,7] float32 as (x, y, z_bottom, w, l, h, ry) in the
-    lidar frame, labels [G] int64, 1-based over ``class_names``).  DontCare rows are dropped, box3d is built in float32
-    (kitti_utils.py:36-37), its centre goes through project_rect_to_velo in float64 and is stored back into float32,
-    Van counts as Car, and only ``class_names`` are kept, in file order.  A frame with no box left gives [0,7] and [0]
-    (the reference's empty array there is 1-D and fails to index)."""
+def labelled_boxes(anno, calib):
+    """One frame's read_label annotation -> (boxes [G,7] float32, names [G]) of its non-DontCare objects in file order,
+    as the reference's prepare_train_img reads them (kitti.py:147-154): box3d built in float32 (kitti_utils.py:36-37),
+    its centre through project_rect_to_velo in float64 and stored back into float32; the raw names, Van included."""
     names = np.asarray(anno["name"]).reshape(-1)
     keep = names != "DontCare"
     box3d = np.concatenate([np.asarray(anno["location"]).reshape(-1, 3),
@@ -103,7 +100,17 @@ def gt_from_anno(anno, calib, class_names):
                             np.asarray(anno["rotation_y"]).reshape(-1, 1)], 1)[keep].astype(np.float32)
     if len(box3d):
         box3d[:, :3] = project_rect_to_velo(box3d[:, :3], calib)
-    types = ["Car" if n == "Van" else str(n) for n in names[keep]]
+    return box3d.reshape(-1, 7), [str(n) for n in names[keep]]
+
+
+def gt_from_anno(anno, calib, class_names):
+    """One frame's read_label annotation -> the ground truth of the reference's labelled test path
+    (prepare_test_img(with_label=True), kitti.py:276-293): (boxes [G,7] float32 as (x, y, z_bottom, w, l, h, ry) in the
+    lidar frame, labels [G] int64, 1-based over ``class_names``).  The boxes are labelled_boxes', Van counts as Car,
+    and only ``class_names`` are kept, in file order.  A frame with no box left gives [0,7] and [0] (the reference's
+    empty array there is 1-D and fails to index)."""
+    box3d, names = labelled_boxes(anno, calib)
+    types = ["Car" if n == "Van" else n for n in names]
     selected = [i for i, n in enumerate(types) if n in class_names]
     labels = np.array([list(class_names).index(types[i]) + 1 for i in selected], dtype=np.int64)
     return box3d[selected].reshape(-1, 7), labels

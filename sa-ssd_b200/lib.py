@@ -49,7 +49,7 @@ GT_CAP_MAX = 256                          # SASSD_GT_CAP_MAX: ground-truth boxes
 OK = 0
 ERRORS = {-1: "SASSD_ERR_ARG", -2: "SASSD_ERR_LAUNCH", -3: "SASSD_ERR_WORKSPACE", -4: "SASSD_ERR_UNSUPPORTED"}
 FLAGS = {1: "VOXEL_CAP", 2: "ROWS_CAP", 4: "GUIDED_CAP", 8: "NMS_CAP", 16: "HASH_FULL", 32: "DET_CAP",
-         64: "GT_CAP", 128: "GATHER_CAP"}
+         64: "GT_CAP", 128: "GATHER_CAP", 256: "POINTS_CAP"}
 GATHER_CAP = 128                          # SASSD_FLAG_GATHER_CAP: sassd_points_in_rbboxes' rows exceed gather_cap
 
 P = c_void_p
@@ -64,6 +64,10 @@ _SIGNATURES = {
     "sassd_image_fov_crop": (c_int, [P, P, c_int, c_int, P, c_float, P, P, P, c_size_t, P]),
     "sassd_points_in_rbboxes_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "sassd_points_in_rbboxes": (c_int, [P, P, c_int, c_int, P, P, P, c_int, P, P, P, c_int, P, P, c_size_t, P]),
+    "sassd_augment_drop_points": (c_int, [P, P, c_int, c_int, P, P, P, P, P, c_size_t, P]),
+    "sassd_augment_noise_search": (c_int, [P, P, P, c_int, c_int, P, P, P, P, P]),
+    "sassd_augment_assemble": (c_int, [P, P, c_int, P, P, c_int, P, P, P, P, P, P, P, c_int, P, P, P, c_int, P, P, P,
+                                       P]),
     "sassd_anchor_mask_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "sassd_anchor_mask": (c_int, [P, P, c_int, c_int, c_int, c_int, P, c_int, c_int, P, P, c_size_t, P]),
     "sassd_hash_build": (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, P]),

@@ -51,7 +51,7 @@ def next_pow2(n):
 
 # --- launch accounting / optional per-call CUDA-event timing (bench.py) ---------------
 # kernels launched by each C-ABI entry point (memsets not counted)
-_KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_points_in_rbboxes": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
+_KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_points_in_rbboxes": 1, "sassd_augment_drop_points": 1, "sassd_augment_noise_search": 1, "sassd_augment_assemble": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
             "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
@@ -187,6 +187,47 @@ def points_in_rbboxes(points, pt_off, batch, planes, centres, nbox, gather_cap, 
           _ptr(nbox), box_cap, _ptr(counts), _ptr(seg_off), _ptr(gathered), int(gather_cap), _ptr(status), _ptr(w),
           w.numel(), _stream())
     return counts, seg_off, gathered, status
+
+
+def augment_drop_points(points, pt_off, batch, planes, box_off, ws=None):
+    """points [Ncap,4] f32, pt_off [batch+1] i32, planes [boxes,6,4] f32, box_off [batch+1] i32 (device).  Returns
+    (points_out [Ncap,4], pt_off_out [batch+1]): each frame's points outside every one of its boxes under the fp32
+    plane test, in input order (the scene crop of the reference's prepare_train_img)."""
+    dev = points.device
+    n_cap = points.shape[0]
+    assert planes.dtype == torch.float32 and planes.shape[1:] == (6, 4), "planes must be float32 [boxes,6,4]"
+    out = torch.empty_like(points)
+    off = torch.empty((batch + 1,), dtype=torch.int32, device=dev)
+    nbytes = _L().sassd_frustum_crop_workspace_bytes(n_cap, batch)
+    w = (ws or _WS).get("frustum", nbytes, dev)
+    _call("sassd_augment_drop_points", None, _ptr(points), _ptr(pt_off), n_cap, batch, _ptr(planes), _ptr(box_off),
+          _ptr(out), _ptr(off), _ptr(w), w.numel(), _stream())
+    return out, off
+
+
+def augment_noise_search(boxes, box_trig, box_off, batch, try_trig, loc, status):
+    """boxes [K,5] f32 (x, y, w, l, ry), box_trig [K,2] f32, box_off [batch+1] i32, try_trig [K,T,2] f32, loc [K,T,3]
+    f64 (device).  Returns sel [K] i32: each box's first collision-free try, or -1 (the reference's noise_per_box)."""
+    tries = loc.shape[1]
+    sel = torch.empty((boxes.shape[0],), dtype=torch.int32, device=boxes.device)
+    _call("sassd_augment_noise_search", None, _ptr(boxes), _ptr(box_trig), _ptr(box_off), batch, tries, _ptr(try_trig),
+          _ptr(loc), _ptr(sel), _ptr(status), _stream())
+    return sel
+
+
+def augment_assemble(kept, kept_off, batch, srow_off, srec_off, srec_db, srec_ctr, db, box_off, planes, centres, sel,
+                     try_trig, loc, frame_tf, out_cap, status):
+    """The augmented cloud of every frame: its sampled database rows, then the kept scene rows, each moved by its box's
+    noise and the frame's flip, rotation and scaling (csrc/augment.cu).  Returns (points [out_cap,4], pt_off
+    [batch+1]); POINTS_CAP in ``status`` when the rows exceed out_cap."""
+    dev = kept.device
+    out = torch.empty((max(int(out_cap), 1), 4), dtype=torch.float32, device=dev)
+    off = torch.empty((batch + 1,), dtype=torch.int32, device=dev)
+    _call("sassd_augment_assemble", None, _ptr(kept), _ptr(kept_off), batch, _ptr(srow_off), _ptr(srec_off),
+          srec_db.numel(), _ptr(srec_db), _ptr(srec_ctr), _ptr(db), _ptr(box_off), _ptr(planes), _ptr(centres),
+          _ptr(sel), loc.shape[1], _ptr(try_trig), _ptr(loc), _ptr(frame_tf), int(out_cap), _ptr(out), _ptr(off),
+          _ptr(status), _stream())
+    return out, off
 
 
 def voxel_mean(voxels, num_points, d_rows=None):
