@@ -158,6 +158,25 @@ __device__ __forceinline__ void store_constant_unit(const Conv2dArgs& p, int b, 
     }
 }
 
+// Zeros in the stored channels [c0, out_split_ch) of a tile that lie past the columns of its units (c0 = nsplit * BN; a
+// BN = 32 layer stores 64 channels), by nthreads threads: the next layer reads them through its 64-channel boxes, and
+// the buffer may hold anything before the call.
+__device__ __forceinline__ void zero_split_tail(const Conv2dArgs& p, int b, int ty, int tx, int c0, int tid,
+                                                int nthreads) {
+    if (!p.out_split || c0 >= p.out_split_ch) return;
+    const int vpp = (p.out_split_ch - c0) >> 3;                        // 16-byte vectors per pixel and plane
+    const size_t plane = (size_t)p.batch * p.H * p.W * p.out_split_ch;
+    const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+    for (int i = tid; i < TILE_H * TILE_W * vpp; i += nthreads) {
+        const int pix = i / vpp;
+        const int y = ty * TILE_H + pix / TILE_W, x = tx * TILE_W + pix % TILE_W;
+        if (y >= p.H || x >= p.W) continue;
+        __half* dst = p.out_split + (((size_t)b * p.H + y) * p.W + x) * p.out_split_ch + c0 + 8 * (i % vpp);
+        *(uint4*)dst = zero;
+        *(uint4*)(dst + plane) = zero;
+    }
+}
+
 template <int BN>
 __global__ void __launch_bounds__(THREADS2, 1)
 conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, const Background bg) {
@@ -344,6 +363,18 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                 }
             }
         }
+        // The stored channels past the units' columns of every tile this CTA walks (computed, stored or copied alike):
+        // zeros, written by this warp while the consumers finish their MMAs (on the consumers' side the stores' address
+        // arithmetic would be hoisted across the accumulators).
+        if (p.out_split && nsplit * BN < p.out_split_ch) {
+            __syncwarp();
+            for (int k = s_walk[5]; k < nunits; k = next_unit(k)) {
+                if (k % nsplit != nsplit - 1) continue;
+                const int tile = tile_ref(k / nsplit) & ~(kConstTile | kBgTile);
+                zero_split_tail(p, tile / (tiles_y * tiles_x), (tile / tiles_x) % tiles_y, tile % tiles_x, nsplit * BN,
+                                lane, 32);
+            }
+        }
     } else {
         // ===================== consumers: warpgroup wg owns pixel rows 64 wg .. 64 wg + 63 of the tile =====================
         const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
@@ -359,7 +390,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
             const bool const_tile = (ref & kConstTile) != 0;
             const int b = tile / (tiles_y * tiles_x);
             const int ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
-            if (ref & kBgTile) continue;                                    // copied after this loop
+            if (ref & kBgTile) continue;                                  // copied after this loop
             if (const_tile) {                                               // no MMAs run for this tile
                 const int ncols = min(BN, p.out_split_ch - n_off);
                 if (p.out_split && !p.out_f32 && (ncols == 64 || ncols == 128 || ncols == 256)) {

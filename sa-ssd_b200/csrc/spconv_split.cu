@@ -446,6 +446,17 @@ __global__ void __launch_bounds__(THREADS3, 1) spconv_split_kernel(const Args p)
                     }
                 }
             }
+            if (p.out_split && p.out_ch > BN) {       // stored channels past the accumulator's columns: zeros
+                const int vpr = (p.out_ch - BN) >> 3;   // 16-byte vectors per row and plane
+                const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+                for (int i = t; i < 64 * vpr; i += 128) {
+                    const int m = tile * BM + wg * 64 + i / vpr;
+                    if (m >= M) continue;
+                    __half* ohi = p.out_split + (size_t)m * p.out_ch + BN + 8 * (i % vpr);
+                    *(uint4*)ohi = zero;
+                    *(uint4*)(ohi + p.out_plane) = zero;
+                }
+            }
         }
         if (p.counters && threadIdx.x == 0 && executed) {
             atomicAdd(&p.counters[0], executed);

@@ -17,6 +17,8 @@ Two entry points:
     eval() mode (csrc/targets.cu).  ``forward_points(..., gt_bboxes=, gt_labels=)`` and ``detect_stream(losses=True)``
     compute them in the detection step itself (validation losses beside the detections, eager or captured).
 """
+import gc
+
 import numpy as np
 import torch
 import torch.nn.functional as F
@@ -620,8 +622,18 @@ class _GraphedStep:
             torch.cuda.synchronize(dev)
             self.graph = torch.cuda.CUDAGraph()
             self.backgrounds = ops.BACKGROUND_PINS = []       # the captured kernels bake their addresses in
-            with torch.cuda.graph(self.graph):
-                self.det, self.d_ndet, self.status, self.aux = self._step()
+            # A dropped detector lives on in its model <-> captured-step cycles until the cyclic collector runs; a
+            # collection during the capture would destroy its CUDA graphs then, which invalidates the capture.  So the
+            # dead cycles go now and the collector stays off until the capture ends.
+            gc_on = gc.isenabled()
+            gc.collect()
+            gc.disable()
+            try:
+                with torch.cuda.graph(self.graph):
+                    self.det, self.d_ndet, self.status, self.aux = self._step()
+            finally:
+                if gc_on:
+                    gc.enable()
         finally:
             ops.BACKGROUND_PINS = None
             ops._WS = shared_ws

@@ -783,9 +783,7 @@ def conv2d_split(x, weight, scale, shift, relu, cout, out_split=True, out_f32=Fa
     osp = of = None
     if out_split:
         cs = (cout + 63) // 64 * 64
-        # the kernel writes the BN (>= cout) columns it computes; stored channels beyond that must read as zero
-        alloc = torch.empty if cs == cout else torch.zeros
-        osp = alloc((2, B, H, W, cs), dtype=torch.float16, device=x.device)
+        osp = torch.empty((2, B, H, W, cs), dtype=torch.float16, device=x.device)   # the kernel zeroes [cout, cs)
         d.out_split_ch = cs
     if out_f32:
         stride = (cout + 3) // 4 * 4

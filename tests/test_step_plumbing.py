@@ -75,6 +75,40 @@ def test_split_detections_per_frame():
 
 
 @pytest.mark.gpu
+def test_capture_collects_dead_detectors_first_and_keeps_the_collector_off(golden_dir, monkeypatch):
+    """A dropped detector lives on in its model <-> captured-step cycles until the cyclic collector runs.  Run during
+    another capture, the collector would destroy those CUDA graphs mid-capture and invalidate it, at whatever allocation
+    it happens to fire.  So a capture collects first and records with the collector off."""
+    import gc
+    import weakref
+    from sassd_b200 import detectors
+    from tests.test_kitti_format import _model, _sweeps_and_metas
+    assert gc.isenabled()
+    pts, _, _ = _sweeps_and_metas(golden_dir, [0])
+    old = _model()
+    old.enable_cuda_graph(1, 32768)
+    old.forward_points(pts)
+    assert old._graphs
+    dead = weakref.ref(old)
+    del old
+    seen = []
+    run = detectors._run_step
+
+    def spy(*args, **kwargs):
+        if torch.cuda.is_current_stream_capturing():
+            seen.append((gc.isenabled(), dead() is None))
+        return run(*args, **kwargs)
+
+    monkeypatch.setattr(detectors, "_run_step", spy)
+    model = _model()
+    model.enable_cuda_graph(1, 32768)
+    got = model.forward_points(pts)
+    assert seen == [(False, True)], "capture ran with the collector on, or with a dead detector's graphs alive"
+    assert gc.isenabled() and len(got) == 1
+    model.disable_cuda_graph()
+
+
+@pytest.mark.gpu
 def test_enable_cuda_graph_recaptures_every_kind_at_the_new_shape(golden_dir):
     """A second enable_cuda_graph at another shape replaces the kinds captured at the first one: a crop graph left at
     batch 1 would never fit a batch of 2 again, and every cropped call would quietly run eagerly."""
