@@ -278,8 +278,22 @@ def test_gt_capacity_overflow_raises():
     many = np.repeat(gts[0], (n + 1) // len(gts[0]) + 1, 0)[:n + 1]
     with pytest.raises(ops._lib.SassdError, match="GT_CAP"):
         model.loss_points(pts, [many], [np.ones(n + 1, np.int64)])
-    ok = model.loss_points(pts, [many[:n]], [np.ones(n, np.int64)])     # exactly the capacity
+    ok, aux = model.loss_points(pts, [many[:n]], [np.ones(n, np.int64)], return_aux=True)     # exactly the capacity
     assert all(np.isfinite(v) for v in ok.values())
+    # the full GT table against the oracle: labels and IoUs bit for bit, targets within 2 ulp, losses within 2e-6
+    anchors = model.anchor_set.anchors
+    A = anchors[None]
+    mask = _host(aux["mask"]).astype(bool)
+    pos, neg = model.rpn_head.thresholds(model.train_cfg.rpn, model.class_names)
+    gt1, lab1 = [many[:n]], [np.ones(n, np.int64)]
+    L, T, M = OT.rpn_targets(A, mask, gt1, [l - 1 for l in lab1], lab1, pos, neg, 1)
+    assert np.array_equal(_host(aux["rpn_labels"]), L)
+    assert np.array_equal(_host(aux["rpn_ious"]).view(np.int32), M.view(np.int32))
+    assert _ulp_diff(_host(aux["rpn_targets"]), T).max() <= 2
+    box, cls, dirp = [t.reshape(1, -1, w) for t, w in zip(model.rpn_head._split(aux["head"]), (7, 1, 2))]
+    exp = OT.rpn_losses(_host(box), _host(cls), _host(dirp), L, T, A)
+    for k, v in exp.items():
+        assert abs(ok[k] - v) <= 2e-6 * abs(v), (k, ok[k], v)
     res = model.loss_points(pts, [g[:0] for g in gts], [l[:0] for l in labels])
     assert res["rpn_loc_loss"] == 0 and res["aux_loss_reg"] == 0 and res["rpn_cls_loss"] > 0
 
