@@ -259,7 +259,12 @@ int sassd_gconv_pack(const float* weight, int taps, int cin, int cout, int preci
  * moved by TMA (cp.async.bulk.tensor) instead of producer warps.  A split map is two fp16 planes
  * [2][batch][H][W][C] (C % 64 == 0): hi = half(x), lo = half((x - hi) * 2048).  Outputs: fp32 NHWC
  * (out_f32, stride out_f32_stride) and/or the next layer's split map (out_split, out_split_ch channels, the
- * channels beyond cout written as zero).  wpack: sassd_gconv_pack(..., SASSD_PREC_F16X3).  16 < cout <= 256. */
+ * channels beyond cout written as zero).  wpack: sassd_conv2d_pack.  16 < cout <= 256. */
+/* The weight pack of sassd_conv2d_f16x3*: weight [taps,cin,cout] fp32 -> packed (sassd_conv2d_pack_bytes bytes, 0 for
+ * an unsupported shape).  cout <= 64: the SASSD_PREC_F16X3 pack of sassd_gconv_pack; cout > 64: the hi / lo fp16
+ * weights in the register-fragment order of the kernel's wgmma A operand.  taps 9 or 1. */
+size_t sassd_conv2d_pack_bytes(int taps, int cin, int cout);
+int sassd_conv2d_pack(const float* weight, int taps, int cin, int cout, void* packed, sassd_stream_t stream);
 typedef struct {
     int32_t batch, H, W;
     int32_t cin, cin_stored;       /* valid / stored input channels */

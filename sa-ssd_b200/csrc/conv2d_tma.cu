@@ -11,9 +11,18 @@
 //     at (y0-1, x0+dx) that all three dy taps read, at 2048-byte row offsets (a 1x1 conv: one column, an 8-row box) —
 //     TMA writes it 128B-swizzled straight into the wgmma operand layout and zero-fills out-of-image pixels (= the
 //     conv's zero padding);
-//   * two rings: A stages (40 KB, released after the box's last tap) and B stages (one (tap, chunk) of weights);
-//   * no producer warps: warp 8 lane 0 issues the TMA boxes (A hi, A lo) and the weight bulk copies, two consumer
-//     warpgroups (pixel rows 0-63 / 64-127 of the tile) issue the MMAs and store the outputs from registers.
+//   * BN <= 64 (the PSWarp 3x3 256->28 conv, the head and PSWarp 1x1 convs): two rings, A stages (40 KB, released
+//     after the box's last tap) and B stages (one (tap, chunk) of weights); no producer warps: warp 8 lane 0 issues
+//     the TMA boxes (A hi, A lo) and the weight bulk copies, two consumer warpgroups (pixel rows 0-63 / 64-127 of the
+//     tile) issue the MMAs and store the outputs from registers;
+//   * BN = 128 (every layer with cout > 64): the operand roles are swapped.  The output channels are wgmma's M and the
+//     tile's 128 pixels its N: consumer warpgroup wg owns channels 64 wg .. 64 wg + 63 of the unit and every pixel,
+//     and issues m64n128k16 with the weights as A in registers and the halo box as B from shared memory.  The weights
+//     go from global memory (L2) straight into registers in wgmma's fragment order (sassd_conv2d_pack), one chunk
+//     ahead, so shared memory carries only the pixels: per K step the SM reads 24 KB of operands instead of 36 KB
+//     and writes no weight ring.  A producer warpgroup (setmaxnreg down to 40 registers, the consumers up to 232)
+//     issues the boxes into a three-stage ring, and the epilogue transposes each warpgroup's 64-channel x 128-pixel
+//     block through shared memory into 16-byte stores.
 // A work unit is a tile and up to 128 of its output channels: the two register accumulators (big, small) of a
 // 64 x 128 block are 128 floats per thread, so 256-channel layers run each tile as two units on the same weight pack.
 #include <cuda.h>
@@ -31,7 +40,6 @@ constexpr int BKC = 64;                         // channels per chunk (one 128-b
 constexpr int kConstTile = 1 << 30;             // tile reference flag: the tile only stores the layer's constant vector
 constexpr int kBgTile = 1 << 29;                // tile reference flag: the tile copies the layer's background map
 constexpr int CONS_WARPS = CONS_THREADS / 32;   // 8
-constexpr int THREADS2 = CONS_THREADS + 32;     // + the TMA / bulk-copy issuing warp
 constexpr int W_LOAD = CONS_WARPS;
 
 // The A operand of a (dx, chunk) step is one halo box per plane: TILE_H + 2 pixel rows (TILE_H for a 1x1 conv) of
@@ -39,14 +47,22 @@ constexpr int W_LOAD = CONS_WARPS;
 constexpr int A_ROWS = TILE_H + 2;
 constexpr int A_PLANE_BYTES = A_ROWS * TILE_W * 128;    // 20 KB (hi) ; same for lo, right after it
 constexpr int A_STAGE_BYTES = 2 * A_PLANE_BYTES;
-constexpr int A_STAGES = 2;
+
+// BN = 128 weight pack (sassd_conv2d_pack): per chunk q of a unit's walk, K step s (16 input channels) and block mb of
+// 64 output channels, 128 threads x 32 bytes: thread t's wgmma A fragment, hi a0..a3 then lo a0..a3.
+constexpr int FRAG_BLOCK_BYTES = 128 * 32;
+constexpr int OUT_PITCH = 64 + 4;               // floats per pixel of the epilogue staging: conflict-free transposes
 
 template <int BN>
 struct Cfg2 {
+    static constexpr bool RS = BN >= 128;                       // weights in registers (see the top of the file)
+    static constexpr int THREADS = CONS_THREADS + (RS ? 128 : 32);
+    static constexpr int A_STAGES = RS ? 3 : 2;
     static constexpr int B_TILE_BYTES = BN * 128;
     static constexpr int B_STAGE_BYTES = 2 * B_TILE_BYTES;     // one (tap, chunk): hi | lo
-    static constexpr int B_STAGES = (BN >= 128) ? 4 : 6;
-    static constexpr int RING_BYTES = A_STAGES * A_STAGE_BYTES + B_STAGES * B_STAGE_BYTES;
+    static constexpr int B_STAGES = RS ? 0 : 6;
+    static constexpr int OUT_BYTES = RS ? 2 * TILE_H * TILE_W * OUT_PITCH * 4 : 0;   // per warpgroup 128 px x 64 ch
+    static constexpr int RING_BYTES = A_STAGES * A_STAGE_BYTES + B_STAGES * B_STAGE_BYTES + OUT_BYTES;
     // tile order (computed tiles first) when the map carries constant-region information: two verdict bits and a uint16
     // per tile, up to 16 frames of the 200 x 176 BEV grid (4400 tiles); the word keeps the tile index in 14 bits
     static constexpr int ORDER_CAP = 4608;
@@ -78,8 +94,7 @@ struct Conv2dArgs {
                           // pack is the 2*BN-wide one)
 };
 
-// Optional: the layer's outputs on an empty scene, batch 1 (same H, W, strides), copied into the far border tiles.  A
-// kernel parameter of its own: grown by two pointers, Conv2dArgs tips the BN = 128 kernel over its 168 registers.
+// Optional: the layer's outputs on an empty scene, batch 1 (same H, W, strides), copied into the far border tiles.
 struct Background {
     const __half* split;
     const float* f32;
@@ -177,16 +192,36 @@ __device__ __forceinline__ void zero_split_tail(const Conv2dArgs& p, int b, int 
     }
 }
 
+// One chunk (four K steps) of the BN = 128 split product with the weights in registers: w holds, per K step s,
+// the hi fragment at w[8 s .. 8 s + 3] and the lo fragment at w[8 s + 4 .. 8 s + 7]; x_hi / x_lo are the pixels'
+// K-major planes.  Same products and order per accumulator as mma_chunk_x3: small += wh*xl, small += wl*xh,
+// big += wh*xh.
+__device__ __forceinline__ void mma_chunk_x3_rs(float (&big)[64], float (&small)[64], const uint32_t (&w)[32],
+                                                uint32_t x_hi, uint32_t x_lo) {
+    const uint64_t dxh = make_desc(x_hi), dxl = make_desc(x_lo);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint64_t ko = 2ull * (uint64_t)k;
+        const uint32_t wh[4] = {w[8 * k], w[8 * k + 1], w[8 * k + 2], w[8 * k + 3]};
+        const uint32_t wl[4] = {w[8 * k + 4], w[8 * k + 5], w[8 * k + 6], w[8 * k + 7]};
+        wgmma_rs_n128(small, wh, dxl + ko);
+        wgmma_rs_n128(small, wl, dxh + ko);
+        wgmma_rs_n128(big, wh, dxh + ko);
+    }
+}
+
 template <int BN>
-__global__ void __launch_bounds__(THREADS2, 1)
+__global__ void __launch_bounds__(Cfg2<BN>::THREADS, 1)
 conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, const Background bg) {
     using C = Cfg2<BN>;
+    constexpr int A_STAGES = C::A_STAGES;
     extern __shared__ uint8_t smem_raw[];
     __shared__ int s_ncomp;       // computed tiles at the head of the tile order
     __shared__ int s_walk[6];     // see next_unit
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    // rings: A stages (halo boxes, hi | lo) at base, B stages (weights of one (tap, chunk), hi | lo) after them
+    // A stages (halo boxes, hi | lo) at base; after them the B stages (weights of one (tap, chunk), hi | lo) for
+    // BN <= 64, the epilogue staging for BN = 128
     const uint32_t b_ring = base + A_STAGES * A_STAGE_BYTES;
     const uint32_t bar_base = base + C::RING_BYTES;
     auto a_full = [&](int s) { return bar_base + 8u * s; };
@@ -234,7 +269,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
     if (small_map) {
         const int nslots = (ntiles + 31) / 32;
 #pragma unroll 1
-        for (int i0 = 4 * warp; i0 < nslots; i0 += 4 * (THREADS2 / 32)) {
+        for (int i0 = 4 * warp; i0 < nslots; i0 += 4 * (C::THREADS / 32)) {
             int dist[4];
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
@@ -318,7 +353,11 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
         return k | tile_skip_flag(p, bg, __ldg(&p.tile_dist[k]), (k / tiles_x) % tiles_y, k % tiles_x, tiles_y, tiles_x);
     };
 
-    if (warp == W_LOAD) {
+    if (warp >= W_LOAD) {
+        if constexpr (C::RS) {
+            setmaxnreg_dec<40>();
+            if (warp != W_LOAD) return;
+        }
         if (lane == 0) {
             int a_stage = 0, b_stage = 0;
             uint32_t a_phase = 0, b_phase = 0;
@@ -341,23 +380,25 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                         tma_load_4d(a_hi, &amap, kc * BKC, x0 + dx, y0 - halo, b, a_full(a_stage));
                         tma_load_4d(a_hi + A_PLANE_BYTES, &amap, kc * BKC, x0 + dx, y0 - halo, p.batch + b, a_full(a_stage));
                         if (++a_stage == A_STAGES) { a_stage = 0; a_phase ^= 1u; }
-                        for (int row = 0; row < nrows; ++row) {
-                            const int t = row * ncols + col;                            // tap (dy + 1) * 3 + dx + 1
-                            mbar_wait(b_empty(b_stage), b_phase ^ 1u);
-                            const uint32_t b_dst = b_ring + b_stage * C::B_STAGE_BYTES;
-                            mbar_expect_tx(b_full(b_stage), C::B_STAGE_BYTES);
-                            // pack: per (tap, chunk) [hi | lo], each nsplit * BN rows of 128 bytes; this unit's BN rows
-                            const uint8_t* src = (const uint8_t*)p.wpack +
-                                                 (size_t)(t * kchunks + kc) * (size_t)(2 * nsplit) * C::B_TILE_BYTES +
-                                                 (size_t)half * C::B_TILE_BYTES;
-                            constexpr uint32_t kPiece = (C::B_TILE_BYTES >= 8192) ? 8192u : (uint32_t)C::B_TILE_BYTES;
+                        if constexpr (!C::RS) {                  // BN = 128: the consumers load their weights themselves
+                            for (int row = 0; row < nrows; ++row) {
+                                const int t = row * ncols + col;                            // tap (dy + 1) * 3 + dx + 1
+                                mbar_wait(b_empty(b_stage), b_phase ^ 1u);
+                                const uint32_t b_dst = b_ring + b_stage * C::B_STAGE_BYTES;
+                                mbar_expect_tx(b_full(b_stage), C::B_STAGE_BYTES);
+                                // pack: per (tap, chunk) [hi | lo], each nsplit * BN rows of 128 bytes; this unit's BN rows
+                                const uint8_t* src = (const uint8_t*)p.wpack +
+                                                     (size_t)(t * kchunks + kc) * (size_t)(2 * nsplit) * C::B_TILE_BYTES +
+                                                     (size_t)half * C::B_TILE_BYTES;
+                                constexpr uint32_t kPiece = (C::B_TILE_BYTES >= 8192) ? 8192u : (uint32_t)C::B_TILE_BYTES;
 #pragma unroll 1
-                            for (int part = 0; part < 2; ++part)
+                                for (int part = 0; part < 2; ++part)
 #pragma unroll 1
-                                for (uint32_t o = 0; o < (uint32_t)C::B_TILE_BYTES; o += kPiece)
-                                    bulk_g2s(b_dst + part * C::B_TILE_BYTES + o,
-                                             src + (size_t)part * nsplit * C::B_TILE_BYTES + o, kPiece, b_full(b_stage));
-                            if (++b_stage == C::B_STAGES) { b_stage = 0; b_phase ^= 1u; }
+                                    for (uint32_t o = 0; o < (uint32_t)C::B_TILE_BYTES; o += kPiece)
+                                        bulk_g2s(b_dst + part * C::B_TILE_BYTES + o,
+                                                 src + (size_t)part * nsplit * C::B_TILE_BYTES + o, kPiece, b_full(b_stage));
+                                if (++b_stage == C::B_STAGES) { b_stage = 0; b_phase ^= 1u; }
+                            }
                         }
                     }
                 }
@@ -376,7 +417,9 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
             }
         }
     } else {
-        // ===================== consumers: warpgroup wg owns pixel rows 64 wg .. 64 wg + 63 of the tile =====================
+        // ============ consumers: warpgroup wg owns pixel rows 64 wg .. 64 wg + 63 of the tile (BN <= 64) or ============
+        // ============ output channels 64 wg .. 64 wg + 63 of the unit (BN = 128)                            ============
+        if constexpr (C::RS) setmaxnreg_inc<232>();
         const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
         const int rl0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);        // tile rows rl0 and rl0 + 8 (= pixel py * 16 + px)
         const size_t plane = (size_t)p.batch * p.H * p.W * p.out_split_ch;
@@ -404,27 +447,71 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                 // stages the previous chunk's MMAs read: released once they are known complete (prev_a only after
                 // the last of the box's nrows taps)
                 int prev_b = -1, prev_a = -1, row = 0;
-                for (int ch = 0; ch < nchunks; ++ch) {
-                    if (row == 0) mbar_wait(a_full(a_stage), a_phase);
-                    mbar_wait(b_full(b_stage), b_phase);
-                    // tap row `row` of this warpgroup's 4 pixel rows: box rows row + 4 wg .. row + 4 wg + 3
-                    const uint32_t ah = base + a_stage * A_STAGE_BYTES + (uint32_t)(row * TILE_W + wg * 64) * 128u;
-                    const uint32_t bh = b_ring + b_stage * C::B_STAGE_BYTES;
-                    wgmma_fence();
-                    mma_chunk_x3<1, BN>(big, small, ah, ah + A_PLANE_BYTES, bh, bh + C::B_TILE_BYTES);
-                    wgmma_commit();
-                    wgmma_wait<1>();            // the previous chunk's MMAs have read their stages
-                    if (t == 0) {
-                        if (prev_b >= 0) mbar_arrive(b_empty(prev_b));
-                        if (prev_a >= 0) mbar_arrive(a_empty(prev_a));
+                if constexpr (C::RS) {
+                    // This thread's fragments in the pack: block 2 (k % nsplit) + wg of the 2 nsplit 64-channel blocks.
+                    const uint32_t kstep = 2u * nsplit * FRAG_BLOCK_BYTES, qstep = 4u * kstep;
+                    const uint8_t* wsrc = (const uint8_t*)p.wpack + (2 * (k % nsplit) + wg) * FRAG_BLOCK_BYTES + t * 32;
+                    auto load_w = [&](uint32_t (&w)[32], int q) {
+                        const uint8_t* src = wsrc + (size_t)q * qstep;
+#pragma unroll
+                        for (int s = 0; s < 4; ++s) {
+                            const uint4 h = ldg_nc_v4(src + s * kstep), l = ldg_nc_v4(src + s * kstep + 16);
+                            w[8 * s] = h.x; w[8 * s + 1] = h.y; w[8 * s + 2] = h.z; w[8 * s + 3] = h.w;
+                            w[8 * s + 4] = l.x; w[8 * s + 5] = l.y; w[8 * s + 6] = l.z; w[8 * s + 7] = l.w;
+                        }
+                    };
+                    // Chunk ch on the fragments in w; the next chunk's go into w_next once the MMAs that read them
+                    // (chunk ch - 1) are complete.
+                    auto chunk = [&](uint32_t (&w)[32], uint32_t (&w_next)[32], int ch) {
+                        if (row == 0) mbar_wait(a_full(a_stage), a_phase);
+                        const uint32_t xh = base + a_stage * A_STAGE_BYTES + (uint32_t)row * (TILE_W * 128u);
+                        wgmma_fence();
+                        mma_chunk_x3_rs(big, small, w, xh, xh + A_PLANE_BYTES);
+                        wgmma_commit();
+                        wgmma_wait<1>();
+                        fence_regs<32>(w_next);
+                        if (t == 0 && prev_a >= 0) mbar_arrive(a_empty(prev_a));
+                        if (ch + 1 < nchunks) load_w(w_next, ch + 1);
+                        prev_a = -1;
+                        if (++row == nrows) {
+                            row = 0;
+                            prev_a = a_stage;
+                            if (++a_stage == A_STAGES) { a_stage = 0; a_phase ^= 1u; }
+                        }
+                    };
+                    uint32_t wa[32], wb[32];
+                    load_w(wa, 0);
+                    for (int ch = 0; ch < nchunks; ch += 2) {
+                        chunk(wa, wb, ch);
+                        if (ch + 1 == nchunks) break;
+                        chunk(wb, wa, ch + 1);
                     }
-                    prev_b = b_stage;
-                    if (++b_stage == C::B_STAGES) { b_stage = 0; b_phase ^= 1u; }
-                    prev_a = -1;
-                    if (++row == nrows) {
-                        row = 0;
-                        prev_a = a_stage;
-                        if (++a_stage == A_STAGES) { a_stage = 0; a_phase ^= 1u; }
+                    wgmma_wait<0>();
+                    fence_regs<32>(wa);
+                    fence_regs<32>(wb);
+                } else {
+                    for (int ch = 0; ch < nchunks; ++ch) {
+                        if (row == 0) mbar_wait(a_full(a_stage), a_phase);
+                        mbar_wait(b_full(b_stage), b_phase);
+                        // tap row `row` of this warpgroup's 4 pixel rows: box rows row + 4 wg .. row + 4 wg + 3
+                        const uint32_t ah = base + a_stage * A_STAGE_BYTES + (uint32_t)(row * TILE_W + wg * 64) * 128u;
+                        const uint32_t bh = b_ring + b_stage * C::B_STAGE_BYTES;
+                        wgmma_fence();
+                        mma_chunk_x3<1, BN>(big, small, ah, ah + A_PLANE_BYTES, bh, bh + C::B_TILE_BYTES);
+                        wgmma_commit();
+                        wgmma_wait<1>();            // the previous chunk's MMAs have read their stages
+                        if (t == 0) {
+                            if (prev_b >= 0) mbar_arrive(b_empty(prev_b));
+                            if (prev_a >= 0) mbar_arrive(a_empty(prev_a));
+                        }
+                        prev_b = b_stage;
+                        if (++b_stage == C::B_STAGES) { b_stage = 0; b_phase ^= 1u; }
+                        prev_a = -1;
+                        if (++row == nrows) {
+                            row = 0;
+                            prev_a = a_stage;
+                            if (++a_stage == A_STAGES) { a_stage = 0; a_phase ^= 1u; }
+                        }
                     }
                 }
                 wgmma_wait<0>();
@@ -435,42 +522,101 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                     if (prev_a >= 0) mbar_arrive(a_empty(prev_a));
                 }
             }
-            // epilogue from registers: folded BN + ReLU (or the layer constant), fp32 and / or split-plane stores
-#pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                const int n = n_off + 8 * j + 2 * (t & 3);
-                float c0, c1, sc0 = 1.f, sc1 = 1.f, sh0 = 0.f, sh1 = 0.f;
-                if (const_tile) {
-                    c0 = n < p.cout ? __ldg(&p.cvec[n]) : 0.f;
-                    c1 = n + 1 < p.cout ? __ldg(&p.cvec[n + 1]) : 0.f;
-                } else {
-                    if (p.scale && n < p.cout) sc0 = __ldg(&p.scale[n]);
-                    if (p.scale && n + 1 < p.cout) sc1 = __ldg(&p.scale[n + 1]);
-                    if (p.shift && n < p.cout) sh0 = __ldg(&p.shift[n]);
-                    if (p.shift && n + 1 < p.cout) sh1 = __ldg(&p.shift[n + 1]);
-                }
+            if constexpr (C::RS) {
+                // Epilogue through shared memory: thread t holds channels m0, m0 + 8 of the warpgroup's 64 at pixels
+                // 8 j + 2 (t % 4) + e; folded BN + ReLU (or the layer constant) into the warpgroup's staging block
+                // [pixel][OUT_PITCH], then whole pixels out with 16-byte fp32 and / or split-plane stores.
+                float* stage = (float*)(base_ptr + A_STAGES * A_STAGE_BYTES) + wg * (TILE_H * TILE_W * OUT_PITCH);
+                const int m0 = 16 * (t >> 5) + ((t & 31) >> 2), c_wg = n_off + 64 * wg;
+                float cv[2], sc[2], sh[2];
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
-                    const int rl = rl0 + 8 * i;
-                    const int y = ty * TILE_H + rl / TILE_W, x = tx * TILE_W + rl % TILE_W;
-                    float o0 = c0, o1 = c1;
-                    if (!const_tile) {
-                        o0 = fmaf(__fadd_rn(big[4 * j + 2 * i], small[4 * j + 2 * i] * (1.f / kF16LoScale)), sc0, sh0);
-                        o1 = fmaf(__fadd_rn(big[4 * j + 2 * i + 1], small[4 * j + 2 * i + 1] * (1.f / kF16LoScale)), sc1, sh1);
-                        if (p.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
-                        if (n >= p.cout) o0 = 0.f;
-                        if (n + 1 >= p.cout) o1 = 0.f;
+                    const int n = c_wg + m0 + 8 * i;
+                    cv[i] = const_tile && n < p.cout ? __ldg(&p.cvec[n]) : 0.f;
+                    sc[i] = p.scale && n < p.cout ? __ldg(&p.scale[n]) : 1.f;
+                    sh[i] = p.shift && n < p.cout ? __ldg(&p.shift[n]) : 0.f;
+                }
+                named_bar_sync(1 + wg, 128);        // the warpgroup's read-back of the previous unit is done
+#pragma unroll
+                for (int j = 0; j < 16; ++j)
+#pragma unroll
+                    for (int i = 0; i < 2; ++i)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            float o = cv[i];
+                            if (!const_tile) {
+                                o = fmaf(__fadd_rn(big[4 * j + 2 * i + e], small[4 * j + 2 * i + e] * (1.f / kF16LoScale)),
+                                         sc[i], sh[i]);
+                                if (p.relu) o = fmaxf(o, 0.f);
+                                if (c_wg + m0 + 8 * i >= p.cout) o = 0.f;
+                            }
+                            stage[(8 * j + 2 * (t & 3) + e) * OUT_PITCH + m0 + 8 * i] = o;
+                        }
+                named_bar_sync(1 + wg, 128);
+                if (p.out_f32) {
+                    for (int v = t; v < TILE_H * TILE_W * 16; v += 128) {
+                        const int pix = v >> 4, c = 4 * (v & 15), n = c_wg + c;
+                        const int y = ty * TILE_H + pix / TILE_W, x = tx * TILE_W + pix % TILE_W;
+                        if (n >= p.out_f32_stride || y >= p.H || x >= p.W) continue;
+                        *(float4*)(p.out_f32 + (((size_t)b * p.H + y) * p.W + x) * p.out_f32_stride + n) =
+                            *(const float4*)(stage + pix * OUT_PITCH + c);
                     }
-                    if (y >= p.H || x >= p.W) continue;
-                    const size_t pix = ((size_t)b * p.H + y) * p.W + x;
-                    if (p.out_f32 && n < p.out_f32_stride)
-                        *(float2*)(p.out_f32 + pix * p.out_f32_stride + n) = make_float2(o0, o1);
-                    if (p.out_split && n < p.out_split_ch) {
-                        uint32_t h, l;
-                        split_f16x2(o0, o1, h, l);
-                        __half* dst = p.out_split + pix * p.out_split_ch + n;
-                        *(uint32_t*)dst = h;
-                        *(uint32_t*)(dst + plane) = l;
+                }
+                if (p.out_split) {
+                    for (int v = t; v < TILE_H * TILE_W * 8; v += 128) {
+                        const int pix = v >> 3, c = 8 * (v & 7), n = c_wg + c;
+                        const int y = ty * TILE_H + pix / TILE_W, x = tx * TILE_W + pix % TILE_W;
+                        if (n >= p.out_split_ch || y >= p.H || x >= p.W) continue;
+                        const float4 f0 = *(const float4*)(stage + pix * OUT_PITCH + c);
+                        const float4 f1 = *(const float4*)(stage + pix * OUT_PITCH + c + 4);
+                        uint4 hi, lo;
+                        split_f16x2(f0.x, f0.y, hi.x, lo.x);
+                        split_f16x2(f0.z, f0.w, hi.y, lo.y);
+                        split_f16x2(f1.x, f1.y, hi.z, lo.z);
+                        split_f16x2(f1.z, f1.w, hi.w, lo.w);
+                        __half* dst = p.out_split + (((size_t)b * p.H + y) * p.W + x) * p.out_split_ch + n;
+                        *(uint4*)dst = hi;
+                        *(uint4*)(dst + plane) = lo;
+                    }
+                }
+            } else {
+                // epilogue from registers: folded BN + ReLU (or the layer constant), fp32 and / or split-plane stores
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int n = n_off + 8 * j + 2 * (t & 3);
+                    float c0, c1, sc0 = 1.f, sc1 = 1.f, sh0 = 0.f, sh1 = 0.f;
+                    if (const_tile) {
+                        c0 = n < p.cout ? __ldg(&p.cvec[n]) : 0.f;
+                        c1 = n + 1 < p.cout ? __ldg(&p.cvec[n + 1]) : 0.f;
+                    } else {
+                        if (p.scale && n < p.cout) sc0 = __ldg(&p.scale[n]);
+                        if (p.scale && n + 1 < p.cout) sc1 = __ldg(&p.scale[n + 1]);
+                        if (p.shift && n < p.cout) sh0 = __ldg(&p.shift[n]);
+                        if (p.shift && n + 1 < p.cout) sh1 = __ldg(&p.shift[n + 1]);
+                    }
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        const int rl = rl0 + 8 * i;
+                        const int y = ty * TILE_H + rl / TILE_W, x = tx * TILE_W + rl % TILE_W;
+                        float o0 = c0, o1 = c1;
+                        if (!const_tile) {
+                            o0 = fmaf(__fadd_rn(big[4 * j + 2 * i], small[4 * j + 2 * i] * (1.f / kF16LoScale)), sc0, sh0);
+                            o1 = fmaf(__fadd_rn(big[4 * j + 2 * i + 1], small[4 * j + 2 * i + 1] * (1.f / kF16LoScale)), sc1, sh1);
+                            if (p.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+                            if (n >= p.cout) o0 = 0.f;
+                            if (n + 1 >= p.cout) o1 = 0.f;
+                        }
+                        if (y >= p.H || x >= p.W) continue;
+                        const size_t pix = ((size_t)b * p.H + y) * p.W + x;
+                        if (p.out_f32 && n < p.out_f32_stride)
+                            *(float2*)(p.out_f32 + pix * p.out_f32_stride + n) = make_float2(o0, o1);
+                        if (p.out_split && n < p.out_split_ch) {
+                            uint32_t h, l;
+                            split_f16x2(o0, o1, h, l);
+                            __half* dst = p.out_split + pix * p.out_split_ch + n;
+                            *(uint32_t*)dst = h;
+                            *(uint32_t*)(dst + plane) = l;
+                        }
                     }
                 }
             }
@@ -523,11 +669,56 @@ static int launch2(const CUtensorMap& map, const Conv2dArgs& a, const Background
     }
     const int units = a.batch * sassd_div_up(a.H, TILE_H) * sassd_div_up(a.W, TILE_W) * a.nsplit;
     const int grid = units < sassd_num_sms() ? units : sassd_num_sms();
-    if (launch_pdl(kern, dim3(grid), dim3(THREADS2), C::SMEM_BYTES, stream, map, a, bg) != cudaSuccess) return SASSD_ERR_LAUNCH;
+    if (launch_pdl(kern, dim3(grid), dim3(C::THREADS), C::SMEM_BYTES, stream, map, a, bg) != cudaSuccess) return SASSD_ERR_LAUNCH;
     return sassd_check_launch();
 }
 
+// The BN = 128 weight pack, W [taps, cin, cout] fp32 -> f16x2 words, one thread per word.  Chunk q of a unit's walk
+// ((dx, chunk) outer, dy inner: q = (col * kchunks + kc) * nrows + row, tap row * ncols + col), K step s, block mb of
+// 64 output channels and thread t hold hi a0..a3 then lo a0..a3, fragment register a (0..3) being output channel
+// 64 mb + 16 (t / 32) + (t % 32) / 4 + 8 (a & 1) at input channels 64 kc + 16 s + 2 (t % 4) + 8 (a >> 1) + {0, 1}.
+__global__ void conv2d_pack_kernel(const float* __restrict__ w, int taps, int cin, int cout, int nblk,
+                                   uint32_t* __restrict__ out) {
+    const int kchunks = (cin + BKC - 1) / BKC, ncols = taps == 9 ? 3 : 1, nrows = ncols;
+    const long long total = (long long)taps * kchunks * 4 * nblk * (FRAG_BLOCK_BYTES / 4);
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int word = (int)(i % 8), t = (int)((i / 8) % 128);
+        long long r = i / (FRAG_BLOCK_BYTES / 4);
+        const int mb = (int)(r % nblk);
+        r /= nblk;
+        const int s = (int)(r % 4), q = (int)(r / 4);
+        const int row = q % nrows, kc = (q / nrows) % kchunks, col = q / (nrows * kchunks);
+        const int tap = row * ncols + col, a = word % 4, lane = t % 32;
+        const int n = 64 * mb + 16 * (t / 32) + lane / 4 + 8 * (a & 1);
+        const int k = kc * BKC + 16 * s + 2 * (lane % 4) + 8 * (a >> 1);
+        float hi[2], lo[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const float v = (k + e < cin && n < cout) ? w[((size_t)tap * cin + k + e) * cout + n] : 0.f;
+            split_f16(v, hi[e], lo[e]);
+        }
+        const __half2 h = word < 4 ? __floats2half2_rn(hi[0], hi[1]) : __floats2half2_rn(lo[0], lo[1]);
+        out[i] = *reinterpret_cast<const uint32_t*>(&h);
+    }
+}
+
 }  // namespace tma
+
+extern "C" size_t sassd_conv2d_pack_bytes(int taps, int cin, int cout) {
+    if (!(taps == 9 || taps == 1) || cin < 1 || cout < 1 || cout > 256) return 0;
+    if (cout <= 64) return sassd_gconv_pack_bytes(taps, cin, cout, SASSD_PREC_F16X3);
+    return (size_t)taps * ((cin + tma::BKC - 1) / tma::BKC) * 4 * (cout <= 128 ? 2 : 4) * tma::FRAG_BLOCK_BYTES;
+}
+
+extern "C" int sassd_conv2d_pack(const float* weight, int taps, int cin, int cout, void* packed,
+                                 sassd_stream_t stream_) {
+    if (!weight || !packed || sassd_conv2d_pack_bytes(taps, cin, cout) == 0) return SASSD_ERR_ARG;
+    if (cout <= 64) return sassd_gconv_pack(weight, taps, cin, cout, SASSD_PREC_F16X3, packed, stream_);
+    const long long words = (long long)sassd_conv2d_pack_bytes(taps, cin, cout) / 4;
+    tma::conv2d_pack_kernel<<<sassd_grid(words, 256), 256, 0, (cudaStream_t)stream_>>>(
+        weight, taps, cin, cout, cout <= 128 ? 2 : 4, (uint32_t*)packed);
+    return sassd_check_launch();
+}
 
 extern "C" int sassd_conv2d_f16x3(const sassd_conv2d_desc* d, const void* in_split, const void* wpack,
                                   const float* scale, const float* shift, float* out_f32, void* out_split,

@@ -82,6 +82,8 @@ _SIGNATURES = {
     "sassd_gconv": (c_int, [ctypes.POINTER(GConvDesc), P, P, P, P, P, P, P, P]),
     "sassd_gconv_pack_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "sassd_gconv_pack": (c_int, [P, c_int, c_int, c_int, c_int, P, P]),
+    "sassd_conv2d_pack_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "sassd_conv2d_pack": (c_int, [P, c_int, c_int, c_int, P, P]),
     "sassd_conv2d_f16x3": (c_int, [ctypes.POINTER(Conv2dDesc), P, P, P, P, P, P, P]),
     "sassd_conv2d_f16x3_occ": (c_int, [ctypes.POINTER(Conv2dDesc), P, P, P, P, P, P, P, c_int, P, P, P]),
     "sassd_conv2d_f16x3_occ_bg": (c_int, [ctypes.POINTER(Conv2dDesc), P, P, P, P, P, P, P, c_int, P, P, P, P, P]),

@@ -53,7 +53,7 @@ def next_pow2(n):
 # kernels launched by each C-ABI entry point (memsets not counted)
 _KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_points_in_rbboxes": 1, "sassd_augment_drop_points": 1, "sassd_augment_noise_search": 1, "sassd_augment_assemble": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
-            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
+            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
             "sassd_boxes_iou_bev": 1, "sassd_points_in_boxes": 2, "sassd_assign_rpn": 3, "sassd_assign_pswarp": 3,
             "sassd_rpn_loss": 2, "sassd_pswarp_loss": 2, "sassd_aux_loss": 2}
@@ -358,6 +358,26 @@ def tc_pack_cached(weight, precision):
         if len(_TC_PACKS) >= 256:
             _TC_PACKS.pop(next(iter(_TC_PACKS)))
         ent = (pack_tc(weight.contiguous(), precision), weight)
+        _TC_PACKS[key] = ent
+    return ent[0]
+
+
+def conv2d_pack_cached(weight):
+    """Weight pack of sassd_conv2d_f16x3 (cached like tc_pack_cached): wgmma register fragments for cout > 64, the
+    F16X3 tensor-core pack otherwise."""
+    key = (weight.data_ptr(), weight._version, tuple(weight.shape), "conv2d")
+    ent = _TC_PACKS.get(key)
+    if ent is None:
+        if len(_TC_PACKS) >= 256:
+            _TC_PACKS.pop(next(iter(_TC_PACKS)))
+        w = weight.contiguous()
+        taps, cin, cout = w.shape
+        nbytes = _L().sassd_conv2d_pack_bytes(taps, cin, cout)
+        if nbytes == 0:
+            raise _lib.SassdError("sassd_conv2d_pack_bytes: unsupported shape taps=%d cin=%d cout=%d" % (taps, cin, cout))
+        packed = torch.empty((nbytes,), dtype=torch.uint8, device=w.device)
+        _call("sassd_conv2d_pack", None, _ptr(w), taps, cin, cout, _ptr(packed), _stream())
+        ent = (packed, weight)
         _TC_PACKS[key] = ent
     return ent[0]
 
@@ -774,7 +794,7 @@ def conv2d_split(x, weight, scale, shift, relu, cout, out_split=True, out_f32=Fa
     """x: SplitMap; weight [taps, cin, cout] fp32 (packed on first use).  Returns (SplitMap | None, fp32 map | None)."""
     B, H, W, cin = x.shape
     taps = weight.shape[0]
-    wp = tc_pack_cached(weight, PREC_F16X3)
+    wp = conv2d_pack_cached(weight)
     d = Conv2dDesc()
     d.batch, d.H, d.W, d.cin, d.cin_stored = B, H, W, cin, x.planes.shape[-1]
     d.cout, d.taps, d.relu = cout, taps, 1 if relu else 0
