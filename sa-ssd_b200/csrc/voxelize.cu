@@ -156,8 +156,10 @@ vox_rank_kernel(const int* __restrict__ pt_off, const int* __restrict__ pt_slot,
 __global__ void vox_offsets_kernel(const int* __restrict__ frame_m, int batch, int rows_cap,
                                    int* __restrict__ frame_rows, int* __restrict__ status) {
     if (threadIdx.x == 0 && blockIdx.x == 0) {
+        // every offset clamped to rows_cap: a frame that starts past the cap owns no rows, and frame_rows stays
+        // non-decreasing and in range for the consumers that take per-frame row counts from it
         int acc = 0;
-        for (int b = 0; b < batch; ++b) { frame_rows[b] = acc; acc += frame_m[b]; }
+        for (int b = 0; b < batch; ++b) { frame_rows[b] = min(acc, rows_cap); acc += frame_m[b]; }
         if (acc > rows_cap) { atomicOr(status, SASSD_FLAG_VOXEL_CAP); acc = rows_cap; }
         frame_rows[batch] = acc;
     }
