@@ -414,6 +414,24 @@ int sassd_kitti_format(const float* det, const int32_t* d_ndet, int batch, int d
                        double* rows, int32_t* n_out, sassd_stream_t stream);
 
 /* ------------------------------------------------------------------------
+ * Detections of a set of single-class models (detectors.DetectorSet), one
+ * block per frame.  Member m (m < n_members <= SASSD_MERGE_MAX) gives
+ * host_dets[m] = det [batch,host_caps[m],9] and host_ndets[m] = d_ndet [batch]
+ * as sassd_rescore_nms writes them (device pointers in host arrays).
+ * det [batch,sum host_caps,9]: frame f holds member 0's first
+ * min(d_ndet_0[f], cap_0) rows, then member 1's, ..., each copied bit for bit
+ * but for its label (column 8), which gains host_label_offsets[m] (the
+ * member's first class in the set's class list).  d_ndet [batch] = the
+ * frame's row count.  Rows past it are left unwritten.  No NMS across
+ * members, no host synchronisation: graph-capturable; sassd_kitti_format
+ * then takes det_cap = sum host_caps.
+ * ---------------------------------------------------------------------- */
+#define SASSD_MERGE_MAX 16
+int sassd_merge_detections(const float* const* host_dets, const int32_t* const* host_ndets, const int* host_caps,
+                           const int* host_label_offsets, int n_members, int batch, float* det, int32_t* d_ndet,
+                           sassd_stream_t stream);
+
+/* ------------------------------------------------------------------------
  * Auxiliary point-wise head, SpMiddleFHD.forward(is_test=False)
  * (cmn.py:121-135, :175-189): per voxel a foreground logit and a centre offset.
  *

@@ -34,3 +34,11 @@ def build_from_config(cfg, device="cuda", data_key="val"):
     model.class_names = list(d.get("class_names", ["Car"]))
     model.attach_data_pipeline(vg, aset)
     return model, vg, aset
+
+
+def __getattr__(name):
+    """``DetectorSet`` (detectors.DetectorSet), imported on first use like the evaluation above."""
+    if name == "DetectorSet":
+        from .detectors import DetectorSet
+        return DetectorSet
+    raise AttributeError("module 'sassd_b200' has no attribute %r" % name)

@@ -18,6 +18,7 @@ Two entry points:
     compute them in the detection step itself (validation losses beside the detections, eager or captured).
 """
 import gc
+import weakref
 
 import numpy as np
 import torch
@@ -58,6 +59,7 @@ class SingleStageDetector(nn.Module):
         self._graph_args = None
         self._stream_slots = None
         self._stream_key = None
+        self._sets = weakref.WeakSet()   # the DetectorSets this model is a member of (refresh_packed_weights)
         if isinstance(pretrained, str):
             from .checkpoint import load_params_from_file
             load_params_from_file(self, pretrained)
@@ -86,6 +88,8 @@ class SingleStageDetector(nn.Module):
         self._graphs = {}
         self._stream_slots = None
         self._stream_key = None
+        for s in list(self._sets):      # a DetectorSet's captured steps bake in this member's weights too
+            s.refresh_packed_weights()
 
     # ------------------------------------------------------------------ reference-signature path
     def merge_second_batch(self, batch_args):
@@ -189,10 +193,21 @@ class SingleStageDetector(nn.Module):
         the auxiliary network's points_mean [cap,4] (b, x, y, z), point_cls [cap] and point_reg [cap,3] (neck.point_head)
         for the voxel rows (frame_rows).  ``guided_thr``: the guided anchors' score threshold (default self.guided_thr;
         the losses use train_cfg.rpn.anchor_thr)."""
-        dev = points.device
-        status = torch.zeros((1,), dtype=torch.int32, device=dev)
-        vg, aset = self.voxel_generator, self.anchor_set
-        voxels, coors, num, mean, frame_rows = vg.generate_device(points, pt_off, batch, max_points_per_frame, status)
+        status = torch.zeros((1,), dtype=torch.int32, device=points.device)
+        vox = self.voxel_generator.generate_device(points, pt_off, batch, max_points_per_frame, status)
+        return self.forward_voxels(vox, batch, status, point_outputs=point_outputs, detections=detections,
+                                   guided_thr=guided_thr)
+
+    def forward_voxels(self, vox, batch, status, sparse_in=None, point_outputs=False, detections=True,
+                       guided_thr=None):
+        """forward_device from the voxelizer's outputs ``vox`` = generate_device's (voxels, coors, num_points, mean,
+        frame_rows) on: the anchor mask, the sparse backbone, the BEV neck, the heads, PSWarp and the rescoring with
+        NMS, on this model's weights.  ``sparse_in``: the level-0 sparse tensor with its rulebooks already queued
+        (SpMiddleFHD.sparse_input over the same voxels), which the members of a DetectorSet share; without it the neck
+        builds them."""
+        aset = self.anchor_set
+        voxels, coors, num, mean, frame_rows = vox
+        dev = coors.device
         d_rows = frame_rows[batch:batch + 1]
         # anchors_mask only feeds the guided-anchor selection: run it on a side stream, next to the backbone
         main = torch.cuda.current_stream()
@@ -201,7 +216,8 @@ class SingleStageDetector(nn.Module):
         self._mask_stream.wait_stream(main)
         with torch.cuda.stream(self._mask_stream):
             mask = aset.mask_device(coors, d_rows, batch)
-        out = self.neck.forward_nhwc(mean, coors, batch, d_rows=d_rows, status=status, point_outputs=point_outputs)
+        out = self.neck.forward_nhwc(mean, coors, batch, d_rows=d_rows, status=status, point_outputs=point_outputs,
+                                     sparse_in=sparse_in)
         y, conv6, xs = out[:3]
         main.wait_stream(self._mask_stream)
         head = self.rpn_head.forward_nhwc(y)
@@ -312,27 +328,7 @@ class SingleStageDetector(nn.Module):
                                   for _ in range(depth)]
             self._copy_stream = torch.cuda.Stream()
             self._stream_key = key
-        slots, pending = self._stream_slots, []
-        for i, item in enumerate(batches):
-            item = tuple(item) if (crop or kitti or losses) else (item,)
-            gt = None
-            if losses:
-                gt, item = self._gt_inputs(*item[-1], len(item[0])), item[:-1]
-            fb = item[0]
-            planes = _frame_planes(item[1], len(fb)) if crop else None
-            metas = item[-1] if kitti else None
-            meta = _meta_blocks(metas, len(fb)) if kitti else None
-            counts = [int(p.shape[0]) for p in fb]
-            slot = slots[i % depth]
-            if len(pending) == depth:                       # the slot we are about to reuse must be drained
-                yield self._collected(*pending.pop(0))
-            if not slot.fits(len(fb), counts):
-                raise ValueError("batch does not fit the captured shape (batch %d, %d points/frame)" %
-                                 (batch, max_points_per_frame))
-            slot.submit(fb, counts, self._copy_stream, own_stream=concurrent, planes=planes, meta=meta, gt=gt)
-            pending.append((slot, metas))
-        for slot, metas in pending:
-            yield self._collected(slot, metas)
+        yield from _stream_through(self, batches, batch, max_points_per_frame, depth, concurrent, crop, kitti, losses)
 
     def _collected(self, slot, metas):
         """Wait for a slot's step and convert its host copy into the caller's per-frame results (and its losses)."""
@@ -473,6 +469,167 @@ class SingleStageDetector(nn.Module):
         return res
 
 
+class DetectorSet:
+    """Several single-class detectors run as one: each KITTI class by a model of its own, as the reference's single-class
+    checkpoints are meant to be used, in one step over shared inputs.
+
+    ``models``: built SingleStageDetectors in eval() mode, each with its class names and data pipeline attached
+    (build_from_config).  They must share the voxel grid - the voxel generator's voxel size, point-cloud range,
+    max_num_points and max_voxels - the neck's output_shape and its row_cap_factor (the rulebooks' capacities), and no
+    class may belong to two members (ValueError otherwise).  Member 0's neck builds the shared rulebooks, so its
+    overlap_rulebooks setting (side streams or not; the rulebooks are the same) applies to the whole set.  The set's class list is the members' class names concatenated in member order, and the
+    labels it returns index that list.
+
+    One step crops (when asked), copies, voxelizes and builds the seven rulebooks once, then runs each member's anchor
+    mask, sparse backbone, BEV neck, heads, PSWarp and rescoring with NMS on its own weights, and gathers the members'
+    detections per frame in member order (ops.merge_detections).  There is no NMS across members: each frame's
+    detections are exactly the concatenation of what each member's forward_points returns for it, and with ``metas`` its
+    KITTI rows are the concatenation of the members' rows.  A set of one model returns what that model returns.
+
+    forward_points, enable_cuda_graph and detect_stream take the items and return the results of the
+    SingleStageDetector methods of the same names (without losses, auxiliary outputs or return_aux).  The set keeps
+    its own captured graphs and stream slots; the members' own are neither used nor changed.  Loading parameters into
+    a member or changing its precision (refresh_packed_weights) drops the set's captured steps too."""
+
+    def __init__(self, models):
+        models = list(models)
+        if not models:
+            raise ValueError("a DetectorSet needs at least one model")
+        if len(models) > ops._lib.MERGE_MAX:
+            raise ValueError("a DetectorSet takes at most %d models, got %d" % (ops._lib.MERGE_MAX, len(models)))
+        for i, m in enumerate(models):
+            if not isinstance(m, SingleStageDetector):
+                raise TypeError("member %d is a %s, not a SingleStageDetector" % (i, type(m).__name__))
+            if m.training:
+                raise ValueError("member %d is in training mode: call .eval() first" % i)
+            if m.voxel_generator is None or m.anchor_set is None or m.class_names is None:
+                raise ValueError("member %d has no data pipeline or class names (build_from_config attaches them)" % i)
+        lead = models[0]
+        for i, m in enumerate(models[1:], 1):
+            diff = voxel_grid_difference(lead.voxel_generator, m.voxel_generator)
+            if diff:
+                raise ValueError("member %d voxelizes differently from member 0 (%s): the set shares one voxelizer "
+                                 "and one set of rulebooks, so run such models separately" % (i, diff))
+            if list(m.neck.sparse_shape) != list(lead.neck.sparse_shape):
+                raise ValueError("member %d's neck output_shape %s differs from member 0's %s" %
+                                 (i, list(m.neck.sparse_shape), list(lead.neck.sparse_shape)))
+            if m.neck.row_cap_factor != lead.neck.row_cap_factor:
+                raise ValueError("member %d's neck row_cap_factor %r differs from member 0's %r: the shared rulebooks "
+                                 "have one set of capacities" % (i, m.neck.row_cap_factor, lead.neck.row_cap_factor))
+            if next(m.parameters()).device != next(lead.parameters()).device:
+                raise ValueError("member %d is on another device than member 0" % i)
+        self.models = models
+        self.class_names, self.label_offsets = merged_classes([m.class_names for m in models])
+        self._pinned = None
+        self._graphs = {}                 # (crop kind, kitti) -> the set's captured step (enable_cuda_graph)
+        self._graph_args = None
+        self._stream_slots = None
+        self._stream_key = None
+        for m in models:
+            m._sets.add(self)
+
+    def parameters(self):
+        for m in self.models:
+            yield from m.parameters()
+
+    @property
+    def det_cap(self):
+        """Detection rows per frame of the merged block: the members' capacities summed."""
+        return sum(m.extra_head.det_cap for m in self.models)
+
+    def refresh_packed_weights(self):
+        """Drop every captured step of the set (a member's parameters or precision changed)."""
+        self._graphs = {}
+        self._stream_slots = None
+        self._stream_key = None
+
+    stage_points = SingleStageDetector.stage_points
+    disable_cuda_graph = SingleStageDetector.disable_cuda_graph
+    _frame_results = SingleStageDetector._frame_results
+    _collected = SingleStageDetector._collected
+
+    def enable_cuda_graph(self, batch, max_points_per_frame=32768):
+        """SingleStageDetector.enable_cuda_graph for the set's step: the plain kind is captured here and returned,
+        the crop and KITTI kinds on their first use."""
+        self._graph_args = (int(batch), int(max_points_per_frame))
+        self._graphs = {}
+        return self._graph_for(CROP_NONE, False)
+
+    def _graph_for(self, crop, kitti):
+        key = (int(crop), kitti)
+        if key not in self._graphs and self._graph_args is not None:
+            self._graphs[key] = _GraphedStep(self, *self._graph_args, latency=True, crop=crop, kitti=kitti,
+                                             run_step=_set_step)
+        return self._graphs.get(key)
+
+    def forward_points(self, points_list, frustum_planes=None, metas=None, image_fov=False):
+        """SingleStageDetector.forward_points for the set: per frame a dict of boxes_lidar, scores and label_preds
+        (None entries when no member keeps a box), or with ``metas`` one KITTI annotation dict, each holding every
+        member's detections in member order."""
+        ops.require_cuda()
+        kind = _crop_kind(frustum_planes is not None, image_fov, metas is not None)
+        B = len(points_list)
+        planes = None if frustum_planes is None else _frame_planes(frustum_planes, B)
+        meta = None if metas is None else _meta_blocks(metas, B)
+        hp, ho, counts = self.stage_points(points_list)
+        g = self._graph_for(kind, meta is not None)
+        if g is not None and g.fits(B, counts):
+            return self._frame_results(g.run_host(hp, ho, sum(counts), planes, meta), metas)
+        dev = next(self.parameters()).device
+        det, d_ndet, status, aux = _set_step(self, hp.to(dev, non_blocking=True), ho.to(dev, non_blocking=True), B,
+                                             max(counts + [1]), _to_device(planes, dev), _to_device(meta, dev),
+                                             image_fov=kind == CROP_IMAGE_FOV)
+        if meta is not None:
+            ops._lib.raise_on_status(status)
+            out = aux["rows"].cpu().numpy(), aux["n_out"].cpu().numpy()
+        else:
+            out = unpack_detections(det, d_ndet, status)
+        return self._frame_results(out, metas)
+
+    def detect_stream(self, batches, batch, max_points_per_frame=32768, depth=4, concurrent=True, crop=False,
+                      kitti=False, image_fov=False):
+        """SingleStageDetector.detect_stream for the set: the same items, ``depth`` captured set steps used
+        round-robin, and per batch the merged results of forward_points."""
+        ops.require_cuda()
+        kind = _crop_kind(bool(crop), image_fov, kitti)
+        key = (batch, max_points_per_frame, depth, kind, bool(kitti))
+        if self._stream_key != key or self._stream_slots is None:
+            self._stream_slots = [_GraphedStep(self, batch, max_points_per_frame, crop=kind, kitti=kitti,
+                                               run_step=_set_step) for _ in range(depth)]
+            self._copy_stream = torch.cuda.Stream()
+            self._stream_key = key
+        yield from _stream_through(self, batches, batch, max_points_per_frame, depth, concurrent, crop, kitti, False)
+
+
+def merged_classes(class_lists):
+    """The class list of a DetectorSet and each member's label offset into it: the members' class names
+    concatenated in member order, member m's labels shifted by the number of classes before it.  A class in two
+    members raises ValueError."""
+    names, offsets = [], []
+    for names_m in class_lists:
+        offsets.append(len(names))
+        names += list(names_m)
+    dup = sorted({n for n in names if names.count(n) > 1})
+    if dup:
+        raise ValueError("class %s belongs to more than one member: a set keeps one model per class" % ", ".join(dup))
+    return names, offsets
+
+
+def voxel_grid_difference(a, b):
+    """What differs between two VoxelGenerators' voxel grids ('' when nothing): voxel size, point-cloud range,
+    max_num_points, max_voxels."""
+    diff = []
+    if not np.array_equal(a.voxel_size, b.voxel_size):
+        diff.append("voxel size %s vs %s" % (list(a.voxel_size), list(b.voxel_size)))
+    if not np.array_equal(a.point_cloud_range, b.point_cloud_range):
+        diff.append("point-cloud range %s vs %s" % (list(a.point_cloud_range), list(b.point_cloud_range)))
+    if a.max_num_points_per_voxel != b.max_num_points_per_voxel:
+        diff.append("max_num_points %d vs %d" % (a.max_num_points_per_voxel, b.max_num_points_per_voxel))
+    if a.max_voxels != b.max_voxels:
+        diff.append("max_voxels %d vs %d" % (a.max_voxels, b.max_voxels))
+    return ", ".join(diff)
+
+
 def _on_device(v, dev):
     """A tensor or a per-class dict of tensors, on ``dev``."""
     return {k: t.to(dev) for k, t in v.items()} if isinstance(v, dict) else v.to(dev)
@@ -525,6 +682,16 @@ def _loss_dict(h):
     return {k: float(v) for k, v in zip(ops.LOSS_KEYS, h.tolist())}
 
 
+def _crop_step(points, pt_off, batch, planes, meta, image_fov):
+    """The crop a step runs first: to the camera frustums of ``planes`` [batch,6,4], to the images of ``meta`` with
+    ``image_fov``, or none."""
+    if planes is not None:
+        return ops.frustum_crop(points, pt_off, batch, planes)
+    if image_fov:
+        return ops.image_fov_crop(points, pt_off, batch, meta)
+    return points, pt_off
+
+
 def _run_step(model, points, pt_off, batch, maxpts, planes=None, meta=None, point_outputs=False, detections=True,
               guided_thr=None, image_fov=False, gt=None):
     """One detector step on the device, no synchronisation; the eager calls and every captured graph build their step
@@ -534,15 +701,60 @@ def _run_step(model, points, pt_off, batch, maxpts, planes=None, meta=None, poin
     loss vector [6] in aux["losses"] and its targets in aux["targets"]; with ``meta`` [batch,36] the detections are
     formatted as KITTI rows (ops.kitti_format) into aux["rows"] / aux["n_out"].  Returns forward_device's (det, d_ndet,
     status, aux)."""
-    if planes is not None:
-        points, pt_off = ops.frustum_crop(points, pt_off, batch, planes)
-    elif image_fov:
-        points, pt_off = ops.image_fov_crop(points, pt_off, batch, meta)
+    points, pt_off = _crop_step(points, pt_off, batch, planes, meta, image_fov)
     det, d_ndet, status, aux = model.forward_device(points, pt_off, batch, maxpts,
                                                     point_outputs=point_outputs or gt is not None,
                                                     detections=detections, guided_thr=guided_thr)
     if gt is not None:
         aux["losses"], aux["targets"] = model.loss_device(aux, batch, *gt, None, status)
+    if meta is not None:
+        aux["rows"], aux["n_out"] = ops.kitti_format(det, d_ndet, meta)
+    return det, d_ndet, status, aux
+
+
+def _stream_through(owner, batches, batch, max_points_per_frame, depth, concurrent, crop, kitti, losses):
+    """detect_stream's loop over ``owner``'s slots (a SingleStageDetector's or a DetectorSet's): stage, submit and
+    collect round-robin, yielding each batch's results in order."""
+    slots, pending = owner._stream_slots, []
+    for i, item in enumerate(batches):
+        item = tuple(item) if (crop or kitti or losses) else (item,)
+        gt = None
+        if losses:
+            gt, item = owner._gt_inputs(*item[-1], len(item[0])), item[:-1]
+        fb = item[0]
+        planes = _frame_planes(item[1], len(fb)) if crop else None
+        metas = item[-1] if kitti else None
+        meta = _meta_blocks(metas, len(fb)) if kitti else None
+        counts = [int(p.shape[0]) for p in fb]
+        slot = slots[i % depth]
+        if len(pending) == depth:                       # the slot we are about to reuse must be drained
+            yield owner._collected(*pending.pop(0))
+        if not slot.fits(len(fb), counts):
+            raise ValueError("batch does not fit the captured shape (batch %d, %d points/frame)" %
+                             (batch, max_points_per_frame))
+        slot.submit(fb, counts, owner._copy_stream, own_stream=concurrent, planes=planes, meta=meta, gt=gt)
+        pending.append((slot, metas))
+    for slot, metas in pending:
+        yield owner._collected(slot, metas)
+
+
+def _set_step(dset, points, pt_off, batch, maxpts, planes=None, meta=None, point_outputs=False, image_fov=False,
+              gt=None):
+    """One DetectorSet step on the device, no synchronisation; the set's eager calls and captured graphs build it here,
+    from the parts of _run_step.  Once: the crop, the voxelizer (the members' generators are equal) and the seven
+    rulebooks (SpMiddleFHD.sparse_input); per member forward_voxels on the shared voxels and rulebooks; then the
+    members' detections gathered per frame (ops.merge_detections) and, with ``meta``, formatted once as KITTI rows.
+    The members share the status word.  Returns (det [batch,det_cap,9], d_ndet, status, aux)."""
+    assert not point_outputs and gt is None, "a DetectorSet step has no auxiliary outputs or losses"
+    points, pt_off = _crop_step(points, pt_off, batch, planes, meta, image_fov)
+    lead = dset.models[0]
+    status = torch.zeros((1,), dtype=torch.int32, device=points.device)
+    vox = lead.voxel_generator.generate_device(points, pt_off, batch, maxpts, status)
+    _, coors, _, mean, frame_rows = vox
+    shared = lead.neck.sparse_input(mean, coors, batch, d_rows=frame_rows[batch:batch + 1], status=status)
+    members = [m.forward_voxels(vox, batch, status, sparse_in=shared)[:2] for m in dset.models]
+    det, d_ndet = ops.merge_detections(members, dset.label_offsets)
+    aux = dict(coors=coors, frame_rows=frame_rows, members=members)
     if meta is not None:
         aux["rows"], aux["n_out"] = ops.kitti_format(det, d_ndet, meta)
     return det, d_ndet, status, aux
@@ -571,7 +783,7 @@ class _GraphedStep:
     """One captured detector step (_run_step) with static input/output buffers."""
 
     def __init__(self, model, batch, max_points_per_frame, latency=False, crop=False, kitti=False, point_outputs=False,
-                 losses=False):
+                 losses=False, run_step=None):
         """latency=True: this step will run alone on the GPU (enable_cuda_graph / forward_points): the dense convs walk
         the computed tiles first so that the constant-region tiles shorten every layer; False (detect_stream slots,
         several steps in flight): round-robin tiles, the SMs a layer leaves idle serve the other steps.
@@ -585,9 +797,11 @@ class _GraphedStep:
         the host (point_results).
         losses=True: the step also computes the losses of the GT in the static buffers gt [batch,SASSD_GT_CAP_MAX,7],
         its classes, labels and per-frame counts (the true counts: a frame with more boxes raises), and copies the loss
-        vector to the host with the detections (loss_results)."""
+        vector to the host with the detections (loss_results).
+        run_step: the step function captured, _run_step's signature (DetectorSet passes _set_step)."""
         dev = next(model.parameters()).device
         self.model, self.batch, self.maxpts = model, int(batch), int(max_points_per_frame)
+        self.run_step = _run_step if run_step is None else run_step
         self.cap = self.batch * self.maxpts
         self.crop, self.kitti, self.point_outputs = int(crop), bool(kitti), bool(point_outputs)
         self.losses = bool(losses)
@@ -660,8 +874,8 @@ class _GraphedStep:
         self.loaded = torch.cuda.Event()
 
     def _step(self):
-        return _run_step(self.model, self.points, self.pt_off, self.batch, self.maxpts, self.planes, self.meta,
-                         point_outputs=self.point_outputs, image_fov=self.crop == CROP_IMAGE_FOV, gt=self.gt)
+        return self.run_step(self.model, self.points, self.pt_off, self.batch, self.maxpts, self.planes, self.meta,
+                             point_outputs=self.point_outputs, image_fov=self.crop == CROP_IMAGE_FOV, gt=self.gt)
 
     def fits(self, batch, counts):
         return batch == self.batch and max(counts + [0]) <= self.maxpts

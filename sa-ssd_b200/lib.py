@@ -45,6 +45,7 @@ KITTI_META, KITTI_ROW = 36, 14            # SASSD_KITTI_META / SASSD_KITTI_ROW
 POINT_LEVEL_CHANNELS = (32, 64, 64)       # sassd_point_aux_head: features of backbone levels 1..3 (conv1, conv2, conv3)
 POINT_FC_IN, POINT_FC_OUT = 160, 64       # point_fc: Linear(160, 64); point_cls / point_reg read its 64 outputs
 GT_CAP_MAX = 256                          # SASSD_GT_CAP_MAX: ground-truth boxes per frame the loss kernels take
+MERGE_MAX = 16                            # SASSD_MERGE_MAX: members sassd_merge_detections takes
 
 OK = 0
 ERRORS = {-1: "SASSD_ERR_ARG", -2: "SASSD_ERR_LAUNCH", -3: "SASSD_ERR_WORKSPACE", -4: "SASSD_ERR_UNSUPPORTED"}
@@ -105,6 +106,7 @@ _SIGNATURES = {
     "sassd_rescore_nms_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "sassd_rescore_nms": (c_int, [P, P, P, P, c_int, c_int, c_float, c_float, c_int, P, P, c_int, P, P, c_size_t, P]),
     "sassd_kitti_format": (c_int, [P, P, c_int, c_int, P, P, P, P]),
+    "sassd_merge_detections": (c_int, [P, P, P, P, c_int, c_int, P, P, P]),
     "sassd_three_nn": (c_int, [P, P, P, c_int, P, P, P, P, P, P, P, P, P, P]),
     "sassd_point_aux_head": (c_int, [P, P, P, c_int, ctypes.POINTER(PointLevels), P, P, P, P, P]),
     "sassd_nms_workspace_bytes": (c_size_t, [c_int]),

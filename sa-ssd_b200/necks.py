@@ -298,23 +298,37 @@ class SpMiddleFHD(nn.Module):
         self.backbone.set_precision(precision if sparse is None else sparse)
         self.fcn.precision = precision
 
-    def forward_nhwc(self, voxel_features, coors, batch_size, d_rows=None, status=None, point_outputs=False):
-        """Device-side entry: capacity-sized inputs + row counter; returns NHWC (x, conv6) and the tensor.  With
-        ``point_outputs`` the auxiliary network runs after conv3, before the dense neck, and its outputs
-        (point_head) come fourth."""
-        if self.training:
-            raise NotImplementedError("sassd_b200 is inference-only: call .eval()")
+    def sparse_input(self, voxel_features, coors, batch_size, d_rows=None, status=None):
+        """The backbone's level-0 tensor with its seven rulebooks queued (VxNet.prebuild_rulebooks on this neck's side
+        streams; with ``overlap_rulebooks`` off the first conv of each level builds them).  The rulebooks depend on the
+        coordinates only, so the members of a detectors.DetectorSet share one such tensor (forward_nhwc's
+        ``sparse_in``)."""
         x = spconv.SparseConvTensor(voxel_features, coors, self.sparse_shape, batch_size, d_rows=d_rows, status=status)
         x.row_cap_factor = self.row_cap_factor
-        x0_mean, x0_coors, rows0 = x._features, x._indices, x.d_rows     # level 0: the voxel means (SimpleVoxel)
         if self.overlap_rulebooks:
             if self._side is None:
                 self._side = torch.cuda.Stream(device=x.device)
                 self._side2 = torch.cuda.Stream(device=x.device)
             self.backbone.prebuild_rulebooks(x, self._side, self._side2)
+        return x
+
+    def forward_nhwc(self, voxel_features, coors, batch_size, d_rows=None, status=None, point_outputs=False,
+                     sparse_in=None):
+        """Device-side entry: capacity-sized inputs + row counter; returns NHWC (x, conv6) and the tensor.  With
+        ``point_outputs`` the auxiliary network runs after conv3, before the dense neck, and its outputs
+        (point_head) come fourth.  ``sparse_in``: a sparse_input() tensor over these voxels, whose rulebooks this
+        call uses instead of building its own."""
+        if self.training:
+            raise NotImplementedError("sassd_b200 is inference-only: call .eval()")
+        if sparse_in is None:
+            x = self.sparse_input(voxel_features, coors, batch_size, d_rows, status)
+        else:       # the shared rulebooks and hash, but this network's own feature chain
+            x = sparse_in._derive(sparse_in._features)
+        side = getattr(sparse_in if sparse_in is not None else x, "_rulebook_stream", None)
+        x0_mean, x0_coors, rows0 = x._features, x._indices, x.d_rows     # level 0: the voxel means (SimpleVoxel)
         x, middle = self.backbone(x)
-        if self.overlap_rulebooks:
-            torch.cuda.current_stream().wait_stream(self._side)   # join (also required to end a graph capture)
+        if side is not None:
+            torch.cuda.current_stream().wait_stream(side)   # join (also required to end a graph capture)
         pts = None
         if point_outputs:
             pts = self.point_head(x0_mean, x0_coors, rows0, middle)

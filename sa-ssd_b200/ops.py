@@ -54,7 +54,7 @@ def next_pow2(n):
 _KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_points_in_rbboxes": 1, "sassd_augment_drop_points": 1, "sassd_augment_noise_search": 1, "sassd_augment_assemble": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
             "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
-            "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
+            "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_merge_detections": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
             "sassd_boxes_iou_bev": 1, "sassd_points_in_boxes": 2, "sassd_assign_rpn": 3, "sassd_assign_pswarp": 3,
             "sassd_rpn_loss": 2, "sassd_pswarp_loss": 2, "sassd_aux_loss": 2}
 LAUNCHES = 0          # running count of kernels launched through this module
@@ -488,6 +488,25 @@ def kitti_format(det, d_ndet, meta):
     _call("sassd_kitti_format", None, _ptr(det), _ptr(d_ndet), B, det_cap, _ptr(meta), _ptr(rows), _ptr(n_out),
           _stream())
     return rows, n_out
+
+
+def merge_detections(dets, label_offsets):
+    """dets: per member (det [B,cap_m,9] f32, d_ndet [B] i32) as rescore_nms returns them; label_offsets: per member
+    the index of its first class in the merged class list.  Returns (det [B,sum cap_m,9], d_ndet [B]): per frame the
+    members' rows in member order, labels offset (csrc/merge.cu).  Rows past d_ndet[b] are left unwritten."""
+    M = len(dets)
+    assert 1 <= M <= _lib.MERGE_MAX and len(label_offsets) == M, "1..%d members, one label offset each" % _lib.MERGE_MAX
+    B = dets[0][0].shape[0]
+    for d, n in dets:
+        assert d.dtype == torch.float32 and d.dim() == 3 and d.shape[0] == B and d.shape[2] == 9 and d.is_contiguous()
+        assert n.dtype == torch.int32 and tuple(n.shape) == (B,)
+    caps = [int(d.shape[1]) for d, _ in dets]
+    det = torch.empty((B, sum(caps), 9), dtype=torch.float32, device=dets[0][0].device)
+    d_ndet = torch.empty((B,), dtype=torch.int32, device=det.device)
+    _call("sassd_merge_detections", None, (ctypes.c_void_p * M)(*[_ptr(d) for d, _ in dets]),
+          (ctypes.c_void_p * M)(*[_ptr(n) for _, n in dets]), (ctypes.c_int * M)(*caps),
+          (ctypes.c_int * M)(*[int(o) for o in label_offsets]), M, B, _ptr(det), _ptr(d_ndet), _stream())
+    return det, d_ndet
 
 
 # ---------------------------------------------------------------------------- auxiliary point-wise head

@@ -5,6 +5,7 @@
                               [--losses] [--r40]
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR --split test --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --drive DRIVE_DIR [--calib-dir DIR] --out DIR [...]
+    python -m sassd_b200.test CONFIG CHECKPOINT --model CONFIG2 CHECKPOINT2 [--model ...] --data-root DIR [...]
 
 Frames are read from disk a few batches ahead (kitti_data.Prefetcher) and streamed through the captured step
 (SingleStageDetector.detect_stream): full sweeps (``--lidar velodyne``) are cropped to the camera frustum on the
@@ -23,6 +24,12 @@ The test split (``testing/``) and raw drives (kitti_data.KittiDrive) have no lab
 files (``--out`` is required) and prints the frame rate and read wait only.  A raw drive's full sweeps are cropped on
 the device to the points that project into image 2 (ops.image_fov_crop, the reference's KittiVideo), and its result
 files are named by the frames' stems, ``%010d.txt``.
+
+``--model CONFIG CHECKPOINT`` (repeatable) adds a model after the positional one: the models run as one
+detectors.DetectorSet, one model per class as the reference's single-class checkpoints are used.  Every step
+voxelizes and builds the rulebooks once for all of them, each frame's result file holds every model's rows in model
+order, and the AP table covers the models' classes in that order.  The models must share the voxel grid and may not
+share a class; ``--losses`` takes one model.
 
 Under torchrun, frame i of the split goes to rank i mod W; at the end every rank contributes one fixed-size block of
 KITTI rows and counts to a single all_gather_into_tensor (dist.DetectionGather) and rank 0 re-interleaves, writes and
@@ -65,9 +72,13 @@ def parse_args(argv=None):
                    help="also compute SA-SSD's losses against the split's labels in the detection step and print "
                         "their means over the batches")
     p.add_argument("--r40", action="store_true", help="also print the AP table at 40 recall positions")
+    p.add_argument("--model", nargs=2, action="append", default=[], metavar=("CONFIG", "CHECKPOINT"),
+                   help="one more single-class model, run with the first as one set (repeatable)")
     args = p.parse_args(argv)
     if args.batch < 1:
         p.error("--batch must be positive")
+    if args.losses and args.model:
+        p.error("--losses computes one model's losses: it does not combine with --model")
     if args.losses and (args.drive or args.split == "test"):
         p.error("--losses needs a labelled split: %s has no labels" % ("--drive" if args.drive else "--split test"))
     if args.r40 and (args.drive or args.split == "test"):
@@ -162,6 +173,15 @@ def run(args, log=print):
     torch.cuda.set_device(device)
     model, _, _ = S.build_from_config(cfg, device=device)
     load_params_from_file(model, args.checkpoint)
+    det_cap = model.extra_head.det_cap
+    if args.model:                      # the positional model and every --model, run as one set
+        members = [model]
+        for cfg_m, ckpt_m in args.model:
+            m, _, _ = S.build_from_config(S.Config.fromfile(cfg_m), device=device)
+            load_params_from_file(m, ckpt_m)
+            members.append(m)
+        model = S.DetectorSet(members)
+        det_cap = model.det_cap
     fov = bool(args.drive)
     crop = args.lidar == "velodyne" and not fov
     class_names = model.class_names
@@ -175,8 +195,9 @@ def run(args, log=print):
                 item += (([b for b, _ in gts[0]], [l for _, l in gts[0]]),)
             yield item
 
+    loss_kw = dict(losses=True) if args.losses else {}
     stream = lambda src: model.detect_stream(src, args.batch, args.max_points, depth=4, crop=crop,  # noqa: E731
-                                             kitti=True, image_fov=fov, losses=args.losses)
+                                             kitti=True, image_fov=fov, **loss_kw)
     for _ in stream([]):                # capture the slots' graphs before the clock starts
         pass
     torch.cuda.synchronize(device)
@@ -194,7 +215,7 @@ def run(args, log=print):
     wall = D.max_over_ranks(wall, device)
 
     if world > 1:
-        dt_annos = gather_annos(annos_local, split.ids, class_names, model.extra_head.det_cap, device)
+        dt_annos = gather_annos(annos_local, split.ids, class_names, det_cap, device)
     else:
         dt_annos = [a for i, a in zip([i for ids in batches for i in ids], annos_local) if i is not None]
     if args.losses:
