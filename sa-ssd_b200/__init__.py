@@ -37,8 +37,8 @@ def build_from_config(cfg, device="cuda", data_key="val"):
 
 
 def __getattr__(name):
-    """``DetectorSet`` (detectors.DetectorSet), imported on first use like the evaluation above."""
-    if name == "DetectorSet":
-        from .detectors import DetectorSet
-        return DetectorSet
+    """``DetectorSet`` and ``CheckpointSweep`` (detectors.*), imported on first use like the evaluation above."""
+    if name in ("DetectorSet", "CheckpointSweep"):
+        from . import detectors
+        return getattr(detectors, name)
     raise AttributeError("module 'sassd_b200' has no attribute %r" % name)

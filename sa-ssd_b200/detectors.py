@@ -198,30 +198,35 @@ class SingleStageDetector(nn.Module):
         return self.forward_voxels(vox, batch, status, point_outputs=point_outputs, detections=detections,
                                    guided_thr=guided_thr)
 
+    def anchor_mask(self, coors, d_rows, batch):
+        """The anchor mask [batch, Na] of the voxel coordinates, queued on a side stream (it only feeds the
+        guided-anchor selection, so it runs next to the backbone).  Returns (mask, the stream to wait for)."""
+        main = torch.cuda.current_stream()
+        if self._mask_stream is None:
+            self._mask_stream = torch.cuda.Stream(device=coors.device)
+        self._mask_stream.wait_stream(main)
+        with torch.cuda.stream(self._mask_stream):
+            mask = self.anchor_set.mask_device(coors, d_rows, batch)
+        return mask, self._mask_stream
+
     def forward_voxels(self, vox, batch, status, sparse_in=None, point_outputs=False, detections=True,
-                       guided_thr=None):
+                       guided_thr=None, mask=None, neighbours=None):
         """forward_device from the voxelizer's outputs ``vox`` = generate_device's (voxels, coors, num_points, mean,
         frame_rows) on: the anchor mask, the sparse backbone, the BEV neck, the heads, PSWarp and the rescoring with
         NMS, on this model's weights.  ``sparse_in``: the level-0 sparse tensor with its rulebooks already queued
         (SpMiddleFHD.sparse_input over the same voxels), which the members of a DetectorSet share; without it the neck
-        builds them."""
-        aset = self.anchor_set
+        builds them.  ``mask``: anchor_mask's (mask, stream) over these voxels, which the checkpoints of a
+        CheckpointSweep share; ``neighbours``: the auxiliary network's three_nn outputs (SpMiddleFHD.point_head)."""
         voxels, coors, num, mean, frame_rows = vox
-        dev = coors.device
         d_rows = frame_rows[batch:batch + 1]
-        # anchors_mask only feeds the guided-anchor selection: run it on a side stream, next to the backbone
         main = torch.cuda.current_stream()
-        if self._mask_stream is None:
-            self._mask_stream = torch.cuda.Stream(device=dev)
-        self._mask_stream.wait_stream(main)
-        with torch.cuda.stream(self._mask_stream):
-            mask = aset.mask_device(coors, d_rows, batch)
+        mask, mask_stream = self.anchor_mask(coors, d_rows, batch) if mask is None else mask
         out = self.neck.forward_nhwc(mean, coors, batch, d_rows=d_rows, status=status, point_outputs=point_outputs,
-                                     sparse_in=sparse_in)
+                                     sparse_in=sparse_in, neighbours=neighbours)
         y, conv6, xs = out[:3]
-        main.wait_stream(self._mask_stream)
+        main.wait_stream(mask_stream)
         head = self.rpn_head.forward_nhwc(y)
-        anchors, _ = aset.device_tensors()
+        anchors, _ = self.anchor_set.device_tensors()
         thr = self.guided_thr if guided_thr is None else guided_thr
         boxes, labels, index, d_k = self.rpn_head.guided_anchors_device(head, anchors, mask, thr, status)
         ps_feat = self.extra_head.convs_nhwc(conv6)
@@ -406,23 +411,42 @@ class SingleStageDetector(nn.Module):
         ret = (res,) + ((pts,) if point_outputs else ()) + ((loss,) if losses else ()) + ((aux,) if return_aux else ())
         return ret if len(ret) > 1 else res
 
-    def loss_device(self, aux, batch, gt, gt_class, gt_label, d_ngt, n_gt_host, status):
+    def loss_targets(self, aux, batch, gt, gt_class, gt_label, d_ngt, status):
+        """The targets of loss_device that read coordinates, anchors, the anchor mask and GT only, no prediction:
+        (points_in_boxes' (labels, offsets, d_npos) of the voxel means, SSDRotateHead.assign's (labels, targets, ious,
+        d_npos)).  The checkpoints of a CheckpointSweep share them."""
+        d_rows = aux["frame_rows"][batch:batch + 1]
+        points = ops.points_in_boxes(aux["points_mean"], d_rows, gt, d_ngt, status)
+        return points, self._assign_rpn(aux, gt, gt_class, gt_label, d_ngt, status)
+
+    def _assign_rpn(self, aux, gt, gt_class, gt_label, d_ngt, status):
+        anchors, _ = self.anchor_set.device_tensors()
+        names = list(self.class_names) if self.class_names is not None else [None]
+        pos, neg = self.rpn_head.thresholds(self.train_cfg.rpn, names)
+        return self.rpn_head.assign(anchors, aux["mask"], gt, gt_class, gt_label, d_ngt, pos, neg, status)
+
+    def loss_device(self, aux, batch, gt, gt_class, gt_label, d_ngt, n_gt_host, status, targets=None):
         """Targets and losses of one forward_device(point_outputs=True) step, on the device: returns the loss vector
         [6] in ops.LOSS_KEYS order and a dict of the targets.  gt [B,gt_cap,7] etc. as stage_gt gives them.  Nothing
         here reads the host: PSWarp scores min(d_ngt[b], gt_cap) GT rows of each frame, the cap applied by the pswarp
-        and assign_pswarp kernels, so the step can be captured; ``n_gt_host`` is not read."""
+        and assign_pswarp kernels, so the step can be captured; ``n_gt_host`` is not read.  ``targets``: loss_targets'
+        outputs for this step's voxels, anchor mask and GT, which are then not computed again."""
         dev = gt.device
         gt_cap = gt.shape[1]
         out = torch.zeros((len(ops.LOSS_KEYS),), dtype=torch.float32, device=dev)
         cfg = self.train_cfg
         d_rows = aux["frame_rows"][batch:batch + 1]
-        p_lab, p_off, p_npos = ops.points_in_boxes(aux["points_mean"], d_rows, gt, d_ngt, status)
+        if targets is None:
+            p_lab, p_off, p_npos = ops.points_in_boxes(aux["points_mean"], d_rows, gt, d_ngt, status)
+        else:
+            (p_lab, p_off, p_npos), rpn = targets
         ops.aux_loss(aux["point_cls"], aux["point_reg"], p_lab, p_off, d_rows, batch, p_npos, out[0:2])
+        if targets is None:
+            rpn = self._assign_rpn(aux, gt, gt_class, gt_label, d_ngt, status)
         anchors, _ = self.anchor_set.device_tensors()
-        names = list(self.class_names) if self.class_names is not None else [None]
-        pos, neg = self.rpn_head.thresholds(cfg.rpn, names)
         r_lab, r_tgt, r_iou, _ = self.rpn_head.loss_device(aux["head"], anchors, aux["mask"], gt, gt_class, gt_label,
-                                                           d_ngt, pos, neg, out[2:5], status)
+                                                           d_ngt, pos_thr=None, neg_thr=None, out=out[2:5],
+                                                           status=status, targets=rpn)
         # PSWarp scores the GT rows the reference prepends to each frame's guided boxes (:364-367) in a slot segment of
         # their own, so the guided capacity does not grow
         gt_scores = self.extra_head.sample(aux["ps_feat"], gt, d_ngt)
@@ -601,6 +625,185 @@ class DetectorSet:
         yield from _stream_through(self, batches, batch, max_points_per_frame, depth, concurrent, crop, kitti, False)
 
 
+class CheckpointSweep:
+    """Several checkpoints of one config validated as one: the same frames, the same step, each checkpoint's detections
+    and losses.  This is how a training run's saved checkpoints are compared on a labelled split.
+
+    ``models``: K >= 1 SingleStageDetectors built from one config (build_from_config), each with its own weights, in
+    eval() mode and on one device.  They must share the voxel grid, the neck's output_shape and row_cap_factor, the
+    anchors, class_names, train_cfg, test_cfg and the detection capacity (ValueError otherwise): the step computes
+    everything that depends on these and not on the weights once.
+
+    One step crops (when asked), copies, voxelizes, builds the seven rulebooks and the anchor mask once; with GT it
+    also computes the auxiliary network's nearest voxel centres (three_nn), the point targets (points_in_boxes) and
+    the RPN targets (assign_rpn) once.  Per checkpoint it runs the sparse backbone, BEV neck, heads, PSWarp, rescoring
+    and NMS, the auxiliary head, the PSWarp targets and the loss reductions, and with ``metas`` the KITTI formatter on
+    that checkpoint's block.  The checkpoints share one status word, checked when the step's results are read.
+
+    forward_points, enable_cuda_graph and detect_stream take the items of the SingleStageDetector methods of the same
+    names (losses included; without auxiliary outputs or return_aux) and return a list of K results in member order:
+    entry k is exactly what member k returns for the same call.  A sweep of one model returns [that model's result].
+    The sweep keeps its own captured graphs and stream slots; reloading a member's parameters or changing its
+    precision drops them.
+
+    Memory: one step holds the front end and one network's activations at a time (each member's are freed before the
+    next runs), so a captured step's graph pool hardly grows with K.  On an H100 80GB HBM3 at batch 16 of full sweeps
+    with the losses it measured 7.9 GB at K = 4 and at K = 10, against 7.2 GB for one model
+    (tests/tools/checkpoint_sweep_memory.py); each checkpoint's weights and cached empty-scene maps add about 0.33 GB.
+    detect_stream's ``depth`` slots each hold one such step: test.py's four take about 32 GB at batch 16."""
+
+    def __init__(self, models):
+        models = list(models)
+        if not models:
+            raise ValueError("a CheckpointSweep needs at least one model")
+        for i, m in enumerate(models):
+            if not isinstance(m, SingleStageDetector):
+                raise TypeError("member %d is a %s, not a SingleStageDetector" % (i, type(m).__name__))
+            if m.training:
+                raise ValueError("member %d is in training mode: call .eval() first" % i)
+            if m.voxel_generator is None or m.anchor_set is None or m.class_names is None:
+                raise ValueError("member %d has no data pipeline or class names (build_from_config attaches them)" % i)
+        lead = models[0]
+        for i, m in enumerate(models[1:], 1):
+            diff = config_difference(lead, m)
+            if diff:
+                raise ValueError("member %d differs from member 0 in %s: a sweep compares checkpoints of one config" %
+                                 (i, diff))
+            if next(m.parameters()).device != next(lead.parameters()).device:
+                raise ValueError("member %d is on another device than member 0" % i)
+        self.models = models
+        self.class_names = list(lead.class_names)
+        self._pinned = None
+        self._graphs = {}                 # (crop kind, kitti, losses) -> the sweep's captured step (enable_cuda_graph)
+        self._graph_args = None
+        self._stream_slots = None
+        self._stream_key = None
+        for m in models:
+            m._sets.add(self)
+
+    parameters = DetectorSet.parameters
+    refresh_packed_weights = DetectorSet.refresh_packed_weights
+    stage_points = SingleStageDetector.stage_points
+    disable_cuda_graph = SingleStageDetector.disable_cuda_graph
+    _gt_inputs = staticmethod(SingleStageDetector._gt_inputs)
+
+    def _require_loss_step(self):
+        for m in self.models:
+            m._require_loss_step()
+
+    def enable_cuda_graph(self, batch, max_points_per_frame=32768):
+        """SingleStageDetector.enable_cuda_graph for the sweep's step: the plain kind is captured here and returned,
+        the crop, KITTI and loss kinds on their first use."""
+        self._graph_args = (int(batch), int(max_points_per_frame))
+        self._graphs = {}
+        return self._graph_for(CROP_NONE, False)
+
+    def _graph_for(self, crop, kitti, losses=False):
+        key = (int(crop), kitti, losses)
+        if key not in self._graphs and self._graph_args is not None:
+            self._graphs[key] = _GraphedStep(self, *self._graph_args, latency=True, crop=crop, kitti=kitti,
+                                             losses=losses, run_step=_sweep_step)
+        return self._graphs.get(key)
+
+    def _frame_results(self, out, metas):
+        """A step's host outputs, the K members' blocks one after another -> per member the frame results of
+        SingleStageDetector._frame_results."""
+        K = len(self.models)
+        if metas is not None:
+            res = annos_from_rows(*out, self.class_names, [m["sample_idx"] for m in metas] * K)
+        else:
+            res = [dict(boxes_lidar=b, scores=s, label_preds=l) for b, s, l in zip(*out)]
+        B = len(res) // K
+        return [res[k * B:(k + 1) * B] for k in range(K)]
+
+    def _loss_results(self, h):
+        """The K members' loss vectors, one after another -> one dict of floats per member."""
+        n = len(ops.LOSS_KEYS)
+        return [_loss_dict(h[k * n:(k + 1) * n]) for k in range(len(self.models))]
+
+    def _collected(self, slot, metas):
+        res = self._frame_results(slot.collect(), metas)
+        return list(zip(res, self._loss_results(slot.h_loss))) if slot.losses else res
+
+    def forward_points(self, points_list, frustum_planes=None, metas=None, image_fov=False, gt_bboxes=None,
+                       gt_labels=None):
+        """SingleStageDetector.forward_points for every member in one step: a list with, per member, what its own
+        forward_points returns for these arguments ((results, losses) with GT)."""
+        ops.require_cuda()
+        kind = _crop_kind(frustum_planes is not None, image_fov, metas is not None)
+        B = len(points_list)
+        losses = gt_bboxes is not None or gt_labels is not None
+        gt_in = None
+        if losses:
+            self._require_loss_step()
+            if gt_bboxes is None or gt_labels is None:
+                raise ValueError("forward_points: gt_bboxes and gt_labels go together")
+            gt_in = self._gt_inputs(gt_bboxes, gt_labels, B)
+        planes = None if frustum_planes is None else _frame_planes(frustum_planes, B)
+        meta = None if metas is None else _meta_blocks(metas, B)
+        hp, ho, counts = self.stage_points(points_list)
+        g = self._graph_for(kind, meta is not None, losses)
+        if g is not None and g.fits(B, counts):
+            res = self._frame_results(g.run_host(hp, ho, sum(counts), planes, meta, gt_in), metas)
+            return list(zip(res, self._loss_results(g.h_loss))) if losses else res
+        dev = next(self.parameters()).device
+        gt = stage_gt(*gt_in, dev) if losses else None
+        det, d_ndet, status, aux = _sweep_step(self, hp.to(dev, non_blocking=True), ho.to(dev, non_blocking=True), B,
+                                               max(counts + [1]), _to_device(planes, dev), _to_device(meta, dev),
+                                               image_fov=kind == CROP_IMAGE_FOV, gt=gt)
+        if meta is not None:
+            ops._lib.raise_on_status(status)
+            out = aux["rows"].cpu().numpy(), aux["n_out"].cpu().numpy()
+        else:
+            out = unpack_detections(det, d_ndet, status)
+        res = self._frame_results(out, metas)
+        return list(zip(res, self._loss_results(aux["losses"].cpu()))) if losses else res
+
+    def detect_stream(self, batches, batch, max_points_per_frame=32768, depth=4, concurrent=True, crop=False,
+                      kitti=False, image_fov=False, losses=False):
+        """SingleStageDetector.detect_stream for the sweep: the same items, ``depth`` captured sweep steps used
+        round-robin, and per batch a list with each member's yield."""
+        ops.require_cuda()
+        kind = _crop_kind(bool(crop), image_fov, kitti)
+        losses = bool(losses)
+        if losses:
+            self._require_loss_step()
+        key = (batch, max_points_per_frame, depth, kind, bool(kitti), losses)
+        if self._stream_key != key or self._stream_slots is None:
+            self._stream_slots = [_GraphedStep(self, batch, max_points_per_frame, crop=kind, kitti=kitti, losses=losses,
+                                               run_step=_sweep_step) for _ in range(depth)]
+            self._copy_stream = torch.cuda.Stream()
+            self._stream_key = key
+        yield from _stream_through(self, batches, batch, max_points_per_frame, depth, concurrent, crop, kitti, losses)
+
+
+def config_difference(a, b):
+    """What differs between two SingleStageDetectors in what a CheckpointSweep computes once for all of its members
+    ('' when nothing): the voxel grid, the neck's output_shape and row_cap_factor, the anchors, class_names,
+    train_cfg, test_cfg, the detection capacity."""
+    diff = []
+    grid = voxel_grid_difference(a.voxel_generator, b.voxel_generator)
+    if grid:
+        diff.append("voxel grid (%s)" % grid)
+    if list(a.neck.sparse_shape) != list(b.neck.sparse_shape):
+        diff.append("neck output_shape %s vs %s" % (list(a.neck.sparse_shape), list(b.neck.sparse_shape)))
+    if a.neck.row_cap_factor != b.neck.row_cap_factor:
+        diff.append("neck row_cap_factor %r vs %r" % (a.neck.row_cap_factor, b.neck.row_cap_factor))
+    sa, sb = a.anchor_set, b.anchor_set
+    if not (np.array_equal(sa.anchors, sb.anchors) and np.array_equal(sa.rects, sb.rects)
+            and sa.grid_hw == sb.grid_hw and sa.threshold == sb.threshold):
+        diff.append("anchors")
+    if list(a.class_names) != list(b.class_names):
+        diff.append("class_names %s vs %s" % (list(a.class_names), list(b.class_names)))
+    if a.train_cfg != b.train_cfg:
+        diff.append("train_cfg")
+    if a.test_cfg != b.test_cfg:
+        diff.append("test_cfg")
+    if a.extra_head.det_cap != b.extra_head.det_cap:
+        diff.append("detection capacity %d vs %d" % (a.extra_head.det_cap, b.extra_head.det_cap))
+    return ", ".join(diff)
+
+
 def merged_classes(class_lists):
     """The class list of a DetectorSet and each member's label offset into it: the members' class names
     concatenated in member order, member m's labels shifted by the number of classes before it.  A class in two
@@ -760,6 +963,52 @@ def _set_step(dset, points, pt_off, batch, maxpts, planes=None, meta=None, point
     return det, d_ndet, status, aux
 
 
+def _sweep_step(sweep, points, pt_off, batch, maxpts, planes=None, meta=None, point_outputs=False, image_fov=False,
+                gt=None):
+    """One CheckpointSweep step on the device, no synchronisation; the sweep's eager calls and captured graphs build it
+    here, from the parts of _run_step.  Once: the crop, the voxelizer, the seven rulebooks and the anchor mask, and
+    with ``gt`` the nearest voxel centres (member 0's auxiliary network computes them, the others reuse them) and
+    loss_targets.  Per member forward_voxels on the shared inputs, loss_device on the shared targets and, with
+    ``meta``, the KITTI formatter.  The members share the status word.  Returns (det [K*batch,det_cap,9], d_ndet
+    [K*batch], status, aux), the members' blocks one after another, with aux["rows"] / aux["n_out"] likewise and
+    aux["losses"] the K loss vectors [K*6]."""
+    assert not point_outputs, "a CheckpointSweep step has no auxiliary outputs"
+    points, pt_off = _crop_step(points, pt_off, batch, planes, meta, image_fov)
+    lead = sweep.models[0]
+    status = torch.zeros((1,), dtype=torch.int32, device=points.device)
+    vox = lead.voxel_generator.generate_device(points, pt_off, batch, maxpts, status)
+    _, coors, _, mean, frame_rows = vox
+    d_rows = frame_rows[batch:batch + 1]
+    mask = lead.anchor_mask(coors, d_rows, batch)
+    shared = lead.neck.sparse_input(mean, coors, batch, d_rows=d_rows, status=status)
+    dets, ndets, rows, n_out, losses = [], [], [], [], []
+    neighbours = targets = None
+    for m in sweep.models:
+        det, d_ndet, _, aux = m.forward_voxels(vox, batch, status, sparse_in=shared, point_outputs=gt is not None,
+                                               mask=mask, neighbours=neighbours)
+        dets.append(det)
+        ndets.append(d_ndet)
+        if gt is not None:
+            if targets is None:
+                neighbours = aux["idx"], aux["dist2"], aux["points_mean"]
+                targets = m.loss_targets(aux, batch, *gt, status)
+            losses.append(m.loss_device(aux, batch, *gt, None, status, targets=targets)[0])
+        # a member's activations (about 4 GB at batch 16) must be free before the next member allocates its own, so
+        # that the step - and its captured graph's private pool - holds one network's, not two
+        aux = None
+        if meta is not None:
+            r, n = ops.kitti_format(det, d_ndet, meta)
+            rows.append(r)
+            n_out.append(n)
+    det, d_ndet = torch.cat(dets), torch.cat(ndets)
+    aux = dict(coors=coors, frame_rows=frame_rows)
+    if gt is not None:
+        aux["losses"] = torch.cat(losses)
+    if meta is not None:
+        aux["rows"], aux["n_out"] = torch.cat(rows), torch.cat(n_out)
+    return det, d_ndet, status, aux
+
+
 def _pinned_pair(n_points, n_off):
     return (torch.empty((n_points, 4), dtype=torch.float32, pin_memory=True),
             torch.empty((n_off,), dtype=torch.int32, pin_memory=True))
@@ -865,7 +1114,7 @@ class _GraphedStep:
             self.h_pts = {k: torch.empty(self.aux[k].shape, dtype=self.aux[k].dtype, pin_memory=True)
                           for k in _POINT_KEYS}
         if self.losses:
-            self.h_loss = torch.empty((len(ops.LOSS_KEYS),), dtype=torch.float32, pin_memory=True)
+            self.h_loss = torch.empty(self.aux["losses"].shape, dtype=torch.float32, pin_memory=True)
         self.h_status = torch.empty((1,), dtype=torch.int32, pin_memory=True)
         self.h_points, self.h_off = _pinned_pair(self.cap, self.batch + 1)
         if self.crop == CROP_FRUSTUM:

@@ -125,26 +125,42 @@ def _d3_from_bev(boxes, qboxes, rinc, criterion=-1):
 
 def calculate_overlaps(gt_annos, dt_annos, metric, overlap_fn=None):
     """overlaps[f][detection, ground truth] as float64 (what calculate_iou_partly(dt, gt, metric) returns)."""
+    return calculate_overlaps_many(gt_annos, [dt_annos], metric, overlap_fn)[0]
+
+
+def calculate_overlaps_many(gt_annos, dt_sets, metric, overlap_fn=None):
+    """calculate_overlaps of each detection set in ``dt_sets`` against the same GT: the rotated overlaps of every
+    (set, frame) pair in one kernel launch."""
     if metric == 0:
-        return [image_box_overlap(np.asarray(d["bbox"], np.float64).reshape(-1, 4),
-                                  np.asarray(g["bbox"], np.float64).reshape(-1, 4)) for g, d in zip(gt_annos, dt_annos)]
+        gts = [np.asarray(g["bbox"], np.float64).reshape(-1, 4) for g in gt_annos]
+        return [[image_box_overlap(np.asarray(d["bbox"], np.float64).reshape(-1, 4), g) for g, d in zip(gts, dts)]
+                for dts in dt_sets]
 
     def cam(a):
         return np.concatenate([np.asarray(a["location"], np.float64).reshape(-1, 3),
                                np.asarray(a["dimensions"], np.float64).reshape(-1, 3),
                                np.asarray(a["rotation_y"], np.float64).reshape(-1, 1)], 1)
-    dts, gts = [cam(d) for d in dt_annos], [cam(g) for g in gt_annos]
+    gts = [cam(g) for g in gt_annos]
+    dts = [cam(d) for dt_annos in dt_sets for d in dt_annos]
     bev = [0, 2, 3, 5, 6]
+    ov = _rotated_overlaps([d[:, bev] for d in dts], [g[:, bev] for g in gts] * len(dt_sets), -1 if metric == 1 else 2,
+                           overlap_fn)
     if metric == 1:
-        ov = _rotated_overlaps([d[:, bev] for d in dts], [g[:, bev] for g in gts], -1, overlap_fn)
-        return [o.astype(np.float64) for o in ov]
-    rinc = _rotated_overlaps([d[:, bev] for d in dts], [g[:, bev] for g in gts], 2, overlap_fn)
-    return [_d3_from_bev(d, g, r).astype(np.float64) for d, g, r in zip(dts, gts, rinc)]
+        ov = [o.astype(np.float64) for o in ov]
+    else:
+        ov = [_d3_from_bev(d, g, r).astype(np.float64) for d, g, r in zip(dts, gts * len(dt_sets), ov)]
+    n = len(gt_annos)
+    return [ov[k * n:(k + 1) * n] for k in range(len(dt_sets))]
 
 
 # ------------------------------------------------------------------ matching
 def clean_data(gt_anno, dt_anno, current_class, difficulty):
     """Ignore flags of one frame (kitti_eval.py:39-92): 0 evaluate, 1 ignore, -1 other class."""
+    return clean_gt(gt_anno, current_class, difficulty) + (clean_dt(dt_anno, current_class, difficulty),)
+
+
+def clean_gt(gt_anno, current_class, difficulty):
+    """clean_data's GT side: (valid GT count, GT ignore flags, DontCare boxes)."""
     cls = CLASS_NAMES[current_class].lower()
     names = np.char.lower(np.asarray(gt_anno["name"], dtype=str)) if len(gt_anno["name"]) else np.zeros((0,), str)
     bbox = np.asarray(gt_anno["bbox"], np.float64).reshape(-1, 4)
@@ -158,11 +174,16 @@ def clean_data(gt_anno, dt_anno, current_class, difficulty):
               | ((bbox[:, 3] - bbox[:, 1]) <= MIN_HEIGHT[difficulty]))
     ign_gt = np.where((valid == 1) & ~ignore, 0, np.where((valid == 0) | (ignore & (valid == 1)), 1, -1)).astype(np.int32)
     dc = bbox[np.asarray(gt_anno["name"], dtype=str) == "DontCare"] if len(names) else np.zeros((0, 4))
+    return int((ign_gt == 0).sum()), ign_gt, dc
+
+
+def clean_dt(dt_anno, current_class, difficulty):
+    """clean_data's detection side: the detections' ignore flags."""
+    cls = CLASS_NAMES[current_class].lower()
     dnames = np.char.lower(np.asarray(dt_anno["name"], dtype=str)) if len(dt_anno["name"]) else np.zeros((0,), str)
     dbox = np.asarray(dt_anno["bbox"], np.float64).reshape(-1, 4)
     height = np.abs(dbox[:, 3] - dbox[:, 1])
-    ign_dt = np.where(height < MIN_HEIGHT[difficulty], 1, np.where(dnames == cls, 0, -1)).astype(np.int32)
-    return int((ign_gt == 0).sum()), ign_gt, ign_dt, dc
+    return np.where(height < MIN_HEIGHT[difficulty], 1, np.where(dnames == cls, 0, -1)).astype(np.int32)
 
 
 def get_thresholds(scores, num_gt, num_sample_pts=41):
@@ -179,39 +200,53 @@ def get_thresholds(scores, num_gt, num_sample_pts=41):
     return np.asarray(thresholds, np.float64)
 
 
-class _Packed:
-    """Per-(class, difficulty) flat arrays for sassd_kitti_match."""
+def _cat(xs, shape, dt):
+    return np.ascontiguousarray(np.concatenate(xs, 0), dtype=dt) if len(xs) else np.zeros(shape, dt)
 
-    def __init__(self, gt_annos, dt_annos, overlaps, current_class, difficulty):
-        prep = [clean_data(g, d, current_class, difficulty) for g, d in zip(gt_annos, dt_annos)]
+
+class _GtSide:
+    """The GT half of sassd_kitti_match's flat arrays for one (class, difficulty): clean_gt of every frame, flattened.
+    Every detection set evaluated against the same GT shares it."""
+
+    def __init__(self, gt_annos, current_class, difficulty):
+        prep = [clean_gt(g, current_class, difficulty) for g in gt_annos]
         self.nframes = len(gt_annos)
         self.total_valid = sum(p[0] for p in prep)
-        ng = [len(p[1]) for p in prep]
-        nd = [len(p[2]) for p in prep]
-        self.gt_off, self.dt_off = _offsets(ng), _offsets(nd)
-        self.dc_off = _offsets([p[3].shape[0] for p in prep])
-        self.ov_off = _offsets(np.asarray(ng, np.int64) * np.asarray(nd, np.int64), np.int64)
-        cat = lambda xs, shape, dt: (np.ascontiguousarray(np.concatenate(xs, 0), dtype=dt) if len(xs) else       # noqa: E731
-                                     np.zeros(shape, dt))
-        self.overlaps = cat([np.asarray(o, np.float64).reshape(-1) for o in overlaps], (0,), np.float64)
-        self.gt_alpha = cat([np.asarray(g["alpha"], np.float64).reshape(-1) for g in gt_annos], (0,), np.float64)
-        self.dt_alpha = cat([np.asarray(d["alpha"], np.float64).reshape(-1) for d in dt_annos], (0,), np.float64)
-        self.dt_score = cat([np.asarray(d["score"], np.float64).reshape(-1) for d in dt_annos], (0,), np.float64)
-        self.dt_bbox = cat([np.asarray(d["bbox"], np.float64).reshape(-1, 4) for d in dt_annos], (0, 4), np.float64)
-        self.dc_bbox = cat([p[3].reshape(-1, 4) for p in prep], (0, 4), np.float64)
-        self.ign_gt = cat([p[1] for p in prep], (0,), np.int32)
-        self.ign_dt = cat([p[2] for p in prep], (0,), np.int32)
+        self.ng = [len(p[1]) for p in prep]
+        self.gt_off = _offsets(self.ng)
+        self.dc_off = _offsets([p[2].shape[0] for p in prep])
+        self.gt_alpha = _cat([np.asarray(g["alpha"], np.float64).reshape(-1) for g in gt_annos], (0,), np.float64)
+        self.dc_bbox = _cat([p[2].reshape(-1, 4) for p in prep], (0, 4), np.float64)
+        self.ign_gt = _cat([p[1] for p in prep], (0,), np.int32)
+
+
+class _Packed:
+    """Per-(class, difficulty) flat arrays for sassd_kitti_match: a _GtSide and one detection set's half."""
+
+    def __init__(self, gt, dt_annos, overlaps, current_class, difficulty):
+        ign_dt = [clean_dt(d, current_class, difficulty) for d in dt_annos]
+        self.gt = gt
+        self.nframes, self.total_valid = gt.nframes, gt.total_valid
+        nd = [len(i) for i in ign_dt]
+        self.dt_off = _offsets(nd)
+        self.ov_off = _offsets(np.asarray(gt.ng, np.int64) * np.asarray(nd, np.int64), np.int64)
+        self.overlaps = _cat([np.asarray(o, np.float64).reshape(-1) for o in overlaps], (0,), np.float64)
+        self.dt_alpha = _cat([np.asarray(d["alpha"], np.float64).reshape(-1) for d in dt_annos], (0,), np.float64)
+        self.dt_score = _cat([np.asarray(d["score"], np.float64).reshape(-1) for d in dt_annos], (0,), np.float64)
+        self.dt_bbox = _cat([np.asarray(d["bbox"], np.float64).reshape(-1, 4) for d in dt_annos], (0, 4), np.float64)
+        self.ign_dt = _cat(ign_dt, (0,), np.int32)
 
     def match(self, metric, min_overlap, thresholds=None, compute_aos=False):
         L = _lib.load()
         nth = 0 if thresholds is None else len(thresholds)
         pr = np.zeros((max(nth, 1), 4), np.float64)
-        tp_scores = np.zeros((max(len(self.gt_alpha), 1),), np.float64)
+        g = self.gt
+        tp_scores = np.zeros((max(len(g.gt_alpha), 1),), np.float64)
         ntp = np.zeros((1,), np.int64)
         th = np.ascontiguousarray(thresholds, np.float64) if nth else None
-        _lib.check(L.sassd_kitti_match(self.nframes, _p(self.overlaps), _p(self.ov_off), _p(self.gt_off), _p(self.dt_off),
-                                       _p(self.dc_off), _p(self.gt_alpha), _p(self.dt_alpha), _p(self.dt_score),
-                                       _p(self.dt_bbox), _p(self.dc_bbox), _p(self.ign_gt), _p(self.ign_dt), int(metric),
+        _lib.check(L.sassd_kitti_match(self.nframes, _p(self.overlaps), _p(self.ov_off), _p(g.gt_off), _p(self.dt_off),
+                                       _p(g.dc_off), _p(g.gt_alpha), _p(self.dt_alpha), _p(self.dt_score),
+                                       _p(self.dt_bbox), _p(g.dc_bbox), _p(g.ign_gt), _p(self.ign_dt), int(metric),
                                        float(min_overlap), int(bool(compute_aos)), nth, _p(th), _p(pr), _p(tp_scores),
                                        _p(ntp)), "sassd_kitti_match")
         return pr[:nth], tp_scores[:int(ntp[0])]
@@ -221,29 +256,41 @@ def eval_class(gt_annos, dt_annos, current_classes, difficultys, metric, min_ove
                overlap_fn=None):
     """precision / recall / orientation [class, difficulty, min_overlap, 41] (eval_class_v3, kitti_eval.py:549-657).
     min_overlaps: [num_minoverlap, metric, class]."""
-    assert len(gt_annos) == len(dt_annos)
-    overlaps = calculate_overlaps(gt_annos, dt_annos, metric, overlap_fn)
+    return eval_class_many(gt_annos, [dt_annos], current_classes, difficultys, metric, min_overlaps, [compute_aos],
+                           overlap_fn)[0]
+
+
+def eval_class_many(gt_annos, dt_sets, current_classes, difficultys, metric, min_overlaps, compute_aos, overlap_fn=None,
+                    gt_sides=None):
+    """eval_class for each detection set of ``dt_sets`` against the same GT (``compute_aos``: one flag per set): one
+    overlap pass for all sets (calculate_overlaps_many) and one GT side per class and difficulty (``gt_sides``:
+    {(class, difficulty): _GtSide}, built here when not given)."""
+    assert all(len(gt_annos) == len(d) for d in dt_sets)
+    overlaps = calculate_overlaps_many(gt_annos, dt_sets, metric, overlap_fn)
     shape = (len(current_classes), len(difficultys), len(min_overlaps), 41)
-    precision, recall, aos = np.zeros(shape), np.zeros(shape), np.zeros(shape)
+    out = [dict(recall=np.zeros(shape), precision=np.zeros(shape), orientation=np.zeros(shape)) for _ in dt_sets]
     for m, cls in enumerate(current_classes):
         for l, diff in enumerate(difficultys):
-            packed = _Packed(gt_annos, dt_annos, overlaps, cls, diff)
-            for k, min_overlap in enumerate(min_overlaps[:, metric, m]):
-                _, tp_scores = packed.match(metric, min_overlap)
-                thresholds = get_thresholds(tp_scores, packed.total_valid)
-                pr, _ = packed.match(metric, min_overlap, thresholds, compute_aos)
-                n = len(thresholds)
-                with np.errstate(divide="ignore", invalid="ignore"):
-                    recall[m, l, k, :n] = pr[:, 0] / (pr[:, 0] + pr[:, 2])
-                    precision[m, l, k, :n] = pr[:, 0] / (pr[:, 0] + pr[:, 1])
-                    if compute_aos:
-                        aos[m, l, k, :n] = pr[:, 3] / (pr[:, 0] + pr[:, 1])
-                for i in range(n):      # monotone envelope over the sampled points (:645-651)
-                    precision[m, l, k, i] = np.max(precision[m, l, k, i:])
-                    recall[m, l, k, i] = np.max(recall[m, l, k, i:])
-                    if compute_aos:
-                        aos[m, l, k, i] = np.max(aos[m, l, k, i:])
-    return dict(recall=recall, precision=precision, orientation=aos)
+            gt = _GtSide(gt_annos, cls, diff) if gt_sides is None else gt_sides[cls, diff]
+            for dt_annos, ov, aos_s, res in zip(dt_sets, overlaps, compute_aos, out):
+                packed = _Packed(gt, dt_annos, ov, cls, diff)
+                recall, precision, aos = res["recall"], res["precision"], res["orientation"]
+                for k, min_overlap in enumerate(min_overlaps[:, metric, m]):
+                    _, tp_scores = packed.match(metric, min_overlap)
+                    thresholds = get_thresholds(tp_scores, packed.total_valid)
+                    pr, _ = packed.match(metric, min_overlap, thresholds, aos_s)
+                    n = len(thresholds)
+                    with np.errstate(divide="ignore", invalid="ignore"):
+                        recall[m, l, k, :n] = pr[:, 0] / (pr[:, 0] + pr[:, 2])
+                        precision[m, l, k, :n] = pr[:, 0] / (pr[:, 0] + pr[:, 1])
+                        if aos_s:
+                            aos[m, l, k, :n] = pr[:, 3] / (pr[:, 0] + pr[:, 1])
+                    for i in range(n):      # monotone envelope over the sampled points (:645-651)
+                        precision[m, l, k, i] = np.max(precision[m, l, k, i:])
+                        recall[m, l, k, i] = np.max(recall[m, l, k, i:])
+                        if aos_s:
+                            aos[m, l, k, i] = np.max(aos[m, l, k, i:])
+    return out
 
 
 def get_mAP(prec):
@@ -262,23 +309,51 @@ def official_eval(gt_annos, dt_annos, current_classes, difficultys=(0, 1, 2), ov
     (get_mAP, the reference's table) or 40 (get_mAP_R40; the text's headings then read AP_R40)."""
     if recall_positions not in (11, 40):
         raise ValueError("recall_positions must be 11 or 40, not %r" % (recall_positions,))
-    get_mAP_n = get_mAP if recall_positions == 11 else get_mAP_R40
-    tag = "AP" if recall_positions == 11 else "AP_R40"
-    if not isinstance(current_classes, (list, tuple)):
-        current_classes = [current_classes]
+    return official_eval_many(gt_annos, [dt_annos], current_classes, (recall_positions,), overlap_fn,
+                              difficultys)[0][recall_positions]
+
+
+def official_eval_many(gt_annos, dt_sets, classes, recall_positions=(11, 40), overlap_fn=None, difficultys=(0, 1, 2)):
+    """official_eval of K detection sets (each a list of per-frame annotation dicts, e.g. one per checkpoint) against
+    the same GT, at each of ``recall_positions`` (11 and / or 40).  Returns one dict per set, {recall positions:
+    official_eval's (text, ap)}.  The rotated overlaps of every (set, frame) pair are one kernel launch for BEV and one
+    for 3D (the 2D box overlaps are vectorised numpy on the host), the GT side of clean_data runs and is flattened once
+    per class and difficulty for all metrics and sets, and R11 and R40 come from one matching pass."""
+    positions = tuple(recall_positions)
+    if not positions or any(r not in (11, 40) for r in positions):
+        raise ValueError("recall_positions must be 11 or 40, not %r" % (recall_positions,))
+    current_classes = classes if isinstance(classes, (list, tuple)) else [classes]
     name_to_class = {v: k for k, v in CLASS_TO_NAME.items()}
     classes = [name_to_class[c] if isinstance(c, str) else c for c in current_classes]
     min_overlaps = np.stack([OVERLAP_0_7, OVERLAP_0_5], axis=0)[:, :, classes]
-    compute_aos = False
-    for anno in dt_annos:                      # :818-823
-        if anno['alpha'].shape[0] != 0:
-            compute_aos = bool(anno['alpha'][0] != -10)
-            break
+    aos_flags = []
+    for dt_annos in dt_sets:
+        compute_aos = False
+        for anno in dt_annos:                      # :818-823
+            if anno['alpha'].shape[0] != 0:
+                compute_aos = bool(anno['alpha'][0] != -10)
+                break
+        aos_flags.append(compute_aos)
     diffs = list(difficultys)
-    r0 = eval_class(gt_annos, dt_annos, classes, diffs, 0, min_overlaps, compute_aos, overlap_fn)
-    ap = dict(bbox=get_mAP_n(r0["precision"]), aos=get_mAP_n(r0["orientation"]) if compute_aos else None,
-              bev=get_mAP_n(eval_class(gt_annos, dt_annos, classes, diffs, 1, min_overlaps, False, overlap_fn)["precision"]),
-              d3=get_mAP_n(eval_class(gt_annos, dt_annos, classes, diffs, 2, min_overlaps, False, overlap_fn)["precision"]))
+    gt_sides = {(c, d): _GtSide(gt_annos, c, d) for c in classes for d in diffs}
+    prec = [eval_class_many(gt_annos, dt_sets, classes, diffs, metric, min_overlaps,
+                            aos_flags if metric == 0 else [False] * len(dt_sets), overlap_fn, gt_sides)
+            for metric in (0, 1, 2)]
+    out = []
+    for s, compute_aos in enumerate(aos_flags):
+        r0, r1, r2 = (p[s] for p in prec)
+        res = {}
+        for rp in positions:
+            get_mAP_n = get_mAP if rp == 11 else get_mAP_R40
+            ap = dict(bbox=get_mAP_n(r0["precision"]), aos=get_mAP_n(r0["orientation"]) if compute_aos else None,
+                      bev=get_mAP_n(r1["precision"]), d3=get_mAP_n(r2["precision"]))
+            res[rp] = (_ap_text(ap, classes, min_overlaps, compute_aos, "AP" if rp == 11 else "AP_R40"), ap)
+        out.append(res)
+    return out
+
+
+def _ap_text(ap, classes, min_overlaps, compute_aos, tag):
+    """The official table of official_eval's AP arrays."""
     lines = []
     for j, cls in enumerate(classes):
         for i in range(min_overlaps.shape[0]):
@@ -287,7 +362,7 @@ def official_eval(gt_annos, dt_annos, current_classes, difficultys=(0, 1, 2), ov
                 lines.append("%s:%.2f, %.2f, %.2f" % (label, ap[key][j, 0, i], ap[key][j, 1, i], ap[key][j, 2, i]))
             if compute_aos:
                 lines.append("aos  AP:%.2f, %.2f, %.2f" % (ap["aos"][j, 0, i], ap["aos"][j, 1, i], ap["aos"][j, 2, i]))
-    return "".join(l + "\n" for l in lines), ap
+    return "".join(l + "\n" for l in lines)
 
 
 def get_official_eval_result(gt_annos, dt_annos, current_classes, difficultys=[0, 1, 2], overlap_fn=None):

@@ -234,14 +234,17 @@ class SpMiddleFHD(nn.Module):
             c = self._point_packed = (ver, fc_t, out)
         return c[1], c[2]
 
-    def point_head(self, mean, coors, d_rows, middle):
+    def point_head(self, mean, coors, d_rows, middle, neighbours=None):
         """The auxiliary network on the device (cmn.py:121-135): ``mean`` / ``coors`` [cap,4] are the voxel rows,
         ``middle`` the outputs of conv1, conv2, conv3.  Returns dict(points_mean [cap,4] (b, x, y, z), point_cls [cap],
         point_reg [cap,3], idx / dist2 [cap,3,3] of the three nearest centres per level); rows past d_rows are
         unwritten.  point_reg is what the reference regresses, the offset from the point to its box centre
-        (points_op.cpp:107-144)."""
-        levels = [(m._indices, m.d_rows) for m in middle]
-        idx, dist2, pm = ops.three_nn(mean, coors, d_rows, levels, points_mean=True)
+        (points_op.cpp:107-144).  ``neighbours``: (idx, dist2, points_mean) of an earlier call over the same voxels and
+        rulebooks; they depend on coordinates only, so the networks of a detectors.CheckpointSweep skip three_nn."""
+        if neighbours is None:
+            levels = [(m._indices, m.d_rows) for m in middle]
+            neighbours = ops.three_nn(mean, coors, d_rows, levels, points_mean=True)
+        idx, dist2, pm = neighbours
         feats = []
         for m, ch in zip(middle, ops._lib.POINT_LEVEL_CHANNELS):
             if m._features is not None:
@@ -313,11 +316,11 @@ class SpMiddleFHD(nn.Module):
         return x
 
     def forward_nhwc(self, voxel_features, coors, batch_size, d_rows=None, status=None, point_outputs=False,
-                     sparse_in=None):
+                     sparse_in=None, neighbours=None):
         """Device-side entry: capacity-sized inputs + row counter; returns NHWC (x, conv6) and the tensor.  With
         ``point_outputs`` the auxiliary network runs after conv3, before the dense neck, and its outputs
-        (point_head) come fourth.  ``sparse_in``: a sparse_input() tensor over these voxels, whose rulebooks this
-        call uses instead of building its own."""
+        (point_head) come fourth; ``neighbours`` as point_head takes them.  ``sparse_in``: a sparse_input() tensor
+        over these voxels, whose rulebooks this call uses instead of building its own."""
         if self.training:
             raise NotImplementedError("sassd_b200 is inference-only: call .eval()")
         if sparse_in is None:
@@ -331,7 +334,7 @@ class SpMiddleFHD(nn.Module):
             torch.cuda.current_stream().wait_stream(side)   # join (also required to end a graph capture)
         pts = None
         if point_outputs:
-            pts = self.point_head(x0_mean, x0_coors, rows0, middle)
+            pts = self.point_head(x0_mean, x0_coors, rows0, middle, neighbours)
         C = x._channels
         D, H, W = x.spatial_shape
         if self.fcn.precision == ops.PREC_F16X3 and self.dense_tma:

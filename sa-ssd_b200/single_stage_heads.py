@@ -146,14 +146,20 @@ class SSDRotateHead(nn.Module):
             names = keys[:1]
         return [float(a[k]["pos_iou_thr"]) for k in names], [float(a[k]["neg_iou_thr"]) for k in names]
 
-    def loss_device(self, head, anchors, mask, gt, gt_class, gt_label, d_ngt, pos_thr, neg_thr, out, status):
-        """No-sync path: targets (create_target_torch with NearestIouSimilarity, per frame and class) and the three
-        RPN losses into out[0:3].  anchors [Na,7] or [B,Na,7], classes concatenated; mask [B,Na] u8.  Returns (labels,
-        targets, ious, d_npos)."""
-        anchors = anchors.contiguous().float()
-        res = ops.assign_rpn(anchors, mask.to(torch.uint8).contiguous(), self._num_class, gt, gt_class, gt_label, d_ngt,
-                             pos_thr, neg_thr, status)
-        ops.rpn_loss(head, self._num_class, anchors, res[0], res[1], res[3], out)
+    def assign(self, anchors, mask, gt, gt_class, gt_label, d_ngt, pos_thr, neg_thr, status):
+        """No-sync path: the RPN targets (create_target_torch with NearestIouSimilarity, per frame and class).  anchors
+        [Na,7] or [B,Na,7], classes concatenated; mask [B,Na] u8.  Returns (labels, targets, ious, d_npos).  They read
+        no prediction, so the checkpoints of one config share them (detectors.CheckpointSweep)."""
+        return ops.assign_rpn(anchors.contiguous().float(), mask.to(torch.uint8).contiguous(), self._num_class, gt,
+                              gt_class, gt_label, d_ngt, pos_thr, neg_thr, status)
+
+    def loss_device(self, head, anchors, mask, gt, gt_class, gt_label, d_ngt, pos_thr, neg_thr, out, status,
+                    targets=None):
+        """No-sync path: the targets (assign, or ``targets`` when it already ran on these inputs) and the three RPN
+        losses into out[0:3].  Returns assign's (labels, targets, ious, d_npos)."""
+        res = self.assign(anchors, mask, gt, gt_class, gt_label, d_ngt, pos_thr, neg_thr, status) \
+            if targets is None else targets
+        ops.rpn_loss(head, self._num_class, anchors.contiguous().float(), res[0], res[1], res[3], out)
         return res
 
     def loss(self, box_preds, cls_preds, dir_cls_preds, gt_bboxes, gt_labels, gt_types, anchors, anchors_mask, cfg):

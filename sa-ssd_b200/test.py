@@ -6,6 +6,7 @@
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR --split test --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --drive DRIVE_DIR [--calib-dir DIR] --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --model CONFIG2 CHECKPOINT2 [--model ...] --data-root DIR [...]
+    python -m sassd_b200.test CONFIG CHECKPOINT --checkpoints CHECKPOINT2 [...] --data-root DIR [--losses] [--r40] [...]
 
 Frames are read from disk a few batches ahead (kitti_data.Prefetcher) and streamed through the captured step
 (SingleStageDetector.detect_stream): full sweeps (``--lidar velodyne``) are cropped to the camera frustum on the
@@ -31,9 +32,18 @@ voxelizes and builds the rulebooks once for all of them, each frame's result fil
 order, and the AP table covers the models' classes in that order.  The models must share the voxel grid and may not
 share a class; ``--losses`` takes one model.
 
+``--checkpoints CHECKPOINT2 [...]`` validates several checkpoints of one config (e.g. those a training run saved) in
+one pass over a labelled split: the models run as one detectors.CheckpointSweep, so every frame is read, cropped and
+voxelized once, the rulebooks and anchor mask are built once and, with ``--losses``, the targets are assigned once, while
+each checkpoint runs its own network.  The driver prints each checkpoint's AP table(s) and loss means under its file
+name, then one summary line per checkpoint (moderate 3D AP per class, rpn_cls_loss and loss_cls means).  ``--out DIR``
+writes each checkpoint's result files to DIR/<checkpoint stem>/.  Each checkpoint's output equals that of a run of its
+own.
+
 Under torchrun, frame i of the split goes to rank i mod W; at the end every rank contributes one fixed-size block of
 KITTI rows and counts to a single all_gather_into_tensor (dist.DetectionGather) and rank 0 re-interleaves, writes and
-evaluates; with ``--losses`` one more all_gather brings every rank's per-batch loss vectors to rank 0.
+evaluates; with ``--losses`` one more all_gather brings every rank's per-batch loss vectors to rank 0.  A checkpoint
+sweep exchanges all checkpoints' rows in the one all_gather and all their loss vectors in the other.
 """
 import argparse
 import json
@@ -74,9 +84,24 @@ def parse_args(argv=None):
     p.add_argument("--r40", action="store_true", help="also print the AP table at 40 recall positions")
     p.add_argument("--model", nargs=2, action="append", default=[], metavar=("CONFIG", "CHECKPOINT"),
                    help="one more single-class model, run with the first as one set (repeatable)")
+    p.add_argument("--checkpoints", nargs="+", default=[], metavar="CHECKPOINT",
+                   help="more checkpoints of CONFIG, validated with CHECKPOINT in one pass over a labelled split")
     args = p.parse_args(argv)
     if args.batch < 1:
         p.error("--batch must be positive")
+    if args.checkpoints:
+        if args.model:
+            p.error("--checkpoints sweeps checkpoints of one config: it does not combine with --model")
+        if args.drive or args.split == "test":
+            p.error("--checkpoints needs a labelled split: %s has no labels" % (
+                "--drive" if args.drive else "--split test"))
+        paths = [os.path.realpath(c) for c in [args.checkpoint] + args.checkpoints]
+        if len(set(paths)) != len(paths):
+            p.error("--checkpoints: a checkpoint is given twice")
+        stems = [checkpoint_stem(c) for c in [args.checkpoint] + args.checkpoints]
+        if args.out and len(set(stems)) != len(stems):
+            p.error("--checkpoints with --out: two checkpoints have the same file stem, so their result directories "
+                    "under %s would clash" % args.out)
     if args.losses and args.model:
         p.error("--losses computes one model's losses: it does not combine with --model")
     if args.losses and (args.drive or args.split == "test"):
@@ -96,6 +121,11 @@ def parse_args(argv=None):
     return args
 
 
+def checkpoint_stem(path):
+    """A checkpoint's file name without its extension: its result directory under --out."""
+    return os.path.splitext(os.path.basename(path))[0]
+
+
 def rank_batches(ids, rank, world, batch):
     """This rank's frames (ids[rank::world]) as padded batches; every rank gets the same number of batches so that the
     result blocks of the final exchange have one size."""
@@ -109,26 +139,35 @@ def rank_batches(ids, rank, world, batch):
 def gather_annos(annos_local, ids, class_names, cap, device):
     """Every rank's per-frame annotation dicts (its frames j*W + rank, padding included) -> the annotations of the
     split's frames ``ids``, in order, on every rank, through one all_gather of [rows | n_out]."""
+    return gather_annos_many([annos_local], ids, class_names, cap, device)[0]
+
+
+def gather_annos_many(annos_sets, ids, class_names, cap, device):
+    """gather_annos for K sets of annotations of the same frames (one per checkpoint), in one all_gather: each local
+    frame's K row blocks go one after another."""
     import torch
     from . import dist as D
     from .results import annos_from_rows, rows_from_annos
-    rows, n_out = rows_from_annos(annos_local, class_names, cap)
-    g = D.DetectionGather(len(annos_local), cap, device, width=2 * rows.shape[2])
+    K, F = len(annos_sets), len(annos_sets[0])
+    rows, n_out = rows_from_annos([a[j] for j in range(F) for a in annos_sets], class_names, cap)
+    g = D.DetectionGather(F * K, cap, device, width=2 * rows.shape[2])
     rows_all, n_all = g(torch.from_numpy(rows).to(device).view(torch.float32),
                         torch.from_numpy(n_out).to(device))
-    rows_all, n_all = D.interleave(rows_all, n_all)
+    W = rows_all.shape[0]          # [W, F*K, ...] -> global frame order (frame j*W + r), then the K blocks
+    rows_all = rows_all.reshape(W, F, K, cap, -1).permute(1, 0, 2, 3, 4).reshape(W * F, K, cap, -1)
+    n_all = n_all.reshape(W, F, K).permute(1, 0, 2).reshape(W * F, K)
     rows_all = rows_all.contiguous().view(torch.float64)[:len(ids)].cpu().numpy()
     n_all = n_all[:len(ids)].cpu().numpy()
-    return annos_from_rows(rows_all, n_all, class_names, ids)
+    return [annos_from_rows(rows_all[:, k], n_all[:, k], class_names, ids) for k in range(K)]
 
 
 def gather_losses(losses_local, n_real, device):
-    """Every rank's per-batch loss vectors (ops.LOSS_KEYS order) and real-frame counts -> the vectors of the batches
-    that hold a real frame, on every rank, in (batch, rank) order, through one all_gather (dist.DetectionGather)."""
+    """Every rank's per-batch loss vectors (ops.LOSS_KEYS order; a checkpoint sweep's K vectors one after another)
+    and real-frame counts -> the vectors of the batches that hold a real frame, on every rank, in (batch, rank) order,
+    through one all_gather (dist.DetectionGather)."""
     import torch
     from . import dist as D
-    from . import ops
-    width = len(ops.LOSS_KEYS)
+    width = len(losses_local[0])
     g = D.DetectionGather(len(n_real), 1, device, width=width)
     vec = torch.tensor(losses_local, dtype=torch.float32).reshape(len(n_real), 1, width)
     vec_all, n_all = D.interleave(*g(vec.to(device), torch.tensor(n_real, dtype=torch.int32).to(device)))
@@ -182,6 +221,15 @@ def run(args, log=print):
             members.append(m)
         model = S.DetectorSet(members)
         det_cap = model.det_cap
+    elif args.checkpoints:              # the positional checkpoint and every --checkpoints one, run as one sweep
+        members = [model]
+        for ckpt in args.checkpoints:
+            m, _, _ = S.build_from_config(cfg, device=device)
+            load_params_from_file(m, ckpt)
+            members.append(m)
+        model = S.CheckpointSweep(members)
+    sweep = bool(args.checkpoints)
+    K = len(args.checkpoints) + 1 if sweep else 1
     fov = bool(args.drive)
     crop = args.lidar == "velodyne" and not fov
     class_names = model.class_names
@@ -203,27 +251,35 @@ def run(args, log=print):
     torch.cuda.synchronize(device)
     reader = Prefetcher(split, batches, depth=args.depth, workers=args.workers)
     t0 = time.perf_counter()
-    annos_local, losses_local = [], []
+    annos_local, losses_local = [[] for _ in range(K)], []      # per checkpoint; per batch (all checkpoints')
     for out in stream(items(reader)):
+        outs = out if sweep else [out]
         if args.losses:
-            out, losses = out
-            losses_local.append([losses[k] for k in ops.LOSS_KEYS])
-        annos_local += out
+            losses_local.append([losses[k] for _, losses in outs for k in ops.LOSS_KEYS])
+            outs = [o for o, _ in outs]
+        for a, o in zip(annos_local, outs):
+            a += o
     torch.cuda.synchronize(device)
     wall = time.perf_counter() - t0
     n_local = sum(i is not None for ids in batches for i in ids)
     wall = D.max_over_ranks(wall, device)
 
     if world > 1:
-        dt_annos = gather_annos(annos_local, split.ids, class_names, det_cap, device)
+        dt_sets = gather_annos_many(annos_local, split.ids, class_names, det_cap, device)
     else:
-        dt_annos = [a for i, a in zip([i for ids in batches for i in ids], annos_local) if i is not None]
+        order = [i for ids in batches for i in ids]
+        dt_sets = [[a for i, a in zip(order, local) if i is not None] for local in annos_local]
+    per_batch = None
     if args.losses:
         per_batch = gather_losses(losses_local, [sum(i is not None for i in ids) for ids in batches], device)
     if rank != 0:
         D.barrier()
         return None
-    if args.out:
+    dt_annos = dt_sets[0]
+    if args.out and sweep:
+        for path, dts in zip([args.checkpoint] + args.checkpoints, dt_sets):
+            write_results(os.path.join(args.out, checkpoint_stem(path)), split.ids, dts, split.result_name)
+    elif args.out:
         write_results(args.out, split.ids, dt_annos, split.result_name)
     fps = len(split.ids) / wall
     rate = "frames: %d (%d rank%s), %.1f frames/s, read wait %.3f s on rank 0 (%d of %d frames on rank 0)" % (
@@ -235,26 +291,75 @@ def run(args, log=print):
         _write_json(args.json, result)
         D.barrier()
         return result
+    if sweep:
+        result["checkpoints"] = _report_sweep(args, split.gt_annos(), dt_sets, class_names, per_batch, log)
+        log(rate)
+        _write_json(args.json, result)
+        D.barrier()
+        return result
     from .kitti_eval import official_eval
     gt_annos = split.gt_annos()
     text, ap = official_eval(gt_annos, dt_annos, class_names)
     log(text, end="")
-    as_lists = lambda ap: {k: (None if v is None else np.asarray(v).tolist()) for k, v in ap.items()}  # noqa: E731
-    result.update(text=text, ap=as_lists(ap))
+    result.update(text=text, ap=_ap_lists(ap))
     if args.r40:
         text40, ap40 = official_eval(gt_annos, dt_annos, class_names, recall_positions=40)
         log(text40, end="")
-        result.update(text_r40=text40, ap_r40=as_lists(ap40))
+        result.update(text_r40=text40, ap_r40=_ap_lists(ap40))
     if args.losses:
-        means = np.mean(np.asarray(per_batch, np.float64), axis=0)
-        log("losses: mean over %d batches of %d frames (per-batch values depend on --batch): %s" % (
-            len(per_batch), args.batch, ", ".join("%s %.6f" % (k, v) for k, v in zip(ops.LOSS_KEYS, means))))
-        result.update(losses=dict(zip(ops.LOSS_KEYS, means.tolist())),
-                      losses_per_batch=[dict(zip(ops.LOSS_KEYS, v)) for v in per_batch])
+        result.update(_loss_means(per_batch, args.batch, log))
     log(rate)
     _write_json(args.json, result)
     D.barrier()
     return result
+
+
+def _ap_lists(ap):
+    return {k: (None if v is None else np.asarray(v).tolist()) for k, v in ap.items()}
+
+
+def _loss_means(per_batch, batch, log):
+    """Print the mean of each loss over the per-batch vectors; returns the result dict's losses entries."""
+    from . import ops
+    means = np.mean(np.asarray(per_batch, np.float64), axis=0)
+    log("losses: mean over %d batches of %d frames (per-batch values depend on --batch): %s" % (
+        len(per_batch), batch, ", ".join("%s %.6f" % (k, v) for k, v in zip(ops.LOSS_KEYS, means))))
+    return dict(losses=dict(zip(ops.LOSS_KEYS, means.tolist())),
+                losses_per_batch=[dict(zip(ops.LOSS_KEYS, v)) for v in per_batch])
+
+
+def _report_sweep(args, gt_annos, dt_sets, class_names, per_batch, log):
+    """Evaluate and print each checkpoint of a sweep (official_eval_many), then one summary line per checkpoint:
+    moderate 3D AP per class at the class's strict overlap (R11, and R40 with --r40) and the rpn_cls_loss / loss_cls
+    means.  Returns the result dict's ``checkpoints`` list."""
+    from . import ops
+    from .kitti_eval import official_eval_many
+    paths = [args.checkpoint] + args.checkpoints
+    positions = (11, 40) if args.r40 else (11,)
+    n = len(ops.LOSS_KEYS)
+    entries, summary = [], []
+    for k, (path, ev) in enumerate(zip(paths, official_eval_many(gt_annos, dt_sets, class_names, positions))):
+        log("== %s ==" % os.path.basename(path))
+        text, ap = ev[11]
+        log(text, end="")
+        entry = dict(path=path, text=text, ap=_ap_lists(ap))
+        line = ["%-24s" % os.path.basename(path)]
+        for j, c in enumerate(class_names):
+            line.append("%s 3d mod R11 %6.2f" % (c, ap["d3"][j, 1, 0]) +
+                        (" R40 %6.2f" % ev[40][1]["d3"][j, 1, 0] if args.r40 else ""))
+        if args.r40:
+            log(ev[40][0], end="")
+            entry.update(text_r40=ev[40][0], ap_r40=_ap_lists(ev[40][1]))
+        if per_batch is not None:
+            entry.update(_loss_means([v[k * n:(k + 1) * n] for v in per_batch], args.batch, log))
+            line.append("rpn_cls_loss %.6f loss_cls %.6f" % (entry["losses"]["rpn_cls_loss"],
+                                                               entry["losses"]["loss_cls"]))
+        entries.append(entry)
+        summary.append("  ".join(line))
+    log("summary: %d checkpoints (moderate 3D AP)" % len(paths))
+    for line in summary:
+        log(line)
+    return entries
 
 
 def _write_json(path, result):
