@@ -566,6 +566,58 @@ int sassd_kitti_match(int nframes, const double* overlaps, const int64_t* ov_off
                       const int32_t* ign_dt, int metric, double min_overlap, int compute_aos, int nthresh,
                       const double* thresholds, double* pr, double* tp_scores, int64_t* n_tp_scores);
 
+/* The same cleaning and matching on the device (csrc/kitti_match.cu), for K detection sets against one GT and any
+ * number of min-overlap rows, with no per-frame host work.  GT rows of all frames are concatenated (gt_off
+ * [nframes + 1]); detection rows of set k's frame f are [dt_off[k * nframes + f], dt_off[k * nframes + f + 1]).
+ * Name ids: each distinct lower-cased class name has one id (-1 for names of no class).
+ *
+ * sassd_kitti_eval_flags: clean_data's flags for every (class c, difficulty entry d), cd = c * ndiff + d:
+ * ign_gt[cd * ngt + row] (0 evaluate, 1 ignore, -1 other class), ign_dt[cd * ndt + row] (1 too low, 0 the class,
+ * -1 other) and n_valid[cd] += the rows flagged 0 (zero it first).  classes[2c] = class c's name id, classes[2c+1] the
+ * id of the name counted as ignored for it (van for car, person_sitting for pedestrian) or -1; limits[3d .. 3d+2] =
+ * (max occlusion, max truncation, min height) of difficulty entry d.  All pointers are device memory. */
+int sassd_kitti_eval_flags(int ngt, const int32_t* gt_name, const double* gt_occ, const double* gt_trunc,
+                           const double* gt_bbox, int ndt, const int32_t* dt_name, const double* dt_bbox, int nclass,
+                           const int32_t* classes, int ndiff, const double* limits, int8_t* ign_gt, int8_t* ign_dt,
+                           int32_t* n_valid, sassd_stream_t stream);
+/* The bbox, BEV and 3-D overlap matrices of every (set, frame) block b = k * nframes + f, row-major [detection, GT]
+ * at ov_off[b] (fp64, bit for bit the host's image_box_overlap / float32 BEV IoU / _d3_from_bev).  bev_iou and
+ * bev_inter are sassd_rotate_overlap_eval's criterion -1 and 2 outputs over the same blocks; cam rows are
+ * (x, y, z, l, h, w, ry) in the camera frame. */
+int sassd_kitti_eval_overlaps(int nsets, int nframes, const int32_t* gt_off, const int32_t* dt_off,
+                              const int64_t* ov_off, const double* gt_cam, const double* dt_cam, const double* gt_bbox,
+                              const double* dt_bbox, const float* bev_iou, const float* bev_inter,
+                              int max_pairs_per_frame, double* ov_bbox, double* ov_bev, double* ov_3d,
+                              sassd_stream_t stream);
+/* HOST function: aos[ov_off[b] + j * ng + i] = (1 + cos(gt_alpha[i] - dt_alpha[j])) / 2 with the host matcher's cos. */
+int sassd_kitti_aos_table(int nsets, int nframes, const int32_t* gt_off, const int32_t* dt_off, const int64_t* ov_off,
+                          const double* gt_alpha, const double* dt_alpha, double* aos);
+
+typedef struct {
+    int nsets, nframes, nclass, ndiff, nover;     /* K, frames, classes, difficulty entries, min-overlap rows */
+    int max_nd, max_ng;                           /* most detections / GT rows of one frame */
+    const int32_t *gt_off, *dt_off;
+    const int64_t* ov_off;
+    const int32_t* gt_dc;                         /* 1 for DontCare GT rows */
+    const double *gt_bbox, *dt_bbox, *dt_score;
+    const double *ov_bbox, *ov_bev, *ov_3d;       /* sassd_kitti_eval_overlaps */
+    const double* aos_table;                      /* sassd_kitti_aos_table, or null */
+    const int32_t* compute_aos;                   /* [nsets] */
+    const double* min_overlaps;                   /* [nover, 3 metrics, nclass] */
+    const int8_t *ign_gt, *ign_dt;
+    const int32_t* n_valid;                       /* sassd_kitti_eval_flags */
+    const int64_t* score_off;                     /* [jobs + 1]: power-of-two region per job, >= n_valid of its cd */
+} SassdKittiEvalDesc;
+/* Job = (((k * nclass + c) * ndiff + d) * 3 + metric) * nover + o.  For every job: the true-positive scores
+ * (compute_fp=False) into scores[score_off[job] ..], n_scores[job] of them; the thresholds of get_thresholds,
+ * thresholds[job * 41 + t] for t < n_thresh[job]; and pr[(job * 41 + t) * 4 + (tp, fp, fn, similarity)] summed over
+ * the frames as fused_compute_statistics does (the similarity in frame order).  Rows past n_thresh are zero.
+ * ws: sassd_kitti_eval_workspace_bytes(max_nd, max_ng) bytes.  SASSD_ERR_ARG for negative counts or a job grid past
+ * 2^31 (job, threshold) items. */
+size_t sassd_kitti_eval_workspace_bytes(int max_nd, int max_ng);
+int sassd_kitti_eval_match(const SassdKittiEvalDesc* desc, double* scores, int32_t* n_scores, double* thresholds,
+                           int32_t* n_thresh, double* pr, void* ws, size_t ws_bytes, sassd_stream_t stream);
+
 /* ------------------------------------------------------------------------
  * Training-time augmentation (the reference's PointAugmentor as
  * prepare_train_img applies it, mmdet/core/point_cloud/point_augmentor.py,

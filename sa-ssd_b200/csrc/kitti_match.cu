@@ -1,0 +1,488 @@
+// The KITTI evaluator's cleaning and matching on the device (mmdet/core/evaluation/kitti_eval.py:39-92 clean_data,
+// :95-154 box / 3-D overlaps, :17-36 get_thresholds, :164-283 compute_statistics_jit, :295-342
+// fused_compute_statistics), for K detection sets against one ground truth and any number of min-overlap rows at once:
+//
+//   sassd_kitti_eval_flags     ignore flags of every GT and detection row for every (class, difficulty);
+//   sassd_kitti_eval_overlaps  the 2-D box, BEV and 3-D overlap matrices of every (set, frame), from the rotated
+//                              overlaps of sassd_rotate_overlap_eval;
+//   sassd_kitti_eval_match     for every job (set, class, difficulty, metric, min-overlap row): the true-positive
+//                              scores, the 41 sampled score thresholds and the per-threshold (tp, fp, fn, similarity)
+//                              sums over all frames, i.e. the host matcher's `pr` array.
+//
+// Every fp64 expression is written with round-to-nearest intrinsics in numpy's (or the host matcher's) operation order
+// and without FMA contraction, so that each array equals what the host path (kitti_eval.py + sassd_kitti_match)
+// computes bit for bit.  The one transcendental, cos() of the AOS similarity, comes from a host table
+// (sassd_kitti_aos_table) made with the host matcher's libm, since the device cos() rounds differently.
+#include <cmath>
+#include <cstdint>
+
+#include "common.cuh"
+
+namespace {
+
+constexpr int kThresh = 41;                  // sampled recall positions (get_thresholds' num_sample_pts)
+constexpr int kMatchCtas = 1024, kMatchThreads = 256;   // persistent grid of the two matching passes
+constexpr long long kScratchThreads = (long long)kMatchCtas * kMatchThreads;
+constexpr double kNo = -10000000.0;          // compute_statistics_jit's NO_DETECTION
+
+__device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
+
+// ------------------------------------------------------------------------------------------------------ flags
+// clean_data (kitti_eval.py:39-92) for every row: GT flags 0 evaluate / 1 ignore / -1 other class, detection flags
+// 1 too low / 0 the class / -1 other class.  limits[3 * d + (0, 1, 2)] = (max occlusion, max truncation, min height)
+// of difficulty entry d; classes[2 * c] is class c's name id, classes[2 * c + 1] the id of the name that counts as
+// "don't care" for it (van for car, person_sitting for pedestrian) or -1.
+__global__ void eval_flags_kernel(int ngt, const int32_t* __restrict__ gt_name, const double* __restrict__ gt_occ,
+                                  const double* __restrict__ gt_trunc, const double* __restrict__ gt_bbox, int ndt,
+                                  const int32_t* __restrict__ dt_name, const double* __restrict__ dt_bbox, int nclass,
+                                  const int32_t* __restrict__ classes, int ndiff, const double* __restrict__ limits,
+                                  int8_t* __restrict__ ign_gt, int8_t* __restrict__ ign_dt, int32_t* __restrict__ n_valid) {
+    const long long rows = (long long)ngt + ndt, total = rows * nclass * ndiff;
+    for (long long w = blockIdx.x * (long long)blockDim.x + threadIdx.x; w < total; w += (long long)gridDim.x * blockDim.x) {
+        const int cd = (int)(w / rows), c = cd / ndiff, d = cd % ndiff;
+        const long long r = w % rows;
+        const int cls = classes[2 * c], alt = classes[2 * c + 1];
+        const double max_occ = limits[3 * d], max_trunc = limits[3 * d + 1], min_h = limits[3 * d + 2];
+        if (r < ngt) {
+            const int nm = gt_name[r];
+            const int valid = nm == cls ? 1 : (alt >= 0 && nm == alt ? 0 : -1);
+            const double h = dsub(gt_bbox[4 * r + 3], gt_bbox[4 * r + 1]);
+            const bool ignore = gt_occ[r] > max_occ || gt_trunc[r] > max_trunc || h <= min_h;
+            const int f = (valid == 1 && !ignore) ? 0 : ((valid == 0 || (ignore && valid == 1)) ? 1 : -1);
+            ign_gt[(long long)cd * ngt + r] = (int8_t)f;
+            if (f == 0) atomicAdd(&n_valid[cd], 1);
+        } else {
+            const long long j = r - ngt;
+            const double h = fabs(dsub(dt_bbox[4 * j + 3], dt_bbox[4 * j + 1]));
+            ign_dt[(long long)cd * ndt + j] = (int8_t)(h < min_h ? 1 : (dt_name[j] == cls ? 0 : -1));
+        }
+    }
+}
+
+// --------------------------------------------------------------------------------------------------- overlaps
+// Block b = k * nframes + f is set k's frame f: detections [dt_off[b], dt_off[b+1]) against GT rows
+// [gt_off[f], gt_off[f+1]), every matrix row-major [detection, GT] at ov_off[b].  cam rows are (x, y, z, l, h, w, ry).
+__global__ void eval_overlaps_kernel(int nsets, int nframes, const int32_t* __restrict__ gt_off,
+                                     const int32_t* __restrict__ dt_off, const long long* __restrict__ ov_off,
+                                     const double* __restrict__ gt_cam, const double* __restrict__ dt_cam,
+                                     const double* __restrict__ gt_bbox, const double* __restrict__ dt_bbox,
+                                     const float* __restrict__ bev_iou, const float* __restrict__ bev_inter,
+                                     double* __restrict__ ov_bbox, double* __restrict__ ov_bev, double* __restrict__ ov_3d) {
+    for (int b = blockIdx.y; b < nsets * nframes; b += gridDim.y) {
+        const int f = b % nframes;
+        const int g0 = gt_off[f], ng = gt_off[f + 1] - g0, d0 = dt_off[b], nd = dt_off[b + 1] - d0;
+        const long long total = (long long)ng * nd, o0 = ov_off[b];
+        for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < total;
+             p += (long long)gridDim.x * blockDim.x) {
+            const int j = (int)(p / ng), i = (int)(p % ng);
+            // image_box_overlap(dt, gt, criterion=-1) (kitti_eval.py:95-122, vectorised in kitti_eval.py)
+            const double* b4 = dt_bbox + 4 * (long long)(d0 + j);
+            const double* q4 = gt_bbox + 4 * (long long)(g0 + i);
+            const double iw = dsub(fmin(b4[2], q4[2]), fmax(b4[0], q4[0]));
+            const double ih = dsub(fmin(b4[3], q4[3]), fmax(b4[1], q4[1]));
+            double v = 0.0;
+            if (iw > 0 && ih > 0) {
+                const double area_b = dmul(dsub(b4[2], b4[0]), dsub(b4[3], b4[1]));
+                const double area_q = dmul(dsub(q4[2], q4[0]), dsub(q4[3], q4[1]));
+                const double inter = dmul(iw, ih);
+                v = ddiv(inter, dsub(dadd(area_b, area_q), inter));
+            }
+            ov_bbox[o0 + p] = v;
+            ov_bev[o0 + p] = (double)bev_iou[o0 + p];
+            // _d3_from_bev (kitti_eval.py:130-154): the height overlap times the float32 BEV intersection area, the
+            // quotient rounded to float32
+            const double* bc = dt_cam + 7 * (long long)(d0 + j);
+            const double* qc = gt_cam + 7 * (long long)(g0 + i);
+            const float rinc = bev_inter[o0 + p];
+            const double hw = dsub(fmin(bc[1], qc[1]), fmax(dsub(bc[1], bc[4]), dsub(qc[1], qc[4])));
+            double v3 = 0.0;
+            if (rinc > 0.f && hw > 0) {
+                const double inc = dmul(hw, (double)rinc);
+                const double a1 = dmul(dmul(bc[3], bc[4]), bc[5]), a2 = dmul(dmul(qc[3], qc[4]), qc[5]);
+                v3 = (double)(float)ddiv(inc, dsub(dadd(a1, a2), inc));
+            }
+            ov_3d[o0 + p] = v3;
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------- matching
+struct Job {
+    int k, c, d, m, o;
+};
+
+__device__ __forceinline__ Job decode_job(const SassdKittiEvalDesc& e, long long job) {
+    Job j;
+    j.o = (int)(job % e.nover); job /= e.nover;
+    j.m = (int)(job % 3); job /= 3;
+    j.d = (int)(job % e.ndiff); job /= e.ndiff;
+    j.c = (int)(job % e.nclass);
+    j.k = (int)(job / e.nclass);
+    return j;
+}
+
+// One frame of one job, everything the matching reads.
+struct Frame {
+    const double* ov;        // [nd, ng]
+    const double* aos;       // [nd, ng] (1 + cos(gt alpha - dt alpha)) / 2, or null
+    const int8_t *igt, *idt;
+    const int32_t* dc;       // DontCare flag of each GT row
+    const double *score, *dt_bbox, *gt_bbox;
+    int ng, nd;
+};
+
+__device__ __forceinline__ Frame frame_of(const SassdKittiEvalDesc& e, const Job& jb, int f) {
+    Frame fr;
+    const int b = jb.k * e.nframes + f, g0 = e.gt_off[f], d0 = e.dt_off[b];
+    const long long ngt = e.gt_off[e.nframes], ndt = e.dt_off[e.nsets * e.nframes];
+    const long long cd = (long long)jb.c * e.ndiff + jb.d;
+    fr.ng = e.gt_off[f + 1] - g0;
+    fr.nd = e.dt_off[b + 1] - d0;
+    const double* ovs[3] = {e.ov_bbox, e.ov_bev, e.ov_3d};
+    fr.ov = ovs[jb.m] + e.ov_off[b];
+    fr.aos = (jb.m == 0 && e.aos_table && e.compute_aos[jb.k]) ? e.aos_table + e.ov_off[b] : nullptr;
+    fr.igt = e.ign_gt + cd * ngt + g0;
+    fr.idt = e.ign_dt + cd * ndt + d0;
+    fr.dc = e.gt_dc + g0;
+    fr.score = e.dt_score + d0;
+    fr.dt_bbox = e.dt_bbox + 4 * (long long)d0;
+    fr.gt_bbox = e.gt_bbox + 4 * (long long)g0;
+    return fr;
+}
+
+__device__ __forceinline__ double min_overlap_of(const SassdKittiEvalDesc& e, const Job& jb) {
+    return e.min_overlaps[((long long)jb.o * 3 + jb.m) * e.nclass + jb.c];   // [nover, metric, class]
+}
+
+// Pass 1 (compute_fp=False): append the score of every true positive to its job's score region.  One thread per
+// (job, frame); `asg` is this thread's assigned-detection scratch, stride kScratchThreads.
+__global__ void __launch_bounds__(kMatchThreads) eval_tp_scores_kernel(SassdKittiEvalDesc e, long long njobs,
+                                                                     char* __restrict__ asg_ws,
+                                                                     double* __restrict__ scores,
+                                                                     int32_t* __restrict__ n_scores) {
+    const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    char* asg = asg_ws + tid;
+    for (long long w = tid; w < njobs * e.nframes; w += kScratchThreads) {
+        const long long job = w / e.nframes;
+        const Job jb = decode_job(e, job);
+        const Frame fr = frame_of(e, jb, (int)(w % e.nframes));
+        if (fr.ng == 0 || fr.nd == 0) continue;
+        const double min_ov = min_overlap_of(e, jb);
+        const long long base = e.score_off[job], cap = e.score_off[job + 1] - base;
+        for (int j = 0; j < fr.nd; ++j) asg[j * kScratchThreads] = 0;
+        for (int i = 0; i < fr.ng; ++i) {
+            const int gi = fr.igt[i];
+            if (gi == -1) continue;
+            int det = -1;
+            double valid = kNo;
+            for (int j = 0; j < fr.nd; ++j) {
+                if (fr.idt[j] == -1 || asg[j * kScratchThreads]) continue;
+                if (fr.ov[(long long)j * fr.ng + i] > min_ov && fr.score[j] > valid) {
+                    det = j;
+                    valid = fr.score[j];
+                }
+            }
+            if (valid == kNo) continue;      // a missed GT (fn) is not counted in this pass
+            if (gi == 1 || fr.idt[det] == 1) {
+                asg[det * kScratchThreads] = 1;
+            } else {
+                const int slot = atomicAdd(&n_scores[job], 1);
+                if (slot < cap) scores[base + slot] = fr.score[det];
+                asg[det * kScratchThreads] = 1;
+            }
+        }
+    }
+}
+
+// get_thresholds (kitti_eval.py:17-36): sort each job's scores descending (bitonic, in its power-of-two region), then
+// pick the scores at the 41 sampled recall positions.  One CTA per job.
+__global__ void eval_thresholds_kernel(SassdKittiEvalDesc e, double* __restrict__ scores,
+                                       const int32_t* __restrict__ n_scores, double* __restrict__ thresholds,
+                                       int32_t* __restrict__ n_thresh) {
+    const long long job = blockIdx.x;
+    const Job jb = decode_job(e, job);
+    double* s = scores + e.score_off[job];
+    const long long P = e.score_off[job + 1] - e.score_off[job];
+    const long long n = n_scores[job] < P ? n_scores[job] : P;
+    for (long long i = n + threadIdx.x; i < P; i += blockDim.x) s[i] = -INFINITY;
+    __syncthreads();
+    for (long long k = 2; k <= P; k <<= 1)
+        for (long long jj = k >> 1; jj > 0; jj >>= 1) {
+            for (long long i = threadIdx.x; i < P; i += blockDim.x) {
+                const long long l = i ^ jj;
+                if (l > i) {
+                    const double a = s[i], b = s[l];
+                    if ((i & k) == 0 ? a < b : a > b) {      // descending runs where (i & k) == 0
+                        s[i] = b;
+                        s[l] = a;
+                    }
+                }
+            }
+            __syncthreads();
+        }
+    if (threadIdx.x != 0) return;
+    const double num_gt = (double)e.n_valid[(long long)jb.c * e.ndiff + jb.d];
+    const double step = 1.0 / (kThresh - 1.0);
+    double cur = 0.0;
+    int nt = 0;
+    for (long long i = 0; i < n && nt < kThresh; ++i) {
+        const double l_recall = ddiv((double)(i + 1), num_gt);
+        const double r_recall = i < n - 1 ? ddiv((double)(i + 2), num_gt) : l_recall;
+        if (dsub(r_recall, cur) < dsub(cur, l_recall) && i < n - 1) continue;
+        thresholds[job * kThresh + nt++] = s[i];
+        cur = dadd(cur, step);
+    }
+    n_thresh[job] = nt;
+}
+
+// np.sum of [0] * nz followed by vals[0 .. n - nz) (stride kScratchThreads): numpy's pairwise summation (blocks of 8
+// partial sums up to 128 elements, halves rounded down to a multiple of 8 above), as the host matcher restates it.
+// The recursion runs on an explicit stack of pending left halves.
+__device__ double pairwise_leaf(const double* vals, int nz, int lo, int n) {
+    auto at = [&](int e) { return lo + e < nz ? 0.0 : vals[(long long)(lo + e - nz) * kScratchThreads]; };
+    if (n < 8) {
+        double s = 0.0;
+        for (int i = 0; i < n; ++i) s = dadd(s, at(i));
+        return s;
+    }
+    double r[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) r[k] = at(k);
+    int i = 8;
+    for (; i + 8 <= n; i += 8)
+#pragma unroll
+        for (int k = 0; k < 8; ++k) r[k] = dadd(r[k], at(i + k));
+    double s = dadd(dadd(dadd(r[0], r[1]), dadd(r[2], r[3])), dadd(dadd(r[4], r[5]), dadd(r[6], r[7])));
+    for (; i < n; ++i) s = dadd(s, at(i));
+    return s;
+}
+
+__device__ double pairwise_sum(const double* vals, int nz, int n) {
+    int lo_s[32], n_s[32];
+    double left_s[32];
+    bool right_s[32];
+    int depth = 0, lo = 0;
+    for (;;) {
+        while (n > 128) {                          // descend into left halves
+            int n2 = n / 2;
+            n2 -= n2 % 8;
+            lo_s[depth] = lo; n_s[depth] = n; right_s[depth] = false;
+            ++depth;
+            n = n2;
+        }
+        double r = pairwise_leaf(vals, nz, lo, n);
+        for (;;) {                                 // climb until a split still owes its right half
+            if (depth == 0) return r;
+            const int d = depth - 1;
+            int n2 = n_s[d] / 2;
+            n2 -= n2 % 8;
+            if (!right_s[d]) {
+                left_s[d] = r; right_s[d] = true;
+                lo = lo_s[d] + n2; n = n_s[d] - n2;
+                break;
+            }
+            r = dadd(left_s[d], r);
+            depth = d;
+        }
+    }
+}
+
+// compute_statistics_jit with compute_fp=True (kitti_eval.py:164-283) for one frame at one threshold.
+__device__ void frame_statistics(const Frame& fr, int metric, double min_ov, double thresh, char* asg, double* vals,
+                                 int* tp_out, int* fp_out, int* fn_out, double* sim_out) {
+    const long long S = kScratchThreads;
+    int tp = 0, fp = 0, fn = 0, nv = 0;
+    for (int j = 0; j < fr.nd; ++j) asg[j * S] = 0;
+    for (int i = 0; i < fr.ng; ++i) {
+        const int gi = fr.igt[i];
+        if (gi == -1) continue;
+        int det = -1;
+        double valid = kNo, max_ov = 0.0;
+        bool assigned_ign = false;
+        for (int j = 0; j < fr.nd; ++j) {
+            const int dj = fr.idt[j];
+            if (dj == -1 || asg[j * S] || fr.score[j] < thresh) continue;
+            const double ov = fr.ov[(long long)j * fr.ng + i];
+            if (ov > min_ov && (ov > max_ov || assigned_ign) && dj == 0) {
+                max_ov = ov; det = j; valid = 1; assigned_ign = false;
+            } else if (ov > min_ov && valid == kNo && dj == 1) {
+                det = j; valid = 1; assigned_ign = true;
+            }
+        }
+        if (valid == kNo && gi == 0) {
+            ++fn;
+        } else if (valid != kNo && (gi == 1 || fr.idt[det] == 1)) {
+            asg[det * S] = 1;
+        } else if (valid != kNo) {
+            ++tp;
+            if (fr.aos) vals[(long long)nv++ * S] = fr.aos[(long long)det * fr.ng + i];
+            asg[det * S] = 1;
+        }
+    }
+    for (int j = 0; j < fr.nd; ++j)
+        if (!(asg[j * S] || fr.idt[j] == -1 || fr.idt[j] == 1 || fr.score[j] < thresh)) ++fp;
+    int nstuff = 0;
+    if (metric == 0)
+        for (int i = 0; i < fr.ng; ++i) {
+            if (!fr.dc[i]) continue;
+            const double* q = fr.gt_bbox + 4 * i;       // a DontCare box
+            for (int j = 0; j < fr.nd; ++j) {
+                if (asg[j * S] || fr.idt[j] == -1 || fr.idt[j] == 1 || fr.score[j] < thresh) continue;
+                const double* b = fr.dt_bbox + 4 * j;    // image_box_overlap with criterion 0
+                const double iw = dsub(fmin(b[2], q[2]), fmax(b[0], q[0]));
+                if (iw <= 0) continue;
+                const double ih = dsub(fmin(b[3], q[3]), fmax(b[1], q[1]));
+                if (ih <= 0) continue;
+                if (ddiv(dmul(iw, ih), dmul(dsub(b[2], b[0]), dsub(b[3], b[1]))) > min_ov) {
+                    asg[j * S] = 1;
+                    ++nstuff;
+                }
+            }
+        }
+    fp -= nstuff;
+    double sim = 0.0;
+    if (fr.aos) sim = (tp > 0 || fp > 0) ? pairwise_sum(vals, fp > 0 ? fp : 0, (fp > 0 ? fp : 0) + nv) : -1.0;
+    *tp_out = tp; *fp_out = fp; *fn_out = fn; *sim_out = sim;
+}
+
+// Pass 2 (fused_compute_statistics): one CTA per (job, threshold), its threads over the frames.  The counts are summed
+// in any order; the similarity is summed in frame order, as the host accumulates pr[t, 3].
+__global__ void __launch_bounds__(kMatchThreads) eval_pr_kernel(SassdKittiEvalDesc e, long long njobs,
+                                                              char* __restrict__ asg_ws, double* __restrict__ vals_ws,
+                                                              const double* __restrict__ thresholds,
+                                                              const int32_t* __restrict__ n_thresh,
+                                                              double* __restrict__ pr) {
+    __shared__ double s_sim[kMatchThreads];
+    __shared__ unsigned long long s_cnt[3];
+    const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    char* asg = asg_ws + tid;
+    double* vals = vals_ws + tid;
+    for (long long w = blockIdx.x; w < njobs * kThresh; w += gridDim.x) {
+        const long long job = w / kThresh;
+        const int t = (int)(w % kThresh);
+        if (t >= n_thresh[job]) continue;                  // uniform over the CTA
+        const Job jb = decode_job(e, job);
+        const double min_ov = min_overlap_of(e, jb), thresh = thresholds[w];
+        const bool aos = jb.m == 0 && e.aos_table && e.compute_aos[jb.k];
+        if (threadIdx.x < 3) s_cnt[threadIdx.x] = 0;
+        long long tp = 0, fp = 0, fn = 0;
+        double sim_sum = 0.0;
+        for (int f0 = 0; f0 < e.nframes; f0 += blockDim.x) {
+            const int f = f0 + threadIdx.x;
+            double sim = -1.0;
+            if (f < e.nframes) {
+                int a, b, c;
+                frame_statistics(frame_of(e, jb, f), jb.m, min_ov, thresh, asg, vals, &a, &b, &c, &sim);
+                tp += a; fp += b; fn += c;
+            }
+            if (aos) {
+                s_sim[threadIdx.x] = sim;
+                __syncthreads();
+                if (threadIdx.x == 0) {
+                    const int nf = min((int)blockDim.x, e.nframes - f0);
+                    for (int i = 0; i < nf; ++i)
+                        if (s_sim[i] != -1.0) sim_sum = dadd(sim_sum, s_sim[i]);
+                }
+                __syncthreads();
+            }
+        }
+        __syncthreads();
+        atomicAdd(&s_cnt[0], (unsigned long long)tp);
+        atomicAdd(&s_cnt[1], (unsigned long long)fp);
+        atomicAdd(&s_cnt[2], (unsigned long long)fn);
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double* o = pr + 4 * w;
+            o[0] = (double)(long long)s_cnt[0];
+            o[1] = (double)(long long)s_cnt[1];
+            o[2] = (double)(long long)s_cnt[2];
+            o[3] = sim_sum;
+        }
+        __syncthreads();
+    }
+}
+
+}  // namespace
+
+extern "C" int sassd_kitti_eval_flags(int ngt, const int32_t* gt_name, const double* gt_occ, const double* gt_trunc,
+                                      const double* gt_bbox, int ndt, const int32_t* dt_name, const double* dt_bbox,
+                                      int nclass, const int32_t* classes, int ndiff, const double* limits,
+                                      int8_t* ign_gt, int8_t* ign_dt, int32_t* n_valid, sassd_stream_t stream) {
+    if (ngt < 0 || ndt < 0 || nclass < 1 || ndiff < 1 || !classes || !limits || !n_valid) return SASSD_ERR_ARG;
+    if (ngt > 0 && (!gt_name || !gt_occ || !gt_trunc || !gt_bbox || !ign_gt)) return SASSD_ERR_ARG;
+    if (ndt > 0 && (!dt_name || !dt_bbox || !ign_dt)) return SASSD_ERR_ARG;
+    const long long total = ((long long)ngt + ndt) * nclass * ndiff;
+    if (total == 0) return SASSD_OK;
+    eval_flags_kernel<<<sassd_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(
+        ngt, gt_name, gt_occ, gt_trunc, gt_bbox, ndt, dt_name, dt_bbox, nclass, classes, ndiff, limits, ign_gt, ign_dt,
+        n_valid);
+    return sassd_check_launch();
+}
+
+extern "C" int sassd_kitti_eval_overlaps(int nsets, int nframes, const int32_t* gt_off, const int32_t* dt_off,
+                                         const int64_t* ov_off, const double* gt_cam, const double* dt_cam,
+                                         const double* gt_bbox, const double* dt_bbox, const float* bev_iou,
+                                         const float* bev_inter, int max_pairs_per_frame, double* ov_bbox,
+                                         double* ov_bev, double* ov_3d, sassd_stream_t stream) {
+    if (nsets < 1 || nframes < 0 || max_pairs_per_frame < 0 || !gt_off || !dt_off || !ov_off) return SASSD_ERR_ARG;
+    if (nframes == 0 || max_pairs_per_frame == 0) return SASSD_OK;
+    if (!gt_cam || !dt_cam || !gt_bbox || !dt_bbox || !bev_iou || !bev_inter || !ov_bbox || !ov_bev || !ov_3d)
+        return SASSD_ERR_ARG;
+    const long long blocks = (long long)nsets * nframes;
+    dim3 grid((unsigned)sassd_div_up(max_pairs_per_frame, 128), (unsigned)(blocks < 32768 ? blocks : 32768));
+    eval_overlaps_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(nsets, nframes, gt_off, dt_off,
+                                                                 (const long long*)ov_off, gt_cam, dt_cam, gt_bbox,
+                                                                 dt_bbox, bev_iou, bev_inter, ov_bbox, ov_bev, ov_3d);
+    return sassd_check_launch();
+}
+
+extern "C" size_t sassd_kitti_eval_workspace_bytes(int max_nd, int max_ng) {
+    if (max_nd < 0 || max_ng < 0) return 0;
+    const size_t asg = ((size_t)kScratchThreads * (size_t)(max_nd > 0 ? max_nd : 1) + 255) / 256 * 256;
+    return asg + (size_t)kScratchThreads * (size_t)(max_ng > 0 ? max_ng : 1) * sizeof(double);
+}
+
+extern "C" int sassd_kitti_eval_match(const SassdKittiEvalDesc* e, double* scores, int32_t* n_scores,
+                                      double* thresholds, int32_t* n_thresh, double* pr, void* ws, size_t ws_bytes,
+                                      sassd_stream_t stream_) {
+    if (!e || e->nsets < 1 || e->nframes < 0 || e->nclass < 1 || e->ndiff < 1 || e->nover < 1 || e->max_nd < 0 ||
+        e->max_ng < 0)
+        return SASSD_ERR_ARG;
+    const long long njobs = (long long)e->nsets * e->nclass * e->ndiff * 3 * e->nover;
+    // one CTA per job sorts its scores; (job, threshold) items and job * frame items are counted in 64 bits
+    if (njobs > 0x7fffffffLL || njobs * kThresh > 0x7fffffffLL) return SASSD_ERR_ARG;
+    if (!e->gt_off || !e->dt_off || !e->ov_off || !e->gt_dc || !e->gt_bbox || !e->dt_bbox || !e->dt_score ||
+        !e->ov_bbox || !e->ov_bev || !e->ov_3d || !e->compute_aos || !e->min_overlaps || !e->ign_gt || !e->ign_dt ||
+        !e->n_valid || !e->score_off || !scores || !n_scores || !thresholds || !n_thresh || !pr || !ws)
+        return SASSD_ERR_ARG;
+    if (ws_bytes < sassd_kitti_eval_workspace_bytes(e->max_nd, e->max_ng)) return SASSD_ERR_WORKSPACE;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    char* asg = (char*)ws;
+    double* vals = (double*)(asg + ((size_t)kScratchThreads * (size_t)(e->max_nd > 0 ? e->max_nd : 1) + 255) / 256 * 256);
+    if (cudaMemsetAsync(n_scores, 0, sizeof(int32_t) * njobs, stream) != cudaSuccess ||
+        cudaMemsetAsync(n_thresh, 0, sizeof(int32_t) * njobs, stream) != cudaSuccess ||
+        cudaMemsetAsync(pr, 0, sizeof(double) * 4 * kThresh * njobs, stream) != cudaSuccess)
+        return SASSD_ERR_LAUNCH;
+    if (e->nframes == 0) return SASSD_OK;
+    eval_tp_scores_kernel<<<kMatchCtas, kMatchThreads, 0, stream>>>(*e, njobs, asg, scores, n_scores);
+    eval_thresholds_kernel<<<(unsigned)njobs, 1024, 0, stream>>>(*e, scores, n_scores, thresholds, n_thresh);
+    eval_pr_kernel<<<kMatchCtas, kMatchThreads, 0, stream>>>(*e, njobs, asg, vals, thresholds, n_thresh, pr);
+    return sassd_check_launch();
+}
+
+// Host function: the AOS term (1 + cos(gt alpha - dt alpha)) / 2 of every (detection, GT) pair, laid out like the
+// overlap matrices, with the libm cos the host matcher (sassd_kitti_match) uses.
+extern "C" int sassd_kitti_aos_table(int nsets, int nframes, const int32_t* gt_off, const int32_t* dt_off,
+                                     const int64_t* ov_off, const double* gt_alpha, const double* dt_alpha, double* out) {
+    if (nsets < 1 || nframes < 0 || !gt_off || !dt_off || !ov_off || !out) return SASSD_ERR_ARG;
+    for (int b = 0; b < nsets * nframes; ++b) {
+        const int f = b % nframes, g0 = gt_off[f], ng = gt_off[f + 1] - g0, d0 = dt_off[b], nd = dt_off[b + 1] - d0;
+        double* o = out + ov_off[b];
+        for (int j = 0; j < nd; ++j)
+            for (int i = 0; i < ng; ++i) o[(size_t)j * ng + i] = (1.0 + std::cos(gt_alpha[g0 + i] - dt_alpha[d0 + j])) / 2.0;
+    }
+    return SASSD_OK;
+}

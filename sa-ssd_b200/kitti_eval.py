@@ -4,12 +4,18 @@ Mirrors the reference's evaluator so that `tools/test.py`-style code can swap th
 
 * `get_official_eval_result(gt_annos, dt_annos, current_classes, difficultys)` -> the same printed table
   (mmdet/core/evaluation/kitti_eval.py:791-851); `official_eval` additionally returns the AP arrays;
+* `get_coco_eval_result(gt_annos, dt_annos, current_classes)` -> the COCO-style table, AP averaged over ten IoU
+  thresholds per class (kitti_eval.py:853-930); `coco_eval` additionally returns the AP arrays;
 * `rotate_iou_gpu_eval(boxes, query_boxes, criterion)` <- mmdet/core/post_processing/rotate_nms_gpu.py:592-627.
 
-What runs where: the rotated-box overlaps of every frame are ONE launch of `sassd_rotate_overlap_eval` (the
-reference launches a numba.cuda kernel per 1/50th of the dataset); the 2-D box and height overlaps are vectorised
-float64 numpy; the greedy matching + per-threshold statistics (numba-jitted CPU loops in the reference) are the
-host C++ function `sassd_kitti_match`.  Annotations are dicts of numpy arrays as produced by
+What runs where: with no ``overlap_fn`` (the product path) everything after flattening the annotations runs on the
+device (csrc/kitti_match.cu, `_eval_device`): the ignore flags, the rotated overlaps (`sassd_rotate_overlap_eval`,
+one launch per criterion for every (set, frame)), the 2-D and 3-D overlaps, both matching passes, the 41 score
+thresholds and the per-threshold sums over frames, for every detection set, class, difficulty, metric and
+min-overlap row at once; only the precision / recall ratios, their envelope and the AP sums run in numpy on the
+downloaded sums.  With an injected ``overlap_fn`` the host path runs: vectorised float64 numpy overlaps, per-frame
+`clean_gt` / `clean_dt` and the host C++ matcher `sassd_kitti_match` (numba-jitted CPU loops in the reference).
+Both paths give the same arrays bit for bit.  Annotations are dicts of numpy arrays as produced by
 `results.kitti_bbox2results` / the reference's `get_label_annos` (camera-frame boxes, dimensions l, h, w).
 """
 import ctypes
@@ -26,6 +32,10 @@ MIN_HEIGHT, MAX_OCCLUSION, MAX_TRUNCATION = (40, 25, 25), (0, 1, 2), (0.15, 0.3,
 OVERLAP_0_7 = np.array([[0.7, 0.5, 0.5, 0.7, 0.5, 0.7, 0.7, 0.7]] * 3)
 OVERLAP_0_5 = np.array([[0.7, 0.5, 0.5, 0.7, 0.5, 0.5, 0.5, 0.5], [0.5, 0.25, 0.25, 0.5, 0.25, 0.5, 0.5, 0.5],
                         [0.5, 0.25, 0.25, 0.5, 0.25, 0.5, 0.5, 0.5]])
+# class -> (start, stop, num) of the COCO-style overlaps, the same for the three metrics (kitti_eval.py:869-879)
+COCO_RANGE = {0: (0.5, 0.95, 10), 1: (0.25, 0.7, 10), 2: (0.25, 0.7, 10), 3: (0.5, 0.95, 10), 4: (0.25, 0.7, 10),
+              5: (0.5, 0.95, 10), 6: (0.5, 0.95, 10), 7: (0.5, 0.95, 10)}
+TABLES = (11, 40, "coco")       # official AP at 11 / 40 recall positions, COCO-style AP
 
 
 def _p(a):
@@ -293,6 +303,126 @@ def eval_class_many(gt_annos, dt_sets, current_classes, difficultys, metric, min
     return out
 
 
+# ------------------------------------------------------------------ device path
+_NAME_IDS = {n: i for i, n in enumerate(dict.fromkeys(CLASS_NAMES))}     # one id per distinct lower-cased class name
+_IGNORED_NAME = {"car": "van", "pedestrian": "person_sitting"}           # counted as ignored, not missed (clean_data)
+
+
+def _flat_names(annos):
+    """(name ids, DontCare flags) of every row of ``annos``, frames concatenated; names are mapped once per distinct
+    name."""
+    names = [np.asarray(a["name"], dtype=str).reshape(-1) for a in annos]
+    names = np.concatenate(names) if names else np.zeros((0,), str)
+    if not len(names):
+        return np.zeros((0,), np.int32), np.zeros((0,), np.int32)
+    uniq, inv = np.unique(names, return_inverse=True)
+    ids = np.array([_NAME_IDS.get(str(u).lower(), -1) for u in uniq], np.int32)
+    return ids[inv.reshape(-1)], (uniq == "DontCare").astype(np.int32)[inv.reshape(-1)]
+
+
+def _flat(annos, key, width):
+    return _cat([np.asarray(a[key], np.float64).reshape(-1, width) for a in annos], (0, width), np.float64)
+
+
+def _flat_cam(annos):
+    return np.concatenate([_flat(annos, "location", 3), _flat(annos, "dimensions", 3), _flat(annos, "rotation_y", 1)], 1)
+
+
+def _eval_device(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flags):
+    """eval_class_many's precision / recall / orientation arrays for the three metrics, [metric][set] ->
+    dict of [class, difficulty, min_overlap, 41], with the flags, overlaps, matching, thresholds and per-threshold sums
+    on the device (csrc/kitti_match.cu); bit for bit what the host path computes."""
+    import torch
+    from . import ops
+    ops.require_cuda()
+    dev = torch.device("cuda", torch.cuda.current_device())
+    K, F, C, Dn, M = len(dt_sets), len(gt_annos), len(classes), len(difficultys), min_overlaps.shape[0]
+    assert all(len(d) == F for d in dt_sets)
+    dt_all = [d for dts in dt_sets for d in dts]
+    ng = np.array([len(g["name"]) for g in gt_annos], np.int64)
+    nd = np.array([len(d["name"]) for d in dt_all], np.int64)
+    npairs = nd * np.tile(ng, K)
+    gt_off, dt_off, ov_off = _offsets(ng), _offsets(nd), _offsets(npairs, np.int64)
+    total = int(ov_off[-1])
+    gt_name, gt_dc = _flat_names(gt_annos)
+    dt_name, _ = _flat_names(dt_all)
+    gt_bbox, dt_bbox = _flat(gt_annos, "bbox", 4), _flat(dt_all, "bbox", 4)
+    gt_cam, dt_cam = _flat_cam(gt_annos), _flat_cam(dt_all)
+    truncs = [np.asarray(g["truncated"]).reshape(-1) for g in gt_annos]
+    trunc = np.concatenate(truncs) if truncs else np.zeros((0,))
+    # numpy compares a float32 column with the Python-float limit in float32: round the limit into the column's dtype
+    tdt = trunc.dtype if trunc.dtype.kind == "f" else np.float64
+    limits = np.array([[MAX_OCCLUSION[d], float(tdt.type(MAX_TRUNCATION[d])), MIN_HEIGHT[d]] for d in difficultys],
+                      np.float64)
+    cls_ids = np.array([[_NAME_IDS[CLASS_NAMES[c].lower()], _NAME_IDS.get(_IGNORED_NAME.get(CLASS_NAMES[c].lower()), -1)]
+                        for c in classes], np.int32)
+
+    def up(a):
+        return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+
+    t = dict(gt_off=up(gt_off), dt_off=up(dt_off), ov_off=up(ov_off), gt_dc=up(gt_dc), gt_bbox=up(gt_bbox),
+             dt_bbox=up(dt_bbox), dt_score=up(_flat(dt_all, "score", 1).reshape(-1)), gt_cam=up(gt_cam),
+             dt_cam=up(dt_cam), min_overlaps=up(np.asarray(min_overlaps, np.float64)),
+             compute_aos=up(np.asarray(aos_flags, np.int32)))
+    ign_gt, ign_dt, n_valid = ops.kitti_eval_flags(
+        up(gt_name), up(_flat(gt_annos, "occluded", 1).reshape(-1)), up(trunc.astype(np.float64)), t["gt_bbox"],
+        up(dt_name), t["dt_bbox"], up(cls_ids), up(limits))
+    # the rotated overlaps of every (set, frame) block: BEV IoU and the intersection area the 3-D overlap builds on
+    bev = [0, 2, 3, 5, 6]
+    dt_bev, gt_bev = up(dt_cam[:, bev].astype(np.float32)), up(np.tile(gt_cam[:, bev].astype(np.float32), (K, 1)))
+    q_off = up(_offsets(np.tile(ng, K)))
+    rot = []
+    for criterion in (-1, 2):
+        out = torch.zeros((max(total, 1),), dtype=torch.float32, device=dev)
+        if total:
+            ops._call("sassd_rotate_overlap_eval", None, ops._ptr(dt_bev), ops._ptr(t["dt_off"]), ops._ptr(gt_bev),
+                      ops._ptr(q_off), ops._ptr(t["ov_off"]), K * F, criterion, int(npairs.max()), ops._ptr(out),
+                      ops._stream())
+        rot.append(out)
+    ov = ops.kitti_eval_overlaps(K, F, t["gt_off"], t["dt_off"], t["ov_off"], t["gt_cam"], t["dt_cam"], t["gt_bbox"],
+                                 t["dt_bbox"], rot[0], rot[1], total, int(npairs.max()) if len(npairs) else 0)
+    aos_table = None
+    if any(aos_flags) and total:
+        table = np.zeros((total,), np.float64)
+        gt_alpha, dt_alpha = _flat(gt_annos, "alpha", 1).reshape(-1), _flat(dt_all, "alpha", 1).reshape(-1)
+        _lib.check(_lib.load().sassd_kitti_aos_table(K, F, _p(gt_off), _p(dt_off), _p(ov_off), _p(gt_alpha),
+                                                     _p(dt_alpha), _p(table)), "sassd_kitti_aos_table")
+        aos_table = up(table)
+    # each job's score region: the next power of two of its (class, difficulty)'s valid GT count
+    nv = n_valid.cpu().numpy().astype(np.int64)
+    region = np.broadcast_to((1 << np.ceil(np.log2(np.maximum(nv, 1))).astype(np.int64))[None, :, :, None, None],
+                             (K, C, Dn, 3, M)).reshape(-1)
+    score_off = up(_offsets(region, np.int64))
+    desc = _lib.KittiEvalDesc(nsets=K, nframes=F, nclass=C, ndiff=Dn, nover=M, max_nd=int(nd.max()) if len(nd) else 0,
+                              max_ng=int(ng.max()) if len(ng) else 0)
+    keep = dict(t, ign_gt=ign_gt, ign_dt=ign_dt, n_valid=n_valid, score_off=score_off, ov_bbox=ov[0], ov_bev=ov[1],
+                ov_3d=ov[2], aos_table=aos_table)
+    for name, _ in desc._fields_[7:]:
+        setattr(desc, name, keep[name].data_ptr() if keep[name] is not None else None)
+    _, n_thresh, pr = ops.kitti_eval_match(desc, len(region), int(region.sum()))
+    n_thresh = n_thresh.cpu().numpy().reshape(K, C, Dn, 3, M)
+    pr = pr.cpu().numpy().reshape(K, C, Dn, 3, M, 41, 4)
+    # precision, recall and AOS of the sampled thresholds and their monotone envelope, as eval_class_many computes them
+    past = np.arange(41) >= n_thresh[..., None]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        recall = pr[..., 0] / (pr[..., 0] + pr[..., 2])
+        precision = pr[..., 0] / (pr[..., 0] + pr[..., 1])
+        aos = pr[..., 3] / (pr[..., 0] + pr[..., 1])
+    out = []
+    for m in range(3):
+        per_set = []
+        for k in range(K):
+            res = {}
+            for key, a in (("recall", recall), ("precision", precision), ("orientation", aos)):
+                v = np.where(past[k, :, :, m], 0.0, a[k, :, :, m])
+                if key == "orientation" and not (m == 0 and aos_flags[k]):
+                    v = np.zeros_like(v)
+                res[key] = np.ascontiguousarray(np.maximum.accumulate(v[..., ::-1], axis=-1)[..., ::-1])
+            per_set.append(res)
+        out.append(per_set)
+    return out
+
+
 def get_mAP(prec):
     """11-point interpolated AP over the 41 samples (get_mAP_v2, kitti_eval.py:683-688)."""
     return sum(prec[..., i] for i in range(0, prec.shape[-1], 4)) / 11 * 100
@@ -316,40 +446,109 @@ def official_eval(gt_annos, dt_annos, current_classes, difficultys=(0, 1, 2), ov
 def official_eval_many(gt_annos, dt_sets, classes, recall_positions=(11, 40), overlap_fn=None, difficultys=(0, 1, 2)):
     """official_eval of K detection sets (each a list of per-frame annotation dicts, e.g. one per checkpoint) against
     the same GT, at each of ``recall_positions`` (11 and / or 40).  Returns one dict per set, {recall positions:
-    official_eval's (text, ap)}.  The rotated overlaps of every (set, frame) pair are one kernel launch for BEV and one
-    for 3D (the 2D box overlaps are vectorised numpy on the host), the GT side of clean_data runs and is flattened once
-    per class and difficulty for all metrics and sets, and R11 and R40 come from one matching pass."""
+    official_eval's (text, ap)}.  One evaluation (eval_many) serves every set and both recall positions."""
     positions = tuple(recall_positions)
     if not positions or any(r not in (11, 40) for r in positions):
         raise ValueError("recall_positions must be 11 or 40, not %r" % (recall_positions,))
-    current_classes = classes if isinstance(classes, (list, tuple)) else [classes]
+    return eval_many(gt_annos, dt_sets, classes, positions, overlap_fn, difficultys)
+
+
+def coco_min_overlaps(classes):
+    """[10, metric, class]: the host's np.linspace(start, stop, 10) of each class's COCO range, for all three metrics
+    (do_coco_style_eval, kitti_eval.py:713-717, with the integer ``num`` NumPy requires)."""
+    out = np.zeros((10, 3, len(classes)))
+    for j, c in enumerate(classes):
+        start, stop, num = COCO_RANGE[c]
+        out[:, :, j] = np.linspace(start, stop, int(num))[:, None]
+    return out
+
+
+def _class_ids(classes):
+    current = classes if isinstance(classes, (list, tuple)) else [classes]
     name_to_class = {v: k for k, v in CLASS_TO_NAME.items()}
-    classes = [name_to_class[c] if isinstance(c, str) else c for c in current_classes]
-    min_overlaps = np.stack([OVERLAP_0_7, OVERLAP_0_5], axis=0)[:, :, classes]
-    aos_flags = []
-    for dt_annos in dt_sets:
-        compute_aos = False
-        for anno in dt_annos:                      # :818-823
-            if anno['alpha'].shape[0] != 0:
-                compute_aos = bool(anno['alpha'][0] != -10)
-                break
-        aos_flags.append(compute_aos)
+    return [name_to_class[c] if isinstance(c, str) else c for c in current]
+
+
+def _aos_flag(dt_annos):
+    """compute_aos as the reference decides it (kitti_eval.py:818-823): from the first frame with detections."""
+    for anno in dt_annos:
+        if anno['alpha'].shape[0] != 0:
+            return bool(anno['alpha'][0] != -10)
+    return False
+
+
+def eval_many(gt_annos, dt_sets, classes, tables=(11,), overlap_fn=None, difficultys=(0, 1, 2)):
+    """Every table of ``tables`` (11 and 40: the official tables at 11 / 40 recall positions; "coco": the COCO-style
+    table) for each of the K detection sets of ``dt_sets`` against the same GT.  Returns one dict per set, {table:
+    (text, ap)}.  The official and COCO overlap rows form one list of min overlaps, so the overlaps, the GT side and
+    the matching run once for all of them; R11 and R40 read the same precision samples."""
+    tables = tuple(tables)
+    if not tables or any(t not in TABLES for t in tables):
+        raise ValueError("tables must be among %r, not %r" % (TABLES, tables))
+    classes = _class_ids(classes)
+    official = any(t in (11, 40) for t in tables)
+    rows = ([np.stack([OVERLAP_0_7, OVERLAP_0_5], axis=0)[:, :, classes]] if official else [])
+    if "coco" in tables:
+        rows.append(coco_min_overlaps(classes))
+    min_overlaps = np.concatenate(rows, 0)
+    n_off = 2 if official else 0
+    aos_flags = [_aos_flag(d) for d in dt_sets]
     diffs = list(difficultys)
-    gt_sides = {(c, d): _GtSide(gt_annos, c, d) for c in classes for d in diffs}
-    prec = [eval_class_many(gt_annos, dt_sets, classes, diffs, metric, min_overlaps,
-                            aos_flags if metric == 0 else [False] * len(dt_sets), overlap_fn, gt_sides)
-            for metric in (0, 1, 2)]
+    if overlap_fn is None:
+        prec = _eval_device(gt_annos, dt_sets, classes, diffs, min_overlaps, aos_flags)
+    else:
+        gt_sides = {(c, d): _GtSide(gt_annos, c, d) for c in classes for d in diffs}
+        prec = [eval_class_many(gt_annos, dt_sets, classes, diffs, metric, min_overlaps,
+                                aos_flags if metric == 0 else [False] * len(dt_sets), overlap_fn, gt_sides)
+                for metric in (0, 1, 2)]
     out = []
     for s, compute_aos in enumerate(aos_flags):
         r0, r1, r2 = (p[s] for p in prec)
         res = {}
-        for rp in positions:
+        for rp in (t for t in tables if t in (11, 40)):
             get_mAP_n = get_mAP if rp == 11 else get_mAP_R40
-            ap = dict(bbox=get_mAP_n(r0["precision"]), aos=get_mAP_n(r0["orientation"]) if compute_aos else None,
-                      bev=get_mAP_n(r1["precision"]), d3=get_mAP_n(r2["precision"]))
-            res[rp] = (_ap_text(ap, classes, min_overlaps, compute_aos, "AP" if rp == 11 else "AP_R40"), ap)
+            ap = dict(bbox=get_mAP_n(r0["precision"][:, :, :n_off]),
+                      aos=get_mAP_n(r0["orientation"][:, :, :n_off]) if compute_aos else None,
+                      bev=get_mAP_n(r1["precision"][:, :, :n_off]), d3=get_mAP_n(r2["precision"][:, :, :n_off]))
+            res[rp] = (_ap_text(ap, classes, min_overlaps[:n_off], compute_aos, "AP" if rp == 11 else "AP_R40"), ap)
+        if "coco" in tables:
+            # do_coco_style_eval (kitti_eval.py:711-729): the mean over the ten overlaps of get_mAP_v2
+            ap = dict(bbox=get_mAP(r0["precision"][:, :, n_off:]).mean(-1),
+                      aos=get_mAP(r0["orientation"][:, :, n_off:]).mean(-1) if compute_aos else None,
+                      bev=get_mAP(r1["precision"][:, :, n_off:]).mean(-1),
+                      d3=get_mAP(r2["precision"][:, :, n_off:]).mean(-1))
+            res["coco"] = (_coco_text(ap, classes, compute_aos), ap)
         out.append(res)
     return out
+
+
+def coco_eval_many(gt_annos, dt_sets, classes, overlap_fn=None):
+    """coco_eval of K detection sets against the same GT in one evaluation: one (text, ap) per set."""
+    return [r["coco"] for r in eval_many(gt_annos, dt_sets, classes, ("coco",), overlap_fn)]
+
+
+def coco_eval(gt_annos, dt_annos, classes, overlap_fn=None):
+    """-> (text, dict(bbox, bev, d3, aos) of AP arrays [class, difficulty]): the reference's COCO-style KITTI AP, each
+    value the mean over the class's ten IoU thresholds of the 11-point AP (``aos`` is None when the detections carry
+    no alpha)."""
+    return coco_eval_many(gt_annos, [dt_annos], classes, overlap_fn)[0]
+
+
+def get_coco_eval_result(gt_annos, dt_annos, current_classes, overlap_fn=None):
+    """Reference signature (kitti_eval.py:853): the printed COCO-style table."""
+    return coco_eval(gt_annos, dt_annos, current_classes, overlap_fn)[0]
+
+
+def _coco_text(ap, classes, compute_aos):
+    """get_coco_eval_result's table (kitti_eval.py:904-930)."""
+    lines = []
+    for j, cls in enumerate(classes):
+        start, stop, num = COCO_RANGE[cls]
+        lines.append("%s coco AP@%.2f:%.2f:%.2f:" % (CLASS_TO_NAME[cls], start, (stop - start) / (num - 1), stop))
+        for key, label in (("bbox", "bbox AP"), ("bev", "bev  AP"), ("d3", "3d   AP")) + ((("aos", "aos  AP"),)
+                                                                                           if compute_aos else ()):
+            lines.append("%s:%.2f, %.2f, %.2f" % (label, ap[key][j, 0], ap[key][j, 1], ap[key][j, 2]))
+    return "".join(l + "\n" for l in lines)
 
 
 def _ap_text(ap, classes, min_overlaps, compute_aos, tag):

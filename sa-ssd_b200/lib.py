@@ -31,6 +31,13 @@ class GConvDesc(ctypes.Structure):
                                               "rows_cap", "batch", "H", "W", "relu")]
 
 
+class KittiEvalDesc(ctypes.Structure):
+    _fields_ = ([(n, ctypes.c_int32) for n in ("nsets", "nframes", "nclass", "ndiff", "nover", "max_nd", "max_ng")]
+                + [(n, c_void_p) for n in ("gt_off", "dt_off", "ov_off", "gt_dc", "gt_bbox", "dt_bbox", "dt_score",
+                                           "ov_bbox", "ov_bev", "ov_3d", "aos_table", "compute_aos", "min_overlaps",
+                                           "ign_gt", "ign_dt", "n_valid", "score_off")])
+
+
 class PointLevels(ctypes.Structure):
     _fields_ = [("rows", c_void_p), ("plane_stride", ctypes.c_int64), ("row_stride", ctypes.c_int32),
                 ("channels", ctypes.c_int32), ("split", ctypes.c_int32), ("pad", ctypes.c_int32)]
@@ -91,6 +98,11 @@ _SIGNATURES = {
     "sassd_rotate_overlap_eval": (c_int, [P, P, P, P, P, c_int, c_int, c_int, P, P]),
     "sassd_kitti_match": (c_int, [c_int, P, P, P, P, P, P, P, P, P, P, P, P, c_int, ctypes.c_double, c_int, c_int, P, P,
                                   P, P]),
+    "sassd_kitti_eval_flags": (c_int, [c_int, P, P, P, P, c_int, P, P, c_int, P, c_int, P, P, P, P, P]),
+    "sassd_kitti_eval_overlaps": (c_int, [c_int, c_int, P, P, P, P, P, P, P, P, P, c_int, P, P, P, P]),
+    "sassd_kitti_aos_table": (c_int, [c_int, c_int, P, P, P, P, P, P]),
+    "sassd_kitti_eval_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "sassd_kitti_eval_match": (c_int, [ctypes.POINTER(KittiEvalDesc), P, P, P, P, P, P, c_size_t, P]),
     "sassd_spconv_pack_bytes": (c_size_t, [c_int, c_int, c_int]),
     "sassd_spconv_pack": (c_int, [P, c_int, c_int, c_int, c_int, P, P]),
     "sassd_spconv_workspace_bytes": (c_size_t, []),

@@ -53,7 +53,7 @@ def next_pow2(n):
 # kernels launched by each C-ABI entry point (memsets not counted)
 _KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_points_in_rbboxes": 1, "sassd_augment_drop_points": 1, "sassd_augment_noise_search": 1, "sassd_augment_assemble": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
-            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
+            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_kitti_eval_flags": 1, "sassd_kitti_eval_overlaps": 1, "sassd_kitti_eval_match": 3, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_merge_detections": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
             "sassd_boxes_iou_bev": 1, "sassd_points_in_boxes": 2, "sassd_assign_rpn": 3, "sassd_assign_pswarp": 3,
             "sassd_rpn_loss": 2, "sassd_pswarp_loss": 2, "sassd_aux_loss": 2}
@@ -488,6 +488,50 @@ def kitti_format(det, d_ndet, meta):
     _call("sassd_kitti_format", None, _ptr(det), _ptr(d_ndet), B, det_cap, _ptr(meta), _ptr(rows), _ptr(n_out),
           _stream())
     return rows, n_out
+
+
+def kitti_eval_flags(gt_name, gt_occ, gt_trunc, gt_bbox, dt_name, dt_bbox, classes, limits):
+    """clean_data's ignore flags on the device (csrc/kitti_match.cu).  gt_name / dt_name [rows] i32 name ids, gt_occ /
+    gt_trunc [G] f64, gt_bbox / dt_bbox [rows,4] f64, classes [C,2] i32 (name id, ignored name id or -1), limits
+    [Dn,3] f64 (max occlusion, max truncation, min height).  Returns (ign_gt [C,Dn,G] i8, ign_dt [C,Dn,D] i8,
+    n_valid [C,Dn] i32)."""
+    dev = gt_bbox.device
+    G, D, C, Dn = gt_name.shape[0], dt_name.shape[0], classes.shape[0], limits.shape[0]
+    ign_gt = torch.empty((C, Dn, G), dtype=torch.int8, device=dev)
+    ign_dt = torch.empty((C, Dn, D), dtype=torch.int8, device=dev)
+    n_valid = torch.zeros((C, Dn), dtype=torch.int32, device=dev)
+    _call("sassd_kitti_eval_flags", None, G, _ptr(gt_name), _ptr(gt_occ), _ptr(gt_trunc), _ptr(gt_bbox), D,
+          _ptr(dt_name), _ptr(dt_bbox), C, _ptr(classes), Dn, _ptr(limits), _ptr(ign_gt), _ptr(ign_dt), _ptr(n_valid),
+          _stream())
+    return ign_gt, ign_dt, n_valid
+
+
+def kitti_eval_overlaps(nsets, nframes, gt_off, dt_off, ov_off, gt_cam, dt_cam, gt_bbox, dt_bbox, bev_iou, bev_inter,
+                        total_pairs, max_pairs):
+    """The bbox, BEV and 3-D overlap matrices (f64 [total_pairs], blocks at ov_off) of every (set, frame) block: gt_cam /
+    dt_cam [rows,7] f64 camera boxes, bev_iou / bev_inter the rotated overlaps at criterion -1 / 2 (f32, same blocks)."""
+    out = [torch.empty((max(int(total_pairs), 1),), dtype=torch.float64, device=gt_cam.device) for _ in range(3)]
+    _call("sassd_kitti_eval_overlaps", None, nsets, nframes, _ptr(gt_off), _ptr(dt_off), _ptr(ov_off), _ptr(gt_cam),
+          _ptr(dt_cam), _ptr(gt_bbox), _ptr(dt_bbox), _ptr(bev_iou), _ptr(bev_inter), int(max_pairs), _ptr(out[0]),
+          _ptr(out[1]), _ptr(out[2]), _stream())
+    return out
+
+
+def kitti_eval_match(desc, njobs, score_total, ws=None):
+    """Pass 1, thresholds and pass 2 of the KITTI matching for every job of ``desc`` (lib.KittiEvalDesc whose pointers
+    are device tensors the caller keeps alive).  Returns (thresholds [njobs,41] f64, n_thresh [njobs] i32,
+    pr [njobs,41,4] f64)."""
+    dev = torch.device("cuda", torch.cuda.current_device())
+    scores = torch.empty((max(int(score_total), 1),), dtype=torch.float64, device=dev)
+    n_scores = torch.empty((njobs,), dtype=torch.int32, device=dev)
+    thresholds = torch.zeros((njobs, 41), dtype=torch.float64, device=dev)
+    n_thresh = torch.empty((njobs,), dtype=torch.int32, device=dev)
+    pr = torch.empty((njobs, 41, 4), dtype=torch.float64, device=dev)
+    nbytes = _L().sassd_kitti_eval_workspace_bytes(desc.max_nd, desc.max_ng)
+    w = (ws or _WS).get("kitti_eval", nbytes, dev)
+    _call("sassd_kitti_eval_match", None, ctypes.byref(desc), _ptr(scores), _ptr(n_scores), _ptr(thresholds),
+          _ptr(n_thresh), _ptr(pr), _ptr(w), w.numel(), _stream())
+    return thresholds, n_thresh, pr
 
 
 def merge_detections(dets, label_offsets):

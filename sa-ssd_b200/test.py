@@ -2,18 +2,20 @@
 
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR [--split val] [--batch 16]
                               [--lidar velodyne|velodyne_reduced] [--out DIR] [--workers N] [--json FILE]
-                              [--losses] [--r40]
+                              [--losses] [--r40] [--coco]
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR --split test --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --drive DRIVE_DIR [--calib-dir DIR] --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --model CONFIG2 CHECKPOINT2 [--model ...] --data-root DIR [...]
-    python -m sassd_b200.test CONFIG CHECKPOINT --checkpoints CHECKPOINT2 [...] --data-root DIR [--losses] [--r40] [...]
+    python -m sassd_b200.test CONFIG CHECKPOINT --checkpoints CHECKPOINT2 [...] --data-root DIR [--losses] [--r40] [--coco] [...]
 
 Frames are read from disk a few batches ahead (kitti_data.Prefetcher) and streamed through the captured step
 (SingleStageDetector.detect_stream): full sweeps (``--lidar velodyne``) are cropped to the camera frustum on the
 device, and every step ends with the KITTI result formatter on the device (ops.kitti_format).  The last batch is
 padded with empty frames whose results are dropped.  Prints the official AP table (kitti_eval), the frame rate (wall
 clock of the streamed detection, the evaluation excluded) and the time spent waiting on reads.  ``--r40`` also prints
-the table at 40 recall positions (kitti_eval.official_eval(recall_positions=40)).
+the table at 40 recall positions (kitti_eval.official_eval(recall_positions=40)), and ``--coco`` the reference's
+COCO-style table, AP averaged over ten IoU thresholds per class (kitti_eval.coco_eval), after the official one(s).
+All tables come from one evaluation (kitti_eval.eval_many), which runs on the device.
 
 ``--losses`` (labelled splits): every frame also carries its ground truth (kitti_data.gt_from_anno) and the captured
 step computes SA-SSD's six losses beside the detections (detect_stream(losses=True)); the result files and AP tables
@@ -36,7 +38,8 @@ share a class; ``--losses`` takes one model.
 one pass over a labelled split: the models run as one detectors.CheckpointSweep, so every frame is read, cropped and
 voxelized once, the rulebooks and anchor mask are built once and, with ``--losses``, the targets are assigned once, while
 each checkpoint runs its own network.  The driver prints each checkpoint's AP table(s) and loss means under its file
-name, then one summary line per checkpoint (moderate 3D AP per class, rpn_cls_loss and loss_cls means).  ``--out DIR``
+name, then one summary line per checkpoint (moderate 3D AP per class, with ``--coco`` also its COCO-style AP,
+rpn_cls_loss and loss_cls means); every checkpoint's tables come from one evaluation.  ``--out DIR``
 writes each checkpoint's result files to DIR/<checkpoint stem>/.  Each checkpoint's output equals that of a run of its
 own.
 
@@ -82,6 +85,8 @@ def parse_args(argv=None):
                    help="also compute SA-SSD's losses against the split's labels in the detection step and print "
                         "their means over the batches")
     p.add_argument("--r40", action="store_true", help="also print the AP table at 40 recall positions")
+    p.add_argument("--coco", action="store_true",
+                   help="also print the COCO-style AP table (AP averaged over ten IoU thresholds per class)")
     p.add_argument("--model", nargs=2, action="append", default=[], metavar=("CONFIG", "CHECKPOINT"),
                    help="one more single-class model, run with the first as one set (repeatable)")
     p.add_argument("--checkpoints", nargs="+", default=[], metavar="CHECKPOINT",
@@ -108,6 +113,8 @@ def parse_args(argv=None):
         p.error("--losses needs a labelled split: %s has no labels" % ("--drive" if args.drive else "--split test"))
     if args.r40 and (args.drive or args.split == "test"):
         p.error("--r40 needs a labelled split: %s has no labels" % ("--drive" if args.drive else "--split test"))
+    if args.coco and (args.drive or args.split == "test"):
+        p.error("--coco needs a labelled split: %s has no labels" % ("--drive" if args.drive else "--split test"))
     if args.drive:
         if args.lidar == "velodyne_reduced":
             p.error("--drive reads full sweeps: --lidar velodyne_reduced does not apply")
@@ -297,21 +304,28 @@ def run(args, log=print):
         _write_json(args.json, result)
         D.barrier()
         return result
-    from .kitti_eval import official_eval
-    gt_annos = split.gt_annos()
-    text, ap = official_eval(gt_annos, dt_annos, class_names)
+    from .kitti_eval import eval_many
+    ev = eval_many(split.gt_annos(), [dt_annos], class_names, _tables(args))[0]
+    text, ap = ev[11]
     log(text, end="")
     result.update(text=text, ap=_ap_lists(ap))
     if args.r40:
-        text40, ap40 = official_eval(gt_annos, dt_annos, class_names, recall_positions=40)
-        log(text40, end="")
-        result.update(text_r40=text40, ap_r40=_ap_lists(ap40))
+        log(ev[40][0], end="")
+        result.update(text_r40=ev[40][0], ap_r40=_ap_lists(ev[40][1]))
+    if args.coco:
+        log(ev["coco"][0], end="")
+        result.update(text_coco=ev["coco"][0], ap_coco=_ap_lists(ev["coco"][1]))
     if args.losses:
         result.update(_loss_means(per_batch, args.batch, log))
     log(rate)
     _write_json(args.json, result)
     D.barrier()
     return result
+
+
+def _tables(args):
+    """The kitti_eval.eval_many tables the arguments ask for."""
+    return (11,) + ((40,) if args.r40 else ()) + (("coco",) if args.coco else ())
 
 
 def _ap_lists(ap):
@@ -329,16 +343,16 @@ def _loss_means(per_batch, batch, log):
 
 
 def _report_sweep(args, gt_annos, dt_sets, class_names, per_batch, log):
-    """Evaluate and print each checkpoint of a sweep (official_eval_many), then one summary line per checkpoint:
-    moderate 3D AP per class at the class's strict overlap (R11, and R40 with --r40) and the rpn_cls_loss / loss_cls
-    means.  Returns the result dict's ``checkpoints`` list."""
+    """Evaluate and print each checkpoint of a sweep (one kitti_eval.eval_many for all of them), then one summary line
+    per checkpoint: moderate 3D AP per class at the class's strict overlap (R11, and R40 with --r40), the moderate 3D
+    COCO-style AP with --coco, and the rpn_cls_loss / loss_cls means.  Returns the result dict's ``checkpoints``
+    list."""
     from . import ops
-    from .kitti_eval import official_eval_many
+    from .kitti_eval import eval_many
     paths = [args.checkpoint] + args.checkpoints
-    positions = (11, 40) if args.r40 else (11,)
     n = len(ops.LOSS_KEYS)
     entries, summary = [], []
-    for k, (path, ev) in enumerate(zip(paths, official_eval_many(gt_annos, dt_sets, class_names, positions))):
+    for k, (path, ev) in enumerate(zip(paths, eval_many(gt_annos, dt_sets, class_names, _tables(args)))):
         log("== %s ==" % os.path.basename(path))
         text, ap = ev[11]
         log(text, end="")
@@ -346,10 +360,14 @@ def _report_sweep(args, gt_annos, dt_sets, class_names, per_batch, log):
         line = ["%-24s" % os.path.basename(path)]
         for j, c in enumerate(class_names):
             line.append("%s 3d mod R11 %6.2f" % (c, ap["d3"][j, 1, 0]) +
-                        (" R40 %6.2f" % ev[40][1]["d3"][j, 1, 0] if args.r40 else ""))
+                        (" R40 %6.2f" % ev[40][1]["d3"][j, 1, 0] if args.r40 else "") +
+                        (" COCO %6.2f" % ev["coco"][1]["d3"][j, 1] if args.coco else ""))
         if args.r40:
             log(ev[40][0], end="")
             entry.update(text_r40=ev[40][0], ap_r40=_ap_lists(ev[40][1]))
+        if args.coco:
+            log(ev["coco"][0], end="")
+            entry.update(text_coco=ev["coco"][0], ap_coco=_ap_lists(ev["coco"][1]))
         if per_batch is not None:
             entry.update(_loss_means([v[k * n:(k + 1) * n] for v in per_batch], args.batch, log))
             line.append("rpn_cls_loss %.6f loss_cls %.6f" % (entry["losses"]["rpn_cls_loss"],
