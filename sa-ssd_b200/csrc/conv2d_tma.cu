@@ -18,11 +18,11 @@
 //   * BN = 128 (every layer with cout > 64): the operand roles are swapped.  The output channels are wgmma's M and the
 //     tile's 128 pixels its N: consumer warpgroup wg owns channels 64 wg .. 64 wg + 63 of the unit and every pixel,
 //     and issues m64n128k16 with the weights as A in registers and the halo box as B from shared memory.  The weights
-//     go from global memory (L2) straight into registers in wgmma's fragment order (sassd_conv2d_pack), one chunk
-//     ahead, so shared memory carries only the pixels: per K step the SM reads 24 KB of operands instead of 36 KB
-//     and writes no weight ring.  A producer warpgroup (setmaxnreg down to 40 registers, the consumers up to 232)
-//     issues the boxes into a three-stage ring, and the epilogue transposes each warpgroup's 64-channel x 128-pixel
-//     block through shared memory into 16-byte stores.
+//     are packed in wgmma's fragment order (sassd_conv2d_pack); one producer warp copies each chunk of them (32 KB)
+//     with bulk copies into a two-stage ring, and the consumers move a chunk from the ring into registers one chunk
+//     ahead of its MMAs and release the stage at once.  A producer warpgroup (setmaxnreg down to 40 registers, the
+//     consumers up to 232) issues the boxes into a two-stage ring and the weights, and the epilogue transposes each
+//     warpgroup's 64-channel x 128-pixel block through shared memory into 16-byte stores.
 // A work unit is a tile and up to 128 of its output channels: the two register accumulators (big, small) of a
 // 64 x 128 block are 128 floats per thread, so 256-channel layers run each tile as two units on the same weight pack.
 #include <cuda.h>
@@ -49,7 +49,8 @@ constexpr int A_PLANE_BYTES = A_ROWS * TILE_W * 128;    // 20 KB (hi) ; same for
 constexpr int A_STAGE_BYTES = 2 * A_PLANE_BYTES;
 
 // BN = 128 weight pack (sassd_conv2d_pack): per chunk q of a unit's walk, K step s (16 input channels) and block mb of
-// 64 output channels, 128 threads x 32 bytes: thread t's wgmma A fragment, hi a0..a3 then lo a0..a3.
+// 64 output channels, 128 threads x 32 bytes: thread t's wgmma A fragment, hi a0..a3 then lo a0..a3.  A unit's two
+// blocks of a K step are contiguous: 8 KB per K step, 32 KB per chunk.
 constexpr int FRAG_BLOCK_BYTES = 128 * 32;
 constexpr int OUT_PITCH = 64 + 4;               // floats per pixel of the epilogue staging: conflict-free transposes
 
@@ -57,10 +58,11 @@ template <int BN>
 struct Cfg2 {
     static constexpr bool RS = BN >= 128;                       // weights in registers (see the top of the file)
     static constexpr int THREADS = CONS_THREADS + (RS ? 128 : 32);
-    static constexpr int A_STAGES = RS ? 3 : 2;
+    static constexpr int A_STAGES = 2;
     static constexpr int B_TILE_BYTES = BN * 128;
-    static constexpr int B_STAGE_BYTES = 2 * B_TILE_BYTES;     // one (tap, chunk): hi | lo
-    static constexpr int B_STAGES = RS ? 0 : 6;
+    static constexpr int B_STAGE_BYTES = 2 * B_TILE_BYTES;     // one (tap, chunk): hi | lo; RS: one chunk of fragments
+    static_assert(!RS || B_STAGE_BYTES == 4 * 2 * FRAG_BLOCK_BYTES, "an RS weight stage holds one chunk of a unit");
+    static constexpr int B_STAGES = RS ? 2 : 6;
     static constexpr int OUT_BYTES = RS ? 2 * TILE_H * TILE_W * OUT_PITCH * 4 : 0;   // per warpgroup 128 px x 64 ch
     static constexpr int RING_BYTES = A_STAGES * A_STAGE_BYTES + B_STAGES * B_STAGE_BYTES + OUT_BYTES;
     // tile order (computed tiles first) when the map carries constant-region information: two verdict bits and a uint16
@@ -220,8 +222,8 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
     __shared__ int s_walk[6];     // see next_unit
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    // A stages (halo boxes, hi | lo) at base; after them the B stages (weights of one (tap, chunk), hi | lo) for
-    // BN <= 64, the epilogue staging for BN = 128
+    // A stages (halo boxes, hi | lo) at base; after them the B stages (BN <= 64: the weights of one (tap, chunk),
+    // hi | lo; BN = 128: one chunk of the unit's weight fragments), then for BN = 128 the epilogue staging
     const uint32_t b_ring = base + A_STAGES * A_STAGE_BYTES;
     const uint32_t bar_base = base + C::RING_BYTES;
     auto a_full = [&](int s) { return bar_base + 8u * s; };
@@ -356,6 +358,26 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
     if (warp >= W_LOAD) {
         if constexpr (C::RS) {
             setmaxnreg_dec<40>();
+            if (warp == W_LOAD + 1 && lane == 0) {
+                // The weights of every computed unit, chunk by chunk in the order of the walk (the pack's): per K step
+                // the unit's two blocks, 8 KB contiguous in the pack.
+                constexpr uint32_t kStep = 2 * FRAG_BLOCK_BYTES;
+                int b_stage = 0;
+                uint32_t b_phase = 0;
+                for (int k = s_walk[5]; k < nunits; k = next_unit(k)) {
+                    if (tile_ref(k / nsplit) & (kConstTile | kBgTile)) continue;
+                    const uint8_t* src = (const uint8_t*)p.wpack + (size_t)(k % nsplit) * kStep;
+                    for (int q = 0; q < nchunks; ++q) {
+                        mbar_wait(b_empty(b_stage), b_phase ^ 1u);
+                        mbar_expect_tx(b_full(b_stage), C::B_STAGE_BYTES);
+                        const uint32_t dst = b_ring + b_stage * C::B_STAGE_BYTES;
+#pragma unroll 1
+                        for (int s = 0; s < 4; ++s, src += (size_t)nsplit * kStep)
+                            bulk_g2s(dst + s * kStep, src, kStep, b_full(b_stage));
+                        if (++b_stage == C::B_STAGES) { b_stage = 0; b_phase ^= 1u; }
+                    }
+                }
+            }
             if (warp != W_LOAD) return;
         }
         if (lane == 0) {
@@ -380,7 +402,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                         tma_load_4d(a_hi, &amap, kc * BKC, x0 + dx, y0 - halo, b, a_full(a_stage));
                         tma_load_4d(a_hi + A_PLANE_BYTES, &amap, kc * BKC, x0 + dx, y0 - halo, p.batch + b, a_full(a_stage));
                         if (++a_stage == A_STAGES) { a_stage = 0; a_phase ^= 1u; }
-                        if constexpr (!C::RS) {                  // BN = 128: the consumers load their weights themselves
+                        if constexpr (!C::RS) {                  // BN = 128: warp W_LOAD + 1 copies the weights
                             for (int row = 0; row < nrows; ++row) {
                                 const int t = row * ncols + col;                            // tap (dy + 1) * 3 + dx + 1
                                 mbar_wait(b_empty(b_stage), b_phase ^ 1u);
@@ -448,17 +470,25 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                 // the last of the box's nrows taps)
                 int prev_b = -1, prev_a = -1, row = 0;
                 if constexpr (C::RS) {
-                    // This thread's fragments in the pack: block 2 (k % nsplit) + wg of the 2 nsplit 64-channel blocks.
-                    const uint32_t kstep = 2u * nsplit * FRAG_BLOCK_BYTES, qstep = 4u * kstep;
-                    const uint8_t* wsrc = (const uint8_t*)p.wpack + (2 * (k % nsplit) + wg) * FRAG_BLOCK_BYTES + t * 32;
-                    auto load_w = [&](uint32_t (&w)[32], int q) {
-                        const uint8_t* src = wsrc + (size_t)q * qstep;
+                    // The next chunk's fragments from the weight ring: per K step s this warpgroup's block at
+                    // 8 KB s + 4 KB wg, thread t's 32 bytes (hi | lo) in it.  Threads with (t / 4) odd read their lo
+                    // half first, so that each 8-thread phase of a 16-byte load covers all 32 banks.  The stage is
+                    // released as soon as every thread of the warpgroup holds its fragments.
+                    auto load_w = [&](uint32_t (&w)[32]) {
+                        mbar_wait(b_full(b_stage), b_phase);
+                        const uint32_t sw = (t & 4) * 4u;
+                        const uint32_t src = b_ring + b_stage * C::B_STAGE_BYTES + wg * FRAG_BLOCK_BYTES + t * 32;
 #pragma unroll
                         for (int s = 0; s < 4; ++s) {
-                            const uint4 h = ldg_nc_v4(src + s * kstep), l = ldg_nc_v4(src + s * kstep + 16);
+                            const uint4 x = lds_v4(src + s * 2 * FRAG_BLOCK_BYTES + sw);
+                            const uint4 y = lds_v4(src + s * 2 * FRAG_BLOCK_BYTES + (sw ^ 16u));
+                            const uint4 h = sw ? y : x, l = sw ? x : y;
                             w[8 * s] = h.x; w[8 * s + 1] = h.y; w[8 * s + 2] = h.z; w[8 * s + 3] = h.w;
                             w[8 * s + 4] = l.x; w[8 * s + 5] = l.y; w[8 * s + 6] = l.z; w[8 * s + 7] = l.w;
                         }
+                        named_bar_sync(3 + wg, 128);
+                        if (t == 0) mbar_arrive(b_empty(b_stage));
+                        if (++b_stage == C::B_STAGES) { b_stage = 0; b_phase ^= 1u; }
                     };
                     // Chunk ch on the fragments in w; the next chunk's go into w_next once the MMAs that read them
                     // (chunk ch - 1) are complete.
@@ -471,7 +501,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                         wgmma_wait<1>();
                         fence_regs<32>(w_next);
                         if (t == 0 && prev_a >= 0) mbar_arrive(a_empty(prev_a));
-                        if (ch + 1 < nchunks) load_w(w_next, ch + 1);
+                        if (ch + 1 < nchunks) load_w(w_next);
                         prev_a = -1;
                         if (++row == nrows) {
                             row = 0;
@@ -480,7 +510,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                         }
                     };
                     uint32_t wa[32], wb[32];
-                    load_w(wa, 0);
+                    load_w(wa);
                     for (int ch = 0; ch < nchunks; ch += 2) {
                         chunk(wa, wb, ch);
                         if (ch + 1 == nchunks) break;
@@ -526,7 +556,8 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                 // Epilogue through shared memory: thread t holds channels m0, m0 + 8 of the warpgroup's 64 at pixels
                 // 8 j + 2 (t % 4) + e; folded BN + ReLU (or the layer constant) into the warpgroup's staging block
                 // [pixel][OUT_PITCH], then whole pixels out with 16-byte fp32 and / or split-plane stores.
-                float* stage = (float*)(base_ptr + A_STAGES * A_STAGE_BYTES) + wg * (TILE_H * TILE_W * OUT_PITCH);
+                float* stage = (float*)(base_ptr + A_STAGES * A_STAGE_BYTES + C::B_STAGES * C::B_STAGE_BYTES) +
+                               wg * (TILE_H * TILE_W * OUT_PITCH);
                 const int m0 = 16 * (t >> 5) + ((t & 31) >> 2), c_wg = n_off + 64 * wg;
                 float cv[2], sc[2], sh[2];
 #pragma unroll
