@@ -618,6 +618,33 @@ size_t sassd_kitti_eval_workspace_bytes(int max_nd, int max_ng);
 int sassd_kitti_eval_match(const SassdKittiEvalDesc* desc, double* scores, int32_t* n_scores, double* thresholds,
                            int32_t* n_thresh, double* pr, void* ws, size_t ws_bytes, sassd_stream_t stream);
 
+/* KITTI label / result files parsed on the device (csrc/kitti_parse.cu), get_label_anno's semantics
+ * (tools/kitti_common.py:560-601).  buf holds every file's bytes back to back, file f at [file_off[f], file_off[f+1])
+ * (int64).  All pointers are device memory.
+ *
+ * sassd_kitti_scan_labels: per file, n_lines[f] its readlines() line count ('\n' ends a line) and flags[f]:
+ * SASSD_KITTI_PARSE_SCORE when its first line has exactly 16 space-separated fields, SASSD_KITTI_PARSE_DEFER when the
+ * file is outside the device grammar (a byte >= 0x80 or a control character, an empty field, a missing converted field,
+ * a number outside [+-]?digits[.digits][(e|E)[+-]?digits], with more than 19 significant digits, a significand >= 2^53
+ * or a decimal exponent beyond +-22, an occluded value beyond int64) and must be read on the host (n_lines[f] = 0).
+ *
+ * sassd_kitti_parse_labels: the rows of every file not deferred, file f's lines at rows row_off[f] .. (row_off [nfiles
+ * + 1], nrows = row_off[nfiles]; a deferred file's rows are left unwritten): name_id (the index of the lower-cased name
+ * in the table names / name_off [nnames + 1], or -1), dontcare (name == "DontCare"), truncated, occluded
+ * (int(float(x)) as fp64), alpha, bbox [rows, 4], cam [rows, 7] (location, the file's h, w, l as l, h, w, rotation_y)
+ * and score (the 16th field with SASSD_KITTI_PARSE_SCORE, else 0), each equal to Python's float() bit for bit.
+ * ws: sassd_kitti_parse_workspace_bytes(nrows) bytes. */
+#define SASSD_KITTI_PARSE_DEFER 1
+#define SASSD_KITTI_PARSE_SCORE 2
+int sassd_kitti_scan_labels(const uint8_t* buf, const int64_t* file_off, int nfiles, int32_t* n_lines, int32_t* flags,
+                            sassd_stream_t stream);
+size_t sassd_kitti_parse_workspace_bytes(int nrows);
+int sassd_kitti_parse_labels(const uint8_t* buf, const int64_t* file_off, int nfiles, const int32_t* flags,
+                             const int32_t* row_off, int nrows, const char* names, const int32_t* name_off, int nnames,
+                             int32_t* name_id, int32_t* dontcare, double* truncated, double* occluded, double* alpha,
+                             double* bbox, double* cam, double* score, void* ws, size_t ws_bytes,
+                             sassd_stream_t stream);
+
 /* ------------------------------------------------------------------------
  * Training-time augmentation (the reference's PointAugmentor as
  * prepare_train_img applies it, mmdet/core/point_cloud/point_augmentor.py,

@@ -16,9 +16,21 @@ min-overlap row at once; only the precision / recall ratios, their envelope and 
 downloaded sums.  With an injected ``overlap_fn`` the host path runs: vectorised float64 numpy overlaps, per-frame
 `clean_gt` / `clean_dt` and the host C++ matcher `sassd_kitti_match` (numba-jitted CPU loops in the reference).
 Both paths give the same arrays bit for bit.  Annotations are dicts of numpy arrays as produced by
-`results.kitti_bbox2results` / the reference's `get_label_annos` (camera-frame boxes, dimensions l, h, w).
+`results.kitti_bbox2results` / the reference's `get_label_annos` (camera-frame boxes, dimensions l, h, w), or an
+AnnoBlock: the same rows as flat columns on the device, built from dicts or parsed from a directory of KITTI files on
+the device (`read_block`, csrc/kitti_parse.cu).
+
+    python -m sassd_b200.kitti_eval --data-root DIR [--split val] --results DIR [DIR ...] [--classes Car ...]
+                                    [--r40] [--coco] [--json FILE]
+
+evaluates directories of result files against a split's labels (`main`, `eval_dirs`).
 """
+import argparse
 import ctypes
+import json
+import os
+import sys
+import time
 
 import numpy as np
 
@@ -308,6 +320,9 @@ _NAME_IDS = {n: i for i, n in enumerate(dict.fromkeys(CLASS_NAMES))}     # one i
 _IGNORED_NAME = {"car": "van", "pedestrian": "person_sitting"}           # counted as ignored, not missed (clean_data)
 
 
+_ID_NAMES = list(_NAME_IDS)
+
+
 def _flat_names(annos):
     """(name ids, DontCare flags) of every row of ``annos``, frames concatenated; names are mapped once per distinct
     name."""
@@ -328,48 +343,175 @@ def _flat_cam(annos):
     return np.concatenate([_flat(annos, "location", 3), _flat(annos, "dimensions", 3), _flat(annos, "rotation_y", 1)], 1)
 
 
-def _eval_device(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flags):
-    """eval_class_many's precision / recall / orientation arrays for the three metrics, [metric][set] ->
-    dict of [class, difficulty, min_overlap, 41], with the flags, overlaps, matching, thresholds and per-threshold sums
-    on the device (csrc/kitti_match.cu); bit for bit what the host path computes."""
+def _cuda_device():
     import torch
     from . import ops
     ops.require_cuda()
-    dev = torch.device("cuda", torch.cuda.current_device())
-    K, F, C, Dn, M = len(dt_sets), len(gt_annos), len(classes), len(difficultys), min_overlaps.shape[0]
-    assert all(len(d) == F for d in dt_sets)
-    dt_all = [d for dts in dt_sets for d in dts]
-    ng = np.array([len(g["name"]) for g in gt_annos], np.int64)
-    nd = np.array([len(d["name"]) for d in dt_all], np.int64)
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+class AnnoBlock:
+    """The annotations of a list of frames as the flat columns the device evaluator reads: ``off`` [frames + 1] int64
+    row offsets (host), and torch tensors on one device, a row per object: ``name_id`` int32 (the index of the
+    lower-cased name among the class names, -1 for any other name), ``dontcare`` int32 (name == "DontCare"),
+    ``truncated``, ``occluded``, ``alpha`` and ``score`` float64, ``bbox`` [rows, 4] float64 and ``cam`` [rows, 7]
+    float64 (location, dimensions l, h, w, rotation_y).  ``trunc_dtype`` is the dtype the truncation values came in:
+    numpy compares a float32 column with the Python-float limit in float32, so the evaluator rounds the limit into it.
+
+    Built from annotation dicts (``from_annos``) or parsed from a directory of KITTI files on the device
+    (``read_block``)."""
+    COLUMNS = ("name_id", "dontcare", "truncated", "occluded", "alpha", "bbox", "cam", "score")
+
+    def __init__(self, off, columns, trunc_dtype=np.float64):
+        self.off = np.asarray(off, np.int64)
+        for name in self.COLUMNS:
+            setattr(self, name, columns[name])
+        self.trunc_dtype = np.dtype(trunc_dtype)
+
+    def __len__(self):
+        return len(self.off) - 1
+
+    @property
+    def counts(self):
+        return np.diff(self.off)
+
+    @classmethod
+    def from_annos(cls, annos, device=None):
+        """The block of a list of annotation dicts (``device``: default the current CUDA device).  A dict without
+        ``score`` (ground truth) gets zeros."""
+        import torch
+        device = _cuda_device() if device is None else torch.device(device)
+        names, dc = _flat_names(annos)
+        truncs = [np.asarray(a["truncated"]).reshape(-1) for a in annos]
+        trunc = np.concatenate(truncs) if truncs else np.zeros((0,))
+        scores = [np.asarray(a["score"], np.float64).reshape(-1) if "score" in a else np.zeros((len(a["name"]),))
+                  for a in annos]
+        cols = dict(name_id=names, dontcare=dc, truncated=trunc.astype(np.float64),
+                    occluded=_flat(annos, "occluded", 1).reshape(-1), alpha=_flat(annos, "alpha", 1).reshape(-1),
+                    bbox=_flat(annos, "bbox", 4), cam=_flat_cam(annos), score=_cat(scores, (0,), np.float64))
+        cols = {k: torch.from_numpy(np.ascontiguousarray(v)).to(device) for k, v in cols.items()}
+        return cls(_offsets([len(a["name"]) for a in annos], np.int64), cols,
+                   trunc.dtype if trunc.dtype.kind == "f" else np.float64)
+
+    def to(self, device):
+        return AnnoBlock(self.off, {k: getattr(self, k).to(device) for k in self.COLUMNS}, self.trunc_dtype)
+
+    def to_annos(self):
+        """Per-frame annotation dicts for the host path: the columns, ``truncated`` in ``trunc_dtype``, and a name per
+        row that the evaluator treats as the original (the class's lower-cased name, "DontCare", or "" for any other
+        name)."""
+        c = {k: getattr(self, k).cpu().numpy() for k in self.COLUMNS}
+        names = np.array([""] + _ID_NAMES + ["DontCare"])[np.where(c["dontcare"] != 0, len(_ID_NAMES) + 1,
+                                                                    c["name_id"] + 1)]
+        out = []
+        for f in range(len(self)):
+            r = slice(self.off[f], self.off[f + 1])
+            out.append(dict(name=names[r], truncated=c["truncated"][r].astype(self.trunc_dtype),
+                            occluded=c["occluded"][r], alpha=c["alpha"][r], bbox=c["bbox"][r],
+                            location=c["cam"][r, :3], dimensions=c["cam"][r, 3:6], rotation_y=c["cam"][r, 6],
+                            score=c["score"][r]))
+        return out
+
+
+def _as_block(annos):
+    return annos if isinstance(annos, AnnoBlock) else AnnoBlock.from_annos(annos)
+
+
+def _as_annos(annos):
+    return annos.to_annos() if isinstance(annos, AnnoBlock) else annos
+
+
+def read_block(directory, ids, device=None, workers=8, times=None):
+    """``directory/%06d.txt`` of every id (KITTI label or result files, a 16th field the score) -> an AnnoBlock, what
+    ``AnnoBlock.from_annos(kitti_data.read_labels(directory, ids))`` gives, bit for bit.  The files are read on a
+    thread pool into one pinned buffer, copied to the device once and parsed there (csrc/kitti_parse.cu); a file
+    outside the device's grammar is read by kitti_data.read_label instead, and so raises what it raises.  A missing
+    file raises FileNotFoundError naming it.  ``times``: a dict whose "read" and "parse" entries accumulate the seconds
+    spent reading the files and parsing them (the device synchronised)."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    import torch
+    from . import lib, ops
+    from .kitti_data import read_label
+    t0 = time.perf_counter()
+    paths = [os.path.join(directory, "%06d.txt" % i) for i in ids]
+
+    def load(path):
+        with open(path, "rb") as fh:
+            return fh.read()
+    with ThreadPoolExecutor(max_workers=max(1, int(workers))) as ex:
+        data = list(ex.map(load, paths))
+    device = _cuda_device() if device is None else torch.device(device)
+    file_off = _offsets([len(d) for d in data], np.int64)
+    host = torch.empty((max(int(file_off[-1]), 1),), dtype=torch.uint8, pin_memory=True)
+    host.numpy()[:file_off[-1]] = np.frombuffer(b"".join(data), np.uint8)
+    t1 = time.perf_counter()
+    buf = host.to(device, non_blocking=True)
+    d_file_off = torch.from_numpy(file_off).to(device)
+    n_lines, flags = ops.kitti_scan_labels(buf, d_file_off)
+    n_lines, flags = torch.stack([n_lines, flags]).cpu().numpy() if len(ids) else np.zeros((2, 0), np.int32)
+    deferred = np.flatnonzero(flags & lib.KITTI_PARSE_DEFER)
+    slow = AnnoBlock.from_annos([read_label(paths[f]) for f in deferred], "cpu")
+    counts = n_lines.astype(np.int64)
+    counts[deferred] = slow.counts
+    row_off = _offsets(counts)
+    nrows = int(row_off[-1])
+    names = "".join(_ID_NAMES).encode()
+    name_off = _offsets([len(n) for n in _ID_NAMES])
+    cols = ops.kitti_parse_labels(buf, d_file_off, torch.from_numpy(flags).to(device), torch.from_numpy(row_off).to(device),
+                                  nrows, torch.frombuffer(bytearray(names), dtype=torch.uint8).to(device),
+                                  torch.from_numpy(name_off).to(device))
+    cols = dict(zip(AnnoBlock.COLUMNS, cols))
+    if len(deferred):
+        rows = np.concatenate([np.arange(row_off[f], row_off[f + 1]) for f in deferred])
+        idx = torch.from_numpy(rows).to(device)
+        for k in AnnoBlock.COLUMNS:
+            cols[k][idx] = getattr(slow, k).to(device)
+    block = AnnoBlock(row_off.astype(np.int64), cols)
+    if times is not None:
+        torch.cuda.synchronize(device)
+        t2 = time.perf_counter()
+        times["read"] = times.get("read", 0.0) + t1 - t0
+        times["parse"] = times.get("parse", 0.0) + t2 - t1
+    return block
+
+
+def _eval_device(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flags):
+    """eval_class_many's precision / recall / orientation arrays for the three metrics, [metric][set] ->
+    dict of [class, difficulty, min_overlap, 41], with the flags, overlaps, matching, thresholds and per-threshold sums
+    on the device (csrc/kitti_match.cu); bit for bit what the host path computes.  The GT and each detection set are
+    AnnoBlocks (lists of annotation dicts are flattened into one first)."""
+    import torch
+    from . import ops
+    dev = _cuda_device()
+    gt = _as_block(gt_annos).to(dev)
+    dts = [_as_block(d).to(dev) for d in dt_sets]
+    K, F, C, Dn, M = len(dts), len(gt), len(classes), len(difficultys), min_overlaps.shape[0]
+    assert all(len(d) == F for d in dts)
+    ng = gt.counts
+    nd = np.concatenate([d.counts for d in dts]) if dts else np.zeros((0,), np.int64)
     npairs = nd * np.tile(ng, K)
     gt_off, dt_off, ov_off = _offsets(ng), _offsets(nd), _offsets(npairs, np.int64)
     total = int(ov_off[-1])
-    gt_name, gt_dc = _flat_names(gt_annos)
-    dt_name, _ = _flat_names(dt_all)
-    gt_bbox, dt_bbox = _flat(gt_annos, "bbox", 4), _flat(dt_all, "bbox", 4)
-    gt_cam, dt_cam = _flat_cam(gt_annos), _flat_cam(dt_all)
-    truncs = [np.asarray(g["truncated"]).reshape(-1) for g in gt_annos]
-    trunc = np.concatenate(truncs) if truncs else np.zeros((0,))
+    dt_name = torch.cat([d.name_id for d in dts])
+    dt_bbox, dt_cam = torch.cat([d.bbox for d in dts]), torch.cat([d.cam for d in dts])
     # numpy compares a float32 column with the Python-float limit in float32: round the limit into the column's dtype
-    tdt = trunc.dtype if trunc.dtype.kind == "f" else np.float64
-    limits = np.array([[MAX_OCCLUSION[d], float(tdt.type(MAX_TRUNCATION[d])), MIN_HEIGHT[d]] for d in difficultys],
-                      np.float64)
+    limits = np.array([[MAX_OCCLUSION[d], float(gt.trunc_dtype.type(MAX_TRUNCATION[d])), MIN_HEIGHT[d]]
+                       for d in difficultys], np.float64)
     cls_ids = np.array([[_NAME_IDS[CLASS_NAMES[c].lower()], _NAME_IDS.get(_IGNORED_NAME.get(CLASS_NAMES[c].lower()), -1)]
                         for c in classes], np.int32)
 
     def up(a):
         return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
 
-    t = dict(gt_off=up(gt_off), dt_off=up(dt_off), ov_off=up(ov_off), gt_dc=up(gt_dc), gt_bbox=up(gt_bbox),
-             dt_bbox=up(dt_bbox), dt_score=up(_flat(dt_all, "score", 1).reshape(-1)), gt_cam=up(gt_cam),
-             dt_cam=up(dt_cam), min_overlaps=up(np.asarray(min_overlaps, np.float64)),
-             compute_aos=up(np.asarray(aos_flags, np.int32)))
-    ign_gt, ign_dt, n_valid = ops.kitti_eval_flags(
-        up(gt_name), up(_flat(gt_annos, "occluded", 1).reshape(-1)), up(trunc.astype(np.float64)), t["gt_bbox"],
-        up(dt_name), t["dt_bbox"], up(cls_ids), up(limits))
+    t = dict(gt_off=up(gt_off), dt_off=up(dt_off), ov_off=up(ov_off), gt_dc=gt.dontcare, gt_bbox=gt.bbox,
+             dt_bbox=dt_bbox, dt_score=torch.cat([d.score for d in dts]), gt_cam=gt.cam, dt_cam=dt_cam,
+             min_overlaps=up(np.asarray(min_overlaps, np.float64)), compute_aos=up(np.asarray(aos_flags, np.int32)))
+    ign_gt, ign_dt, n_valid = ops.kitti_eval_flags(gt.name_id, gt.occluded, gt.truncated, t["gt_bbox"], dt_name,
+                                                   t["dt_bbox"], up(cls_ids), up(limits))
     # the rotated overlaps of every (set, frame) block: BEV IoU and the intersection area the 3-D overlap builds on
     bev = [0, 2, 3, 5, 6]
-    dt_bev, gt_bev = up(dt_cam[:, bev].astype(np.float32)), up(np.tile(gt_cam[:, bev].astype(np.float32), (K, 1)))
+    dt_bev, gt_bev = dt_cam[:, bev].float().contiguous(), gt.cam[:, bev].float().repeat(K, 1)
     q_off = up(_offsets(np.tile(ng, K)))
     rot = []
     for criterion in (-1, 2):
@@ -384,7 +526,8 @@ def _eval_device(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flag
     aos_table = None
     if any(aos_flags) and total:
         table = np.zeros((total,), np.float64)
-        gt_alpha, dt_alpha = _flat(gt_annos, "alpha", 1).reshape(-1), _flat(dt_all, "alpha", 1).reshape(-1)
+        gt_alpha = gt.alpha.cpu().numpy()
+        dt_alpha = torch.cat([d.alpha for d in dts]).cpu().numpy()
         _lib.check(_lib.load().sassd_kitti_aos_table(K, F, _p(gt_off), _p(dt_off), _p(ov_off), _p(gt_alpha),
                                                      _p(dt_alpha), _p(table)), "sassd_kitti_aos_table")
         aos_table = up(table)
@@ -471,6 +614,8 @@ def _class_ids(classes):
 
 def _aos_flag(dt_annos):
     """compute_aos as the reference decides it (kitti_eval.py:818-823): from the first frame with detections."""
+    if isinstance(dt_annos, AnnoBlock):
+        return bool(dt_annos.off[-1] > 0 and float(dt_annos.alpha[0]) != -10)
     for anno in dt_annos:
         if anno['alpha'].shape[0] != 0:
             return bool(anno['alpha'][0] != -10)
@@ -481,7 +626,8 @@ def eval_many(gt_annos, dt_sets, classes, tables=(11,), overlap_fn=None, difficu
     """Every table of ``tables`` (11 and 40: the official tables at 11 / 40 recall positions; "coco": the COCO-style
     table) for each of the K detection sets of ``dt_sets`` against the same GT.  Returns one dict per set, {table:
     (text, ap)}.  The official and COCO overlap rows form one list of min overlaps, so the overlaps, the GT side and
-    the matching run once for all of them; R11 and R40 read the same precision samples."""
+    the matching run once for all of them; R11 and R40 read the same precision samples.  The GT and each set are a
+    list of annotation dicts or an AnnoBlock."""
     tables = tuple(tables)
     if not tables or any(t not in TABLES for t in tables):
         raise ValueError("tables must be among %r, not %r" % (TABLES, tables))
@@ -497,6 +643,7 @@ def eval_many(gt_annos, dt_sets, classes, tables=(11,), overlap_fn=None, difficu
     if overlap_fn is None:
         prec = _eval_device(gt_annos, dt_sets, classes, diffs, min_overlaps, aos_flags)
     else:
+        gt_annos, dt_sets = _as_annos(gt_annos), [_as_annos(d) for d in dt_sets]
         gt_sides = {(c, d): _GtSide(gt_annos, c, d) for c in classes for d in diffs}
         prec = [eval_class_many(gt_annos, dt_sets, classes, diffs, metric, min_overlaps,
                                 aos_flags if metric == 0 else [False] * len(dt_sets), overlap_fn, gt_sides)
@@ -567,3 +714,112 @@ def _ap_text(ap, classes, min_overlaps, compute_aos, tag):
 def get_official_eval_result(gt_annos, dt_annos, current_classes, difficultys=[0, 1, 2], overlap_fn=None):
     """Reference signature (kitti_eval.py:791): the printed result table."""
     return official_eval(gt_annos, dt_annos, current_classes, difficultys, overlap_fn)[0]
+
+
+# ------------------------------------------------------------------ result directories
+def ap_lists(ap):
+    """An AP dict as JSON-ready nested lists."""
+    return {k: (None if v is None else np.asarray(v).tolist()) for k, v in ap.items()}
+
+
+def report_sets(entries, labels, evs, class_names, noun, log=print, extra=None):
+    """Print each evaluated set's tables (``evs``: eval_many's dicts, with table 11) under ``== label ==``, then one
+    summary line per set: moderate 3D AP per class at the class's strict overlap (R11, and R40 / COCO when evaluated).
+    Each set's texts and AP lists go into its dict of ``entries`` (returned).  ``extra(k, entry)`` may add to set k's
+    entry after its tables and returns more summary fields."""
+    summary = []
+    for k, (entry, label, ev) in enumerate(zip(entries, labels, evs)):
+        log("== %s ==" % label)
+        text, ap = ev[11]
+        log(text, end="")
+        entry.update(text=text, ap=ap_lists(ap))
+        line = ["%-24s" % label]
+        for j, c in enumerate(class_names):
+            line.append("%s 3d mod R11 %6.2f" % (c, ap["d3"][j, 1, 0]) +
+                        (" R40 %6.2f" % ev[40][1]["d3"][j, 1, 0] if 40 in ev else "") +
+                        (" COCO %6.2f" % ev["coco"][1]["d3"][j, 1] if "coco" in ev else ""))
+        if 40 in ev:
+            log(ev[40][0], end="")
+            entry.update(text_r40=ev[40][0], ap_r40=ap_lists(ev[40][1]))
+        if "coco" in ev:
+            log(ev["coco"][0], end="")
+            entry.update(text_coco=ev["coco"][0], ap_coco=ap_lists(ev["coco"][1]))
+        if extra is not None:
+            line += extra(k, entry)
+        summary.append("  ".join(line))
+    log("summary: %d %s (moderate 3D AP)" % (len(labels), noun))
+    for line in summary:
+        log(line)
+    return entries
+
+
+def eval_dirs(label_dir, result_dirs, ids, classes, tables=(11,), times=None):
+    """Every table of ``tables`` for each directory of KITTI result files in ``result_dirs`` against the label files
+    of ``label_dir``, over the frames ``ids``: the GT is read once, every directory is read and parsed on the device
+    (read_block), and one eval_many evaluates them all.  Returns eval_many's list, one dict per directory.
+    ``times``: a dict whose "read", "parse" and "eval" entries accumulate seconds."""
+    times = {} if times is None else times
+    gt = read_block(label_dir, ids, times=times)
+    dts = [read_block(d, ids, times=times) for d in result_dirs]
+    t0 = time.perf_counter()
+    out = eval_many(gt, dts, classes, tables)
+    times["eval"] = times.get("eval", 0.0) + time.perf_counter() - t0
+    return out
+
+
+def parse_args(argv=None):
+    p = argparse.ArgumentParser(prog="python -m sassd_b200.kitti_eval", description=main.__doc__.split("\n\n")[0])
+    p.add_argument("--data-root", required=True, help="KITTI root holding ImageSets/ and training/label_2/")
+    p.add_argument("--split", default="val", help="the frames of ImageSets/<split>.txt (default val)")
+    p.add_argument("--results", nargs="+", required=True, metavar="DIR",
+                   help="directories of KITTI result files %%06d.txt (a 16th field the score)")
+    p.add_argument("--classes", nargs="+", default=["Car"], metavar="CLASS",
+                   help="classes to evaluate, among %s (default Car)" % ", ".join(CLASS_TO_NAME.values()))
+    p.add_argument("--r40", action="store_true", help="also print the AP table at 40 recall positions")
+    p.add_argument("--coco", action="store_true",
+                   help="also print the COCO-style AP table (AP averaged over ten IoU thresholds per class)")
+    p.add_argument("--json", default=None, help="write the AP arrays and times here")
+    args = p.parse_args(argv)
+    unknown = [c for c in args.classes if c not in CLASS_TO_NAME.values()]
+    if unknown:
+        p.error("--classes: unknown class %s (known: %s)" % (", ".join(unknown), ", ".join(CLASS_TO_NAME.values())))
+    if not os.path.isfile(os.path.join(args.data_root, "ImageSets", args.split + ".txt")):
+        p.error("--split %s: %s does not exist" % (args.split, os.path.join(args.data_root, "ImageSets",
+                                                                              args.split + ".txt")))
+    if not os.path.isdir(os.path.join(args.data_root, "training", "label_2")):
+        p.error("--data-root %s has no training/label_2 directory" % args.data_root)
+    missing = [d for d in args.results if not os.path.isdir(d)]
+    if missing:
+        p.error("--results: %s is not a directory" % missing[0])
+    return args
+
+
+def main(argv=None, log=print):
+    """Evaluate directories of KITTI result files against a split's labels (SECOND's kitti-object-eval-python):
+
+    python -m sassd_b200.kitti_eval --data-root DIR [--split val] --results DIR [DIR ...]
+                                    [--classes Car Pedestrian Cyclist] [--r40] [--coco] [--json FILE]
+
+    The labels are ``training/label_2/%06d.txt`` and the frames those of ``ImageSets/<split>.txt``; files a result
+    directory holds beyond them are ignored.  Every file is read into pinned memory, copied to the device once and
+    parsed there (read_block), and all directories are evaluated in one pass (eval_many) on the device.  Prints each
+    directory's tables under ``== DIR ==``, one summary line per directory and the seconds spent reading, parsing and
+    evaluating.  Returns the result dict that ``--json`` writes."""
+    from .kitti_data import read_split
+    args = parse_args(argv)
+    ids = read_split(args.data_root, args.split)
+    tables = (11,) + ((40,) if args.r40 else ()) + (("coco",) if args.coco else ())
+    times = {}
+    evs = eval_dirs(os.path.join(args.data_root, "training", "label_2"), args.results, ids, args.classes, tables, times)
+    entries = report_sets([dict(dir=d) for d in args.results], args.results, evs, args.classes, "directories", log)
+    log("frames: %d, directories: %d, read %.3f s, parse %.3f s, evaluate %.3f s" % (
+        len(ids), len(args.results), times["read"], times["parse"], times["eval"]))
+    result = dict(split=args.split, frames=len(ids), classes=args.classes, results=entries, times_s=times)
+    if args.json:
+        with open(args.json, "w") as fh:
+            json.dump(result, fh, indent=1)
+    return result
+
+
+if __name__ == "__main__":
+    main(sys.argv[1:])

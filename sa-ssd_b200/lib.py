@@ -51,6 +51,7 @@ SPCONV_TILE_ROWS = 128                    # SASSD_SPCONV_TILE_ROWS
 KITTI_META, KITTI_ROW = 36, 14            # SASSD_KITTI_META / SASSD_KITTI_ROW
 POINT_LEVEL_CHANNELS = (32, 64, 64)       # sassd_point_aux_head: features of backbone levels 1..3 (conv1, conv2, conv3)
 POINT_FC_IN, POINT_FC_OUT = 160, 64       # point_fc: Linear(160, 64); point_cls / point_reg read its 64 outputs
+KITTI_PARSE_DEFER, KITTI_PARSE_SCORE = 1, 2     # SASSD_KITTI_PARSE_DEFER / _SCORE: sassd_kitti_scan_labels' flags
 GT_CAP_MAX = 256                          # SASSD_GT_CAP_MAX: ground-truth boxes per frame the loss kernels take
 MERGE_MAX = 16                            # SASSD_MERGE_MAX: members sassd_merge_detections takes
 
@@ -103,6 +104,9 @@ _SIGNATURES = {
     "sassd_kitti_aos_table": (c_int, [c_int, c_int, P, P, P, P, P, P]),
     "sassd_kitti_eval_workspace_bytes": (c_size_t, [c_int, c_int]),
     "sassd_kitti_eval_match": (c_int, [ctypes.POINTER(KittiEvalDesc), P, P, P, P, P, P, c_size_t, P]),
+    "sassd_kitti_scan_labels": (c_int, [P, P, c_int, P, P, P]),
+    "sassd_kitti_parse_workspace_bytes": (c_size_t, [c_int]),
+    "sassd_kitti_parse_labels": (c_int, [P, P, c_int, P, P, c_int, P, P, c_int, P, P, P, P, P, P, P, P, P, c_size_t, P]),
     "sassd_spconv_pack_bytes": (c_size_t, [c_int, c_int, c_int]),
     "sassd_spconv_pack": (c_int, [P, c_int, c_int, c_int, c_int, P, P]),
     "sassd_spconv_workspace_bytes": (c_size_t, []),

@@ -53,7 +53,7 @@ def next_pow2(n):
 # kernels launched by each C-ABI entry point (memsets not counted)
 _KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_points_in_rbboxes": 1, "sassd_augment_drop_points": 1, "sassd_augment_noise_search": 1, "sassd_augment_assemble": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
-            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_kitti_eval_flags": 1, "sassd_kitti_eval_overlaps": 1, "sassd_kitti_eval_match": 3, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
+            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_kitti_eval_flags": 1, "sassd_kitti_eval_overlaps": 1, "sassd_kitti_eval_match": 3, "sassd_kitti_scan_labels": 1, "sassd_kitti_parse_labels": 2, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_merge_detections": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
             "sassd_boxes_iou_bev": 1, "sassd_points_in_boxes": 2, "sassd_assign_rpn": 3, "sassd_assign_pswarp": 3,
             "sassd_rpn_loss": 2, "sassd_pswarp_loss": 2, "sassd_aux_loss": 2}
@@ -532,6 +532,34 @@ def kitti_eval_match(desc, njobs, score_total, ws=None):
     _call("sassd_kitti_eval_match", None, ctypes.byref(desc), _ptr(scores), _ptr(n_scores), _ptr(thresholds),
           _ptr(n_thresh), _ptr(pr), _ptr(w), w.numel(), _stream())
     return thresholds, n_thresh, pr
+
+
+def kitti_scan_labels(buf, file_off):
+    """buf [bytes] u8: every file's bytes back to back, file f at [file_off[f], file_off[f+1]) (file_off [F+1] i64;
+    device).  Returns (n_lines [F] i32, flags [F] i32 of lib.KITTI_PARSE_DEFER / KITTI_PARSE_SCORE), csrc/kitti_parse.cu:
+    a deferred file is outside the device grammar and is read on the host."""
+    F = file_off.shape[0] - 1
+    n_lines = torch.empty((F,), dtype=torch.int32, device=buf.device)
+    flags = torch.empty((F,), dtype=torch.int32, device=buf.device)
+    _call("sassd_kitti_scan_labels", None, _ptr(buf), _ptr(file_off), F, _ptr(n_lines), _ptr(flags), _stream())
+    return n_lines, flags
+
+
+def kitti_parse_labels(buf, file_off, flags, row_off, nrows, names, name_off, ws=None):
+    """The rows of every file kitti_scan_labels did not defer, file f's lines at rows row_off[f] .. (row_off [F+1] i32;
+    names / name_off: the lower-cased class-name table, u8 bytes and [N+1] i32 offsets).  Returns the columns
+    (name_id [R] i32, dontcare [R] i32, truncated, occluded, alpha [R] f64, bbox [R,4] f64, cam [R,7] f64, score [R]
+    f64); a deferred file's rows are left unwritten."""
+    dev = buf.device
+    F = file_off.shape[0] - 1
+    f64 = dict(dtype=torch.float64, device=dev)
+    out = [torch.empty((nrows,), dtype=torch.int32, device=dev), torch.empty((nrows,), dtype=torch.int32, device=dev),
+           torch.empty((nrows,), **f64), torch.empty((nrows,), **f64), torch.empty((nrows,), **f64),
+           torch.empty((nrows, 4), **f64), torch.empty((nrows, 7), **f64), torch.empty((nrows,), **f64)]
+    w = (ws or _WS).get("kitti_parse", _L().sassd_kitti_parse_workspace_bytes(nrows), dev)
+    _call("sassd_kitti_parse_labels", None, _ptr(buf), _ptr(file_off), F, _ptr(flags), _ptr(row_off), nrows,
+          _ptr(names), _ptr(name_off), name_off.shape[0] - 1, *[_ptr(t) for t in out], _ptr(w), w.numel(), _stream())
+    return out
 
 
 def merge_detections(dets, label_offsets):

@@ -15,7 +15,8 @@ padded with empty frames whose results are dropped.  Prints the official AP tabl
 clock of the streamed detection, the evaluation excluded) and the time spent waiting on reads.  ``--r40`` also prints
 the table at 40 recall positions (kitti_eval.official_eval(recall_positions=40)), and ``--coco`` the reference's
 COCO-style table, AP averaged over ten IoU thresholds per class (kitti_eval.coco_eval), after the official one(s).
-All tables come from one evaluation (kitti_eval.eval_many), which runs on the device.
+All tables come from one evaluation (kitti_eval.eval_many), which runs on the device, against the split's labels as
+kitti_eval.read_block parses them on the device.
 
 ``--losses`` (labelled splits): every frame also carries its ground truth (kitti_data.gt_from_anno) and the captured
 step computes SA-SSD's six losses beside the detections (detect_stream(losses=True)); the result files and AP tables
@@ -298,23 +299,24 @@ def run(args, log=print):
         _write_json(args.json, result)
         D.barrier()
         return result
+    from .kitti_eval import ap_lists, eval_many, read_block
+    gt = read_block(os.path.join(split.dir, "label_2"), split.ids)
     if sweep:
-        result["checkpoints"] = _report_sweep(args, split.gt_annos(), dt_sets, class_names, per_batch, log)
+        result["checkpoints"] = _report_sweep(args, gt, dt_sets, class_names, per_batch, log)
         log(rate)
         _write_json(args.json, result)
         D.barrier()
         return result
-    from .kitti_eval import eval_many
-    ev = eval_many(split.gt_annos(), [dt_annos], class_names, _tables(args))[0]
+    ev = eval_many(gt, [dt_annos], class_names, _tables(args))[0]
     text, ap = ev[11]
     log(text, end="")
-    result.update(text=text, ap=_ap_lists(ap))
+    result.update(text=text, ap=ap_lists(ap))
     if args.r40:
         log(ev[40][0], end="")
-        result.update(text_r40=ev[40][0], ap_r40=_ap_lists(ev[40][1]))
+        result.update(text_r40=ev[40][0], ap_r40=ap_lists(ev[40][1]))
     if args.coco:
         log(ev["coco"][0], end="")
-        result.update(text_coco=ev["coco"][0], ap_coco=_ap_lists(ev["coco"][1]))
+        result.update(text_coco=ev["coco"][0], ap_coco=ap_lists(ev["coco"][1]))
     if args.losses:
         result.update(_loss_means(per_batch, args.batch, log))
     log(rate)
@@ -328,10 +330,6 @@ def _tables(args):
     return (11,) + ((40,) if args.r40 else ()) + (("coco",) if args.coco else ())
 
 
-def _ap_lists(ap):
-    return {k: (None if v is None else np.asarray(v).tolist()) for k, v in ap.items()}
-
-
 def _loss_means(per_batch, batch, log):
     """Print the mean of each loss over the per-batch vectors; returns the result dict's losses entries."""
     from . import ops
@@ -342,42 +340,23 @@ def _loss_means(per_batch, batch, log):
                 losses_per_batch=[dict(zip(ops.LOSS_KEYS, v)) for v in per_batch])
 
 
-def _report_sweep(args, gt_annos, dt_sets, class_names, per_batch, log):
+def _report_sweep(args, gt, dt_sets, class_names, per_batch, log):
     """Evaluate and print each checkpoint of a sweep (one kitti_eval.eval_many for all of them), then one summary line
     per checkpoint: moderate 3D AP per class at the class's strict overlap (R11, and R40 with --r40), the moderate 3D
     COCO-style AP with --coco, and the rpn_cls_loss / loss_cls means.  Returns the result dict's ``checkpoints``
     list."""
     from . import ops
-    from .kitti_eval import eval_many
+    from .kitti_eval import eval_many, report_sets
     paths = [args.checkpoint] + args.checkpoints
     n = len(ops.LOSS_KEYS)
-    entries, summary = [], []
-    for k, (path, ev) in enumerate(zip(paths, eval_many(gt_annos, dt_sets, class_names, _tables(args)))):
-        log("== %s ==" % os.path.basename(path))
-        text, ap = ev[11]
-        log(text, end="")
-        entry = dict(path=path, text=text, ap=_ap_lists(ap))
-        line = ["%-24s" % os.path.basename(path)]
-        for j, c in enumerate(class_names):
-            line.append("%s 3d mod R11 %6.2f" % (c, ap["d3"][j, 1, 0]) +
-                        (" R40 %6.2f" % ev[40][1]["d3"][j, 1, 0] if args.r40 else "") +
-                        (" COCO %6.2f" % ev["coco"][1]["d3"][j, 1] if args.coco else ""))
-        if args.r40:
-            log(ev[40][0], end="")
-            entry.update(text_r40=ev[40][0], ap_r40=_ap_lists(ev[40][1]))
-        if args.coco:
-            log(ev["coco"][0], end="")
-            entry.update(text_coco=ev["coco"][0], ap_coco=_ap_lists(ev["coco"][1]))
-        if per_batch is not None:
-            entry.update(_loss_means([v[k * n:(k + 1) * n] for v in per_batch], args.batch, log))
-            line.append("rpn_cls_loss %.6f loss_cls %.6f" % (entry["losses"]["rpn_cls_loss"],
-                                                               entry["losses"]["loss_cls"]))
-        entries.append(entry)
-        summary.append("  ".join(line))
-    log("summary: %d checkpoints (moderate 3D AP)" % len(paths))
-    for line in summary:
-        log(line)
-    return entries
+
+    def losses(k, entry):
+        if per_batch is None:
+            return []
+        entry.update(_loss_means([v[k * n:(k + 1) * n] for v in per_batch], args.batch, log))
+        return ["rpn_cls_loss %.6f loss_cls %.6f" % (entry["losses"]["rpn_cls_loss"], entry["losses"]["loss_cls"])]
+    return report_sets([dict(path=p) for p in paths], [os.path.basename(p) for p in paths],
+                       eval_many(gt, dt_sets, class_names, _tables(args)), class_names, "checkpoints", log, losses)
 
 
 def _write_json(path, result):
