@@ -322,6 +322,9 @@ typedef struct {
     int32_t cin, cout, taps;         /* cin = stored channels of the input planes */
     int32_t rows_cap, in_rows_cap;   /* output rows capacity; rows of the input planes (plane stride) */
     int32_t relu, out_ch, out_f32_stride;
+    int32_t fixed_walk;              /* 1: every tile walks its K chunks from chunk 0; 0 (default): from a tile-dependent
+                                        chunk, which spreads the CTAs' weight reads over L2 but makes a row's fp32
+                                        summation order depend on the index of its tile, i.e. on the rows before it */
 } sassd_spconv_desc;
 /* wpack for sassd_spconv_f16x3: weight [taps, cin, cout] fp32 -> sassd_spconv_pack_bytes(taps, cin_stored, cout)
  * bytes.  Narrow inputs are tap-packed: a 64-wide K chunk holds 64 / cin_stored taps (cin_stored 8, 16, 32). */

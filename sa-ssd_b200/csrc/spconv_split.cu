@@ -88,6 +88,7 @@ struct Args {
                             // (null: no chunk deal)
     int* counters;          // optional [2]: executed (tile, chunk) pairs, tiles (bench instrumentation)
     int cin, cout, taps, rows_cap, relu, out_ch, out_f32_stride;
+    int fixed_walk;         // every tile walks its chunks from chunk 0 (see rot_of)
 };
 
 // Chunk g of a tile is active when one of its `tpg` taps is in the tile's tap mask.
@@ -171,8 +172,9 @@ __global__ void __launch_bounds__(THREADS3, 1) spconv_split_kernel(const Args p)
     // Every CTA streams the same weight chunks.  If they all walked the taps in the same order they would ask the
     // same few L2 lines for the same 16 KB at the same time; each tile therefore starts at a different tap
     // (rotation by a tile-dependent offset, identical in all roles; the sum over taps is order-independent up to fp32
-    // rounding and deterministic per tile).
-    auto rot_of = [&](int tile) { return (int)(((unsigned)tile * 11u) % (unsigned)nchunks); };
+    // rounding and deterministic per tile).  A tile holds the rows of whichever frames fall into it, so with the
+    // rotation a frame's bits depend on how many rows the frames before it have; fixed_walk takes it away.
+    auto rot_of = [&](int tile) { return p.fixed_walk ? 0 : (int)(((unsigned)tile * 11u) % (unsigned)nchunks); };
     // Work decomposition, uniform over the grid.  Chunk deal (tiles <= CTAs): deal_pre[t] = active chunks of the tiles
     // before t, S = all of them; CTA c < D = min(G, S) takes chunks [c S / D, (c + 1) S / D) of that list (at least
     // one each, so every CTA that owns part of a tile has work in it).  Otherwise rounds of one tile per CTA.
@@ -565,6 +567,7 @@ extern "C" int sassd_spconv_f16x3(const sassd_spconv_desc* d, const void* in_spl
     a.counters = counters;
     a.cin = d->cin; a.cout = d->cout; a.taps = d->taps; a.rows_cap = d->rows_cap; a.relu = d->relu;
     a.out_ch = d->out_ch; a.out_f32_stride = d->out_f32_stride;
+    a.fixed_walk = d->fixed_walk;
     const int tiles = sassd_div_up(d->rows_cap, sps::BM), tpg = spconv_tpg(d->cin);
     if (d->taps == 1) return sps::dispatch3<0>(a, tiles, (cudaStream_t)stream_);
     return sps::dispatch3<1>(a, ws ? tiles * ((d->taps + tpg - 1) / tpg) : tiles, (cudaStream_t)stream_);

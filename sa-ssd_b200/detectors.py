@@ -193,6 +193,7 @@ class SingleStageDetector(nn.Module):
         the auxiliary network's points_mean [cap,4] (b, x, y, z), point_cls [cap] and point_reg [cap,3] (neck.point_head)
         for the voxel rows (frame_rows).  ``guided_thr``: the guided anchors' score threshold (default self.guided_thr;
         the losses use train_cfg.rpn.anchor_thr)."""
+        _require_batch(self, batch)
         status = torch.zeros((1,), dtype=torch.int32, device=points.device)
         vox = self.voxel_generator.generate_device(points, pt_off, batch, max_points_per_frame, status)
         return self.forward_voxels(vox, batch, status, point_outputs=point_outputs, detections=detections,
@@ -885,6 +886,16 @@ def _loss_dict(h):
     return {k: float(v) for k, v in zip(ops.LOSS_KEYS, h.tolist())}
 
 
+def _require_batch(model, batch):
+    """Refuse a step of more frames than the level-0 hash can key before any of its kernels is launched (the hash
+    build would refuse it midway, after the voxelizer and the anchor mask ran)."""
+    limit = model.neck.max_batch()
+    if batch > limit:
+        grid = "x".join(map(str, model.neck.sparse_shape))
+        raise ops._lib.SassdError("batch %d exceeds the level-0 hash limit of %d frames: its 31-bit keys flatten "
+                                  "(b, z, y, x) over the %s grid" % (batch, limit, grid))
+
+
 def _crop_step(points, pt_off, batch, planes, meta, image_fov):
     """The crop a step runs first: to the camera frustums of ``planes`` [batch,6,4], to the images of ``meta`` with
     ``image_fov``, or none."""
@@ -904,6 +915,7 @@ def _run_step(model, points, pt_off, batch, maxpts, planes=None, meta=None, poin
     loss vector [6] in aux["losses"] and its targets in aux["targets"]; with ``meta`` [batch,36] the detections are
     formatted as KITTI rows (ops.kitti_format) into aux["rows"] / aux["n_out"].  Returns forward_device's (det, d_ndet,
     status, aux)."""
+    _require_batch(model, batch)
     points, pt_off = _crop_step(points, pt_off, batch, planes, meta, image_fov)
     det, d_ndet, status, aux = model.forward_device(points, pt_off, batch, maxpts,
                                                     point_outputs=point_outputs or gt is not None,
@@ -949,8 +961,9 @@ def _set_step(dset, points, pt_off, batch, maxpts, planes=None, meta=None, point
     members' detections gathered per frame (ops.merge_detections) and, with ``meta``, formatted once as KITTI rows.
     The members share the status word.  Returns (det [batch,det_cap,9], d_ndet, status, aux)."""
     assert not point_outputs and gt is None, "a DetectorSet step has no auxiliary outputs or losses"
-    points, pt_off = _crop_step(points, pt_off, batch, planes, meta, image_fov)
     lead = dset.models[0]
+    _require_batch(lead, batch)
+    points, pt_off = _crop_step(points, pt_off, batch, planes, meta, image_fov)
     status = torch.zeros((1,), dtype=torch.int32, device=points.device)
     vox = lead.voxel_generator.generate_device(points, pt_off, batch, maxpts, status)
     _, coors, _, mean, frame_rows = vox
@@ -973,8 +986,9 @@ def _sweep_step(sweep, points, pt_off, batch, maxpts, planes=None, meta=None, po
     [K*batch], status, aux), the members' blocks one after another, with aux["rows"] / aux["n_out"] likewise and
     aux["losses"] the K loss vectors [K*6]."""
     assert not point_outputs, "a CheckpointSweep step has no auxiliary outputs"
-    points, pt_off = _crop_step(points, pt_off, batch, planes, meta, image_fov)
     lead = sweep.models[0]
+    _require_batch(lead, batch)
+    points, pt_off = _crop_step(points, pt_off, batch, planes, meta, image_fov)
     status = torch.zeros((1,), dtype=torch.int32, device=points.device)
     vox = lead.voxel_generator.generate_device(points, pt_off, batch, maxpts, status)
     _, coors, _, mean, frame_rows = vox

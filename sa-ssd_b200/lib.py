@@ -23,7 +23,7 @@ class Conv2dDesc(ctypes.Structure):
 
 class SpconvDesc(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in ("cin", "cout", "taps", "rows_cap", "in_rows_cap", "relu", "out_ch",
-                                              "out_f32_stride")]
+                                              "out_f32_stride", "fixed_walk")]
 
 
 class GConvDesc(ctypes.Structure):

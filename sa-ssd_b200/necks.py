@@ -222,6 +222,12 @@ class SpMiddleFHD(nn.Module):
         self._side = None
         self._point_packed = None
 
+    def max_batch(self):
+        """The most frames one step can hold: the level-0 hash keys each voxel by its flattened (b, z, y, x) cell in
+        31 bits (sassd_hash_build refuses batch * D * H * W >= 2^31 - 1); 23 on the 40 x 1600 x 1408 grid."""
+        D, H, W = self.sparse_shape
+        return (2147483647 - 1) // (D * H * W)
+
     def _point_weights(self):
         """(point_fc.weight^T [160,64], [point_cls.weight; point_reg.weight] [4,64]) fp32, re-derived when a reload
         changes the parameters (the same version check as BEVNet._weights)."""

@@ -936,6 +936,10 @@ def split_rows_float(planes, channels):
 SPCONV_COUNTERS = None     # bench instrumentation: int32[2] device tensor -> += executed (tile, chunk) pairs, += tiles
 SPCONV_TAP_SKIP = os.environ.get("SASSD_SPS_SKIP", "1") != "0"      # use the rulebook's tile masks
 SPCONV_TAP_SPLIT = os.environ.get("SASSD_SPS_SPLIT", "1") != "0"    # chunk deal over all SMs for layers with few tiles
+# Each tile walks its chunks from a tile-dependent chunk (spreads the weight reads over L2).  A row's summation order
+# then depends on its tile's index, i.e. on the rows of the frames before it in the batch; False walks every tile from
+# chunk 0, which makes each frame's bits independent of its batch (with SPCONV_TAP_SPLIT False too).
+SPCONV_TAP_ROTATE = True
 
 
 def spconv_split(planes, weight, scale, shift, relu, cout, rows_cap, nbr=None, d_rows=None, want_f32=False,
@@ -948,6 +952,7 @@ def spconv_split(planes, weight, scale, shift, relu, cout, rows_cap, nbr=None, d
     d.cin, d.cout, d.taps = planes.shape[2], cout, taps
     d.rows_cap, d.in_rows_cap, d.relu = rows_cap, planes.shape[1], 1 if relu else 0
     d.out_ch = (cout + 7) // 8 * 8
+    d.fixed_walk = 0 if SPCONV_TAP_ROTATE else 1
     out = torch.empty((2, rows_cap, d.out_ch), dtype=torch.float16, device=planes.device)
     of = None
     if want_f32:
