@@ -669,8 +669,10 @@ int sassd_kitti_parse_labels(const uint8_t* buf, const int64_t* file_off, int nf
  *
  * sassd_augment_assemble: per frame, the database rows of its sampled
  * records (records s in [d_srow_off..] order: rows db[d_srec_db[s] ..] of
- * count d_srec_off[s+1] - d_srec_off[s], each x, y, z plus srec_ctr[s] fp64)
- * followed by the rows sassd_augment_drop_points kept; each row then takes
+ * count d_srec_off[s+1] - d_srec_off[s], each x, y, z plus srec_ctr[s] fp64,
+ * then, when srec_dz [n_rec] is not null, z minus srec_dz[s] fp64, rounded
+ * again: the record's move onto the frame's road plane; null: no move, and
+ * a non-null srec_dz needs n_rec > 0) followed by the rows sassd_augment_drop_points kept; each row then takes
  * the transform of the first box whose fp32 planes contain it (centres
  * [boxes][3] fp32, its try sel[k]), the frame's flip, rotation and scale
  * (frame_tf [batch][6]: flip, R00, R01, R10, R11, scale).  More than out_cap
@@ -685,7 +687,7 @@ int sassd_augment_noise_search(const float* boxes, const float* box_trig, const 
                                int32_t* d_status, sassd_stream_t stream);
 int sassd_augment_assemble(const float* kept, const int32_t* d_kept_off, int batch, const int32_t* d_srow_off,
                            const int32_t* d_srec_off, int n_rec, const int32_t* d_srec_db, const double* srec_ctr,
-                           const float* db, const int32_t* d_box_off, const float* planes, const float* centres,
+                           const double* srec_dz, const float* db, const int32_t* d_box_off, const float* planes, const float* centres,
                            const int32_t* sel, int tries, const float* try_trig, const double* loc,
                            const float* frame_tf, int out_cap, float* points_out, int32_t* d_pt_off_out,
                            int32_t* d_status, sassd_stream_t stream);

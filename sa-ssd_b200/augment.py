@@ -3,7 +3,9 @@
 with the per-point work and the noise search on the GPU (csrc/augment.cu).
 
     python -m sassd_b200.augment CONFIG --data-root R [--split train] [--lidar velodyne|velodyne_reduced] [--seed S]
-                                 [--batch B] [--frames K] [--out DIR]
+                                 [--batch B] [--frames K] [--out DIR] [--checkpoint CKPT]
+
+With the config's data.train.with_plane, the driver also reads each frame's training/planes/%06d.txt (read_plane).
 
 Per frame, in order, the host makes the reference's draws on ``rng`` (a np.random.RandomState; numpy's global state by
 default): the database picks of each class's sampler (and the shuffle when a sampler wraps), the location and rotation
@@ -22,8 +24,12 @@ Semantics kept from the reference, as it runs with numba compiled:
   * rotations round as numpy's float32 matmul: out_k = fma(z, R2k, fma(y, R1k, fma(x, R0k, +0))).
 A frame with no box left after the range filter is reported through the keep mask; the caller picks a replacement.
 The reference draws that replacement inside the stream with np.random.choice, so a seeded stream with a rejected frame
-differs from the reference's after that frame.  Road planes (``with_plane``) are not supported.  NaN coordinates come
-out NaN, with the device's NaN bits.
+differs from the reference's after that frame.  NaN coordinates come out NaN, with the device's NaN bits.
+
+Road planes (the reference's ``with_plane``; ``augment(road_planes=, calibs=)``): once a frame's records are picked,
+their boxes move vertically onto its road plane in float64 (plane_shift, the reference's sample_all); the moved float32
+boxes replace the database boxes everywhere after the sampler's collision filter, and the records' points move by the
+same height on the device, rounded after the centre add and again after the move.  No draw changes.
 """
 import argparse
 import ctypes
@@ -143,6 +149,41 @@ def rotation_z32(angle):
     return np.array([[c, -s, 0], [s, c, 0], [0, 0, 1]], dtype=np.float32)
 
 
+def plane_shift(sampled64, plane, calib):
+    """Sampled database boxes [S,7] (their float64 box3d_lidar, in sample order) moved vertically onto the frame's
+    road plane (kitti_data.read_plane's float64 (a, b, c, d), rectified camera frame), as the reference's sample_all
+    does with road_planes (point_augmentor.py:225-245): each centre goes to the camera frame, takes the plane's height
+    there, comes back, and z moves by mv = z - that height.  Returns (boxes [S,7] float32, mv [S] float64); the
+    sampled records' points move by -mv after their centre add."""
+    from .results import project_rect_to_velo, project_velo_to_rect
+    boxes = np.array(sampled64, np.float64).reshape(-1, 7)
+    a, b, c, d = np.asarray(plane, np.float64)
+    center_cam = project_velo_to_rect(boxes[:, 0:3], calib)
+    center_cam[:, 1] = (-d - a * center_cam[:, 0] - c * center_cam[:, 2]) / b
+    cur = project_rect_to_velo(center_cam, calib)[:, 2]
+    mv = boxes[:, 2] - cur
+    boxes[:, 2] -= mv        # not z = cur: z - (z - cur) need not round to cur
+    return boxes.astype(np.float32), mv
+
+
+def check_planes(road_planes, calibs, batch):
+    """augment's road_planes / calibs -> per-frame lists (of None without planes): both None, or both one entry per
+    frame with each plane 4 finite numbers."""
+    if road_planes is None and calibs is None:
+        return [None] * batch, [None] * batch
+    if road_planes is None or calibs is None:
+        raise ValueError("road_planes and calibs go together: pass both or neither")
+    road_planes, calibs = list(road_planes), list(calibs)
+    if len(road_planes) != batch or len(calibs) != batch:
+        raise ValueError("road_planes and calibs need one entry per frame (%d frames; %d planes, %d calibs)"
+                         % (batch, len(road_planes), len(calibs)))
+    for b, p in enumerate(road_planes):
+        p = np.asarray(p)
+        if p.shape != (4,) or not np.issubdtype(p.dtype, np.number) or not np.isfinite(p).all():
+            raise ValueError("frame %d: a road plane is 4 finite numbers (a, b, c, d), not %r" % (b, p))
+    return road_planes, calibs
+
+
 # ---------------------------------------------------------------------------------------------------- augmentor
 class _ClassSampler:
     """The reference's BatchSampler over one class's records: a shuffled index order consumed in runs, reshuffled
@@ -176,7 +217,9 @@ class PointAugmentor:
                  gt_rot_range=None, global_rot_range=None, center_noise_std=None, scale_range=None, rng=None,
                  device="cuda", with_plane=False):
         if with_plane:
-            raise NotImplementedError("road-plane height correction is not supported")
+            raise NotImplementedError("with_plane is a dataset option (data.train.with_plane), not an augmentor "
+                                      "argument: pass each frame's road plane and calibration to "
+                                      "augment(road_planes=, calibs=)")
         if global_rot_range is None or center_noise_std is None or scale_range is None:
             raise ValueError("global_rot_range, center_noise_std and scale_range are required")
         sample_classes = list(sample_classes)
@@ -218,10 +261,12 @@ class PointAugmentor:
         self.db = torch.from_numpy(np.ascontiguousarray(cat if len(cat) else np.zeros((1, 4), np.float32))).to(device)
 
     # -------------------------------------------------------------------------------------------- host, per frame
-    def draw(self, gt_boxes, gt_names, class_names):
+    def draw(self, gt_boxes, gt_names, class_names, plane=None, calib=None):
         """One frame's host part, in the reference's draw order: gt_boxes [G,7] float32 (every non-DontCare label box,
         LiDAR frame) and their raw names.  Returns a dict: the sampled record ids, the selected boxes (float32, before
-        noise), their labels, the noise draws and the frame's flip, rotation and scale."""
+        noise), their labels, the noise draws and the frame's flip, rotation and scale.  With the frame's road
+        ``plane`` and ``calib``, the sampled boxes are plane_shift's (the collision filter has run on the database
+        boxes, as in the reference) and ``mv`` holds each sampled record's height move; otherwise ``mv`` is None."""
         rng = self.rng
         gt_boxes = np.asarray(gt_boxes, np.float32).reshape(-1, 7)
         gt_names = [str(n) for n in gt_names]
@@ -238,6 +283,9 @@ class PointAugmentor:
                 avoid = np.concatenate([avoid, np.stack([self.records[r]["box3d_lidar"] for r in valid], 0)], 0)
         sampled = (np.stack([self.records[r]["box3d_lidar"] for r in picked], 0).astype(np.float32) if picked
                    else np.zeros((0, 7), np.float32))
+        mv = None
+        if plane is not None and picked:
+            sampled, mv = plane_shift(np.stack([self.records[r]["box3d_lidar"] for r in picked], 0), plane, calib)
         boxes = np.concatenate([gt_boxes, sampled], 0)
         names = ["Car" if n == "Van" else n for n in gt_names + [self.records[r]["name"] for r in picked]]
         sel = [i for i, n in enumerate(names) if n in class_names]
@@ -249,7 +297,7 @@ class PointAugmentor:
         flip = bool(rng.choice([False, True], replace=False, p=[0.5, 0.5]))
         angle = rng.uniform(self.global_rot_range[0], self.global_rot_range[1])
         scale = rng.uniform(self.scale_range[0], self.scale_range[1])
-        return dict(records=picked, sampled=sampled, boxes=boxes, labels=labels, loc=loc, rot=rot, flip=flip,
+        return dict(records=picked, sampled=sampled, mv=mv, boxes=boxes, labels=labels, loc=loc, rot=rot, flip=flip,
                     angle=angle, scale=scale)
 
     @staticmethod
@@ -279,24 +327,30 @@ class PointAugmentor:
 
     # -------------------------------------------------------------------------------------------- device, per batch
     def augment(self, points, pt_off, batch, gt_boxes, gt_names, class_names=None, point_cloud_range=DEFAULT_RANGE,
-                max_points=None):
+                max_points=None, road_planes=None, calibs=None):
         """points [Ncap,4] f32 and pt_off [batch+1] i32 on the device (frustum_crop's layout); per frame the
         non-DontCare boxes (float32 [G,7], LiDAR frame) and raw KITTI names.  Returns (points [cap,4], pt_off
         [batch+1], boxes list, labels list, keep [batch] bool, sel list): per frame its GT boxes (float32) and labels
         (int64, 1-based over ``class_names``) after the range filter and limit_period, keep false where the reference
         would reject the frame (no box left), and each selected box's chosen noise try (int32, -1: none), in the order
         of the selected boxes before the range filter.  ``max_points`` (default: the input's rows plus every sampled
-        row) caps the output rows; overflow raises."""
+        row) caps the output rows; overflow raises.
+
+        ``road_planes`` and ``calibs`` (the reference's data.train.with_plane): per frame its road plane
+        (kitti_data.read_plane) and its results.Calibration.  The sampled boxes then sit on the frame's road
+        (plane_shift) for the scene crop, the noise search, the point masks and the returned boxes, and each sampled
+        record's points move by the same height as its box."""
         import torch
         from . import ops
         from .lib import GT_CAP_MAX, raise_on_status
+        road_planes, calibs = check_planes(road_planes, calibs, batch)
         if self.device is None:
             raise ValueError("this augmentor was built without a device database")
         class_names = list(self.sample_classes if class_names is None else class_names)
         if len(gt_boxes) != batch or len(gt_names) != batch:
             raise ValueError("gt_boxes and gt_names need one entry per frame")
         dev = points.device
-        plans = [self.draw(gt_boxes[b], gt_names[b], class_names) for b in range(batch)]
+        plans = [self.draw(gt_boxes[b], gt_names[b], class_names, road_planes[b], calibs[b]) for b in range(batch)]
         for p in plans:
             if len(p["boxes"]) > GT_CAP_MAX:
                 raise ValueError("a frame has %d boxes after sampling; at most %d are supported"
@@ -339,11 +393,14 @@ class PointAugmentor:
                        for p in plans], np.float32)
         out_cap = int(points.shape[0] + srow_off[-1]) if max_points is None else int(max_points)
         srec_db = torch.from_numpy(np.array([self.db_start[r] for r in recs], np.int32)).to(dev)
+        dz = None
+        if recs and road_planes[0] is not None:
+            dz = dev_t(np.concatenate([p["mv"] for p in plans if p["records"]]), np.float64)
         out, out_off = ops.augment_assemble(
             kept, kept_off, batch, dev_t(srow_off, np.int32), dev_t(srec_off, np.int32), srec_db, dev_t(ctr, np.float64),
             self.db, d_box_off, dev_t(np.concatenate([box_planes32(p["boxes"]) for p in plans], 0).reshape(-1, 6, 4),
                                       np.float32),
-            dev_t(boxes[:, :3], np.float32), sel, d_trig, d_loc, dev_t(tf, np.float32), out_cap, status)
+            dev_t(boxes[:, :3], np.float32), sel, d_trig, d_loc, dev_t(tf, np.float32), out_cap, status, dz=dz)
         sel_h = sel.cpu().numpy()
         raise_on_status(int(status.cpu()))
         sels = [sel_h[box_off[b]:box_off[b + 1]].copy() for b in range(batch)]
@@ -384,10 +441,11 @@ def main(argv=None):
         ap.error("--batch must be >= 1")
     import torch
     from . import Config, ops
-    from .kitti_data import KittiSplit, Prefetcher, labelled_boxes, read_label
+    from .kitti_data import KittiSplit, Prefetcher, labelled_boxes, read_label, read_plane
     cfg = Config.fromfile(args.config)
     if "train" not in cfg.data:
         ap.error("%s has no data.train section" % args.config)
+    with_plane = bool(cfg.data["train"].get("with_plane", False))
     class_names = list(cfg.data["train"].get("class_names", cfg.data["val"]["class_names"]))
     pc_range = cfg.data["train"]["generator"]["point_cloud_range"]
     if args.seed is not None:
@@ -410,7 +468,10 @@ def main(argv=None):
     class _Labelled:
         def frame(self, idx):
             pts, meta = split.frame(idx)
-            return pts, meta, labelled_boxes(read_label(split.path("label_2", idx, "txt")), meta["calib"])
+            gt = labelled_boxes(read_label(split.path("label_2", idx, "txt")), meta["calib"])
+            if with_plane:
+                return pts, meta, gt, read_plane(split.path("planes", idx, "txt"))
+            return pts, meta, gt
 
         def pad_frame(self):
             raise AssertionError("frames are not padded")
@@ -419,7 +480,7 @@ def main(argv=None):
     if args.out:
         os.makedirs(args.out, exist_ok=True)
     n_frames, n_kept, t0 = 0, 0, time.perf_counter()
-    for bids, pts, metas, gts in pf:
+    for bids, pts, metas, gts, *road in pf:
         B = len(bids)
         off = np.concatenate([[0], np.cumsum([len(p) for p in pts])]).astype(np.int32)
         d_pts = torch.from_numpy(np.concatenate(pts, 0) if off[-1] else np.zeros((1, 4), np.float32)).to(dev)
@@ -427,8 +488,9 @@ def main(argv=None):
         if args.lidar == "velodyne":
             planes = np.stack([split.planes(m["calib"], m["img_shape"]) for m in metas])
             d_pts, d_off = ops.frustum_crop(d_pts, d_off, B, torch.from_numpy(planes).to(dev))
-        out, out_off, boxes, lbls, keep, _ = aug.augment(d_pts, d_off, B, [g[0] for g in gts], [g[1] for g in gts],
-                                                         class_names, pc_range)
+        out, out_off, boxes, lbls, keep, _ = aug.augment(
+            d_pts, d_off, B, [g[0] for g in gts], [g[1] for g in gts], class_names, pc_range,
+            road_planes=road[0] if with_plane else None, calibs=[m["calib"] for m in metas] if with_plane else None)
         n_frames += B
         n_kept += int(keep.sum())
         if args.out or (model is not None and keep.any()):

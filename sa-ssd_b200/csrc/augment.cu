@@ -150,14 +150,16 @@ extern "C" int sassd_augment_noise_search(const float* boxes, const float* box_t
     return sassd_check_launch();
 }
 
-// The augmented cloud: per frame, the sampled records' database rows (sample order, each plus its box centre) and then
-// the scene rows the crop kept.  Each row then takes the transform of the first box (in box order) whose fp32 planes
-// contain it (points_transform_: -centre, the noise rotation, +centre, +location noise; a box without a successful try
-// rotates by 0), the frame's flip of y, its global rotation and its scaling.
+// The augmented cloud: per frame, the sampled records' database rows (sample order, each plus its box centre; with
+// srec_dz, z then minus srec_dz[s], the box's move onto the frame's road plane, rounded again as numpy's
+// `f32_array[:, 2] -= f64` does) and then the scene rows the crop kept.  Each row then takes the transform of the first
+// box (in box order) whose fp32 planes contain it (points_transform_: -centre, the noise rotation, +centre, +location
+// noise; a box without a successful try rotates by 0), the frame's flip of y, its global rotation and its scaling.
 __global__ void __launch_bounds__(AUG_THREADS)
 aug_assemble_kernel(const float4* __restrict__ kept, const int* __restrict__ kept_off, int batch,
                     const int* __restrict__ srow_off, const int* __restrict__ srec_off, int n_rec,
-                    const int* __restrict__ srec_db, const double* __restrict__ srec_ctr, const float4* __restrict__ db,
+                    const int* __restrict__ srec_db, const double* __restrict__ srec_ctr,
+                    const double* __restrict__ srec_dz, const float4* __restrict__ db,
                     const int* __restrict__ box_off, const float* __restrict__ planes, const float* __restrict__ centres,
                     const int* __restrict__ sel, int tries, const float* __restrict__ try_trig,
                     const double* __restrict__ loc, const float* __restrict__ frame_tf, int out_cap,
@@ -181,6 +183,7 @@ aug_assemble_kernel(const float4* __restrict__ kept, const int* __restrict__ kep
             p.x = aug_addd(p.x, __ldg(&srec_ctr[3 * s]));
             p.y = aug_addd(p.y, __ldg(&srec_ctr[3 * s + 1]));
             p.z = aug_addd(p.z, __ldg(&srec_ctr[3 * s + 2]));
+            if (srec_dz) p.z = aug_addd(p.z, -__ldg(&srec_dz[s]));
         } else {
             p = __ldg(&kept[__ldg(&kept_off[b]) + q - ns]);
         }
@@ -214,7 +217,8 @@ aug_assemble_kernel(const float4* __restrict__ kept, const int* __restrict__ kep
 
 extern "C" int sassd_augment_assemble(const float* kept, const int32_t* d_kept_off, int batch, const int32_t* d_srow_off,
                                       const int32_t* d_srec_off, int n_rec, const int32_t* d_srec_db,
-                                      const double* srec_ctr, const float* db, const int32_t* d_box_off,
+                                      const double* srec_ctr, const double* srec_dz, const float* db,
+                                      const int32_t* d_box_off,
                                       const float* planes, const float* centres, const int32_t* sel, int tries,
                                       const float* try_trig, const double* loc, const float* frame_tf, int out_cap,
                                       float* points_out, int32_t* d_pt_off_out, int32_t* d_status,
@@ -225,11 +229,12 @@ extern "C" int sassd_augment_assemble(const float* kept, const int32_t* d_kept_o
     if (batch < 1 || batch > AUG_MAX_BATCH || n_rec < 0 || tries < 1 || tries > AUG_TRIES_MAX || out_cap < 0)
         return SASSD_ERR_ARG;
     if (n_rec > 0 && (!d_srec_db || !srec_ctr || !db)) return SASSD_ERR_ARG;
+    if (srec_dz && n_rec == 0) return SASSD_ERR_ARG;
     if (points_out == kept) return SASSD_ERR_ARG;
     const int grid = sassd_grid(out_cap, AUG_THREADS, 4);
     aug_assemble_kernel<<<grid, AUG_THREADS, 0, (cudaStream_t)stream>>>(
-        (const float4*)kept, d_kept_off, batch, d_srow_off, d_srec_off, n_rec, d_srec_db, srec_ctr, (const float4*)db,
-        d_box_off, planes, centres, sel, tries, try_trig, loc, frame_tf, out_cap, (float4*)points_out, d_pt_off_out,
-        d_status);
+        (const float4*)kept, d_kept_off, batch, d_srow_off, d_srec_off, n_rec, d_srec_db, srec_ctr, srec_dz,
+        (const float4*)db, d_box_off, planes, centres, sel, tries, try_trig, loc, frame_tf, out_cap,
+        (float4*)points_out, d_pt_off_out, d_status);
     return sassd_check_launch();
 }

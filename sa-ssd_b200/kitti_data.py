@@ -59,6 +59,23 @@ def read_points(path):
     return np.fromfile(path, dtype=np.float32).reshape(-1, 4)
 
 
+def read_plane(path):
+    """One ``planes/%06d.txt`` road plane (the format AVOD ships for KITTI: three header lines, then ``a b c d`` of
+    a x + b y + c z + d = 0 in the rectified camera frame) -> float64 [4], as the reference's get_road_plane
+    (kitti.py:96-108): the normal turned up (negated when b > 0), then the whole vector divided by the normal's
+    length."""
+    if not os.path.isfile(path):
+        raise FileNotFoundError("road plane file %s not found" % path)
+    with open(path) as fh:
+        lines = fh.readlines()
+    if len(lines) < 4:
+        raise ValueError("%s: a road plane file has its coefficients on line 4" % path)
+    plane = np.asarray([float(v) for v in lines[3].split()])
+    if plane[1] > 0:
+        plane = -plane
+    return plane / np.linalg.norm(plane[0:3])
+
+
 def read_label(path):
     """One ``label_2`` file -> ground-truth annotation dict (get_label_anno's semantics).
 

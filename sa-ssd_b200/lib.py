@@ -75,8 +75,8 @@ _SIGNATURES = {
     "sassd_points_in_rbboxes": (c_int, [P, P, c_int, c_int, P, P, P, c_int, P, P, P, c_int, P, P, c_size_t, P]),
     "sassd_augment_drop_points": (c_int, [P, P, c_int, c_int, P, P, P, P, P, c_size_t, P]),
     "sassd_augment_noise_search": (c_int, [P, P, P, c_int, c_int, P, P, P, P, P]),
-    "sassd_augment_assemble": (c_int, [P, P, c_int, P, P, c_int, P, P, P, P, P, P, P, c_int, P, P, P, c_int, P, P, P,
-                                       P]),
+    "sassd_augment_assemble": (c_int, [P, P, c_int, P, P, c_int, P, P, P, P, P, P, P, P, c_int, P, P, P, c_int, P, P,
+                                       P, P]),
     "sassd_anchor_mask_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "sassd_anchor_mask": (c_int, [P, P, c_int, c_int, c_int, c_int, P, c_int, c_int, P, P, c_size_t, P]),
     "sassd_hash_build": (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, P]),

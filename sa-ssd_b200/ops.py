@@ -216,15 +216,18 @@ def augment_noise_search(boxes, box_trig, box_off, batch, try_trig, loc, status)
 
 
 def augment_assemble(kept, kept_off, batch, srow_off, srec_off, srec_db, srec_ctr, db, box_off, planes, centres, sel,
-                     try_trig, loc, frame_tf, out_cap, status):
+                     try_trig, loc, frame_tf, out_cap, status, dz=None):
     """The augmented cloud of every frame: its sampled database rows, then the kept scene rows, each moved by its box's
-    noise and the frame's flip, rotation and scaling (csrc/augment.cu).  Returns (points [out_cap,4], pt_off
-    [batch+1]); POINTS_CAP in ``status`` when the rows exceed out_cap."""
+    noise and the frame's flip, rotation and scaling (csrc/augment.cu).  ``dz`` [records] f64 (optional): each sampled
+    record's height move onto its frame's road plane, subtracted from its rows' z after the centre add.  Returns
+    (points [out_cap,4], pt_off [batch+1]); POINTS_CAP in ``status`` when the rows exceed out_cap."""
+    if dz is not None:
+        assert dz.dtype == torch.float64 and dz.numel() >= srec_db.numel(), "dz must be float64 [records]"
     dev = kept.device
     out = torch.empty((max(int(out_cap), 1), 4), dtype=torch.float32, device=dev)
     off = torch.empty((batch + 1,), dtype=torch.int32, device=dev)
     _call("sassd_augment_assemble", None, _ptr(kept), _ptr(kept_off), batch, _ptr(srow_off), _ptr(srec_off),
-          srec_db.numel(), _ptr(srec_db), _ptr(srec_ctr), _ptr(db), _ptr(box_off), _ptr(planes), _ptr(centres),
+          srec_db.numel(), _ptr(srec_db), _ptr(srec_ctr), _ptr(dz), _ptr(db), _ptr(box_off), _ptr(planes), _ptr(centres),
           _ptr(sel), loc.shape[1], _ptr(try_trig), _ptr(loc), _ptr(frame_tf), int(out_cap), _ptr(out), _ptr(off),
           _ptr(status), _stream())
     return out, off
