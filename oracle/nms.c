@@ -82,7 +82,9 @@ static inline pt_t rot_about(pt_t ctr, float c, float s, pt_t p)
     return r;
 }
 
-float oracle_box_overlap(const float *a, const float *b)
+/* The reference keeps 16 polygon points; this restatement has room for every point the loops can add (16 edge
+ * hits and 8 corners) so that it can report a pair that would need more (*count), without writing out of bounds. */
+static float box_overlap_count(const float *a, const float *b, int *count)
 {
     pt_t ca = { (a[0] + a[2]) / 2, (a[1] + a[3]) / 2 };
     pt_t cb = { (b[0] + b[2]) / 2, (b[1] + b[3]) / 2 };
@@ -97,7 +99,7 @@ float oracle_box_overlap(const float *a, const float *b)
     A[4] = A[0];
     B[4] = B[0];
 
-    pt_t poly[16];
+    pt_t poly[24];
     pt_t ctr = { 0.f, 0.f };
     int cnt = 0;
     for (int i = 0; i < 4; ++i)
@@ -117,6 +119,7 @@ float oracle_box_overlap(const float *a, const float *b)
             poly[cnt++] = A[k];
         }
     }
+    *count = cnt;
     ctr.x /= cnt;
     ctr.y /= cnt;
     /* bubble sort, ascending polar angle about the centroid (iou3d_kernel.cu:183-193) */
@@ -133,6 +136,18 @@ float oracle_box_overlap(const float *a, const float *b)
         area += cross2(u, v);
     }
     return fabsf(area) / 2.0f;
+}
+
+float oracle_box_overlap(const float *a, const float *b)
+{
+    int cnt;
+    return box_overlap_count(a, b, &cnt);
+}
+
+/* polygon point count of each pair (a[i], b[i]), i < n: the reference's box_overlap needs cnt <= 16 */
+void oracle_overlap_points(const float *a, const float *b, int n, int32_t *count)
+{
+    for (int i = 0; i < n; ++i) box_overlap_count(a + (size_t)i * 5, b + (size_t)i * 5, &count[i]);
 }
 
 float oracle_iou_bev(const float *a, const float *b)

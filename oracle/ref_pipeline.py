@@ -453,6 +453,17 @@ def nms_mask(boxes_sorted, thr):
     return mask[:, :cb]
 
 
+def overlap_points(a, b):
+    """polygon point count of box_overlap(a[i], b[i]) for BEV box pairs [n,5]: the reference keeps at most 16"""
+    a = np.ascontiguousarray(a, np.float32)
+    b = np.ascontiguousarray(b, np.float32)
+    assert a.shape == b.shape and a.shape[-1] == 5
+    out = np.zeros((a.shape[0],), np.int32)
+    if len(out):
+        lib().oracle_overlap_points(_p(a, ctypes.c_float), _p(b, ctypes.c_float), len(out), _p(out, ctypes.c_int32))
+    return out
+
+
 def iou_matrix(boxes):
     b = np.ascontiguousarray(boxes, np.float32)
     n = b.shape[0]

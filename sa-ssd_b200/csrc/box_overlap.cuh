@@ -87,14 +87,16 @@ __device__ float rotated_overlap(const float* box_a, const float* box_b) {
                 pc.y = pc.y + poly[cnt].y;
                 cnt++;
             }
+    // 16 edge pairs give at most 16 points; a contained corner past them would write beyond poly[16] (the
+    // reference's behaviour is undefined there), so it is dropped.  No pair within the bound changes.
     for (int k = 0; k < 4; k++) {
-        if (point_in_box(box_a, cb[k])) {
+        if (cnt < 16 && point_in_box(box_a, cb[k])) {
             pc.x = pc.x + cb[k].x;
             pc.y = pc.y + cb[k].y;
             poly[cnt] = cb[k];
             cnt++;
         }
-        if (point_in_box(box_b, ca[k])) {
+        if (cnt < 16 && point_in_box(box_b, ca[k])) {
             pc.x = pc.x + ca[k].x;
             pc.y = pc.y + ca[k].y;
             poly[cnt] = ca[k];

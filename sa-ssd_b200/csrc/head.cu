@@ -25,7 +25,8 @@ __device__ __forceinline__ void anchor_decompose(const HeadLayout& L, int a, int
     pix = t - cls_a * hw;
 }
 
-// max_c sigmoid(cls logits) and its argmax (first maximum on ties, like torch.max on CPU)
+// max_c sigmoid(cls logits) and its argmax like torch.max on CPU: the first maximum on ties, and the first NaN wins
+// both the value and the index (so a NaN class score is never selected: NaN > thr is false)
 __device__ __forceinline__ float anchor_score(const HeadLayout& L, const float* __restrict__ head_b, int a, int& label) {
     int cls_a, pix, rot;
     anchor_decompose(L, a, cls_a, pix, rot);
@@ -34,7 +35,7 @@ __device__ __forceinline__ float anchor_score(const HeadLayout& L, const float* 
     label = 0;
     for (int c = 1; c < L.ncls; ++c) {
         const float s = sigmoidf_(__ldg(p + c));
-        if (s > best) { best = s; label = c; }
+        if (s > best || (s != s && best == best)) { best = s; label = c; }
     }
     return best;
 }
@@ -124,9 +125,11 @@ ds_emit_kernel(const float* __restrict__ head, HeadLayout L, const float* __rest
             const float hg = __fmul_rn(expf(__ldg(e + 5)), ha);
             float rg = __fadd_rn(__ldg(e + 6), ra);
             zg = __fsub_rn(zg, __fdiv_rn(hg, 2.f));
-            // direction classifier: dir_label = argmax (first max on ties); flip when (r > 0) != dir_label
+            // direction classifier: dir_label = torch.max's argmax (first max on ties, the first NaN wins); flip when
+            // (r > 0) != dir_label
             const float* dp = px + L.dir_off + cls_a * 4 + rot * 2;
-            const bool dir_label = __ldg(dp + 1) > __ldg(dp + 0);
+            const float d0 = __ldg(dp + 0), d1 = __ldg(dp + 1);
+            const bool dir_label = d0 == d0 && (d1 > d0 || d1 != d1);
             if ((rg > 0.f) != dir_label) rg = __fadd_rn(rg, 3.14159274101257324f);
             float* ob = boxes + ((size_t)b * k_cap + pos) * 7;
             ob[0] = xg; ob[1] = yg; ob[2] = zg; ob[3] = wg; ob[4] = lg; ob[5] = hg; ob[6] = rg;
@@ -200,16 +203,23 @@ pswarp_kernel(const float* __restrict__ feat, int stride, int H, int W, const fl
             const float fx = floorf(ix), fy = floorf(iy);
             const float w_e = __fsub_rn(ix, fx), w_w = __fsub_rn(1.f, w_e);
             const float w_s = __fsub_rn(iy, fy), w_n = __fsub_rn(1.f, w_s);
-            const int x0 = (int)fx, y0 = (int)fy, x1 = x0 + 1, y1 = y0 + 1;
-            const bool vx0 = x0 >= 0 && x0 < W, vx1 = x1 >= 0 && x1 < W;
-            const bool vy0 = y0 >= 0 && y0 < H, vy1 = y1 >= 0 && y1 < H;
+            // Each tap's validity is decided on the floats (false for NaN), and only a valid tap's corner is converted
+            // to int: converting an out-of-range float is undefined, and an int x0 + 1 may wrap (x0 = INT_MAX gave
+            // x1 = INT_MIN, which passed x1 >= 0 once the compiler rewrote it as x0 > -2).  Off the map a tap adds
+            // exactly 0, however far off it is.
+            const bool vx0 = fx >= 0.f && fx < (float)W, vx1 = fx >= -1.f && fx < (float)(W - 1);
+            const bool vy0 = fy >= 0.f && fy < (float)H, vy1 = fy >= -1.f && fy < (float)(H - 1);
+            const int x0 = vx0 || vx1 ? (int)fx : 0, y0 = vy0 || vy1 ? (int)fy : 0, x1 = x0 + 1, y1 = y0 + 1;
             const float* fp = feat_b + lane;
             float acc = 0.f;
             if (vy0 && vx0) acc = __fadd_rn(acc, __fmul_rn(__ldg(fp + ((size_t)y0 * W + x0) * stride), __fmul_rn(w_n, w_w)));
             if (vy0 && vx1) acc = __fadd_rn(acc, __fmul_rn(__ldg(fp + ((size_t)y0 * W + x1) * stride), __fmul_rn(w_n, w_e)));
             if (vy1 && vx0) acc = __fadd_rn(acc, __fmul_rn(__ldg(fp + ((size_t)y1 * W + x0) * stride), __fmul_rn(w_s, w_w)));
             if (vy1 && vx1) acc = __fadd_rn(acc, __fmul_rn(__ldg(fp + ((size_t)y1 * W + x1) * stride), __fmul_rn(w_s, w_e)));
-            val = acc;
+            // A non-finite sample coordinate (a box with an infinite or NaN centre, size or yaw) has no position on
+            // the map: the part is NaN, so the box's score is NaN and the rescoring threshold drops it.  The float
+            // predicates above alone would give it 0, a finite score.
+            val = isfinite(ix) && isfinite(iy) ? acc : __int_as_float(0x7fc00000);
         }
 #pragma unroll
         for (int d = 16; d > 0; d >>= 1) val += __shfl_down_sync(0xffffffffu, val, d);

@@ -135,16 +135,25 @@ __device__ __forceinline__ void bev_box(const float* b, float* q) {
     q[4] = b[6];
 }
 
+// torch.min / torch.max / torch.clamp: a NaN operand gives NaN (fminf / fmaxf would return the other operand)
+__device__ __forceinline__ float min_nan(float x, float y) {
+    return x != x || y != y ? __int_as_float(0x7fffffff) : fminf(x, y);
+}
+__device__ __forceinline__ float max_nan(float x, float y) {
+    return x != x || y != y ? __int_as_float(0x7fffffff) : fmaxf(x, y);
+}
+
 // boxes_iou3d_gpu (iou3d_utils.py:79-111): rotated BEV overlap (box_overlap) x bottom-based height overlap over
 // clamp(vol_a + vol_b - overlap, 1e-7).  a = the box being assigned, g = the GT (the reference's argument order).
+// The guided boxes come from the weights, so a NaN in one must give the reference's NaN IoU.
 __device__ __forceinline__ float iou3d(const float* a, const float* qa, const float* g, const float* qg) {
     const float bev = rotated_overlap(qa, qg);
-    const float top = fminf(__fadd_rn(a[2], a[5]), __fadd_rn(g[2], g[5]));
-    const float oh = fmaxf(__fsub_rn(top, fmaxf(a[2], g[2])), 0.f);
+    const float top = min_nan(__fadd_rn(a[2], a[5]), __fadd_rn(g[2], g[5]));
+    const float oh = max_nan(__fsub_rn(top, max_nan(a[2], g[2])), 0.f);
     const float ov = __fmul_rn(bev, oh);
     const float va = __fmul_rn(__fmul_rn(a[3], a[4]), a[5]);
     const float vg = __fmul_rn(__fmul_rn(g[3], g[4]), g[5]);
-    return __fdiv_rn(ov, fmaxf(__fsub_rn(__fadd_rn(va, vg), ov), 1e-7f));
+    return __fdiv_rn(ov, max_nan(__fsub_rn(__fadd_rn(va, vg), ov), 1e-7f));
 }
 
 // second_box_encode (ssd_rotate_head.py:15-51) in fp32: z to the centre, offsets over the anchor diagonal, log sizes.
@@ -217,9 +226,13 @@ __global__ void __launch_bounds__(kThreads) assign_kernel(const AssignParams p, 
         for (int j = 0; j < ngt; ++j) {
             if (s_cls[j] != c) continue;
             const float v = p.mode == 0 ? near_iou(qa, s_q + j * 5) : iou3d(ab, qa, s_gt + j * 7, s_q + j * 5);
-            if (arg < 0 || v > best) { best = v; arg = j; }     // argmax: the first maximum
+            // argmax: the first maximum, and as in torch.max the first NaN wins (a NaN maximum is neither >= pos nor
+            // < neg, so the box is ignored unless forced)
+            if (arg < 0 || v > best || (v != v && best == best)) { best = v; arg = j; }
             if (phase == 0) {
-                if (v > 0.f) atomicMax(&s_max[j], __float_as_int(v));
+                // a NaN IoU makes the GT's maximum NaN (0x7fffffff is above every other float's bits), so that GT
+                // forces nothing, as gt_max == overlaps never holds for NaN in the reference
+                if (v > 0.f || v != v) atomicMax(&s_max[j], v != v ? 0x7fffffff : __float_as_int(v));
             } else {
                 // a GT whose maximum is 0 gets -1 (target_ops.py:211-212) and forces nothing
                 const int m = s_max[j];
