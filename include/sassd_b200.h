@@ -55,8 +55,15 @@ enum { /* bits of *d_status */
                                    (sassd_points_in_boxes, sassd_assign_*, sassd_points_in_rbboxes) */
     SASSD_FLAG_GATHER_CAP = 128, /* gathered rows exceed gather_cap: rows past it are not written
                                    (sassd_points_in_rbboxes) */
-    SASSD_FLAG_POINTS_CAP = 256 /* augmented rows exceed out_cap: rows past it are not written
+    SASSD_FLAG_POINTS_CAP = 256, /* augmented rows exceed out_cap: rows past it are not written
                                    (sassd_augment_assemble) */
+    SASSD_FLAG_F16_RANGE = 512  /* a finite value at or above 65520 in magnitude was split into fp16 planes: its hi half is
+                                   +-inf and its lo half -+inf, so every output that reads it becomes NaN.  Set by the
+                                   split stores of the *_status entry points (sassd_conv2d_f16x3_occ_bg_status,
+                                   sassd_spconv_f16x3_status, sassd_features_to_split_status,
+                                   sassd_sparse_to_bev_split_status, and sassd_gconv_status's on-the-fly input split at
+                                   SASSD_PREC_F16X3); values that are already inf or NaN do not set it.  The FP32 and
+                                   TF32X3 precisions have fp32's range */
 };
 
 int sassd_version(void);
@@ -232,7 +239,8 @@ int sassd_rulebook_pairs(const int32_t* nbr, const int32_t* d_rows_out, int rows
  * mode ROWS  : taps == 1, row(m,0) = m                (1x1 convs / plain GEMM)
  * weight [taps, Cin, Cout] f32; scale/shift [Cout] (folded BatchNorm or bias); Cin % 4 == 0.
  * precision: SASSD_PREC_FP32 = CUDA-core FFMA; SASSD_PREC_TF32X3 / SASSD_PREC_F16X3 = Hopper tensor cores (wgmma) with a
- * 3-product hi/lo split of both operands (tf32: 21 bits, any range; fp16: 22 bits, |x| < 65504, 2x the MMA rate).
+ * 3-product hi/lo split of both operands (tf32: 21 bits, any range; fp16: 22 bits, |x| < 65520, 2x the MMA rate).
+ * With relu a NaN output stays NaN (as torch.relu).
  * ---------------------------------------------------------------------- */
 enum { SASSD_GCONV_TABLE = 0, SASSD_GCONV_CONV2D = 1, SASSD_GCONV_ROWS = 2 };
 enum { SASSD_PREC_FP32 = 0, SASSD_PREC_TF32X3 = 1, SASSD_PREC_F16X3 = 2 };
@@ -246,6 +254,11 @@ typedef struct {
 } sassd_gconv_desc;
 int sassd_gconv(const sassd_gconv_desc* host_desc, const float* in, const float* weight, const float* scale,
                 const float* shift, const int32_t* nbr, const int32_t* d_rows, float* out, sassd_stream_t stream);
+/* Same, with a status word (nullable): SASSD_PREC_F16X3 sets SASSD_FLAG_F16_RANGE in it when an input value overflows
+ * the split. */
+int sassd_gconv_status(const sassd_gconv_desc* host_desc, const float* in, const float* weight, const float* scale,
+                       const float* shift, const int32_t* nbr, const int32_t* d_rows, float* out, int32_t* d_status,
+                       sassd_stream_t stream);
 
 /* The tensor-core precisions take their weights pre-split (hi / lo) and pre-swizzled for the shared-memory
  * operand layout: pack once per layer with sassd_gconv_pack (weight [taps,cin,cout] fp32 -> packed,
@@ -259,7 +272,8 @@ int sassd_gconv_pack(const float* weight, int taps, int cin, int cout, int preci
  * moved by TMA (cp.async.bulk.tensor) instead of producer warps.  A split map is two fp16 planes
  * [2][batch][H][W][C] (C % 64 == 0): hi = half(x), lo = half((x - hi) * 2048).  Outputs: fp32 NHWC
  * (out_f32, stride out_f32_stride) and/or the next layer's split map (out_split, out_split_ch channels, the
- * channels beyond cout written as zero).  wpack: sassd_conv2d_pack.  16 < cout <= 256. */
+ * channels beyond cout written as zero).  wpack: sassd_conv2d_pack.  16 < cout <= 256.  With relu a NaN output stays
+ * NaN (as torch.relu). */
 /* The weight pack of sassd_conv2d_f16x3*: weight [taps,cin,cout] fp32 -> packed (sassd_conv2d_pack_bytes bytes, 0 for
  * an unsupported shape).  cout <= 64: the SASSD_PREC_F16X3 pack of sassd_gconv_pack; cout > 64: the hi / lo fp16
  * weights in the register-fragment order of the kernel's wgmma A operand.  taps 9 or 1. */
@@ -309,10 +323,20 @@ int sassd_conv2d_f16x3_occ_bg(const sassd_conv2d_desc* host_desc, const void* in
                               const float* scale, const float* shift, float* out_f32, void* out_split,
                               const int32_t* tile_dist, int reach, const float* const_out, const void* bg_split,
                               const float* bg_f32, int32_t* counters, sassd_stream_t stream);
+/* Same, with a status word (nullable; the three entry points above pass NULL): SASSD_FLAG_F16_RANGE is set when an
+ * output stored into out_split overflows the split (|x| >= 65520). */
+int sassd_conv2d_f16x3_occ_bg_status(const sassd_conv2d_desc* host_desc, const void* in_split, const void* wpack,
+                                     const float* scale, const float* shift, float* out_f32, void* out_split,
+                                     const int32_t* tile_dist, int reach, const float* const_out, const void* bg_split,
+                                     const float* bg_f32, int32_t* counters, int32_t* d_status, sassd_stream_t stream);
 /* dense() of the last sparse tensor straight into a (pre-zeroed) split map [2,batch,H,W,D*C]. */
 int sassd_sparse_to_bev_split(const float* feat, const int32_t* coors, const int32_t* d_rows, int rows_cap, int C,
                               int D, int H, int W, int batch, void* bev_split, int32_t* tile_dist,
                               sassd_stream_t stream);   /* tile_dist: optional, pre-filled with a large value, see above */
+/* Same, with a status word (nullable): SASSD_FLAG_F16_RANGE when a finite input has |x| >= 65520. */
+int sassd_sparse_to_bev_split_status(const float* feat, const int32_t* coors, const int32_t* d_rows, int rows_cap,
+                                     int C, int D, int H, int W, int batch, void* bev_split, int32_t* tile_dist,
+                                     int32_t* d_status, sassd_stream_t stream);
 
 /* Ruled sparse conv on "split rows" (two fp16 planes [2][rows][C], C % 8 == 0; hi = half(x), lo = half((x-hi)*2048)):
  * same semantics as sassd_gconv TABLE / ROWS mode with SASSD_PREC_F16X3, but the gather is 16-byte cp.async copies
@@ -338,16 +362,26 @@ int sassd_spconv_pack(const float* weight, int taps, int cin, int cin_stored, in
  * the same time): with it, a layer that has at most as many tiles as CTAs, and whose longest tile would otherwise
  * dominate, deals its tiles' active K chunks evenly over all CTAs; the fp32 partial sums of tiles cut between CTAs and the counters that pick the CTA finishing each tile live
  * in it, and every call leaves the counters zero again.  Without it, one CTA per tile.
- * counters (optional, int32[2], caller-zeroed): += executed (tile, chunk) pairs, += tiles (instrumentation). */
+ * counters (optional, int32[2], caller-zeroed): += executed (tile, chunk) pairs, += tiles (instrumentation).
+ * With relu a NaN output stays NaN (as torch.relu); the columns >= cout are written as exact zeros whatever the inputs
+ * hold. */
 #define SASSD_SPCONV_TILE_ROWS 128
 size_t sassd_spconv_workspace_bytes(void);
 int sassd_spconv_f16x3(const sassd_spconv_desc* host_desc, const void* in_split, const void* wpack, const float* scale,
                        const float* shift, const int32_t* nbr, const int32_t* tile_mask, const int32_t* d_rows,
                        void* out_split, float* out_f32, void* ws, size_t ws_bytes, int32_t* counters,
                        sassd_stream_t stream);
+/* Same, with a status word (nullable): SASSD_FLAG_F16_RANGE when an output stored into out_split overflows the split. */
+int sassd_spconv_f16x3_status(const sassd_spconv_desc* host_desc, const void* in_split, const void* wpack,
+                              const float* scale, const float* shift, const int32_t* nbr, const int32_t* tile_mask,
+                              const int32_t* d_rows, void* out_split, float* out_f32, void* ws, size_t ws_bytes,
+                              int32_t* counters, int32_t* d_status, sassd_stream_t stream);
 /* fp32 rows [rows, cin] -> split rows [2][rows_cap][cs] (cs >= cin, cs % 8 == 0, padding zero). */
 int sassd_features_to_split(const float* feat, const int32_t* d_rows, int rows_cap, int cin, int cs, void* out_split,
                             sassd_stream_t stream);
+/* Same, with a status word (nullable): SASSD_FLAG_F16_RANGE when a finite input has |x| >= 65520. */
+int sassd_features_to_split_status(const float* feat, const int32_t* d_rows, int rows_cap, int cin, int cs,
+                                   void* out_split, int32_t* d_status, sassd_stream_t stream);
 /* dense() of split rows into a (pre-zeroed) split BEV map [2,batch,H,W,D*C]. */
 int sassd_split_rows_to_bev(const void* feat_split, const int32_t* coors, const int32_t* d_rows, int rows_cap, int C,
                             int D, int H, int W, int batch, void* bev_split, int32_t* tile_dist, sassd_stream_t stream);

@@ -37,6 +37,14 @@ static inline int sassd_grid(long long work, int block, int ctas_per_sm = 8) {
     return (int)(need < cap ? need : cap);
 }
 
+// The convs' ReLU.  max.NaN returns NaN when an operand is NaN (as torch.relu; fmaxf would return 0) and the same bits
+// as fmaxf(o, 0) for every other value, in one instruction.
+__device__ __forceinline__ float sassd_relu(float o) {
+    float r;
+    asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(o));
+    return r;
+}
+
 // Frame of point i of concatenated frames: the b with off[b] <= i < off[b+1] (off in shared memory, off[0] <= i).
 __device__ __forceinline__ int sassd_frame_of(const int* s_off, int batch, int i) {
     int lo = 0, hi = batch;

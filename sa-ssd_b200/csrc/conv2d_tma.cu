@@ -94,6 +94,7 @@ struct Conv2dArgs {
     int tile_order;       // 1: computed tiles first, 0: round-robin
     int nsplit;           // work units per tile: 1, or 2 = each unit computes BN of the 2*BN output channels (the weight
                           // pack is the 2*BN-wide one)
+    int* status;          // optional: SASSD_FLAG_F16_RANGE when a value stored into out_split overflows the split
 };
 
 // Optional: the layer's outputs on an empty scene, batch 1 (same H, W, strides), copied into the far border tiles.
@@ -162,6 +163,8 @@ __device__ __forceinline__ void store_constant_unit(const Conv2dArgs& p, int b, 
     split_f16x2(v[2], v[3], hi.y, lo.y);
     split_f16x2(v[4], v[5], hi.z, lo.z);
     split_f16x2(v[6], v[7], hi.w, lo.w);
+    F16Range ovf;
+    ovf.add(lo.x); ovf.add(lo.y); ovf.add(lo.z); ovf.add(lo.w);
     const size_t plane = (size_t)p.batch * p.H * p.W * p.out_split_ch;
 #pragma unroll 4
     for (int pg = warp; pg * ppi < TILE_H * TILE_W; pg += EW) {
@@ -173,6 +176,7 @@ __device__ __forceinline__ void store_constant_unit(const Conv2dArgs& p, int b, 
             *(uint4*)(dst + plane) = lo;
         }
     }
+    report_f16_range(p.status, ovf.overflowed());
 }
 
 // Zeros in the stored channels [c0, out_split_ch) of a tile that lie past the columns of its units (c0 = nsplit * BN; a
@@ -578,7 +582,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                             if (!const_tile) {
                                 o = fmaf(__fadd_rn(big[4 * j + 2 * i + e], small[4 * j + 2 * i + e] * (1.f / kF16LoScale)),
                                          sc[i], sh[i]);
-                                if (p.relu) o = fmaxf(o, 0.f);
+                                if (p.relu) o = sassd_relu(o);
                                 if (c_wg + m0 + 8 * i >= p.cout) o = 0.f;
                             }
                             stage[(8 * j + 2 * (t & 3) + e) * OUT_PITCH + m0 + 8 * i] = o;
@@ -594,6 +598,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                     }
                 }
                 if (p.out_split) {
+                    F16Range ovf;             // one vote per unit: no register lives across the MMA loop for it
                     for (int v = t; v < TILE_H * TILE_W * 8; v += 128) {
                         const int pix = v >> 3, c = 8 * (v & 7), n = c_wg + c;
                         const int y = ty * TILE_H + pix / TILE_W, x = tx * TILE_W + pix % TILE_W;
@@ -605,13 +610,16 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                         split_f16x2(f0.z, f0.w, hi.y, lo.y);
                         split_f16x2(f1.x, f1.y, hi.z, lo.z);
                         split_f16x2(f1.z, f1.w, hi.w, lo.w);
+                        ovf.add(lo.x); ovf.add(lo.y); ovf.add(lo.z); ovf.add(lo.w);
                         __half* dst = p.out_split + (((size_t)b * p.H + y) * p.W + x) * p.out_split_ch + n;
                         *(uint4*)dst = hi;
                         *(uint4*)(dst + plane) = lo;
                     }
+                    report_f16_range(p.status, ovf.overflowed());
                 }
             } else {
                 // epilogue from registers: folded BN + ReLU (or the layer constant), fp32 and / or split-plane stores
+                F16Range ovf;
 #pragma unroll
                 for (int j = 0; j < BN / 8; ++j) {
                     const int n = n_off + 8 * j + 2 * (t & 3);
@@ -633,7 +641,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                         if (!const_tile) {
                             o0 = fmaf(__fadd_rn(big[4 * j + 2 * i], small[4 * j + 2 * i] * (1.f / kF16LoScale)), sc0, sh0);
                             o1 = fmaf(__fadd_rn(big[4 * j + 2 * i + 1], small[4 * j + 2 * i + 1] * (1.f / kF16LoScale)), sc1, sh1);
-                            if (p.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+                            if (p.relu) { o0 = sassd_relu(o0); o1 = sassd_relu(o1); }
                             if (n >= p.cout) o0 = 0.f;
                             if (n + 1 >= p.cout) o1 = 0.f;
                         }
@@ -644,12 +652,14 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                         if (p.out_split && n < p.out_split_ch) {
                             uint32_t h, l;
                             split_f16x2(o0, o1, h, l);
+                            ovf.add(l);
                             __half* dst = p.out_split + pix * p.out_split_ch + n;
                             *(uint32_t*)dst = h;
                             *(uint32_t*)(dst + plane) = l;
                         }
                     }
                 }
+                report_f16_range(p.status, ovf.overflowed());
             }
         }
         // Background tiles in a pass of their own: interleaved with the MMA units, the copy's address arithmetic is
@@ -754,16 +764,16 @@ extern "C" int sassd_conv2d_pack(const float* weight, int taps, int cin, int cou
 extern "C" int sassd_conv2d_f16x3(const sassd_conv2d_desc* d, const void* in_split, const void* wpack,
                                   const float* scale, const float* shift, float* out_f32, void* out_split,
                                   sassd_stream_t stream_) {
-    return sassd_conv2d_f16x3_occ_bg(d, in_split, wpack, scale, shift, out_f32, out_split, nullptr, 0, nullptr, nullptr,
-                                     nullptr, nullptr, stream_);
+    return sassd_conv2d_f16x3_occ_bg_status(d, in_split, wpack, scale, shift, out_f32, out_split, nullptr, 0, nullptr,
+                                            nullptr, nullptr, nullptr, nullptr, stream_);
 }
 
 extern "C" int sassd_conv2d_f16x3_occ(const sassd_conv2d_desc* d, const void* in_split, const void* wpack,
                                       const float* scale, const float* shift, float* out_f32, void* out_split,
                                       const int32_t* tile_dist, int reach, const float* const_out, int32_t* counters,
                                       sassd_stream_t stream_) {
-    return sassd_conv2d_f16x3_occ_bg(d, in_split, wpack, scale, shift, out_f32, out_split, tile_dist, reach, const_out,
-                                     nullptr, nullptr, counters, stream_);
+    return sassd_conv2d_f16x3_occ_bg_status(d, in_split, wpack, scale, shift, out_f32, out_split, tile_dist, reach,
+                                            const_out, nullptr, nullptr, counters, nullptr, stream_);
 }
 
 extern "C" int sassd_conv2d_f16x3_occ_bg(const sassd_conv2d_desc* d, const void* in_split, const void* wpack,
@@ -771,6 +781,15 @@ extern "C" int sassd_conv2d_f16x3_occ_bg(const sassd_conv2d_desc* d, const void*
                                          const int32_t* tile_dist, int reach, const float* const_out,
                                          const void* bg_split, const float* bg_f32, int32_t* counters,
                                          sassd_stream_t stream_) {
+    return sassd_conv2d_f16x3_occ_bg_status(d, in_split, wpack, scale, shift, out_f32, out_split, tile_dist, reach,
+                                            const_out, bg_split, bg_f32, counters, nullptr, stream_);
+}
+
+extern "C" int sassd_conv2d_f16x3_occ_bg_status(const sassd_conv2d_desc* d, const void* in_split, const void* wpack,
+                                                const float* scale, const float* shift, float* out_f32,
+                                                void* out_split, const int32_t* tile_dist, int reach,
+                                                const float* const_out, const void* bg_split, const float* bg_f32,
+                                                int32_t* counters, int32_t* d_status, sassd_stream_t stream_) {
     if (tile_dist && (!const_out || reach < 0)) return SASSD_ERR_ARG;
     // a background must hold every output the layer writes
     if ((bg_split || bg_f32) && ((out_split && !bg_split) || (out_f32 && !bg_f32))) return SASSD_ERR_ARG;
@@ -811,6 +830,7 @@ extern "C" int sassd_conv2d_f16x3_occ_bg(const sassd_conv2d_desc* d, const void*
     a.tile_dist = tile_dist; a.reach = reach; a.cvec = const_out; a.counters = counters;
     a.tile_order = d->tile_order;
     a.nsplit = 1;
+    a.status = d_status;
     const Background bg = {out_split ? (const __half*)bg_split : nullptr, out_f32 ? bg_f32 : nullptr};
     cudaStream_t stream = (cudaStream_t)stream_;
     if (d->cout <= 32) return launch2<32>(map, a, bg, stream);
@@ -824,9 +844,11 @@ extern "C" int sassd_conv2d_f16x3_occ_bg(const sassd_conv2d_desc* d, const void*
 // SparseConvTensor.dense() into the split BEV map: hi / lo*2048 fp16 planes [2,B,H,W,D*C] (channel d*C + c).
 __global__ void sparse_to_bev_split_kernel(const float4* __restrict__ feat, const int4* __restrict__ coors,
                                            const int* __restrict__ d_rows, int rows_cap, int C4, int D, int H, int W,
-                                           size_t plane, __half* __restrict__ bev, int* __restrict__ tile_dist) {
+                                           size_t plane, __half* __restrict__ bev, int* __restrict__ tile_dist,
+                                           int* __restrict__ status) {
     const int rows = min(*d_rows, rows_cap);
     const long long total = (long long)rows * C4;
+    tc::F16Range ovf;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
          i += (long long)gridDim.x * blockDim.x) {
         const int r = (int)(i / C4), q = (int)(i % C4);
@@ -835,20 +857,31 @@ __global__ void sparse_to_bev_split_kernel(const float4* __restrict__ feat, cons
         uint32_t h0, h1, l0, l1;
         tc::split_f16x2(v.x, v.y, h0, l0);
         tc::split_f16x2(v.z, v.w, h1, l1);
+        ovf.add(l0);
+        ovf.add(l1);
         __half* dst = bev + ((((size_t)c.x * H + c.z) * W + c.w) * (size_t)(D * C4) + (size_t)c.y * C4 + q) * 4;
         *(uint2*)dst = make_uint2(h0, h1);
         *(uint2*)(dst + plane) = make_uint2(l0, l1);
         if (tile_dist && q == 0) sassd_mark_conv2d_tiles(tile_dist, c.x, c.z, c.w, H, W);
     }
+    tc::report_f16_range(status, ovf.overflowed());
 }
 
 extern "C" int sassd_sparse_to_bev_split(const float* feat, const int32_t* coors, const int32_t* d_rows, int rows_cap,
                                          int C, int D, int H, int W, int batch, void* bev_split, int32_t* tile_dist,
                                          sassd_stream_t stream_) {
+    return sassd_sparse_to_bev_split_status(feat, coors, d_rows, rows_cap, C, D, H, W, batch, bev_split, tile_dist,
+                                            nullptr, stream_);
+}
+
+extern "C" int sassd_sparse_to_bev_split_status(const float* feat, const int32_t* coors, const int32_t* d_rows,
+                                                int rows_cap, int C, int D, int H, int W, int batch, void* bev_split,
+                                                int32_t* tile_dist, int32_t* d_status, sassd_stream_t stream_) {
     if (!feat || !coors || !d_rows || !bev_split || (C & 3) || batch < 1) return SASSD_ERR_ARG;
     if (rows_cap <= 0) return SASSD_OK;
     const size_t plane = (size_t)batch * H * W * D * C;
     sparse_to_bev_split_kernel<<<sassd_grid((long long)rows_cap * (C / 4), 256), 256, 0, (cudaStream_t)stream_>>>(
-        (const float4*)feat, (const int4*)coors, d_rows, rows_cap, C / 4, D, H, W, plane, (__half*)bev_split, tile_dist);
+        (const float4*)feat, (const int4*)coors, d_rows, rows_cap, C / 4, D, H, W, plane, (__half*)bev_split, tile_dist,
+        d_status);
     return sassd_check_launch();
 }

@@ -184,7 +184,7 @@ gconv_ffma_kernel(const float* __restrict__ in, const float* __restrict__ weight
 #pragma unroll
         for (int j = 0; j < TN; ++j) {
             v[j] = fmaf(acc[i][j], sc[j], sh[j]);
-            if (relu) v[j] = fmaxf(v[j], 0.f);
+            if (relu) v[j] = sassd_relu(v[j]);
         }
         if (TN >= 4 && (out_stride & 3) == 0 && n0 + tx * TN + TN <= cout) {
 #pragma unroll
@@ -226,11 +226,18 @@ static int dispatch_ffma(const sassd_gconv_desc* d, const float* in, const float
 }
 
 int sassd_gconv_tc(const sassd_gconv_desc* d, const float* in, const float* weight, const float* scale,
-                   const float* shift, const int32_t* nbr, const int32_t* d_rows, float* out, cudaStream_t stream);
+                   const float* shift, const int32_t* nbr, const int32_t* d_rows, float* out, int32_t* d_status,
+                   cudaStream_t stream);
 
 extern "C" int sassd_gconv(const sassd_gconv_desc* d, const float* in, const float* weight, const float* scale,
                            const float* shift, const int32_t* nbr, const int32_t* d_rows, float* out,
                            sassd_stream_t stream_) {
+    return sassd_gconv_status(d, in, weight, scale, shift, nbr, d_rows, out, nullptr, stream_);
+}
+
+extern "C" int sassd_gconv_status(const sassd_gconv_desc* d, const float* in, const float* weight, const float* scale,
+                                  const float* shift, const int32_t* nbr, const int32_t* d_rows, float* out,
+                                  int32_t* d_status, sassd_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (!d || !in || !weight || !out) return SASSD_ERR_ARG;
     if (d->cin <= 0 || (d->cin & 3) || d->cout <= 0 || d->taps <= 0 || (d->in_stride & 3) || d->rows_cap < 0)
@@ -240,7 +247,7 @@ extern "C" int sassd_gconv(const sassd_gconv_desc* d, const float* in, const flo
     if (d->mode == SASSD_GCONV_ROWS && d->taps != 1) return SASSD_ERR_ARG;
     if (d->rows_cap == 0) return SASSD_OK;
     if (d->precision == SASSD_PREC_TF32X3 || d->precision == SASSD_PREC_F16X3)
-        return sassd_gconv_tc(d, in, weight, scale, shift, nbr, d_rows, out, stream);
+        return sassd_gconv_tc(d, in, weight, scale, shift, nbr, d_rows, out, d_status, stream);
     if (d->precision != SASSD_PREC_FP32) return SASSD_ERR_ARG;
     switch (d->mode) {
         case SASSD_GCONV_TABLE: return dispatch_ffma<SASSD_GCONV_TABLE>(d, in, weight, scale, shift, nbr, d_rows, out, stream);

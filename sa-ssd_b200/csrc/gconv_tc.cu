@@ -60,7 +60,7 @@ __global__ void __launch_bounds__(GC_THREADS, 1)
 gconv_tc_kernel(const float* __restrict__ in, const float* __restrict__ wpack, const float* __restrict__ scale,
                 const float* __restrict__ shift, const int* __restrict__ nbr, const int* __restrict__ d_rows,
                 float* __restrict__ out, int cin, int cout, int taps, int in_stride, int out_stride, int rows_cap,
-                int H, int W, int relu, int bn, int nparts) {
+                int H, int W, int relu, int bn, int nparts, int* __restrict__ status) {
     using C = Cfg<NB>;
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment is required by the 128B swizzle
@@ -139,6 +139,8 @@ gconv_tc_kernel(const float* __restrict__ in, const float* __restrict__ wpack, c
                     if (ch >= nchunks) break;
                     float4 (&vn)[NF4H] = ring[u];
                     uint4 ph[4], pl[4];       // this thread's 4 of the 8 16-byte chunks of the hi / lo rows
+                    F16Range ovf;             // the lo halves of this chunk (one vote per chunk: no register
+                                              // lives across the chunk loop for it)
                     if (!ring_live[u]) {      // missing neighbour (most sparse (row, offset) slots): no split math
 #pragma unroll
                         for (int c = 0; c < 4; ++c) { ph[c] = make_uint4(0u, 0u, 0u, 0u); pl[c] = ph[c]; }
@@ -164,8 +166,10 @@ gconv_tc_kernel(const float* __restrict__ in, const float* __restrict__ wpack, c
                             split_f16x2(b.z, b.w, h3, l3);
                             ph[c] = make_uint4(h0, h1, h2, h3);
                             pl[c] = make_uint4(l0, l1, l2, l3);
+                            ovf.add(l0); ovf.add(l1); ovf.add(l2); ovf.add(l3);
                         }
                     }
+                    report_f16_range(status, ovf.overflowed());
                     if (ch + PF < nchunks) fetch(vn, ring_live[u]);        // refill this ring slot
                     if (lane == 0) {                                        // one polling lane per warp
                         mbar_wait(empty(stage), phase ^ 1u);
@@ -243,7 +247,7 @@ gconv_tc_kernel(const float* __restrict__ in, const float* __restrict__ wpack, c
                     for (int e = 0; e < 2; ++e) {
                         const float sm = PREC == 0 ? small[4 * j + 2 * i + e] : small[4 * j + 2 * i + e] * (1.f / kF16LoScale);
                         float val = fmaf(__fadd_rn(sum[4 * j + 2 * i + e], sm), sc[e], sh[e]);
-                        if (relu) val = fmaxf(val, 0.f);
+                        if (relu) val = sassd_relu(val);
                         o[e] = val;
                     }
                     float* orow = out + (size_t)m * out_stride;
@@ -260,7 +264,7 @@ gconv_tc_kernel(const float* __restrict__ in, const float* __restrict__ wpack, c
 
 template <int MODE, int NB, int PREC>
 static int launch(const sassd_gconv_desc* d, const float* in, const float* w, const float* scale, const float* shift,
-                  const int* nbr, const int* d_rows, float* out, cudaStream_t stream, int bn) {
+                  const int* nbr, const int* d_rows, float* out, int* status, cudaStream_t stream, int bn) {
     using C = Cfg<NB>;
     auto kern = gconv_tc_kernel<MODE, NB, PREC>;
     static bool configured = false;
@@ -274,28 +278,28 @@ static int launch(const sassd_gconv_desc* d, const float* in, const float* w, co
     const int grid = units < sassd_num_sms() ? (units > 0 ? units : 1) : sassd_num_sms();
     kern<<<grid, GC_THREADS, C::SMEM_BYTES, stream>>>(in, w, scale, shift, nbr, d_rows, out, d->cin, d->cout, d->taps,
                                                       d->in_stride, d->out_stride, d->rows_cap, d->H, d->W, d->relu,
-                                                      bn, nparts);
+                                                      bn, nparts, status);
     return sassd_check_launch();
 }
 
 template <int MODE, int PREC>
 static int dispatch(const sassd_gconv_desc* d, const float* in, const float* w, const float* scale, const float* shift,
-                    const int* nbr, const int* d_rows, float* out, cudaStream_t s) {
-    if (d->cout <= 16) return launch<MODE, 16, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s, 16);
-    if (d->cout <= 32) return launch<MODE, 32, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s, 32);
-    if (d->cout <= 64) return launch<MODE, 64, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s, 64);
-    if (d->cout <= 128) return launch<MODE, 64, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s, 128);
-    if (d->cout <= 256) return launch<MODE, 64, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s, 256);
+                    const int* nbr, const int* d_rows, float* out, int* st, cudaStream_t s) {
+    if (d->cout <= 16) return launch<MODE, 16, PREC>(d, in, w, scale, shift, nbr, d_rows, out, st, s, 16);
+    if (d->cout <= 32) return launch<MODE, 32, PREC>(d, in, w, scale, shift, nbr, d_rows, out, st, s, 32);
+    if (d->cout <= 64) return launch<MODE, 64, PREC>(d, in, w, scale, shift, nbr, d_rows, out, st, s, 64);
+    if (d->cout <= 128) return launch<MODE, 64, PREC>(d, in, w, scale, shift, nbr, d_rows, out, st, s, 128);
+    if (d->cout <= 256) return launch<MODE, 64, PREC>(d, in, w, scale, shift, nbr, d_rows, out, st, s, 256);
     return SASSD_ERR_UNSUPPORTED;
 }
 
 template <int PREC>
 static int dispatch_mode(const sassd_gconv_desc* d, const float* in, const float* w, const float* scale,
-                         const float* shift, const int* nbr, const int* d_rows, float* out, cudaStream_t s) {
+                         const float* shift, const int* nbr, const int* d_rows, float* out, int* st, cudaStream_t s) {
     switch (d->mode) {
-        case SASSD_GCONV_TABLE: return dispatch<SASSD_GCONV_TABLE, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s);
-        case SASSD_GCONV_CONV2D: return dispatch<SASSD_GCONV_CONV2D, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s);
-        case SASSD_GCONV_ROWS: return dispatch<SASSD_GCONV_ROWS, PREC>(d, in, w, scale, shift, nbr, d_rows, out, s);
+        case SASSD_GCONV_TABLE: return dispatch<SASSD_GCONV_TABLE, PREC>(d, in, w, scale, shift, nbr, d_rows, out, st, s);
+        case SASSD_GCONV_CONV2D: return dispatch<SASSD_GCONV_CONV2D, PREC>(d, in, w, scale, shift, nbr, d_rows, out, st, s);
+        case SASSD_GCONV_ROWS: return dispatch<SASSD_GCONV_ROWS, PREC>(d, in, w, scale, shift, nbr, d_rows, out, st, s);
     }
     return SASSD_ERR_ARG;
 }
@@ -306,9 +310,12 @@ static int dispatch_mode(const sassd_gconv_desc* d, const float* in, const float
 //   TF32X3: [taps*ceil(cin/32)][hi|lo][BN rows (n)][32 fp32]   F16X3: [taps*ceil(cin/64)][hi|lo][BN][64 fp16]
 // every row is 128 bytes, its 16-byte chunks XOR-swizzled by (n & 7).
 int sassd_gconv_tc(const sassd_gconv_desc* d, const float* in, const float* weight, const float* scale,
-                   const float* shift, const int32_t* nbr, const int32_t* d_rows, float* out, cudaStream_t stream) {
-    if (d->precision == SASSD_PREC_TF32X3) return tc::dispatch_mode<0>(d, in, weight, scale, shift, nbr, d_rows, out, stream);
-    if (d->precision == SASSD_PREC_F16X3) return tc::dispatch_mode<1>(d, in, weight, scale, shift, nbr, d_rows, out, stream);
+                   const float* shift, const int32_t* nbr, const int32_t* d_rows, float* out, int32_t* d_status,
+                   cudaStream_t stream) {
+    if (d->precision == SASSD_PREC_TF32X3)
+        return tc::dispatch_mode<0>(d, in, weight, scale, shift, nbr, d_rows, out, d_status, stream);
+    if (d->precision == SASSD_PREC_F16X3)
+        return tc::dispatch_mode<1>(d, in, weight, scale, shift, nbr, d_rows, out, d_status, stream);
     return SASSD_ERR_ARG;
 }
 

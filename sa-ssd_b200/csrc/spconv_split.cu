@@ -87,6 +87,7 @@ struct Args {
     int* arrivals;          // [MAX_CTAS][2] pieces of a shared tile done, per consumer warpgroup; zero between launches
                             // (null: no chunk deal)
     int* counters;          // optional [2]: executed (tile, chunk) pairs, tiles (bench instrumentation)
+    int* status;            // optional: SASSD_FLAG_F16_RANGE when a value stored into out_split overflows the split
     int cin, cout, taps, rows_cap, relu, out_ch, out_f32_stride;
     int fixed_walk;         // every tile walks its chunks from chunk 0 (see rot_of)
 };
@@ -349,6 +350,7 @@ __global__ void __launch_bounds__(THREADS3, 1) spconv_split_kernel(const Args p)
         int stage = 0;
         uint32_t phase = 0;
         int executed = 0, tiles_done = 0;
+        F16Range ovf;                 // the lo halves this thread stored into out_split
         for (int ii = 0; ii < n_items; ++ii) {
             const Item item = item_at(ii);
             const int tile = item.tile;
@@ -432,15 +434,18 @@ __global__ void __launch_bounds__(THREADS3, 1) spconv_split_kernel(const Args p)
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
                     const int m = tile * BM + rl0 + 8 * i;
-                    // columns >= cout: zero weights, scale 1, shift 0 -> exactly 0
                     float o0 = fmaf(big[4 * j + 2 * i], scl0, shl0), o1 = fmaf(big[4 * j + 2 * i + 1], scl1, shl1);
-                    if (p.relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+                    if (p.relu) { o0 = sassd_relu(o0); o1 = sassd_relu(o1); }
+                    // columns >= cout: exactly 0 (their zero weights alone would turn a NaN input into NaN)
+                    if (n >= p.cout) o0 = 0.f;
+                    if (n + 1 >= p.cout) o1 = 0.f;
                     if (m < M) {
                         if (p.out_f32 && n < p.out_f32_stride)
                             *(float2*)(p.out_f32 + (size_t)m * p.out_f32_stride + n) = make_float2(o0, o1);
                         if (p.out_split && 8 * j < p.out_ch) {
                             uint32_t h, l;
                             split_f16x2(o0, o1, h, l);
+                            ovf.add(l);
                             __half* ohi = p.out_split + (size_t)m * p.out_ch + n;
                             *(uint32_t*)ohi = h;
                             *(uint32_t*)(ohi + p.out_plane) = l;
@@ -460,6 +465,7 @@ __global__ void __launch_bounds__(THREADS3, 1) spconv_split_kernel(const Args p)
                 }
             }
         }
+        report_f16_range(p.status, ovf.overflowed());
         if (p.counters && threadIdx.x == 0 && executed) {
             atomicAdd(&p.counters[0], executed);
             atomicAdd(&p.counters[1], tiles_done);
@@ -549,6 +555,15 @@ extern "C" int sassd_spconv_f16x3(const sassd_spconv_desc* d, const void* in_spl
                                   const float* scale, const float* shift, const int32_t* nbr,
                                   const int32_t* tile_mask, const int32_t* d_rows, void* out_split, float* out_f32,
                                   void* ws, size_t ws_bytes, int32_t* counters, sassd_stream_t stream_) {
+    return sassd_spconv_f16x3_status(d, in_split, wpack, scale, shift, nbr, tile_mask, d_rows, out_split, out_f32, ws,
+                                     ws_bytes, counters, nullptr, stream_);
+}
+
+extern "C" int sassd_spconv_f16x3_status(const sassd_spconv_desc* d, const void* in_split, const void* wpack,
+                                         const float* scale, const float* shift, const int32_t* nbr,
+                                         const int32_t* tile_mask, const int32_t* d_rows, void* out_split,
+                                         float* out_f32, void* ws, size_t ws_bytes, int32_t* counters,
+                                         int32_t* d_status, sassd_stream_t stream_) {
     if (!d || !in_split || !wpack || (!out_split && !out_f32)) return SASSD_ERR_ARG;
     if (d->cin < 8 || (d->cin & 7) || d->cin > 64 || d->cout < 1 || d->cout > 64 || d->taps < 1 || d->rows_cap < 0)
         return SASSD_ERR_ARG;
@@ -565,6 +580,7 @@ extern "C" int sassd_spconv_f16x3(const sassd_spconv_desc* d, const void* in_spl
     a.parts = (float*)ws;
     a.arrivals = ws ? (int*)((char*)ws + spconv_parts_bytes()) : nullptr;
     a.counters = counters;
+    a.status = d_status;
     a.cin = d->cin; a.cout = d->cout; a.taps = d->taps; a.rows_cap = d->rows_cap; a.relu = d->relu;
     a.out_ch = d->out_ch; a.out_f32_stride = d->out_f32_stride;
     a.fixed_walk = d->fixed_walk;
@@ -575,25 +591,36 @@ extern "C" int sassd_spconv_f16x3(const sassd_spconv_desc* d, const void* in_spl
 
 // fp32 rows [rows, cin] -> split rows [2][rows_cap][cs] (cs >= cin, multiple of 8; padding channels zero)
 __global__ void features_to_split_kernel(const float* __restrict__ feat, const int* __restrict__ d_rows, int rows_cap,
-                                         int cin, int cs, __half* __restrict__ out) {
+                                         int cin, int cs, __half* __restrict__ out, int* __restrict__ status) {
     const int rows = d_rows ? min(*d_rows, rows_cap) : rows_cap;
     const long long total = (long long)rows * cs;
     const size_t plane = (size_t)rows_cap * cs;
+    bool ovf = false;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         const int r = (int)(i / cs), c = (int)(i % cs);
         float hi = 0.f, lo = 0.f;
-        if (c < cin) tc::split_f16(feat[(size_t)r * cin + c], hi, lo);
+        if (c < cin) {
+            const float x = feat[(size_t)r * cin + c];
+            tc::split_f16(x, hi, lo);
+            ovf |= isinf(lo);             // -+inf exactly when a finite x overflowed (NaN when x is inf or NaN)
+        }
         out[i] = __float2half_rn(hi);
         out[i + plane] = __float2half_rn(lo);
     }
+    tc::report_f16_range(status, ovf);
 }
 
 extern "C" int sassd_features_to_split(const float* feat, const int32_t* d_rows, int rows_cap, int cin, int cs,
                                        void* out_split, sassd_stream_t stream_) {
+    return sassd_features_to_split_status(feat, d_rows, rows_cap, cin, cs, out_split, nullptr, stream_);
+}
+
+extern "C" int sassd_features_to_split_status(const float* feat, const int32_t* d_rows, int rows_cap, int cin, int cs,
+                                              void* out_split, int32_t* d_status, sassd_stream_t stream_) {
     if (!feat || !out_split || cin < 1 || cs < cin || (cs & 7)) return SASSD_ERR_ARG;
     if (rows_cap <= 0) return SASSD_OK;
     features_to_split_kernel<<<sassd_grid((long long)rows_cap * cs, 256), 256, 0, (cudaStream_t)stream_>>>(
-        feat, d_rows, rows_cap, cin, cs, (__half*)out_split);
+        feat, d_rows, rows_cap, cin, cs, (__half*)out_split, d_status);
     return sassd_check_launch();
 }
 

@@ -58,7 +58,9 @@ MERGE_MAX = 16                            # SASSD_MERGE_MAX: members sassd_merge
 OK = 0
 ERRORS = {-1: "SASSD_ERR_ARG", -2: "SASSD_ERR_LAUNCH", -3: "SASSD_ERR_WORKSPACE", -4: "SASSD_ERR_UNSUPPORTED"}
 FLAGS = {1: "VOXEL_CAP", 2: "ROWS_CAP", 4: "GUIDED_CAP", 8: "NMS_CAP", 16: "HASH_FULL", 32: "DET_CAP",
-         64: "GT_CAP", 128: "GATHER_CAP", 256: "POINTS_CAP"}
+         64: "GT_CAP", 128: "GATHER_CAP", 256: "POINTS_CAP", 512: "F16_RANGE"}
+F16_RANGE = 512                           # SASSD_FLAG_F16_RANGE: a finite value with |x| >= 65520 overflowed the fp16 split
+F16_SPLIT_MAX = 65520.0                   # the least magnitude the 3xFP16 split cannot hold (half_rn rounds it to inf)
 GATHER_CAP = 128                          # SASSD_FLAG_GATHER_CAP: sassd_points_in_rbboxes' rows exceed gather_cap
 
 P = c_void_p
@@ -89,6 +91,7 @@ _SIGNATURES = {
     "sassd_rulebook_conv_nbr": (c_int, [P, P, c_int, c_int, c_int, c_int, P, P, c_int, P, P, P]),
     "sassd_rulebook_pairs": (c_int, [P, P, c_int, P, P, P]),
     "sassd_gconv": (c_int, [ctypes.POINTER(GConvDesc), P, P, P, P, P, P, P, P]),
+    "sassd_gconv_status": (c_int, [ctypes.POINTER(GConvDesc), P, P, P, P, P, P, P, P, P]),
     "sassd_gconv_pack_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "sassd_gconv_pack": (c_int, [P, c_int, c_int, c_int, c_int, P, P]),
     "sassd_conv2d_pack_bytes": (c_size_t, [c_int, c_int, c_int]),
@@ -96,6 +99,8 @@ _SIGNATURES = {
     "sassd_conv2d_f16x3": (c_int, [ctypes.POINTER(Conv2dDesc), P, P, P, P, P, P, P]),
     "sassd_conv2d_f16x3_occ": (c_int, [ctypes.POINTER(Conv2dDesc), P, P, P, P, P, P, P, c_int, P, P, P]),
     "sassd_conv2d_f16x3_occ_bg": (c_int, [ctypes.POINTER(Conv2dDesc), P, P, P, P, P, P, P, c_int, P, P, P, P, P]),
+    "sassd_conv2d_f16x3_occ_bg_status": (c_int, [ctypes.POINTER(Conv2dDesc), P, P, P, P, P, P, P, c_int, P, P, P, P, P,
+                                                 P]),
     "sassd_rotate_overlap_eval": (c_int, [P, P, P, P, P, c_int, c_int, c_int, P, P]),
     "sassd_kitti_match": (c_int, [c_int, P, P, P, P, P, P, P, P, P, P, P, P, c_int, ctypes.c_double, c_int, c_int, P, P,
                                   P, P]),
@@ -111,9 +116,12 @@ _SIGNATURES = {
     "sassd_spconv_pack": (c_int, [P, c_int, c_int, c_int, c_int, P, P]),
     "sassd_spconv_workspace_bytes": (c_size_t, []),
     "sassd_spconv_f16x3": (c_int, [ctypes.POINTER(SpconvDesc), P, P, P, P, P, P, P, P, P, P, c_size_t, P, P]),
+    "sassd_spconv_f16x3_status": (c_int, [ctypes.POINTER(SpconvDesc), P, P, P, P, P, P, P, P, P, P, c_size_t, P, P, P]),
     "sassd_features_to_split": (c_int, [P, P, c_int, c_int, c_int, P, P]),
+    "sassd_features_to_split_status": (c_int, [P, P, c_int, c_int, c_int, P, P, P]),
     "sassd_split_rows_to_bev": (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P]),
     "sassd_sparse_to_bev_split": (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P]),
+    "sassd_sparse_to_bev_split_status": (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P, P]),
     "sassd_sparse_to_bev": (c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, P, P]),
     "sassd_decode_select_workspace_bytes": (c_size_t, [c_int, c_int]),
     "sassd_decode_select": (c_int, [P, c_int, c_int, c_int, c_int, c_int, P, c_int, P, c_int, c_float, P, P, P, P, c_int, P,
@@ -186,5 +194,8 @@ def raise_on_status(word):
     """Raise SassdError naming the capacities that overflowed if the status word ``d_status`` of a step has a
     SASSD_FLAG_* bit set.  ``word`` is an int or a one-element tensor (a device tensor is read with a sync)."""
     word = int(word)
+    if word & F16_RANGE:
+        raise SassdError("activation out of the fp16 split's range on device (|x| >= 65520), outputs that read it are "
+                         "NaN: %s; run the model at set_precision(PREC_FP32) (fp32 range)" % decode_flags(word))
     if word:
         raise SassdError("capacity overflow on device: %s" % decode_flags(word))

@@ -346,9 +346,10 @@ class SpMiddleFHD(nn.Module):
         if self.fcn.precision == ops.PREC_F16X3 and self.dense_tma:
             # split fp16 planes + TMA-fed tensor-core convs (conv2d_tma.cu); y / conv6 are ops.SplitMap
             if x._split is not None and x._split.shape[2] == C:
-                bev = ops.split_rows_to_bev(x._split, x._indices, x.d_rows, C, D, H, W, batch_size)
+                bev = ops.split_rows_to_bev(x._split, x._indices, x.d_rows, C, D, H, W, batch_size, x.status)
             else:
-                bev = ops.sparse_to_bev_split(x.features_cap(), x._indices, x.d_rows, C, D, H, W, batch_size)
+                bev = ops.sparse_to_bev_split(x.features_cap(), x._indices, x.d_rows, C, D, H, W, batch_size,
+                                              x.status)
         else:
             feats = x.features_cap()
             bev = torch.zeros((batch_size, H, W, D * C), dtype=torch.float32, device=feats.device)

@@ -53,7 +53,7 @@ def next_pow2(n):
 # kernels launched by each C-ABI entry point (memsets not counted)
 _KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_points_in_rbboxes": 1, "sassd_augment_drop_points": 1, "sassd_augment_noise_search": 1, "sassd_augment_assemble": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
-            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_kitti_eval_flags": 1, "sassd_kitti_eval_overlaps": 1, "sassd_kitti_eval_match": 3, "sassd_kitti_scan_labels": 1, "sassd_kitti_parse_labels": 2, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
+            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_kitti_eval_flags": 1, "sassd_kitti_eval_overlaps": 1, "sassd_kitti_eval_match": 3, "sassd_kitti_scan_labels": 1, "sassd_kitti_parse_labels": 2, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_conv2d_f16x3_occ_bg_status": 1, "sassd_gconv_status": 1, "sassd_spconv_f16x3_status": 1, "sassd_features_to_split_status": 1, "sassd_sparse_to_bev_split_status": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_merge_detections": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
             "sassd_boxes_iou_bev": 1, "sassd_points_in_boxes": 2, "sassd_assign_rpn": 3, "sassd_assign_pswarp": 3,
             "sassd_rpn_loss": 2, "sassd_pswarp_loss": 2, "sassd_aux_loss": 2}
@@ -343,6 +343,17 @@ def rulebook_pairs(nbr, d_rows):
 _TC_PACKS = {}
 
 
+def check_f16_weight(weight, what):
+    """Refuse a weight the 3xFP16 split cannot hold: |w| >= 65520 would pack as hi = +-inf, lo = -+inf and turn every
+    output of the layer into NaN.  One host read per pack (packs are made once per load, before any capture)."""
+    if weight.numel() == 0:
+        return
+    m = float(weight.detach().abs().max())     # a NaN weight passes (NaN >= x is false): the convs propagate it
+    if m >= _lib.F16_SPLIT_MAX:
+        raise ValueError("%s: weight magnitude %g is out of the 3xFP16 split's range (|w| < 65520); run the layer at "
+                         "PREC_FP32" % (what, m))
+
+
 def pack_tc(weight, precision):
     """weight [taps, cin, cout] fp32 (device) -> tensor-core pack (hi/lo split, 128B-swizzled K-major blocks)."""
     taps, cin, cout = weight.shape
@@ -358,6 +369,9 @@ def tc_pack_cached(weight, precision):
     key = (weight.data_ptr(), weight._version, tuple(weight.shape), precision)
     ent = _TC_PACKS.get(key)
     if ent is None:
+        if precision == PREC_F16X3:
+            taps, cin, cout = weight.shape
+            check_f16_weight(weight, "gconv[taps=%d %d->%d]" % (taps, cin, cout))
         if len(_TC_PACKS) >= 256:
             _TC_PACKS.pop(next(iter(_TC_PACKS)))
         ent = (pack_tc(weight.contiguous(), precision), weight)
@@ -375,6 +389,7 @@ def conv2d_pack_cached(weight):
             _TC_PACKS.pop(next(iter(_TC_PACKS)))
         w = weight.contiguous()
         taps, cin, cout = w.shape
+        check_f16_weight(w, "conv2d_tma[taps=%d %d->%d]" % (taps, cin, cout))
         nbytes = _L().sassd_conv2d_pack_bytes(taps, cin, cout)
         if nbytes == 0:
             raise _lib.SassdError("sassd_conv2d_pack_bytes: unsupported shape taps=%d cin=%d cout=%d" % (taps, cin, cout))
@@ -394,6 +409,7 @@ def spconv_pack_cached(weight, cin_stored):
             _TC_PACKS.pop(next(iter(_TC_PACKS)))
         w = weight.contiguous()
         taps, cin, cout = w.shape
+        check_f16_weight(w, "spconv_split[taps=%d %d->%d]" % (taps, cin, cout))
         nbytes = _L().sassd_spconv_pack_bytes(taps, cin_stored, cout)
         if nbytes == 0:
             raise _lib.SassdError("sassd_spconv_pack_bytes: unsupported shape taps=%d cin_stored=%d cout=%d"
@@ -406,8 +422,9 @@ def spconv_pack_cached(weight, cin_stored):
 
 
 def gconv(inp, weight, scale, shift, out, *, mode, taps, cin, cout, relu, nbr=None, d_rows=None, rows_cap=None,
-          batch=0, H=0, W=0, precision=PREC_FP32):
-    """out[m,:] = act((sum_t in[row(m,t),:] @ W[t]) * scale + shift); see sassd_b200.h."""
+          batch=0, H=0, W=0, precision=PREC_FP32, status=None):
+    """out[m,:] = act((sum_t in[row(m,t),:] @ W[t]) * scale + shift); see sassd_b200.h.  ``status``: the step's status
+    word, F16_RANGE when PREC_F16X3 meets an input it cannot split."""
     if precision in (PREC_TF32X3, PREC_F16X3):
         weight = tc_pack_cached(weight, precision)
     d = GConvDesc()
@@ -419,8 +436,8 @@ def gconv(inp, weight, scale, shift, out, *, mode, taps, cin, cout, relu, nbr=No
     d.batch, d.H, d.W = batch, H, W
     d.relu = 1 if relu else 0
     label = "gconv[%s taps=%d %d->%d]" % (("table", "conv2d", "rows")[mode], taps, cin, cout)
-    _call("sassd_gconv", label, ctypes.byref(d), _ptr_any(inp), _ptr(weight), _ptr(scale), _ptr(shift), _ptr(nbr),
-                           _ptr(d_rows), _ptr_any(out), _stream())
+    _call("sassd_gconv_status", label, ctypes.byref(d), _ptr_any(inp), _ptr(weight), _ptr(scale), _ptr(shift), _ptr(nbr),
+                           _ptr(d_rows), _ptr_any(out), _ptr(status), _stream())
     return out
 
 
@@ -750,7 +767,7 @@ class SplitMap:
     """Activation map as two fp16 planes [2, B, H, W, C_stored] (hi, lo*2048) — the operand format of
     sassd_conv2d_f16x3; ``channels`` of the C_stored are meaningful, the rest are zero."""
 
-    def __init__(self, planes, channels, tile_dist=None, reach=0, const=None, background=None):
+    def __init__(self, planes, channels, tile_dist=None, reach=0, const=None, background=None, status=None):
         # Maps that descend from a scattered sparse tensor are constant over large regions.  tile_dist: int32
         # [B * tiles_y * tiles_x], pixel distance of every conv tile to the nearest active cell of the scattered map;
         # reach: number of 3x3 convs applied since; const: fp32 [channels] value of the constant region (None = 0);
@@ -760,6 +777,9 @@ class SplitMap:
         self.planes, self.channels = planes, channels
         self.tile_dist, self.reach, self.const = tile_dist, reach, const
         self.background = background
+        # status: the step's int32 status word, which every conv on this map and the maps derived from it flags
+        # F16_RANGE in when a value it stores overflows the split (None: unchecked)
+        self.status = status
 
     @property
     def shape(self):
@@ -876,12 +896,12 @@ def conv_background(x, weight, scale, shift, relu, cout, out_split, out_f32):
     return ent[0]
 
 
-def sparse_to_bev_split(feat, coors, d_rows, C, D, H, W, batch):
+def sparse_to_bev_split(feat, coors, d_rows, C, D, H, W, batch, status=None):
     planes = torch.zeros((2, batch, H, W, D * C), dtype=torch.float16, device=feat.device)
     dist = _tile_dist(batch, H, W, feat.device)
-    _call("sassd_sparse_to_bev_split", None, _ptr(feat), _ptr(coors), _ptr(d_rows), feat.shape[0], C, D, H, W, batch,
-          _ptr(planes), _ptr(dist), _stream())
-    return SplitMap(planes, D * C, dist)
+    _call("sassd_sparse_to_bev_split_status", None, _ptr(feat), _ptr(coors), _ptr(d_rows), feat.shape[0], C, D, H, W, batch,
+          _ptr(planes), _ptr(dist), _ptr(status), _stream())
+    return SplitMap(planes, D * C, dist, status=status)
 
 
 def conv2d_split(x, weight, scale, shift, relu, cout, out_split=True, out_f32=False):
@@ -915,19 +935,21 @@ def conv2d_split(x, weight, scale, shift, relu, cout, out_split=True, out_f32=Fa
         bg = conv_background(x, weight, scale, shift, relu, cout, out_split, out_f32)
         if bg is not None:
             bg_sp, bg_f = bg
-    _call("sassd_conv2d_f16x3_occ_bg", label, ctypes.byref(d), _ptr(x.planes), _ptr(wp), _ptr(scale), _ptr(shift),
+    _call("sassd_conv2d_f16x3_occ_bg_status", label, ctypes.byref(d), _ptr(x.planes), _ptr(wp), _ptr(scale), _ptr(shift),
           _ptr(of), _ptr(osp), _ptr(dist), reach, _ptr(cvec), _ptr(bg_sp.planes if bg_sp is not None else None),
-          _ptr(bg_f), _ptr(CONV2D_COUNTERS.get(label) if CONV2D_COUNTERS is not None else None), _stream())
-    return (SplitMap(osp, cout, dist, reach, cvec, bg_sp) if osp is not None else None), of
+          _ptr(bg_f), _ptr(CONV2D_COUNTERS.get(label) if CONV2D_COUNTERS is not None else None), _ptr(x.status),
+          _stream())
+    return (SplitMap(osp, cout, dist, reach, cvec, bg_sp, x.status) if osp is not None else None), of
 
 
 # ---------------------------------------------------------------------------- sparse conv on split rows
-def features_to_split(feat, d_rows=None):
-    """fp32 rows [cap, C] -> split rows [2, cap, cs] fp16 (cs = C rounded up to 8)."""
+def features_to_split(feat, d_rows=None, status=None):
+    """fp32 rows [cap, C] -> split rows [2, cap, cs] fp16 (cs = C rounded up to 8); F16_RANGE in ``status`` when a
+    finite value has |x| >= 65520."""
     cap, C = feat.shape
     cs = (C + 7) // 8 * 8
     out = torch.empty((2, cap, cs), dtype=torch.float16, device=feat.device)
-    _call("sassd_features_to_split", None, _ptr(feat), _ptr(d_rows), cap, C, cs, _ptr(out), _stream())
+    _call("sassd_features_to_split_status", None, _ptr(feat), _ptr(d_rows), cap, C, cs, _ptr(out), _ptr(status), _stream())
     return out
 
 
@@ -946,9 +968,10 @@ SPCONV_TAP_ROTATE = True
 
 
 def spconv_split(planes, weight, scale, shift, relu, cout, rows_cap, nbr=None, d_rows=None, want_f32=False,
-                 tile_mask=None, ws=None):
+                 tile_mask=None, ws=None, status=None):
     """planes [2, in_cap, cin_stored] fp16; weight [taps, cin, cout] fp32 (packed on first use).
-    Returns (out planes [2, rows_cap, out_ch], fp32 rows or None)."""
+    Returns (out planes [2, rows_cap, out_ch], fp32 rows or None).  F16_RANGE in ``status`` when an output overflows
+    the split."""
     taps = weight.shape[0]
     wp = spconv_pack_cached(weight, planes.shape[2])
     d = SpconvDesc()
@@ -965,15 +988,15 @@ def spconv_split(planes, weight, scale, shift, relu, cout, rows_cap, nbr=None, d
     w = None
     if SPCONV_TAP_SPLIT and taps > 1:
         w = (ws or _WS).get("spconv_split", _L().sassd_spconv_workspace_bytes(), planes.device, zeroed=True)
-    _call("sassd_spconv_f16x3", label, ctypes.byref(d), _ptr(planes), _ptr(wp), _ptr(scale), _ptr(shift), _ptr(nbr),
+    _call("sassd_spconv_f16x3_status", label, ctypes.byref(d), _ptr(planes), _ptr(wp), _ptr(scale), _ptr(shift), _ptr(nbr),
           _ptr(tile_mask if SPCONV_TAP_SKIP else None), _ptr(d_rows), _ptr(out), _ptr(of), _ptr(w),
-          0 if w is None else w.numel(), _ptr(SPCONV_COUNTERS), _stream())
+          0 if w is None else w.numel(), _ptr(SPCONV_COUNTERS), _ptr(status), _stream())
     return out, of
 
 
-def split_rows_to_bev(planes, coors, d_rows, C, D, H, W, batch):
+def split_rows_to_bev(planes, coors, d_rows, C, D, H, W, batch, status=None):
     bev = torch.zeros((2, batch, H, W, D * C), dtype=torch.float16, device=planes.device)
     dist = _tile_dist(batch, H, W, planes.device)
     _call("sassd_split_rows_to_bev", None, _ptr(planes), _ptr(coors), _ptr(d_rows), planes.shape[1], C, D, H, W, batch,
           _ptr(bev), _ptr(dist), _stream())
-    return SplitMap(bev, D * C, dist)
+    return SplitMap(bev, D * C, dist, status=status)

@@ -69,7 +69,7 @@ class SparseConvTensor:
 
     def split_planes(self):
         if self._split is None:
-            self._split = ops.features_to_split(self._features, self.d_rows)
+            self._split = ops.features_to_split(self._features, self.d_rows, self.status)
         return self._split
 
     @property
@@ -170,11 +170,11 @@ class _SparseConvBase(nn.Module):
             planes = x.split_planes()
             if taps == 1:
                 out, _ = ops.spconv_split(planes, wp, scale, shift, relu, self.out_channels, x.rows_cap,
-                                          d_rows=x.d_rows)
+                                          d_rows=x.d_rows, status=x.status)
                 return x._derive(None, split=out, channels=self.out_channels)
             rb = self._rulebook(x)
             out, _ = ops.spconv_split(planes, wp, scale, shift, relu, self.out_channels, rb.nbr.shape[0], nbr=rb.nbr,
-                                      d_rows=rb.d_rows_out, tile_mask=rb.tile_mask)
+                                      d_rows=rb.d_rows_out, tile_mask=rb.tile_mask, status=x.status)
             if self.subm:
                 return x._derive(None, split=out, channels=self.out_channels)
             return x._derive(None, indices=rb.coors_out, spatial_shape=rb.shape_out, d_rows=rb.d_rows_out,
@@ -185,14 +185,14 @@ class _SparseConvBase(nn.Module):
             out = torch.empty((x.rows_cap, self.out_channels), dtype=torch.float32, device=wp.device)
             ops.gconv(x._features, wp, scale, shift, out, mode=ops.GCONV_ROWS, taps=1, cin=self.in_channels,
                       cout=self.out_channels, relu=relu, d_rows=x.d_rows, rows_cap=x.rows_cap,
-                      precision=self.precision)
+                      precision=self.precision, status=x.status)
             return x._derive(out)
         rb = self._rulebook(x)
         cap = rb.nbr.shape[0]
         out = torch.empty((cap, self.out_channels), dtype=torch.float32, device=wp.device)
         ops.gconv(x._features, wp, scale, shift, out, mode=ops.GCONV_TABLE, taps=27, cin=self.in_channels,
                   cout=self.out_channels, relu=relu, nbr=rb.nbr, d_rows=rb.d_rows_out, rows_cap=cap,
-                  precision=self.precision)
+                  precision=self.precision, status=x.status)
         if self.subm:
             return x._derive(out)
         return x._derive(out, indices=rb.coors_out, spatial_shape=rb.shape_out, d_rows=rb.d_rows_out,
