@@ -602,6 +602,13 @@ int sassd_kitti_match(int nframes, const double* overlaps, const int64_t* ov_off
                       const double* dt_score, const double* dt_bbox, const double* dc_bbox, const int32_t* ign_gt,
                       const int32_t* ign_dt, int metric, double min_overlap, int compute_aos, int nthresh,
                       const double* thresholds, double* pr, double* tp_scores, int64_t* n_tp_scores);
+/* HOST function: the same matching's assignment for sassd_kitti_eval_assign's table, one (class, difficulty, metric)
+ * of one set (compute_fp=True at a threshold below every score): gt_det[row] the matched detection's row or -1,
+ * gt_ov[row] their overlap (0 when unmatched), dt_state[row] SASSD_KITTI_DT_* of every detection row. */
+int sassd_kitti_assign(int nframes, const double* overlaps, const int64_t* ov_off, const int32_t* gt_off,
+                       const int32_t* dt_off, const int32_t* dc_off, const double* dt_score, const double* dt_bbox,
+                       const double* dc_bbox, const int32_t* ign_gt, const int32_t* ign_dt, int metric,
+                       double min_overlap, int32_t* gt_det, double* gt_ov, int8_t* dt_state);
 
 /* The same cleaning and matching on the device (csrc/kitti_match.cu), for K detection sets against one GT and any
  * number of min-overlap rows, with no per-frame host work.  GT rows of all frames are concatenated (gt_off
@@ -617,6 +624,19 @@ int sassd_kitti_eval_flags(int ngt, const int32_t* gt_name, const double* gt_occ
                            const double* gt_bbox, int ndt, const int32_t* dt_name, const double* dt_bbox, int nclass,
                            const int32_t* classes, int ndiff, const double* limits, int8_t* ign_gt, int8_t* ign_dt,
                            int32_t* n_valid, sassd_stream_t stream);
+/* sassd_kitti_eval_flags with a range bin per difficulty entry.  A row's range is its ground distance from the camera,
+ * sqrt(x * x + z * z) of its camera-frame location (gt_cam / dt_cam rows x, y, z, l, h, w, ry; fp64).  Entry d keeps
+ * the rows with ranges[2d] <= range < ranges[2d+1]: a GT row of the class outside it is flagged 1 (ignored, as a GT
+ * harder than the difficulty is), a detection of the class outside it 1 (as a low one is); other classes and DontCare
+ * rows are not range-tested, and a NaN range falls in no bin.  ranges null, or an entry whose lower edge is -inf, means
+ * no range test.  gt_range / dt_range, when not null, receive every row's range.  With ranges null and no range
+ * outputs this is sassd_kitti_eval_flags, which calls it so. */
+int sassd_kitti_eval_flags_ranged(int ngt, const int32_t* gt_name, const double* gt_occ, const double* gt_trunc,
+                                  const double* gt_bbox, const double* gt_cam, int ndt, const int32_t* dt_name,
+                                  const double* dt_bbox, const double* dt_cam, int nclass, const int32_t* classes,
+                                  int ndiff, const double* limits, const double* ranges, int8_t* ign_gt,
+                                  int8_t* ign_dt, int32_t* n_valid, double* gt_range, double* dt_range,
+                                  sassd_stream_t stream);
 /* The bbox, BEV and 3-D overlap matrices of every (set, frame) block b = k * nframes + f, row-major [detection, GT]
  * at ov_off[b] (fp64, bit for bit the host's image_box_overlap / float32 BEV IoU / _d3_from_bev).  bev_iou and
  * bev_inter are sassd_rotate_overlap_eval's criterion -1 and 2 outputs over the same blocks; cam rows are
@@ -654,6 +674,30 @@ typedef struct {
 size_t sassd_kitti_eval_workspace_bytes(int max_nd, int max_ng);
 int sassd_kitti_eval_match(const SassdKittiEvalDesc* desc, double* scores, int32_t* n_scores, double* thresholds,
                            int32_t* n_thresh, double* pr, void* ws, size_t ws_bytes, sassd_stream_t stream);
+
+/* Match-table states of a detection row (compute_statistics_jit's fate of the detection). */
+#define SASSD_KITTI_DT_NOT_COUNTED 0   /* flag -1 (other class) or 1 (ignored) and not assigned */
+#define SASSD_KITTI_DT_TP 1            /* true positive */
+#define SASSD_KITTI_DT_FP 2            /* false positive */
+#define SASSD_KITTI_DT_DONTCARE 3      /* unassigned, inside a DontCare area (bbox metric only): not a false positive */
+#define SASSD_KITTI_DT_IGNORED 4       /* assigned to an ignored GT, or an ignored detection assigned to a GT */
+
+/* The match table: compute_statistics_jit's assignment (compute_fp=True at a threshold below every score, so every
+ * detection counts) for every (set k, class c, difficulty entry d < ndiff, metric m) at min-overlap row `row` of the
+ * desc (whose flags and overlaps it reads; aos_table, compute_aos, n_valid and score_off are not read).  With G / D the
+ * GT / detection rows of all sets:
+ *   gt_det[(((k * nclass + c) * ndiff + d) * 3 + m) * G + i]   the matched detection's row within set k, or -1;
+ *   gt_ov[same]                                                  their overlap, 0 when unmatched;
+ *   dt_state[((c * ndiff + d) * 3 + m) * D + j]                  SASSD_KITTI_DT_* of detection row j;
+ *   tp_err[(((k * nclass + c) * ndiff + d) * G + i) * 3 + e]     the 3-D metric's TP errors (ATE, ASE, AOE) of GT row
+ *                                                                i, NaN when it has no true positive there.
+ * ATE = sqrt(dx * dx + dz * dz) of the camera-frame centres (detection minus GT); ASE = 1 - vi / ((vg + vd) - vi) with
+ * vi = (min l * min h) * min w and vg, vd = (l * h) * w; AOE = min(|w|, pi) with dr = ry_det - ry_gt and
+ * w = dr - 2pi * floor((dr + pi) / 2pi).  All fp64, rounded operation by operation.  gt_cam / dt_cam are the camera
+ * rows of the flags.  ws as sassd_kitti_eval_match's. */
+int sassd_kitti_eval_assign(const SassdKittiEvalDesc* desc, int row, int ndiff, const double* gt_cam,
+                            const double* dt_cam, int32_t* gt_det, double* gt_ov, int8_t* dt_state, double* tp_err,
+                            void* ws, size_t ws_bytes, sassd_stream_t stream);
 
 /* KITTI label / result files parsed on the device (csrc/kitti_parse.cu), get_label_anno's semantics
  * (tools/kitti_common.py:560-601).  buf holds every file's bytes back to back, file f at [file_off[f], file_off[f+1])

@@ -152,10 +152,25 @@ struct FrameView {
     const int32_t *ign_gt, *ign_dt;
 };
 
-// compute_statistics_jit (:164-283).  Returns tp; fills fp, fn, similarity; appends TP scores when asked.
+// Where frame_statistics records its assignment (sassd_kitti_assign): per GT row the matched detection's row (row0 +
+// its index in the frame) or -1 and their overlap, per detection its SASSD_KITTI_DT_* state.
+struct AssignRecord {
+    int32_t* gt_det;
+    double* gt_ov;
+    int8_t* dt_state;
+    int row0;
+};
+
+// compute_statistics_jit (:164-283).  Returns tp; fills fp, fn, similarity; appends TP scores when asked; records the
+// assignment when `rec` is given.
 int frame_statistics(const FrameView& f, int metric, double min_overlap, double thresh, bool compute_fp, bool compute_aos,
                      int* fp_out, int* fn_out, double* sim_out, double* tp_scores, long long* n_tp_scores,
-                     std::vector<char>& assigned, std::vector<char>& below, std::vector<double>& delta) {
+                     std::vector<char>& assigned, std::vector<char>& below, std::vector<double>& delta,
+                     const AssignRecord* rec = nullptr) {
+    if (rec) {
+        for (int i = 0; i < f.ng; ++i) { rec->gt_det[i] = -1; rec->gt_ov[i] = 0.0; }
+        for (int j = 0; j < f.nd; ++j) rec->dt_state[j] = SASSD_KITTI_DT_NOT_COUNTED;
+    }
     assigned.assign(f.nd, 0);
     below.assign(f.nd, 0);
     delta.clear();
@@ -183,17 +198,26 @@ int frame_statistics(const FrameView& f, int metric, double min_overlap, double 
             ++fn;
         } else if (valid != NO && (f.ign_gt[i] == 1 || f.ign_dt[det] == 1)) {
             assigned[det] = 1;
+            if (rec) rec->dt_state[det] = SASSD_KITTI_DT_IGNORED;
         } else if (valid != NO) {
             ++tp;
             if (tp_scores) tp_scores[(*n_tp_scores)++] = f.dt_score[det];
             if (compute_aos) delta.push_back(f.gt_alpha[i] - f.dt_alpha[det]);
             assigned[det] = 1;
+            if (rec) rec->dt_state[det] = SASSD_KITTI_DT_TP;
+        }
+        if (rec && valid != NO) {
+            rec->gt_det[i] = rec->row0 + det;
+            rec->gt_ov[i] = f.ov[(size_t)det * f.ng + i];
         }
     }
     double similarity = 0;
     if (compute_fp) {
         for (int j = 0; j < f.nd; ++j)
-            if (!(assigned[j] || f.ign_dt[j] == -1 || f.ign_dt[j] == 1 || below[j])) ++fp;
+            if (!(assigned[j] || f.ign_dt[j] == -1 || f.ign_dt[j] == 1 || below[j])) {
+                ++fp;
+                if (rec) rec->dt_state[j] = SASSD_KITTI_DT_FP;
+            }
         int nstuff = 0;
         if (metric == 0)
             for (int i = 0; i < f.ndc; ++i)
@@ -202,6 +226,7 @@ int frame_statistics(const FrameView& f, int metric, double min_overlap, double 
                     if (box_overlap_first(f.dt_bbox + 4 * (size_t)j, f.dc_bbox + 4 * (size_t)i) > min_overlap) {
                         assigned[j] = 1;
                         ++nstuff;
+                        if (rec) rec->dt_state[j] = SASSD_KITTI_DT_DONTCARE;
                     }
                 }
         fp -= nstuff;
@@ -291,5 +316,32 @@ extern "C" int sassd_kitti_match(int nframes, const double* overlaps, const int6
         }
     }
     if (n_tp_scores) *n_tp_scores = ntp;
+    return SASSD_OK;
+}
+
+// Host function: frame_statistics' assignment at a threshold below every score, recorded frame by frame.
+extern "C" int sassd_kitti_assign(int nframes, const double* overlaps, const int64_t* ov_off, const int32_t* gt_off,
+                                  const int32_t* dt_off, const int32_t* dc_off, const double* dt_score,
+                                  const double* dt_bbox, const double* dc_bbox, const int32_t* ign_gt,
+                                  const int32_t* ign_dt, int metric, double min_overlap, int32_t* gt_det, double* gt_ov,
+                                  int8_t* dt_state) {
+    if (nframes < 0 || !ov_off || !gt_off || !dt_off || !dc_off || metric < 0 || metric > 2) return SASSD_ERR_ARG;
+    if (nframes > 0 && (gt_off[nframes] > 0 && (!gt_det || !gt_ov || !ign_gt))) return SASSD_ERR_ARG;
+    if (nframes > 0 && (dt_off[nframes] > 0 && (!dt_state || !ign_dt || !dt_score || !dt_bbox))) return SASSD_ERR_ARG;
+    std::vector<char> assigned, below;
+    std::vector<double> delta;
+    for (int f = 0; f < nframes; ++f) {
+        FrameView v;
+        v.ng = gt_off[f + 1] - gt_off[f]; v.nd = dt_off[f + 1] - dt_off[f]; v.ndc = dc_off[f + 1] - dc_off[f];
+        v.ov = overlaps + ov_off[f];
+        v.gt_alpha = nullptr; v.dt_alpha = nullptr; v.dt_score = dt_score + dt_off[f];
+        v.dt_bbox = dt_bbox + 4 * (size_t)dt_off[f]; v.dc_bbox = dc_bbox + 4 * (size_t)dc_off[f];
+        v.ign_gt = ign_gt + gt_off[f]; v.ign_dt = ign_dt + dt_off[f];
+        AssignRecord rec{gt_det + gt_off[f], gt_ov + gt_off[f], dt_state + dt_off[f], dt_off[f]};
+        int fp, fn;
+        double sim;
+        frame_statistics(v, metric, min_overlap, -INFINITY, true, false, &fp, &fn, &sim, nullptr, nullptr, assigned,
+                         below, delta, &rec);
+    }
     return SASSD_OK;
 }

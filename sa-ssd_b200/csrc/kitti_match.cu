@@ -31,15 +31,33 @@ __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a,
 __device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
 
 // ------------------------------------------------------------------------------------------------------ flags
+// The ground distance of a camera-frame row (x, y, z, ...): sqrt(x * x + z * z), numpy's operation order.
+__device__ __forceinline__ double ground_range(const double* cam) {
+    return __dsqrt_rn(dadd(dmul(cam[0], cam[0]), dmul(cam[2], cam[2])));
+}
+
+// Whether range r falls in difficulty entry d's bin [ranges[2d], ranges[2d+1]).  No ranges, or an entry whose lower
+// edge is -inf, means no range test (every row, a NaN range included); otherwise a NaN range falls in no bin.
+__device__ __forceinline__ bool in_bin(const double* ranges, int d, double r) {
+    if (!ranges) return true;
+    const double lo = ranges[2 * d], hi = ranges[2 * d + 1];
+    return lo == -INFINITY || (lo <= r && r < hi);
+}
+
 // clean_data (kitti_eval.py:39-92) for every row: GT flags 0 evaluate / 1 ignore / -1 other class, detection flags
 // 1 too low / 0 the class / -1 other class.  limits[3 * d + (0, 1, 2)] = (max occlusion, max truncation, min height)
 // of difficulty entry d; classes[2 * c] is class c's name id, classes[2 * c + 1] the id of the name that counts as
-// "don't care" for it (van for car, person_sitting for pedestrian) or -1.
+// "don't care" for it (van for car, person_sitting for pedestrian) or -1.  With ranges, a GT row of the class outside
+// entry d's bin is ignored (1) as a GT harder than the difficulty is, and a detection of the class outside it is
+// ignored (1) as a low one is; gt_range / dt_range (when given) receive every row's ground distance.
 __global__ void eval_flags_kernel(int ngt, const int32_t* __restrict__ gt_name, const double* __restrict__ gt_occ,
-                                  const double* __restrict__ gt_trunc, const double* __restrict__ gt_bbox, int ndt,
-                                  const int32_t* __restrict__ dt_name, const double* __restrict__ dt_bbox, int nclass,
+                                  const double* __restrict__ gt_trunc, const double* __restrict__ gt_bbox,
+                                  const double* __restrict__ gt_cam, int ndt, const int32_t* __restrict__ dt_name,
+                                  const double* __restrict__ dt_bbox, const double* __restrict__ dt_cam, int nclass,
                                   const int32_t* __restrict__ classes, int ndiff, const double* __restrict__ limits,
-                                  int8_t* __restrict__ ign_gt, int8_t* __restrict__ ign_dt, int32_t* __restrict__ n_valid) {
+                                  const double* __restrict__ ranges, int8_t* __restrict__ ign_gt,
+                                  int8_t* __restrict__ ign_dt, int32_t* __restrict__ n_valid,
+                                  double* __restrict__ gt_range, double* __restrict__ dt_range) {
     const long long rows = (long long)ngt + ndt, total = rows * nclass * ndiff;
     for (long long w = blockIdx.x * (long long)blockDim.x + threadIdx.x; w < total; w += (long long)gridDim.x * blockDim.x) {
         const int cd = (int)(w / rows), c = cd / ndiff, d = cd % ndiff;
@@ -47,17 +65,22 @@ __global__ void eval_flags_kernel(int ngt, const int32_t* __restrict__ gt_name, 
         const int cls = classes[2 * c], alt = classes[2 * c + 1];
         const double max_occ = limits[3 * d], max_trunc = limits[3 * d + 1], min_h = limits[3 * d + 2];
         if (r < ngt) {
+            const double rg = (ranges || gt_range) ? ground_range(gt_cam + 7 * r) : 0.0;
+            if (cd == 0 && gt_range) gt_range[r] = rg;
             const int nm = gt_name[r];
             const int valid = nm == cls ? 1 : (alt >= 0 && nm == alt ? 0 : -1);
             const double h = dsub(gt_bbox[4 * r + 3], gt_bbox[4 * r + 1]);
-            const bool ignore = gt_occ[r] > max_occ || gt_trunc[r] > max_trunc || h <= min_h;
+            const bool ignore = gt_occ[r] > max_occ || gt_trunc[r] > max_trunc || h <= min_h || !in_bin(ranges, d, rg);
             const int f = (valid == 1 && !ignore) ? 0 : ((valid == 0 || (ignore && valid == 1)) ? 1 : -1);
             ign_gt[(long long)cd * ngt + r] = (int8_t)f;
             if (f == 0) atomicAdd(&n_valid[cd], 1);
         } else {
             const long long j = r - ngt;
+            const double rd = (ranges || dt_range) ? ground_range(dt_cam + 7 * j) : 0.0;
+            if (cd == 0 && dt_range) dt_range[j] = rd;
             const double h = fabs(dsub(dt_bbox[4 * j + 3], dt_bbox[4 * j + 1]));
-            ign_dt[(long long)cd * ndt + j] = (int8_t)(h < min_h ? 1 : (dt_name[j] == cls ? 0 : -1));
+            ign_dt[(long long)cd * ndt + j] =
+                (int8_t)(h < min_h ? 1 : (dt_name[j] == cls ? (in_bin(ranges, d, rd) ? 0 : 1) : -1));
         }
     }
 }
@@ -290,12 +313,27 @@ __device__ double pairwise_sum(const double* vals, int nz, int n) {
     }
 }
 
-// compute_statistics_jit with compute_fp=True (kitti_eval.py:164-283) for one frame at one threshold.
+// Where frame_statistics records its assignment (the match table): per GT row the matched detection (its row in the
+// set, or -1) and their overlap (0 when unmatched); per detection row its SASSD_KITTI_DT_* state.
+struct Record {
+    int32_t* gt_det;
+    double* gt_ov;
+    int8_t* dt_state;
+    int row0;            // the set's row of the frame's first detection
+};
+
+// compute_statistics_jit with compute_fp=True (kitti_eval.py:164-283) for one frame at one threshold; with kRecord
+// also the frame's assignment into `rec`.
+template <bool kRecord>
 __device__ void frame_statistics(const Frame& fr, int metric, double min_ov, double thresh, char* asg, double* vals,
-                                 int* tp_out, int* fp_out, int* fn_out, double* sim_out) {
+                                 int* tp_out, int* fp_out, int* fn_out, double* sim_out, const Record& rec = Record{}) {
     const long long S = kScratchThreads;
     int tp = 0, fp = 0, fn = 0, nv = 0;
     for (int j = 0; j < fr.nd; ++j) asg[j * S] = 0;
+    if constexpr (kRecord) {
+        for (int i = 0; i < fr.ng; ++i) { rec.gt_det[i] = -1; rec.gt_ov[i] = 0.0; }
+        for (int j = 0; j < fr.nd; ++j) rec.dt_state[j] = SASSD_KITTI_DT_NOT_COUNTED;
+    }
     for (int i = 0; i < fr.ng; ++i) {
         const int gi = fr.igt[i];
         if (gi == -1) continue;
@@ -316,14 +354,24 @@ __device__ void frame_statistics(const Frame& fr, int metric, double min_ov, dou
             ++fn;
         } else if (valid != kNo && (gi == 1 || fr.idt[det] == 1)) {
             asg[det * S] = 1;
+            if constexpr (kRecord) rec.dt_state[det] = SASSD_KITTI_DT_IGNORED;
         } else if (valid != kNo) {
             ++tp;
             if (fr.aos) vals[(long long)nv++ * S] = fr.aos[(long long)det * fr.ng + i];
             asg[det * S] = 1;
+            if constexpr (kRecord) rec.dt_state[det] = SASSD_KITTI_DT_TP;
         }
+        if constexpr (kRecord)
+            if (valid != kNo) {
+                rec.gt_det[i] = rec.row0 + det;
+                rec.gt_ov[i] = fr.ov[(long long)det * fr.ng + i];
+            }
     }
     for (int j = 0; j < fr.nd; ++j)
-        if (!(asg[j * S] || fr.idt[j] == -1 || fr.idt[j] == 1 || fr.score[j] < thresh)) ++fp;
+        if (!(asg[j * S] || fr.idt[j] == -1 || fr.idt[j] == 1 || fr.score[j] < thresh)) {
+            ++fp;
+            if constexpr (kRecord) rec.dt_state[j] = SASSD_KITTI_DT_FP;
+        }
     int nstuff = 0;
     if (metric == 0)
         for (int i = 0; i < fr.ng; ++i) {
@@ -339,6 +387,7 @@ __device__ void frame_statistics(const Frame& fr, int metric, double min_ov, dou
                 if (ddiv(dmul(iw, ih), dmul(dsub(b[2], b[0]), dsub(b[3], b[1]))) > min_ov) {
                     asg[j * S] = 1;
                     ++nstuff;
+                    if constexpr (kRecord) rec.dt_state[j] = SASSD_KITTI_DT_DONTCARE;
                 }
             }
         }
@@ -375,7 +424,7 @@ __global__ void __launch_bounds__(kMatchThreads) eval_pr_kernel(SassdKittiEvalDe
             double sim = -1.0;
             if (f < e.nframes) {
                 int a, b, c;
-                frame_statistics(frame_of(e, jb, f), jb.m, min_ov, thresh, asg, vals, &a, &b, &c, &sim);
+                frame_statistics<false>(frame_of(e, jb, f), jb.m, min_ov, thresh, asg, vals, &a, &b, &c, &sim);
                 tp += a; fp += b; fn += c;
             }
             if (aos) {
@@ -405,20 +454,98 @@ __global__ void __launch_bounds__(kMatchThreads) eval_pr_kernel(SassdKittiEvalDe
     }
 }
 
+// ------------------------------------------------------------------------------------------------- match table
+constexpr double kPi = 3.141592653589793, kTwoPi = 6.283185307179586;
+
+// The TP errors of a 3-D-metric true positive, GT row g against detection row q (camera rows x, y, z, l, h, w, ry):
+// ATE the BEV centre distance, ASE 1 - IoU of the boxes aligned at one centre and heading, AOE the heading difference
+// wrapped to [0, pi].  fp64 in a fixed order with sqrt the only non-arithmetic operation, as kitti_eval.tp_errors.
+__device__ void tp_errors(const double* g, const double* q, double* out) {
+    const double dx = dsub(q[0], g[0]), dz = dsub(q[2], g[2]);
+    out[0] = __dsqrt_rn(dadd(dmul(dx, dx), dmul(dz, dz)));
+    const double vi = dmul(dmul(fmin(q[3], g[3]), fmin(q[4], g[4])), fmin(q[5], g[5]));
+    const double vg = dmul(dmul(g[3], g[4]), g[5]), vd = dmul(dmul(q[3], q[4]), q[5]);
+    out[1] = dsub(1.0, ddiv(vi, dsub(dadd(vg, vd), vi)));
+    const double d = dsub(q[6], g[6]);
+    out[2] = fmin(fabs(dsub(d, dmul(kTwoPi, floor(ddiv(dadd(d, kPi), kTwoPi))))), kPi);
+}
+
+// compute_statistics_jit's assignment (compute_fp=True, a threshold below every score) of every (set, class,
+// difficulty entry < ndiff, metric) job at min-overlap row `row`, one thread per (job, frame), written out instead of
+// summed; each 3-D-metric job also writes its TP errors (NaN for a GT row without a true positive).
+__global__ void __launch_bounds__(kMatchThreads) eval_assign_kernel(SassdKittiEvalDesc e, int row, int ndiff,
+                                                                  long long njobs, char* __restrict__ asg_ws,
+                                                                  const double* __restrict__ gt_cam,
+                                                                  const double* __restrict__ dt_cam,
+                                                                  int32_t* __restrict__ gt_det,
+                                                                  double* __restrict__ gt_ov,
+                                                                  int8_t* __restrict__ dt_state,
+                                                                  double* __restrict__ tp_err) {
+    const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    char* asg = asg_ws + tid;
+    const long long ngt = e.gt_off[e.nframes], ndt = e.dt_off[e.nsets * e.nframes];
+    for (long long w = tid; w < njobs * e.nframes; w += kScratchThreads) {
+        const long long job = w / e.nframes;             // ((k * nclass + c) * ndiff + d) * 3 + m
+        const int f = (int)(w % e.nframes);
+        Job jb;
+        jb.m = (int)(job % 3);
+        jb.d = (int)(job / 3 % ndiff);
+        jb.c = (int)(job / 3 / ndiff % e.nclass);
+        jb.k = (int)(job / 3 / ndiff / e.nclass);
+        jb.o = row;
+        Frame fr = frame_of(e, jb, f);
+        fr.aos = nullptr;                                // the table sums no AOS similarity: no `vals` scratch
+        const int b = jb.k * e.nframes + f, g0 = e.gt_off[f], d0 = e.dt_off[b];
+        const long long cdm = ((long long)jb.c * ndiff + jb.d) * 3 + jb.m;
+        Record rec;
+        rec.gt_det = gt_det + job * ngt + g0;
+        rec.gt_ov = gt_ov + job * ngt + g0;
+        rec.dt_state = dt_state + cdm * ndt + d0;
+        rec.row0 = d0 - e.dt_off[jb.k * e.nframes];
+        int tp, fp, fn;
+        double sim;
+        frame_statistics<true>(fr, jb.m, min_overlap_of(e, jb), -INFINITY, asg, nullptr, &tp, &fp, &fn, &sim, rec);
+        if (jb.m != 2) continue;
+        double* err = tp_err + ((((long long)jb.k * e.nclass + jb.c) * ndiff + jb.d) * ngt + g0) * 3;
+        for (int i = 0; i < fr.ng; ++i) {
+            const int j = rec.gt_det[i] - rec.row0;
+            if (j >= 0 && rec.dt_state[j] == SASSD_KITTI_DT_TP) {
+                tp_errors(gt_cam + 7 * (long long)(g0 + i), dt_cam + 7 * (long long)(d0 + j), err + 3 * i);
+            } else {
+                err[3 * i] = err[3 * i + 1] = err[3 * i + 2] = __longlong_as_double(0x7ff8000000000000LL);
+            }
+        }
+    }
+}
+
 }  // namespace
 
 extern "C" int sassd_kitti_eval_flags(int ngt, const int32_t* gt_name, const double* gt_occ, const double* gt_trunc,
                                       const double* gt_bbox, int ndt, const int32_t* dt_name, const double* dt_bbox,
                                       int nclass, const int32_t* classes, int ndiff, const double* limits,
                                       int8_t* ign_gt, int8_t* ign_dt, int32_t* n_valid, sassd_stream_t stream) {
+    return sassd_kitti_eval_flags_ranged(ngt, gt_name, gt_occ, gt_trunc, gt_bbox, nullptr, ndt, dt_name, dt_bbox,
+                                         nullptr, nclass, classes, ndiff, limits, nullptr, ign_gt, ign_dt, n_valid,
+                                         nullptr, nullptr, stream);
+}
+
+extern "C" int sassd_kitti_eval_flags_ranged(int ngt, const int32_t* gt_name, const double* gt_occ,
+                                             const double* gt_trunc, const double* gt_bbox, const double* gt_cam,
+                                             int ndt, const int32_t* dt_name, const double* dt_bbox,
+                                             const double* dt_cam, int nclass, const int32_t* classes, int ndiff,
+                                             const double* limits, const double* ranges, int8_t* ign_gt,
+                                             int8_t* ign_dt, int32_t* n_valid, double* gt_range, double* dt_range,
+                                             sassd_stream_t stream) {
     if (ngt < 0 || ndt < 0 || nclass < 1 || ndiff < 1 || !classes || !limits || !n_valid) return SASSD_ERR_ARG;
     if (ngt > 0 && (!gt_name || !gt_occ || !gt_trunc || !gt_bbox || !ign_gt)) return SASSD_ERR_ARG;
     if (ndt > 0 && (!dt_name || !dt_bbox || !ign_dt)) return SASSD_ERR_ARG;
+    if (ngt > 0 && (ranges || gt_range) && !gt_cam) return SASSD_ERR_ARG;
+    if (ndt > 0 && (ranges || dt_range) && !dt_cam) return SASSD_ERR_ARG;
     const long long total = ((long long)ngt + ndt) * nclass * ndiff;
     if (total == 0) return SASSD_OK;
     eval_flags_kernel<<<sassd_grid(total, 256), 256, 0, (cudaStream_t)stream>>>(
-        ngt, gt_name, gt_occ, gt_trunc, gt_bbox, ndt, dt_name, dt_bbox, nclass, classes, ndiff, limits, ign_gt, ign_dt,
-        n_valid);
+        ngt, gt_name, gt_occ, gt_trunc, gt_bbox, gt_cam, ndt, dt_name, dt_bbox, dt_cam, nclass, classes, ndiff, limits,
+        ranges, ign_gt, ign_dt, n_valid, gt_range, dt_range);
     return sassd_check_launch();
 }
 
@@ -485,4 +612,22 @@ extern "C" int sassd_kitti_aos_table(int nsets, int nframes, const int32_t* gt_o
             for (int i = 0; i < ng; ++i) o[(size_t)j * ng + i] = (1.0 + std::cos(gt_alpha[g0 + i] - dt_alpha[d0 + j])) / 2.0;
     }
     return SASSD_OK;
+}
+
+extern "C" int sassd_kitti_eval_assign(const SassdKittiEvalDesc* e, int row, int ndiff, const double* gt_cam,
+                                       const double* dt_cam, int32_t* gt_det, double* gt_ov, int8_t* dt_state,
+                                       double* tp_err, void* ws, size_t ws_bytes, sassd_stream_t stream) {
+    if (!e || e->nsets < 1 || e->nframes < 0 || e->nclass < 1 || e->ndiff < 1 || e->nover < 1 || e->max_nd < 0 ||
+        e->max_ng < 0 || row < 0 || row >= e->nover || ndiff < 1 || ndiff > e->ndiff)
+        return SASSD_ERR_ARG;
+    if (!e->gt_off || !e->dt_off || !e->ov_off || !e->gt_dc || !e->gt_bbox || !e->dt_bbox || !e->dt_score ||
+        !e->ov_bbox || !e->ov_bev || !e->ov_3d || !e->min_overlaps || !e->ign_gt || !e->ign_dt || !gt_cam || !dt_cam ||
+        !gt_det || !gt_ov || !dt_state || !tp_err || !ws)
+        return SASSD_ERR_ARG;
+    if (ws_bytes < sassd_kitti_eval_workspace_bytes(e->max_nd, e->max_ng)) return SASSD_ERR_WORKSPACE;
+    if (e->nframes == 0) return SASSD_OK;
+    const long long njobs = (long long)e->nsets * e->nclass * ndiff * 3;
+    eval_assign_kernel<<<kMatchCtas, kMatchThreads, 0, (cudaStream_t)stream>>>(*e, row, ndiff, njobs, (char*)ws, gt_cam,
+                                                                             dt_cam, gt_det, gt_ov, dt_state, tp_err);
+    return sassd_check_launch();
 }

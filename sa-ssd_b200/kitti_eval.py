@@ -20,8 +20,12 @@ Both paths give the same arrays bit for bit.  Annotations are dicts of numpy arr
 AnnoBlock: the same rows as flat columns on the device, built from dicts or parsed from a directory of KITTI files on
 the device (`read_block`, csrc/kitti_parse.cu).
 
+``eval_many(..., ranges=[e0, e1, ...])`` adds every table per bin [e_i, e_i+1) of ground distance from the camera (more
+difficulty entries of the same evaluation), and ``match_table`` / ``eval_many(..., match=True)`` the evaluator's own
+per-object assignment with the 3-D true positives' ATE / ASE / AOE (``tp_errors``).
+
     python -m sassd_b200.kitti_eval --data-root DIR [--split val] --results DIR [DIR ...] [--classes Car ...]
-                                    [--r40] [--coco] [--json FILE]
+                                    [--r40] [--coco] [--json FILE] [--ranges EDGE ...] [--matches FILE.npz]
 
 evaluates directories of result files against a split's labels (`main`, `eval_dirs`).
 """
@@ -176,13 +180,26 @@ def calculate_overlaps_many(gt_annos, dt_sets, metric, overlap_fn=None):
 
 
 # ------------------------------------------------------------------ matching
-def clean_data(gt_anno, dt_anno, current_class, difficulty):
+def clean_data(gt_anno, dt_anno, current_class, difficulty, rng=None):
     """Ignore flags of one frame (kitti_eval.py:39-92): 0 evaluate, 1 ignore, -1 other class."""
-    return clean_gt(gt_anno, current_class, difficulty) + (clean_dt(dt_anno, current_class, difficulty),)
+    return clean_gt(gt_anno, current_class, difficulty, rng) + (clean_dt(dt_anno, current_class, difficulty, rng),)
 
 
-def clean_gt(gt_anno, current_class, difficulty):
-    """clean_data's GT side: (valid GT count, GT ignore flags, DontCare boxes)."""
+def ground_range(anno):
+    """Each row's ground distance from the camera: sqrt(x * x + z * z) of its camera-frame location, fp64."""
+    loc = np.asarray(anno["location"], np.float64).reshape(-1, 3)
+    return np.sqrt(loc[:, 0] * loc[:, 0] + loc[:, 2] * loc[:, 2])
+
+
+def _in_bin(anno, rng):
+    """Rows whose ground range lies in the bin ``rng`` = (lo, hi), lo <= range < hi; a NaN range lies in no bin."""
+    r = ground_range(anno)
+    return (rng[0] <= r) & (r < rng[1])
+
+
+def clean_gt(gt_anno, current_class, difficulty, rng=None):
+    """clean_data's GT side: (valid GT count, GT ignore flags, DontCare boxes).  ``rng`` = (lo, hi): a GT of the class
+    outside that range bin is ignored (1), as one harder than the difficulty is."""
     cls = CLASS_NAMES[current_class].lower()
     names = np.char.lower(np.asarray(gt_anno["name"], dtype=str)) if len(gt_anno["name"]) else np.zeros((0,), str)
     bbox = np.asarray(gt_anno["bbox"], np.float64).reshape(-1, 4)
@@ -194,18 +211,22 @@ def clean_gt(gt_anno, current_class, difficulty):
     ignore = ((np.asarray(gt_anno["occluded"]) > MAX_OCCLUSION[difficulty])
               | (np.asarray(gt_anno["truncated"]) > MAX_TRUNCATION[difficulty])
               | ((bbox[:, 3] - bbox[:, 1]) <= MIN_HEIGHT[difficulty]))
+    if rng is not None:
+        ignore = ignore | ~_in_bin(gt_anno, rng)
     ign_gt = np.where((valid == 1) & ~ignore, 0, np.where((valid == 0) | (ignore & (valid == 1)), 1, -1)).astype(np.int32)
     dc = bbox[np.asarray(gt_anno["name"], dtype=str) == "DontCare"] if len(names) else np.zeros((0, 4))
     return int((ign_gt == 0).sum()), ign_gt, dc
 
 
-def clean_dt(dt_anno, current_class, difficulty):
-    """clean_data's detection side: the detections' ignore flags."""
+def clean_dt(dt_anno, current_class, difficulty, rng=None):
+    """clean_data's detection side: the detections' ignore flags.  ``rng`` = (lo, hi): a detection of the class
+    outside that range bin is ignored (1), as a low one is."""
     cls = CLASS_NAMES[current_class].lower()
     dnames = np.char.lower(np.asarray(dt_anno["name"], dtype=str)) if len(dt_anno["name"]) else np.zeros((0,), str)
     dbox = np.asarray(dt_anno["bbox"], np.float64).reshape(-1, 4)
     height = np.abs(dbox[:, 3] - dbox[:, 1])
-    return np.where(height < MIN_HEIGHT[difficulty], 1, np.where(dnames == cls, 0, -1)).astype(np.int32)
+    own = 0 if rng is None else np.where(_in_bin(dt_anno, rng), 0, 1)
+    return np.where(height < MIN_HEIGHT[difficulty], 1, np.where(dnames == cls, own, -1)).astype(np.int32)
 
 
 def get_thresholds(scores, num_gt, num_sample_pts=41):
@@ -230,8 +251,8 @@ class _GtSide:
     """The GT half of sassd_kitti_match's flat arrays for one (class, difficulty): clean_gt of every frame, flattened.
     Every detection set evaluated against the same GT shares it."""
 
-    def __init__(self, gt_annos, current_class, difficulty):
-        prep = [clean_gt(g, current_class, difficulty) for g in gt_annos]
+    def __init__(self, gt_annos, current_class, difficulty, rng=None):
+        prep = [clean_gt(g, current_class, difficulty, rng) for g in gt_annos]
         self.nframes = len(gt_annos)
         self.total_valid = sum(p[0] for p in prep)
         self.ng = [len(p[1]) for p in prep]
@@ -245,8 +266,8 @@ class _GtSide:
 class _Packed:
     """Per-(class, difficulty) flat arrays for sassd_kitti_match: a _GtSide and one detection set's half."""
 
-    def __init__(self, gt, dt_annos, overlaps, current_class, difficulty):
-        ign_dt = [clean_dt(d, current_class, difficulty) for d in dt_annos]
+    def __init__(self, gt, dt_annos, overlaps, current_class, difficulty, rng=None):
+        ign_dt = [clean_dt(d, current_class, difficulty, rng) for d in dt_annos]
         self.gt = gt
         self.nframes, self.total_valid = gt.nframes, gt.total_valid
         nd = [len(i) for i in ign_dt]
@@ -273,6 +294,20 @@ class _Packed:
                                        _p(ntp)), "sassd_kitti_match")
         return pr[:nth], tp_scores[:int(ntp[0])]
 
+    def assign(self, metric, min_overlap):
+        """The match table's columns of this (class, difficulty) at one metric (sassd_kitti_assign): per GT row the
+        matched detection's row or -1 and their overlap, per detection row its lib.KITTI_DT_* state."""
+        g = self.gt
+        gt_det = np.zeros((len(g.ign_gt),), np.int32)
+        gt_ov = np.zeros((len(g.ign_gt),), np.float64)
+        state = np.zeros((len(self.ign_dt),), np.int8)
+        _lib.check(_lib.load().sassd_kitti_assign(self.nframes, _p(self.overlaps), _p(self.ov_off), _p(g.gt_off),
+                                                  _p(self.dt_off), _p(g.dc_off), _p(self.dt_score), _p(self.dt_bbox),
+                                                  _p(g.dc_bbox), _p(g.ign_gt), _p(self.ign_dt), int(metric),
+                                                  float(min_overlap), _p(gt_det), _p(gt_ov), _p(state)),
+                   "sassd_kitti_assign")
+        return gt_det, gt_ov, state
+
 
 def eval_class(gt_annos, dt_annos, current_classes, difficultys, metric, min_overlaps, compute_aos=False,
                overlap_fn=None):
@@ -283,19 +318,21 @@ def eval_class(gt_annos, dt_annos, current_classes, difficultys, metric, min_ove
 
 
 def eval_class_many(gt_annos, dt_sets, current_classes, difficultys, metric, min_overlaps, compute_aos, overlap_fn=None,
-                    gt_sides=None):
+                    gt_sides=None, bins=None):
     """eval_class for each detection set of ``dt_sets`` against the same GT (``compute_aos``: one flag per set): one
-    overlap pass for all sets (calculate_overlaps_many) and one GT side per class and difficulty (``gt_sides``:
-    {(class, difficulty): _GtSide}, built here when not given)."""
+    overlap pass for all sets (calculate_overlaps_many) and one GT side per class and difficulty entry (``gt_sides``:
+    {(class, difficulty, bin): _GtSide}, built here when not given).  ``bins``: a range bin (lo, hi) or None per entry
+    of ``difficultys`` (clean_gt / clean_dt's ``rng``); None: no bins."""
     assert all(len(gt_annos) == len(d) for d in dt_sets)
+    bins = [None] * len(difficultys) if bins is None else list(bins)
     overlaps = calculate_overlaps_many(gt_annos, dt_sets, metric, overlap_fn)
     shape = (len(current_classes), len(difficultys), len(min_overlaps), 41)
     out = [dict(recall=np.zeros(shape), precision=np.zeros(shape), orientation=np.zeros(shape)) for _ in dt_sets]
     for m, cls in enumerate(current_classes):
-        for l, diff in enumerate(difficultys):
-            gt = _GtSide(gt_annos, cls, diff) if gt_sides is None else gt_sides[cls, diff]
+        for l, (diff, rng) in enumerate(zip(difficultys, bins)):
+            gt = _GtSide(gt_annos, cls, diff, rng) if gt_sides is None else gt_sides[cls, diff, rng]
             for dt_annos, ov, aos_s, res in zip(dt_sets, overlaps, compute_aos, out):
-                packed = _Packed(gt, dt_annos, ov, cls, diff)
+                packed = _Packed(gt, dt_annos, ov, cls, diff, rng)
                 recall, precision, aos = res["recall"], res["precision"], res["orientation"]
                 for k, min_overlap in enumerate(min_overlaps[:, metric, m]):
                     _, tp_scores = packed.match(metric, min_overlap)
@@ -481,6 +518,15 @@ def _eval_device(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flag
     dict of [class, difficulty, min_overlap, 41], with the flags, overlaps, matching, thresholds and per-threshold sums
     on the device (csrc/kitti_match.cu); bit for bit what the host path computes.  The GT and each detection set are
     AnnoBlocks (lists of annotation dicts are flattened into one first)."""
+    return _eval_device_full(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flags)[0]
+
+
+def _eval_device_full(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flags, bins=None, assign=None,
+                      ap=True):
+    """_eval_device with a range bin (lo, hi) or None per difficulty entry (``bins``), and with ``assign`` = (row,
+    ndiff) also the match table of the first ndiff entries at min-overlap row ``row`` (match_table's dicts, one per
+    set), from the flags and overlaps already on the device.  ``ap`` False skips the AP matching (the arrays are then
+    None).  Returns (arrays, tables)."""
     import torch
     from . import ops
     dev = _cuda_device()
@@ -507,8 +553,16 @@ def _eval_device(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flag
     t = dict(gt_off=up(gt_off), dt_off=up(dt_off), ov_off=up(ov_off), gt_dc=gt.dontcare, gt_bbox=gt.bbox,
              dt_bbox=dt_bbox, dt_score=torch.cat([d.score for d in dts]), gt_cam=gt.cam, dt_cam=dt_cam,
              min_overlaps=up(np.asarray(min_overlaps, np.float64)), compute_aos=up(np.asarray(aos_flags, np.int32)))
-    ign_gt, ign_dt, n_valid = ops.kitti_eval_flags(gt.name_id, gt.occluded, gt.truncated, t["gt_bbox"], dt_name,
-                                                   t["dt_bbox"], up(cls_ids), up(limits))
+    ranged = bins is not None and any(b is not None for b in bins)
+    if ranged or assign is not None:
+        # an entry without a bin has a lower edge of -inf: no range test
+        ranges = up(np.array([(-np.inf, np.inf) if b is None else b for b in bins], np.float64)) if ranged else None
+        ign_gt, ign_dt, n_valid, gt_range, dt_range = ops.kitti_eval_flags_ranged(
+            gt.name_id, gt.occluded, gt.truncated, t["gt_bbox"], gt.cam, dt_name, t["dt_bbox"], dt_cam, up(cls_ids),
+            up(limits), ranges)
+    else:
+        ign_gt, ign_dt, n_valid = ops.kitti_eval_flags(gt.name_id, gt.occluded, gt.truncated, t["gt_bbox"], dt_name,
+                                                       t["dt_bbox"], up(cls_ids), up(limits))
     # the rotated overlaps of every (set, frame) block: BEV IoU and the intersection area the 3-D overlap builds on
     bev = [0, 2, 3, 5, 6]
     dt_bev, gt_bev = dt_cam[:, bev].float().contiguous(), gt.cam[:, bev].float().repeat(K, 1)
@@ -542,6 +596,23 @@ def _eval_device(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flag
                 ov_3d=ov[2], aos_table=aos_table)
     for name, _ in desc._fields_[7:]:
         setattr(desc, name, keep[name].data_ptr() if keep[name] is not None else None)
+    tables = None
+    if assign is not None:
+        row, nd_t = assign
+        gt_det, gt_ov, dt_state, tp_err = (x.cpu().numpy() for x in ops.kitti_eval_assign(desc, row, nd_t, gt.cam,
+                                                                                            dt_cam))
+        gt_flag, dt_flag = ign_gt[:, :nd_t].cpu().numpy(), ign_dt[:, :nd_t].cpu().numpy()
+        gt_range, dt_range = gt_range.cpu().numpy(), dt_range.cpu().numpy()
+        rows = _offsets([int(d.off[-1]) for d in dts], np.int64)
+        tables = []
+        for k in range(K):
+            r = slice(rows[k], rows[k + 1])
+            tables.append(dict(gt_off=gt.off.copy(), dt_off=dts[k].off.copy(), gt_range=gt_range, dt_range=dt_range[r],
+                               gt_flag=gt_flag, dt_flag=np.ascontiguousarray(dt_flag[..., r]), gt_det=gt_det[k],
+                               gt_overlap=gt_ov[k], dt_state=np.ascontiguousarray(dt_state[..., r]),
+                               tp_errors=tp_err[k]))
+    if not ap:
+        return None, tables
     _, n_thresh, pr = ops.kitti_eval_match(desc, len(region), int(region.sum()))
     n_thresh = n_thresh.cpu().numpy().reshape(K, C, Dn, 3, M)
     pr = pr.cpu().numpy().reshape(K, C, Dn, 3, M, 41, 4)
@@ -563,7 +634,7 @@ def _eval_device(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flag
                 res[key] = np.ascontiguousarray(np.maximum.accumulate(v[..., ::-1], axis=-1)[..., ::-1])
             per_set.append(res)
         out.append(per_set)
-    return out
+    return out, tables
 
 
 def get_mAP(prec):
@@ -622,51 +693,177 @@ def _aos_flag(dt_annos):
     return False
 
 
-def eval_many(gt_annos, dt_sets, classes, tables=(11,), overlap_fn=None, difficultys=(0, 1, 2)):
+def check_ranges(ranges):
+    """The range bin edges e0 < e1 < ... as a tuple of floats: at least two, non-negative and strictly increasing (the
+    last may be inf); anything else is a ValueError."""
+    try:
+        edges = np.asarray(ranges, np.float64).reshape(-1)
+    except (TypeError, ValueError):
+        raise ValueError("ranges must be numbers, not %r" % (ranges,)) from None
+    with np.errstate(invalid="ignore"):
+        bad = len(edges) < 2 or not np.all(edges >= 0) or not np.all(np.diff(edges) > 0)
+    if bad:
+        raise ValueError("ranges must be two or more non-negative, strictly increasing edges, not %r" % (ranges,))
+    return tuple(float(e) for e in edges)
+
+
+def range_bins(edges):
+    """The half-open bins [e_i, e_i+1) of the edges."""
+    return list(zip(edges[:-1], edges[1:]))
+
+
+def eval_many(gt_annos, dt_sets, classes, tables=(11,), overlap_fn=None, difficultys=(0, 1, 2), ranges=None,
+              match=False):
     """Every table of ``tables`` (11 and 40: the official tables at 11 / 40 recall positions; "coco": the COCO-style
     table) for each of the K detection sets of ``dt_sets`` against the same GT.  Returns one dict per set, {table:
     (text, ap)}.  The official and COCO overlap rows form one list of min overlaps, so the overlaps, the GT side and
     the matching run once for all of them; R11 and R40 read the same precision samples.  The GT and each set are a
-    list of annotation dicts or an AnnoBlock."""
+    list of annotation dicts or an AnnoBlock.
+
+    ``ranges``: bin edges (check_ranges); each set's dict then also holds ``"ranges"``: [(lo, hi, {table: (text,
+    ap)}), ...], the tables over the objects whose ground range (ground_range) lies in [lo, hi), each text naming its
+    range.  The bins are more difficulty entries of the same evaluation: a GT or detection of the class outside a bin is
+    ignored there (clean_gt / clean_dt).  ``match``: each set's dict also holds ``"matches"``, its match_table."""
     tables = tuple(tables)
     if not tables or any(t not in TABLES for t in tables):
         raise ValueError("tables must be among %r, not %r" % (TABLES, tables))
+    return _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, ranges, match)
+
+
+def match_table(gt_annos, dt_sets, classes, difficultys=(0, 1, 2), overlap_fn=None):
+    """compute_statistics_jit's whole-range assignment (kitti_eval.py:164-283, compute_fp=True at a threshold below
+    every score, each class's first official min overlap) of each detection set, for every class, difficulty and metric
+    (bbox, BEV, 3-D).  One dict per set of numpy arrays, with G GT rows and D_k detection rows (frames concatenated):
+
+    * ``gt_off`` / ``dt_off`` [frames + 1]: each frame's first row;
+    * ``gt_range`` [G] / ``dt_range`` [D_k]: each row's ground range;
+    * ``gt_flag`` [C, Dn, G] / ``dt_flag`` [C, Dn, D_k]: clean_data's flags;
+    * ``gt_det`` [C, Dn, 3, G]: the matched detection row or -1; ``gt_overlap`` [C, Dn, 3, G] their overlap (0 when
+      unmatched);
+    * ``dt_state`` [C, Dn, 3, D_k]: lib.KITTI_DT_TP, _FP, _DONTCARE (in a DontCare area, bbox metric only), _IGNORED
+      (assigned to an ignored GT or through an ignored detection) or _NOT_COUNTED (flag -1 or 1);
+    * ``tp_errors`` [C, Dn, G, 3]: the 3-D metric's true positives' ATE, ASE, AOE (tp_errors) on their GT rows, NaN
+      elsewhere.
+
+    On the device this is one kernel over the flags and overlaps of the evaluation (csrc/kitti_match.cu); with
+    ``overlap_fn`` the host matcher records the same assignment."""
+    return [r["matches"] for r in _evaluate(gt_annos, dt_sets, classes, (), overlap_fn, difficultys, None, True)]
+
+
+def tp_errors(gt_cam, dt_cam):
+    """[n, 3] (ATE, ASE, AOE) of camera rows (x, y, z, l, h, w, ry) of GTs against their detections': ATE the BEV
+    centre distance in camera x-z, ASE 1 - vi / (vg + vd - vi) with vi = min(l) * min(h) * min(w), AOE |ry_d - ry_g|
+    wrapped to [0, pi].  fp64, in the device kernel's operation order."""
+    g, q = np.asarray(gt_cam, np.float64).reshape(-1, 7), np.asarray(dt_cam, np.float64).reshape(-1, 7)
+    dx, dz = q[:, 0] - g[:, 0], q[:, 2] - g[:, 2]
+    vi = np.fmin(q[:, 3], g[:, 3]) * np.fmin(q[:, 4], g[:, 4]) * np.fmin(q[:, 5], g[:, 5])
+    vg, vd = g[:, 3] * g[:, 4] * g[:, 5], q[:, 3] * q[:, 4] * q[:, 5]
+    d = q[:, 6] - g[:, 6]
+    aoe = np.fmin(np.abs(d - 2 * np.pi * np.floor((d + np.pi) / (2 * np.pi))), np.pi)
+    return np.stack([np.sqrt(dx * dx + dz * dz), 1.0 - vi / (vg + vd - vi), aoe], 1)
+
+
+def _table_host(gt_annos, dt_sets, classes, difficultys, row, overlap_fn, gt_sides):
+    """match_table on the host path: the host matcher's recorded assignment per (class, difficulty, metric)."""
+    ovs = [calculate_overlaps_many(gt_annos, dt_sets, m, overlap_fn) for m in range(3)]
+    gt_cam = _flat_cam(gt_annos)
+    gt_range = _cat([ground_range(g) for g in gt_annos], (0,), np.float64)
+    C, Dn, G = len(classes), len(difficultys), len(gt_range)
+    gt_flag = np.zeros((C, Dn, G), np.int8)
+    out = []
+    for k, dts in enumerate(dt_sets):
+        dt_cam = _flat_cam(dts)
+        D = dt_cam.shape[0]
+        t = dict(gt_off=_offsets([len(g["name"]) for g in gt_annos], np.int64),
+                 dt_off=_offsets([len(d["name"]) for d in dts], np.int64), gt_range=gt_range,
+                 dt_range=_cat([ground_range(d) for d in dts], (0,), np.float64), gt_flag=gt_flag,
+                 dt_flag=np.zeros((C, Dn, D), np.int8), gt_det=np.zeros((C, Dn, 3, G), np.int32),
+                 gt_overlap=np.zeros((C, Dn, 3, G)), dt_state=np.zeros((C, Dn, 3, D), np.int8),
+                 tp_errors=np.full((C, Dn, G, 3), np.nan))
+        for ci, c in enumerate(classes):
+            for di, d in enumerate(difficultys):
+                side = gt_sides[c, d, None]
+                gt_flag[ci, di] = side.ign_gt
+                for m in range(3):
+                    packed = _Packed(side, dts, ovs[m][k], c, d)
+                    t["gt_det"][ci, di, m], t["gt_overlap"][ci, di, m], t["dt_state"][ci, di, m] = packed.assign(
+                        m, row[m, ci])
+                t["dt_flag"][ci, di] = packed.ign_dt
+                j = t["gt_det"][ci, di, 2]
+                tp = np.flatnonzero(j >= 0)
+                tp = tp[t["dt_state"][ci, di, 2][j[tp]] == _lib.KITTI_DT_TP]
+                t["tp_errors"][ci, di, tp] = tp_errors(gt_cam[tp], dt_cam[j[tp]])
+        out.append(t)
+    return out
+
+
+def _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, ranges, match):
+    """eval_many's work: the AP tables of ``tables`` (none: no AP matching) over the whole range and each bin of
+    ``ranges``, and with ``match`` the match table."""
     classes = _class_ids(classes)
+    edges = None if ranges is None else check_ranges(ranges)
+    diffs = list(difficultys)
+    bins = [None] + ([] if edges is None else range_bins(edges))
+    entries = [(d, b) for b in bins for d in diffs]     # difficulty entries: the whole range, then bin by bin
     official = any(t in (11, 40) for t in tables)
     rows = ([np.stack([OVERLAP_0_7, OVERLAP_0_5], axis=0)[:, :, classes]] if official else [])
     if "coco" in tables:
         rows.append(coco_min_overlaps(classes))
+    table_row = 0
+    if match and not official:          # the match table is at each class's first official min overlap
+        table_row = sum(r.shape[0] for r in rows)
+        rows.append(OVERLAP_0_7[None][:, :, classes])
     min_overlaps = np.concatenate(rows, 0)
     n_off = 2 if official else 0
     aos_flags = [_aos_flag(d) for d in dt_sets]
-    diffs = list(difficultys)
+    ent_diffs, ent_bins = [d for d, _ in entries], [b for _, b in entries]
     if overlap_fn is None:
-        prec = _eval_device(gt_annos, dt_sets, classes, diffs, min_overlaps, aos_flags)
+        prec, matches = _eval_device_full(gt_annos, dt_sets, classes, ent_diffs, min_overlaps, aos_flags,
+                                          ent_bins, (table_row, len(diffs)) if match else None, bool(tables))
     else:
         gt_annos, dt_sets = _as_annos(gt_annos), [_as_annos(d) for d in dt_sets]
-        gt_sides = {(c, d): _GtSide(gt_annos, c, d) for c in classes for d in diffs}
-        prec = [eval_class_many(gt_annos, dt_sets, classes, diffs, metric, min_overlaps,
-                                aos_flags if metric == 0 else [False] * len(dt_sets), overlap_fn, gt_sides)
-                for metric in (0, 1, 2)]
+        gt_sides = {(c, d, b): _GtSide(gt_annos, c, d, b) for c in classes for d, b in entries}
+        prec = [eval_class_many(gt_annos, dt_sets, classes, ent_diffs, metric, min_overlaps,
+                                aos_flags if metric == 0 else [False] * len(dt_sets), overlap_fn, gt_sides, ent_bins)
+                for metric in (0, 1, 2)] if tables else None
+        matches = (_table_host(gt_annos, dt_sets, classes, diffs, min_overlaps[table_row], overlap_fn, gt_sides)
+                   if match else None)
     out = []
+    Dn = len(diffs)
     for s, compute_aos in enumerate(aos_flags):
-        r0, r1, r2 = (p[s] for p in prec)
         res = {}
-        for rp in (t for t in tables if t in (11, 40)):
-            get_mAP_n = get_mAP if rp == 11 else get_mAP_R40
-            ap = dict(bbox=get_mAP_n(r0["precision"][:, :, :n_off]),
-                      aos=get_mAP_n(r0["orientation"][:, :, :n_off]) if compute_aos else None,
-                      bev=get_mAP_n(r1["precision"][:, :, :n_off]), d3=get_mAP_n(r2["precision"][:, :, :n_off]))
-            res[rp] = (_ap_text(ap, classes, min_overlaps[:n_off], compute_aos, "AP" if rp == 11 else "AP_R40"), ap)
-        if "coco" in tables:
-            # do_coco_style_eval (kitti_eval.py:711-729): the mean over the ten overlaps of get_mAP_v2
-            ap = dict(bbox=get_mAP(r0["precision"][:, :, n_off:]).mean(-1),
-                      aos=get_mAP(r0["orientation"][:, :, n_off:]).mean(-1) if compute_aos else None,
-                      bev=get_mAP(r1["precision"][:, :, n_off:]).mean(-1),
-                      d3=get_mAP(r2["precision"][:, :, n_off:]).mean(-1))
-            res["coco"] = (_coco_text(ap, classes, compute_aos), ap)
+        if tables:
+            r = [p[s] for p in prec]
+            res = _ap_tables(r, 0, Dn, tables, classes, min_overlaps, n_off, compute_aos, None)
+            if edges is not None:
+                res["ranges"] = [(lo, hi, _ap_tables(r, (b + 1) * Dn, Dn, tables, classes, min_overlaps, n_off,
+                                                     compute_aos, (lo, hi)))
+                                 for b, (lo, hi) in enumerate(bins[1:])]
+        if match:
+            res["matches"] = matches[s]
         out.append(res)
     return out
+
+
+def _ap_tables(r, e0, Dn, tables, classes, min_overlaps, n_off, compute_aos, rng):
+    """{table: (text, ap)} of difficulty entries [e0, e0 + Dn) of one set's precision arrays r[metric]."""
+    r0, r1, r2 = ({k: v[:, e0:e0 + Dn] for k, v in m.items()} for m in r)
+    res = {}
+    for rp in (t for t in tables if t in (11, 40)):
+        get_mAP_n = get_mAP if rp == 11 else get_mAP_R40
+        ap = dict(bbox=get_mAP_n(r0["precision"][:, :, :n_off]),
+                  aos=get_mAP_n(r0["orientation"][:, :, :n_off]) if compute_aos else None,
+                  bev=get_mAP_n(r1["precision"][:, :, :n_off]), d3=get_mAP_n(r2["precision"][:, :, :n_off]))
+        res[rp] = (_ap_text(ap, classes, min_overlaps[:n_off], compute_aos, "AP" if rp == 11 else "AP_R40", rng), ap)
+    if "coco" in tables:
+        # do_coco_style_eval (kitti_eval.py:711-729): the mean over the ten overlaps of get_mAP_v2
+        c0 = n_off + 10
+        ap = dict(bbox=get_mAP(r0["precision"][:, :, n_off:c0]).mean(-1),
+                  aos=get_mAP(r0["orientation"][:, :, n_off:c0]).mean(-1) if compute_aos else None,
+                  bev=get_mAP(r1["precision"][:, :, n_off:c0]).mean(-1),
+                  d3=get_mAP(r2["precision"][:, :, n_off:c0]).mean(-1))
+        res["coco"] = (_coco_text(ap, classes, compute_aos, rng), ap)
+    return res
 
 
 def coco_eval_many(gt_annos, dt_sets, classes, overlap_fn=None):
@@ -686,24 +883,31 @@ def get_coco_eval_result(gt_annos, dt_annos, current_classes, overlap_fn=None):
     return coco_eval(gt_annos, dt_annos, current_classes, overlap_fn)[0]
 
 
-def _coco_text(ap, classes, compute_aos):
-    """get_coco_eval_result's table (kitti_eval.py:904-930)."""
+def _range_label(rng):
+    """The heading suffix of a range bin's table ("" for the whole range)."""
+    return "" if rng is None else " range [%g, %g) m" % rng
+
+
+def _coco_text(ap, classes, compute_aos, rng=None):
+    """get_coco_eval_result's table (kitti_eval.py:904-930); a range bin's names its range in each heading."""
     lines = []
     for j, cls in enumerate(classes):
         start, stop, num = COCO_RANGE[cls]
-        lines.append("%s coco AP@%.2f:%.2f:%.2f:" % (CLASS_TO_NAME[cls], start, (stop - start) / (num - 1), stop))
+        lines.append("%s coco AP@%.2f:%.2f:%.2f%s:" % (CLASS_TO_NAME[cls], start, (stop - start) / (num - 1), stop,
+                                                      _range_label(rng)))
         for key, label in (("bbox", "bbox AP"), ("bev", "bev  AP"), ("d3", "3d   AP")) + ((("aos", "aos  AP"),)
                                                                                            if compute_aos else ()):
             lines.append("%s:%.2f, %.2f, %.2f" % (label, ap[key][j, 0], ap[key][j, 1], ap[key][j, 2]))
     return "".join(l + "\n" for l in lines)
 
 
-def _ap_text(ap, classes, min_overlaps, compute_aos, tag):
-    """The official table of official_eval's AP arrays."""
+def _ap_text(ap, classes, min_overlaps, compute_aos, tag, rng=None):
+    """The official table of official_eval's AP arrays; a range bin's names its range in each heading."""
     lines = []
     for j, cls in enumerate(classes):
         for i in range(min_overlaps.shape[0]):
-            lines.append("%s %s@%.2f, %.2f, %.2f:" % ((CLASS_TO_NAME[cls], tag) + tuple(min_overlaps[i, :, j])))
+            lines.append("%s %s@%.2f, %.2f, %.2f%s:" % ((CLASS_TO_NAME[cls], tag) + tuple(min_overlaps[i, :, j])
+                                                       + (_range_label(rng),)))
             for key, label in (("bbox", "bbox AP"), ("bev", "bev  AP"), ("d3", "3d   AP")):
                 lines.append("%s:%.2f, %.2f, %.2f" % (label, ap[key][j, 0, i], ap[key][j, 1, i], ap[key][j, 2, i]))
             if compute_aos:
@@ -722,11 +926,87 @@ def ap_lists(ap):
     return {k: (None if v is None else np.asarray(v).tolist()) for k, v in ap.items()}
 
 
-def report_sets(entries, labels, evs, class_names, noun, log=print, extra=None):
+def tp_error_summary(table, classes, difficultys=(0, 1, 2), ranges=None):
+    """Per class, at moderate difficulty: the 3-D metric's true-positive count and the means (numpy's) of their ATE,
+    ASE and AOE (None without a true positive), over the whole range and, with ``ranges``, per bin of the GT's range.
+    ``table``: one set's match_table.  A list of dicts (class, tp, ate, ase, aoe[, ranges: [dict(lo, hi, tp, ...)]])."""
+    d = list(difficultys).index(1)
+    out = []
+    for ci, c in enumerate(_class_ids(classes)):
+        j = table["gt_det"][ci, d, 2]
+        tp = j >= 0
+        tp[tp] = table["dt_state"][ci, d, 2][j[tp]] == _lib.KITTI_DT_TP
+        err = table["tp_errors"][ci, d]
+
+        def stats(mask):
+            e = err[mask]
+            return dict(tp=int(mask.sum()), **{k: (float(np.mean(e[:, i])) if len(e) else None)
+                                                for i, k in enumerate(("ate", "ase", "aoe"))})
+        entry = dict(cls=CLASS_TO_NAME[c], **stats(tp))
+        if ranges is not None:
+            r = table["gt_range"]
+            entry["ranges"] = [dict(lo=lo, hi=_json_edge(hi), **stats(tp & (lo <= r) & (r < hi)))
+                               for lo, hi in range_bins(check_ranges(ranges))]
+        out.append(entry)
+    return out
+
+
+def _json_edge(e):
+    """A bin edge for JSON: inf as None."""
+    return None if np.isinf(e) else e
+
+
+def _fmt_err(st):
+    return "TP %d ATE %s ASE %s AOE %s" % ((st["tp"],) + tuple("-" if st[k] is None else "%.4f" % st[k]
+                                                               for k in ("ate", "ase", "aoe")))
+
+
+def range_report(entry, ev, class_names, log=print, tp_err=None):
+    """Print a set's per-range tables (``ev``: eval_many's dict with ``ranges``, or without: nothing) after its
+    whole-range ones and put their texts and AP lists into ``entry`` (text_ranges / ap_ranges and the _r40 / _coco
+    variants evaluated), and ``tp_err`` (tp_error_summary) as ``tp_errors``.  Returns the summary fields: moderate 3D
+    AP per class per bin, then the TP error means per class."""
+    fields = []
+    if "ranges" in ev:
+        for suffix, t in (("", 11), ("_r40", 40), ("_coco", "coco")):
+            if t not in ev:
+                continue
+            for _, _, res in ev["ranges"]:
+                log(res[t][0], end="")
+            entry["text_ranges" + suffix] = [res[t][0] for _, _, res in ev["ranges"]]
+            entry["ap_ranges" + suffix] = [dict(lo=lo, hi=_json_edge(hi), ap=ap_lists(res[t][1]))
+                                           for lo, hi, res in ev["ranges"]]
+        for j, c in enumerate(class_names):
+            for lo, hi, res in ev["ranges"]:
+                fields.append("%s 3d mod [%g, %g) R11 %6.2f" % (c, lo, hi, res[11][1]["d3"][j, 1, 0]) +
+                              (" R40 %6.2f" % res[40][1]["d3"][j, 1, 0] if 40 in res else "") +
+                              (" COCO %6.2f" % res["coco"][1]["d3"][j, 1] if "coco" in res else ""))
+    if tp_err is not None:
+        entry["tp_errors"] = tp_err
+        for st in tp_err:
+            fields.append("%s %s" % (st["cls"], _fmt_err(st)))
+            for b in st.get("ranges", []):
+                fields.append("%s [%g, %g) %s" % (st["cls"], b["lo"], np.inf if b["hi"] is None else b["hi"],
+                                                  _fmt_err(b)))
+    return fields
+
+
+def write_matches(path, labels, tables):
+    """Write each set's match_table to an .npz: set k's arrays as ``set<k>_<name>``, ``labels`` [K] the sets' labels
+    and the KITTI_DT_* state names ``states``."""
+    out = dict(labels=np.array([str(l) for l in labels]),
+               states=np.array(["not_counted", "tp", "fp", "dontcare", "ignored"]))
+    for k, t in enumerate(tables):
+        out.update({"set%d_%s" % (k, name): v for name, v in t.items()})
+    np.savez_compressed(path, **out)
+
+
+def report_sets(entries, labels, evs, class_names, noun, log=print, extra=None, ranges=None):
     """Print each evaluated set's tables (``evs``: eval_many's dicts, with table 11) under ``== label ==``, then one
     summary line per set: moderate 3D AP per class at the class's strict overlap (R11, and R40 / COCO when evaluated).
     Each set's texts and AP lists go into its dict of ``entries`` (returned).  ``extra(k, entry)`` may add to set k's
-    entry after its tables and returns more summary fields."""
+    entry after its tables and returns more summary fields.  A set evaluated with ranges or a match table also prints
+    its per-range tables, and its summary line gains range_report's fields (``ranges``: the bin edges)."""
     summary = []
     for k, (entry, label, ev) in enumerate(zip(entries, labels, evs)):
         log("== %s ==" % label)
@@ -744,6 +1024,9 @@ def report_sets(entries, labels, evs, class_names, noun, log=print, extra=None):
         if "coco" in ev:
             log(ev["coco"][0], end="")
             entry.update(text_coco=ev["coco"][0], ap_coco=ap_lists(ev["coco"][1]))
+        if "ranges" in ev or "matches" in ev:
+            tp_err = tp_error_summary(ev["matches"], class_names, ranges=ranges) if "matches" in ev else None
+            line += range_report(entry, ev, class_names, log, tp_err)
         if extra is not None:
             line += extra(k, entry)
         summary.append("  ".join(line))
@@ -753,16 +1036,16 @@ def report_sets(entries, labels, evs, class_names, noun, log=print, extra=None):
     return entries
 
 
-def eval_dirs(label_dir, result_dirs, ids, classes, tables=(11,), times=None):
+def eval_dirs(label_dir, result_dirs, ids, classes, tables=(11,), times=None, ranges=None, match=False):
     """Every table of ``tables`` for each directory of KITTI result files in ``result_dirs`` against the label files
     of ``label_dir``, over the frames ``ids``: the GT is read once, every directory is read and parsed on the device
-    (read_block), and one eval_many evaluates them all.  Returns eval_many's list, one dict per directory.
-    ``times``: a dict whose "read", "parse" and "eval" entries accumulate seconds."""
+    (read_block), and one eval_many evaluates them all (``ranges``, ``match``: eval_many's).  Returns eval_many's list,
+    one dict per directory.  ``times``: a dict whose "read", "parse" and "eval" entries accumulate seconds."""
     times = {} if times is None else times
     gt = read_block(label_dir, ids, times=times)
     dts = [read_block(d, ids, times=times) for d in result_dirs]
     t0 = time.perf_counter()
-    out = eval_many(gt, dts, classes, tables)
+    out = eval_many(gt, dts, classes, tables, ranges=ranges, match=match)
     times["eval"] = times.get("eval", 0.0) + time.perf_counter() - t0
     return out
 
@@ -779,7 +1062,9 @@ def parse_args(argv=None):
     p.add_argument("--coco", action="store_true",
                    help="also print the COCO-style AP table (AP averaged over ten IoU thresholds per class)")
     p.add_argument("--json", default=None, help="write the AP arrays and times here")
+    add_range_args(p)
     args = p.parse_args(argv)
+    check_range_args(p, args)
     unknown = [c for c in args.classes if c not in CLASS_TO_NAME.values()]
     if unknown:
         p.error("--classes: unknown class %s (known: %s)" % (", ".join(unknown), ", ".join(CLASS_TO_NAME.values())))
@@ -794,24 +1079,49 @@ def parse_args(argv=None):
     return args
 
 
+def add_range_args(p):
+    """The --ranges / --matches options of the evaluation commands."""
+    p.add_argument("--ranges", nargs="+", type=float, default=None, metavar="EDGE",
+                   help="also print the tables per range bin [e_i, e_i+1) of ground distance from the camera, in m "
+                        "(e.g. 0 20 40 inf), and the true positives' mean ATE / ASE / AOE")
+    p.add_argument("--matches", default=None, metavar="NPZ",
+                   help="write each set's per-object match table (kitti_eval.match_table) to this .npz")
+
+
+def check_range_args(p, args):
+    if args.ranges is not None:
+        try:
+            args.ranges = list(check_ranges(args.ranges))
+        except ValueError as e:
+            p.error("--ranges: %s" % e)
+
+
 def main(argv=None, log=print):
     """Evaluate directories of KITTI result files against a split's labels (SECOND's kitti-object-eval-python):
 
     python -m sassd_b200.kitti_eval --data-root DIR [--split val] --results DIR [DIR ...]
                                     [--classes Car Pedestrian Cyclist] [--r40] [--coco] [--json FILE]
+                                    [--ranges EDGE EDGE [...]] [--matches FILE.npz]
 
     The labels are ``training/label_2/%06d.txt`` and the frames those of ``ImageSets/<split>.txt``; files a result
     directory holds beyond them are ignored.  Every file is read into pinned memory, copied to the device once and
     parsed there (read_block), and all directories are evaluated in one pass (eval_many) on the device.  Prints each
     directory's tables under ``== DIR ==``, one summary line per directory and the seconds spent reading, parsing and
-    evaluating.  Returns the result dict that ``--json`` writes."""
+    evaluating.  ``--ranges`` adds each directory's tables per range bin and, with ``--matches``, the true positives'
+    TP errors to its summary line; ``--matches`` writes every directory's match table.  Returns the result dict that
+    ``--json`` writes."""
     from .kitti_data import read_split
     args = parse_args(argv)
     ids = read_split(args.data_root, args.split)
     tables = (11,) + ((40,) if args.r40 else ()) + (("coco",) if args.coco else ())
     times = {}
-    evs = eval_dirs(os.path.join(args.data_root, "training", "label_2"), args.results, ids, args.classes, tables, times)
-    entries = report_sets([dict(dir=d) for d in args.results], args.results, evs, args.classes, "directories", log)
+    match = args.ranges is not None or args.matches is not None
+    evs = eval_dirs(os.path.join(args.data_root, "training", "label_2"), args.results, ids, args.classes, tables, times,
+                    args.ranges, match)
+    entries = report_sets([dict(dir=d) for d in args.results], args.results, evs, args.classes, "directories", log,
+                          ranges=args.ranges)
+    if args.matches:
+        write_matches(args.matches, args.results, [ev["matches"] for ev in evs])
     log("frames: %d, directories: %d, read %.3f s, parse %.3f s, evaluate %.3f s" % (
         len(ids), len(args.results), times["read"], times["parse"], times["eval"]))
     result = dict(split=args.split, frames=len(ids), classes=args.classes, results=entries, times_s=times)

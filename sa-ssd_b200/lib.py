@@ -54,6 +54,8 @@ POINT_FC_IN, POINT_FC_OUT = 160, 64       # point_fc: Linear(160, 64); point_cls
 KITTI_PARSE_DEFER, KITTI_PARSE_SCORE = 1, 2     # SASSD_KITTI_PARSE_DEFER / _SCORE: sassd_kitti_scan_labels' flags
 GT_CAP_MAX = 256                          # SASSD_GT_CAP_MAX: ground-truth boxes per frame the loss kernels take
 MERGE_MAX = 16                            # SASSD_MERGE_MAX: members sassd_merge_detections takes
+# SASSD_KITTI_DT_*: a detection's state in the KITTI match table
+KITTI_DT_NOT_COUNTED, KITTI_DT_TP, KITTI_DT_FP, KITTI_DT_DONTCARE, KITTI_DT_IGNORED = 0, 1, 2, 3, 4
 
 OK = 0
 ERRORS = {-1: "SASSD_ERR_ARG", -2: "SASSD_ERR_LAUNCH", -3: "SASSD_ERR_WORKSPACE", -4: "SASSD_ERR_UNSUPPORTED"}
@@ -105,10 +107,14 @@ _SIGNATURES = {
     "sassd_kitti_match": (c_int, [c_int, P, P, P, P, P, P, P, P, P, P, P, P, c_int, ctypes.c_double, c_int, c_int, P, P,
                                   P, P]),
     "sassd_kitti_eval_flags": (c_int, [c_int, P, P, P, P, c_int, P, P, c_int, P, c_int, P, P, P, P, P]),
+    "sassd_kitti_eval_flags_ranged": (c_int, [c_int, P, P, P, P, P, c_int, P, P, P, c_int, P, c_int, P, P, P, P, P,
+                                              P, P, P]),
     "sassd_kitti_eval_overlaps": (c_int, [c_int, c_int, P, P, P, P, P, P, P, P, P, c_int, P, P, P, P]),
     "sassd_kitti_aos_table": (c_int, [c_int, c_int, P, P, P, P, P, P]),
     "sassd_kitti_eval_workspace_bytes": (c_size_t, [c_int, c_int]),
     "sassd_kitti_eval_match": (c_int, [ctypes.POINTER(KittiEvalDesc), P, P, P, P, P, P, c_size_t, P]),
+    "sassd_kitti_eval_assign": (c_int, [ctypes.POINTER(KittiEvalDesc), c_int, c_int, P, P, P, P, P, P, P, c_size_t, P]),
+    "sassd_kitti_assign": (c_int, [c_int, P, P, P, P, P, P, P, P, P, P, c_int, ctypes.c_double, P, P, P]),
     "sassd_kitti_scan_labels": (c_int, [P, P, c_int, P, P, P]),
     "sassd_kitti_parse_workspace_bytes": (c_size_t, [c_int]),
     "sassd_kitti_parse_labels": (c_int, [P, P, c_int, P, P, c_int, P, P, c_int, P, P, P, P, P, P, P, P, P, c_size_t, P]),

@@ -53,7 +53,7 @@ def next_pow2(n):
 # kernels launched by each C-ABI entry point (memsets not counted)
 _KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_points_in_rbboxes": 1, "sassd_augment_drop_points": 1, "sassd_augment_noise_search": 1, "sassd_augment_assemble": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
-            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_kitti_eval_flags": 1, "sassd_kitti_eval_overlaps": 1, "sassd_kitti_eval_match": 3, "sassd_kitti_scan_labels": 1, "sassd_kitti_parse_labels": 2, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_conv2d_f16x3_occ_bg_status": 1, "sassd_gconv_status": 1, "sassd_spconv_f16x3_status": 1, "sassd_features_to_split_status": 1, "sassd_sparse_to_bev_split_status": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
+            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_kitti_eval_flags": 1, "sassd_kitti_eval_flags_ranged": 1, "sassd_kitti_eval_assign": 1, "sassd_kitti_eval_overlaps": 1, "sassd_kitti_eval_match": 3, "sassd_kitti_scan_labels": 1, "sassd_kitti_parse_labels": 2, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_conv2d_f16x3_occ_bg_status": 1, "sassd_gconv_status": 1, "sassd_spconv_f16x3_status": 1, "sassd_features_to_split_status": 1, "sassd_sparse_to_bev_split_status": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_merge_detections": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
             "sassd_boxes_iou_bev": 1, "sassd_points_in_boxes": 2, "sassd_assign_rpn": 3, "sassd_assign_pswarp": 3,
             "sassd_rpn_loss": 2, "sassd_pswarp_loss": 2, "sassd_aux_loss": 2}
@@ -526,6 +526,26 @@ def kitti_eval_flags(gt_name, gt_occ, gt_trunc, gt_bbox, dt_name, dt_bbox, class
     return ign_gt, ign_dt, n_valid
 
 
+def kitti_eval_flags_ranged(gt_name, gt_occ, gt_trunc, gt_bbox, gt_cam, dt_name, dt_bbox, dt_cam, classes, limits,
+                            ranges):
+    """kitti_eval_flags with a range bin per difficulty entry (csrc/kitti_match.cu): gt_cam / dt_cam [rows,7] f64
+    camera rows, ranges [Dn,2] f64 (lo, hi) or None (no range test; an entry whose lo is -inf has none either).
+    Returns (ign_gt, ign_dt, n_valid, gt_range [G] f64, dt_range [D] f64): the flags and every row's ground distance
+    sqrt(x * x + z * z)."""
+    dev = gt_bbox.device
+    G, D, C, Dn = gt_name.shape[0], dt_name.shape[0], classes.shape[0], limits.shape[0]
+    ign_gt = torch.empty((C, Dn, G), dtype=torch.int8, device=dev)
+    ign_dt = torch.empty((C, Dn, D), dtype=torch.int8, device=dev)
+    n_valid = torch.zeros((C, Dn), dtype=torch.int32, device=dev)
+    gt_range = torch.empty((G,), dtype=torch.float64, device=dev)
+    dt_range = torch.empty((D,), dtype=torch.float64, device=dev)
+    _call("sassd_kitti_eval_flags_ranged", None, G, _ptr(gt_name), _ptr(gt_occ), _ptr(gt_trunc), _ptr(gt_bbox),
+          _ptr(gt_cam), D, _ptr(dt_name), _ptr(dt_bbox), _ptr(dt_cam), C, _ptr(classes), Dn, _ptr(limits),
+          _ptr(ranges) if ranges is not None else None, _ptr(ign_gt), _ptr(ign_dt), _ptr(n_valid), _ptr(gt_range),
+          _ptr(dt_range), _stream())
+    return ign_gt, ign_dt, n_valid, gt_range, dt_range
+
+
 def kitti_eval_overlaps(nsets, nframes, gt_off, dt_off, ov_off, gt_cam, dt_cam, gt_bbox, dt_bbox, bev_iou, bev_inter,
                         total_pairs, max_pairs):
     """The bbox, BEV and 3-D overlap matrices (f64 [total_pairs], blocks at ov_off) of every (set, frame) block: gt_cam /
@@ -552,6 +572,22 @@ def kitti_eval_match(desc, njobs, score_total, ws=None):
     _call("sassd_kitti_eval_match", None, ctypes.byref(desc), _ptr(scores), _ptr(n_scores), _ptr(thresholds),
           _ptr(n_thresh), _ptr(pr), _ptr(w), w.numel(), _stream())
     return thresholds, n_thresh, pr
+
+
+def kitti_eval_assign(desc, row, ndiff, gt_cam, dt_cam, ws=None):
+    """The match table of the first ``ndiff`` difficulty entries of ``desc`` at min-overlap row ``row`` (csrc/
+    kitti_match.cu).  Returns (gt_det [K,C,ndiff,3,G] i32, gt_ov [K,C,ndiff,3,G] f64, dt_state [C,ndiff,3,D] i8,
+    tp_err [K,C,ndiff,G,3] f64)."""
+    dev = gt_cam.device
+    K, C, G, D = desc.nsets, desc.nclass, gt_cam.shape[0], dt_cam.shape[0]
+    gt_det = torch.empty((K, C, ndiff, 3, G), dtype=torch.int32, device=dev)
+    gt_ov = torch.empty((K, C, ndiff, 3, G), dtype=torch.float64, device=dev)
+    dt_state = torch.empty((C, ndiff, 3, D), dtype=torch.int8, device=dev)
+    tp_err = torch.empty((K, C, ndiff, G, 3), dtype=torch.float64, device=dev)
+    w = (ws or _WS).get("kitti_eval", _L().sassd_kitti_eval_workspace_bytes(desc.max_nd, desc.max_ng), dev)
+    _call("sassd_kitti_eval_assign", None, ctypes.byref(desc), int(row), int(ndiff), _ptr(gt_cam), _ptr(dt_cam),
+          _ptr(gt_det), _ptr(gt_ov), _ptr(dt_state), _ptr(tp_err), _ptr(w), w.numel(), _stream())
+    return gt_det, gt_ov, dt_state, tp_err
 
 
 def kitti_scan_labels(buf, file_off):

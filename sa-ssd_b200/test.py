@@ -2,7 +2,7 @@
 
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR [--split val] [--batch 16]
                               [--lidar velodyne|velodyne_reduced] [--out DIR] [--workers N] [--json FILE]
-                              [--losses] [--r40] [--coco]
+                              [--losses] [--r40] [--coco] [--ranges EDGE EDGE [...]] [--matches FILE.npz]
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR --split test --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --drive DRIVE_DIR [--calib-dir DIR] --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --model CONFIG2 CHECKPOINT2 [--model ...] --data-root DIR [...]
@@ -16,7 +16,10 @@ clock of the streamed detection, the evaluation excluded) and the time spent wai
 the table at 40 recall positions (kitti_eval.official_eval(recall_positions=40)), and ``--coco`` the reference's
 COCO-style table, AP averaged over ten IoU thresholds per class (kitti_eval.coco_eval), after the official one(s).
 All tables come from one evaluation (kitti_eval.eval_many), which runs on the device, against the split's labels as
-kitti_eval.read_block parses them on the device.
+kitti_eval.read_block parses them on the device.  ``--ranges 0 20 40 inf`` adds the same tables per bin of ground
+distance from the camera after the whole-range ones (kitti_eval.eval_many(ranges=...)) and the true positives' mean
+ATE / ASE / AOE per class (kitti_eval.tp_error_summary); ``--matches FILE.npz`` writes every set's per-object match
+table (kitti_eval.match_table).  Both come from the same one evaluation, for every checkpoint and bin.
 
 ``--losses`` (labelled splits): every frame also carries its ground truth (kitti_data.gt_from_anno) and the captured
 step computes SA-SSD's six losses beside the detections (detect_stream(losses=True)); the result files and AP tables
@@ -92,7 +95,10 @@ def parse_args(argv=None):
                    help="one more single-class model, run with the first as one set (repeatable)")
     p.add_argument("--checkpoints", nargs="+", default=[], metavar="CHECKPOINT",
                    help="more checkpoints of CONFIG, validated with CHECKPOINT in one pass over a labelled split")
+    from .kitti_eval import add_range_args, check_range_args
+    add_range_args(p)
     args = p.parse_args(argv)
+    check_range_args(p, args)
     if args.batch < 1:
         p.error("--batch must be positive")
     if args.checkpoints:
@@ -116,6 +122,9 @@ def parse_args(argv=None):
         p.error("--r40 needs a labelled split: %s has no labels" % ("--drive" if args.drive else "--split test"))
     if args.coco and (args.drive or args.split == "test"):
         p.error("--coco needs a labelled split: %s has no labels" % ("--drive" if args.drive else "--split test"))
+    for flag, given in (("--ranges", args.ranges is not None), ("--matches", args.matches is not None)):
+        if given and (args.drive or args.split == "test"):
+            p.error("%s needs a labelled split: %s has no labels" % (flag, "--drive" if args.drive else "--split test"))
     if args.drive:
         if args.lidar == "velodyne_reduced":
             p.error("--drive reads full sweeps: --lidar velodyne_reduced does not apply")
@@ -299,7 +308,7 @@ def run(args, log=print):
         _write_json(args.json, result)
         D.barrier()
         return result
-    from .kitti_eval import ap_lists, eval_many, read_block
+    from .kitti_eval import ap_lists, eval_many, range_report, read_block, tp_error_summary, write_matches
     gt = read_block(os.path.join(split.dir, "label_2"), split.ids)
     if sweep:
         result["checkpoints"] = _report_sweep(args, gt, dt_sets, class_names, per_batch, log)
@@ -307,7 +316,7 @@ def run(args, log=print):
         _write_json(args.json, result)
         D.barrier()
         return result
-    ev = eval_many(gt, [dt_annos], class_names, _tables(args))[0]
+    ev = eval_many(gt, [dt_annos], class_names, _tables(args), **_range_kw(args))[0]
     text, ap = ev[11]
     log(text, end="")
     result.update(text=text, ap=ap_lists(ap))
@@ -317,6 +326,12 @@ def run(args, log=print):
     if args.coco:
         log(ev["coco"][0], end="")
         result.update(text_coco=ev["coco"][0], ap_coco=ap_lists(ev["coco"][1]))
+    if "matches" in ev:
+        fields = range_report(result, ev, class_names, log,
+                              tp_error_summary(ev["matches"], class_names, ranges=args.ranges))
+        log("summary: " + "  ".join(fields))
+        if args.matches:
+            write_matches(args.matches, [os.path.basename(args.checkpoint)], [ev["matches"]])
     if args.losses:
         result.update(_loss_means(per_batch, args.batch, log))
     log(rate)
@@ -328,6 +343,13 @@ def run(args, log=print):
 def _tables(args):
     """The kitti_eval.eval_many tables the arguments ask for."""
     return (11,) + ((40,) if args.r40 else ()) + (("coco",) if args.coco else ())
+
+
+def _range_kw(args):
+    """eval_many's ranges / match arguments: a match table whenever --ranges or --matches is given."""
+    if args.ranges is None and args.matches is None:
+        return {}
+    return dict(ranges=args.ranges, match=True)
 
 
 def _loss_means(per_batch, batch, log):
@@ -355,8 +377,12 @@ def _report_sweep(args, gt, dt_sets, class_names, per_batch, log):
             return []
         entry.update(_loss_means([v[k * n:(k + 1) * n] for v in per_batch], args.batch, log))
         return ["rpn_cls_loss %.6f loss_cls %.6f" % (entry["losses"]["rpn_cls_loss"], entry["losses"]["loss_cls"])]
-    return report_sets([dict(path=p) for p in paths], [os.path.basename(p) for p in paths],
-                       eval_many(gt, dt_sets, class_names, _tables(args)), class_names, "checkpoints", log, losses)
+    from .kitti_eval import write_matches
+    evs = eval_many(gt, dt_sets, class_names, _tables(args), **_range_kw(args))
+    if args.matches:
+        write_matches(args.matches, [os.path.basename(p) for p in paths], [ev["matches"] for ev in evs])
+    return report_sets([dict(path=p) for p in paths], [os.path.basename(p) for p in paths], evs, class_names,
+                       "checkpoints", log, losses, ranges=args.ranges)
 
 
 def _write_json(path, result):
