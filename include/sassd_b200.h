@@ -57,6 +57,8 @@ enum { /* bits of *d_status */
                                    (sassd_points_in_rbboxes) */
     SASSD_FLAG_POINTS_CAP = 256, /* augmented rows exceed out_cap: rows past it are not written
                                    (sassd_augment_assemble) */
+    SASSD_FLAG_TILE_WAIT = 1024, /* a dense conv waited longer than about a second for its input tiles' ready counters
+                                   (sassd_conv2d_desc.in_ready) and went on without them: its outputs are undefined */
     SASSD_FLAG_F16_RANGE = 512  /* a finite value at or above 65520 in magnitude was split into fp16 planes: its hi half is
                                    +-inf and its lo half -+inf, so every output that reads it becomes NaN.  Set by the
                                    split stores of the *_status entry points (sassd_conv2d_f16x3_occ_bg_status,
@@ -72,6 +74,8 @@ int sassd_version(void);
  * else off).  Worth ~2 % for a step that runs alone on the GPU, costs throughput when several steps are in flight, so set
  * it around the capture of a latency-oriented graph only.  Returns the previous setting.  Results never change. */
 int sassd_set_pdl(int on);
+/* Whether launches are programmatic dependents now (sassd_set_pdl, else the environment). */
+int sassd_pdl_enabled(void);
 
 /* ------------------------------------------------------------------------
  * Voxelization.  Replaces mmdet/ops/points_op/points_ops.py:104-164
@@ -291,6 +295,17 @@ typedef struct {
     int32_t n_split;               /* accepted for ABI compatibility and ignored: a work unit is a tile and at most 128 of
                                       its output channels (the register accumulators' budget), so cout > 128 always runs
                                       as two units per tile */
+    /* Tile ready counters (NULL: off; only for cout > 64 with out_split_ch at most the units' 128 or 256 channels),
+     * int32 [batch * tiles_y * tiles_x + 1] over the SASSD_CONV2D_TILE_H x SASSD_CONV2D_TILE_W tiles, zeroed before
+     * the chain of launches that uses them and never reset by a kernel.  out_ready: this launch adds to a tile's
+     * counter as its units store it, and to the last word once per CTA past its prologue.  in_ready: the out_ready of
+     * the launch that wrote in_split, which must be the previous launch on the stream (anything launched in between
+     * may still be running when this one reads what it wrote).  This launch then does not wait for that one to
+     * complete before it starts, but loads each tile's inputs once the tiles they read are stored, and completes only
+     * after it (results are the same bit for bit).  Needs d_status: a wait longer than about a second (a bug) stops
+     * waiting and sets SASSD_FLAG_TILE_WAIT. */
+    const int32_t* in_ready;
+    int32_t* out_ready;
 } sassd_conv2d_desc;
 int sassd_conv2d_f16x3(const sassd_conv2d_desc* host_desc, const void* in_split, const void* wpack, const float* scale,
                        const float* shift, float* out_f32, void* out_split, sassd_stream_t stream);

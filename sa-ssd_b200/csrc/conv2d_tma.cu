@@ -97,6 +97,56 @@ struct Conv2dArgs {
     int* status;          // optional: SASSD_FLAG_F16_RANGE when a value stored into out_split overflows the split
 };
 
+// BN = 128 only, optional (see sassd_conv2d_desc): [B * tiles_y * tiles_x + 1] counters of the input map, written by
+// the previous launch, and of this layer's output.  With in_ready the kernel starts without waiting for the previous
+// grid and loads a unit's boxes once the tiles they read are ready.  A parameter of its own after the others: grown,
+// Conv2dArgs moves the kernel's other parameters and costs the consumers of the kernel without counters a spill.
+struct Ready {
+    const int* in_ready;
+    int* out_ready;
+};
+
+// Tile ready counters: every unit adds 2 / nsplit per warpgroup once its stores are done, so a tile's counter reaches
+// kTileReady when all of its units have stored.  Word ntiles (after the tiles) counts the CTAs past their prologue.
+constexpr int kTileReady = 4;
+constexpr uint32_t kWaitCycles = 2000000000u;      // ~1 s at the H100's SM clocks: a wait past it is a bug, reported
+
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
+    int v;
+    asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+// After a barrier over the threads whose stores it publishes.
+__device__ __forceinline__ void signal_ready(int* p, int v) {
+    asm volatile("fence.acq_rel.gpu;\n\tred.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+// Spins until *c >= target; false (and SASSD_FLAG_TILE_WAIT in the status word) once clock() is kWaitCycles past t0.
+__device__ __forceinline__ bool wait_ready(const Conv2dArgs& p, const int* c, int target, uint32_t t0) {
+    while (ld_acquire_gpu(c) < target) {
+        if ((uint32_t)clock() - t0 > kWaitCycles) {
+            if (p.status) atomicOr(p.status, SASSD_FLAG_TILE_WAIT);
+            return false;
+        }
+        __nanosleep(64);
+    }
+    return true;
+}
+// The input tiles a unit of `tile` (b, ty, tx) reads: its halo box spans pixel rows y0 - halo .. y0 + TILE_H - 1 + halo
+// and columns x0 - halo .. x0 + TILE_W - 1 + halo, i.e. the tiles ty - halo .. ty + halo, tx - halo .. tx + halo of
+// frame b (halo = 1 <= TILE_H, TILE_W), clipped at the map edge, where TMA fills zeros.  Compact: it runs in the
+// producer warpgroup's 40 registers.
+__device__ __forceinline__ bool wait_input_tiles(const Conv2dArgs& p, const int* in_ready, int tile, int halo,
+                                                 int tiles_y, int tiles_x) {
+    const uint32_t t0 = (uint32_t)clock();
+    const int ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
+    for (int dy = -halo; dy <= halo; ++dy)
+        for (int dx = -halo; dx <= halo; ++dx) {
+            if (ty + dy < 0 || ty + dy >= tiles_y || tx + dx < 0 || tx + dx >= tiles_x) continue;
+            if (!wait_ready(p, in_ready + tile + dy * tiles_x + dx, kTileReady, t0)) return false;
+        }
+    return true;
+}
+
 // Optional: the layer's outputs on an empty scene, batch 1 (same H, W, strides), copied into the far border tiles.
 struct Background {
     const __half* split;
@@ -216,9 +266,11 @@ __device__ __forceinline__ void mma_chunk_x3_rs(float (&big)[64], float (&small)
     }
 }
 
-template <int BN>
+// READY: the launch has tile ready counters (in_ready and / or out_ready, BN = 128 only); without them the kernel is
+// compiled without their code.
+template <int BN, bool READY>
 __global__ void __launch_bounds__(Cfg2<BN>::THREADS, 1)
-conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, const Background bg) {
+conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, const Background bg, const Ready r) {
     using C = Cfg2<BN>;
     constexpr int A_STAGES = C::A_STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -257,7 +309,16 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
         s_walk[5] = blockIdx.x;
     }
     __syncthreads();
-    pdl_wait();                   // the producing layer has completed; nothing above touched global data
+    if (READY && r.in_ready) {
+        // The producing layer may still be running; its units are waited for tile by tile before their boxes load.
+        // The tile distances below were written before it started: reading them waits only until one of its CTAs
+        // has passed this point, which orders them (and the zeroed counters) before everything this grid reads.
+        if (threadIdx.x == 0) wait_ready(p, r.in_ready + ntiles, 1, (uint32_t)clock());
+        __syncthreads();
+    } else {
+        pdl_wait();               // the producing layer has completed; nothing above touched global data
+    }
+    if (READY && r.out_ready && threadIdx.x == 0) signal_ready(r.out_ready + ntiles, 1);
 
     // With constant-region information most tiles only store a constant or copy the background.  Static round-robin
     // leaves some CTAs with two computed tiles and others with none (on the 11-tile-wide BEV grid a stride of 132 units
@@ -389,6 +450,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
             uint32_t a_phase = 0, b_phase = 0;
             // one box per plane and (dx, chunk): rows y0 - halo .. y0 + TILE_H - 1 + halo (the TMA box height of the map)
             const uint32_t a_bytes = 2u * (TILE_H + 2 * halo) * TILE_W * 128;
+            bool waiting = READY && r.in_ready != nullptr;     // false after a timed-out wait: the status word reports it
             for (int k = s_walk[5]; k < nunits; k = next_unit(k)) {
                 const int ref = tile_ref(k / nsplit), half = k % nsplit;
                 if (ref & (kConstTile | kBgTile)) continue;                             // nothing to load
@@ -396,6 +458,11 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                 const int b = tile / (tiles_y * tiles_x);
                 const int ty = (tile / tiles_x) % tiles_y, tx = tile % tiles_x;
                 const int y0 = ty * TILE_H, x0 = tx * TILE_W;
+                if (READY && r.in_ready) {
+                    if (waiting) waiting = wait_input_tiles(p, r.in_ready, tile, halo, tiles_y, tiles_x);
+                    // the tiles were stored through the generic proxy on other SMs; the boxes read them through TMA
+                    asm volatile("fence.proxy.async.global;" ::: "memory");
+                }
                 for (int col = 0; col < ncols; ++col) {
                     const int dx = col - halo;
                     for (int kc = 0; kc < kchunks; ++kc) {
@@ -453,6 +520,17 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
         int a_stage = 0, b_stage = 0;
         uint32_t a_phase = 0, b_phase = 0;
         int computed = 0;
+        // A unit of tile (b, ty, tx) has stored everything this warpgroup writes of it: publish the warpgroup's share.
+        auto unit_stored = [&](int b, int ty, int tx) {
+            if constexpr (READY) {
+                if (r.out_ready) {
+                    // everything from the thread index and the parameters: no register is kept across the MMA loop
+                    named_bar_sync(1 + (threadIdx.x >> 7), 128);
+                    const int ntx = (p.W + TILE_W - 1) / TILE_W, nty = (p.H + TILE_H - 1) / TILE_H;
+                    if ((threadIdx.x & 127) == 0) signal_ready(r.out_ready + (b * nty + ty) * ntx + tx, 2 / p.nsplit);
+                }
+            }
+        };
         for (int k = s_walk[5]; k < nunits; k = next_unit(k)) {
             const int ref = tile_ref(k / nsplit), n_off = (k % nsplit) * BN;
             const int tile = ref & ~(kConstTile | kBgTile);
@@ -464,6 +542,7 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                 const int ncols = min(BN, p.out_split_ch - n_off);
                 if (p.out_split && !p.out_f32 && (ncols == 64 || ncols == 128 || ncols == 256)) {
                     store_constant_unit<CONS_WARPS>(p, b, ty, tx, n_off, ncols, warp, lane);
+                    if constexpr (READY) goto stored;      // one signal site: a second costs the consumers a spill
                     continue;
                 }
             } else {
@@ -661,6 +740,8 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                 }
                 report_f16_range(p.status, ovf.overflowed());
             }
+        stored:
+            unit_stored(b, ty, tx);
         }
         // Background tiles in a pass of their own: interleaved with the MMA units, the copy's address arithmetic is
         // hoisted across the accumulators and spills them.
@@ -671,12 +752,17 @@ conv2d_tma_kernel(const __grid_constant__ CUtensorMap amap, const Conv2dArgs p, 
                 const int tile = ref & ~kBgTile;
                 copy_background_unit(p, bg, tile / (tiles_y * tiles_x), (tile / tiles_x) % tiles_y, tile % tiles_x,
                                      (k % nsplit) * BN, BN, threadIdx.x, CONS_THREADS);
+                if constexpr (READY) unit_stored(tile / (tiles_y * tiles_x), (tile / tiles_x) % tiles_y, tile % tiles_x);
             }
         }
         if (p.counters && threadIdx.x == 0) {
             if (computed) atomicAdd(&p.counters[0], computed);
             if (blockIdx.x == 0) atomicAdd(&p.counters[1], ntiles);
         }
+        // Without the wait at the start, this grid could complete before the producing layer.  Waiting here keeps
+        // "this layer complete" implying "every earlier layer complete", which every launch after the chain relies on
+        // (a grid completes only when all of its threads have exited, so the consumer threads' wait suffices).
+        if (READY && r.in_ready) pdl_wait();
     }
 }
 
@@ -698,10 +784,11 @@ static EncodeTiledFn get_encode() {
     return fn;
 }
 
-template <int BN>
-static int launch2(const CUtensorMap& map, const Conv2dArgs& a, const Background& bg, cudaStream_t stream) {
+template <int BN, bool READY = false>
+static int launch2(const CUtensorMap& map, const Conv2dArgs& a, const Background& bg, const Ready& r,
+                   cudaStream_t stream) {
     using C = Cfg2<BN>;
-    auto kern = conv2d_tma_kernel<BN>;
+    auto kern = conv2d_tma_kernel<BN, READY>;
     static bool configured = false;
     if (!configured) {
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) != cudaSuccess)
@@ -710,7 +797,8 @@ static int launch2(const CUtensorMap& map, const Conv2dArgs& a, const Background
     }
     const int units = a.batch * sassd_div_up(a.H, TILE_H) * sassd_div_up(a.W, TILE_W) * a.nsplit;
     const int grid = units < sassd_num_sms() ? units : sassd_num_sms();
-    if (launch_pdl(kern, dim3(grid), dim3(C::THREADS), C::SMEM_BYTES, stream, map, a, bg) != cudaSuccess) return SASSD_ERR_LAUNCH;
+    if (launch_pdl(kern, dim3(grid), dim3(C::THREADS), C::SMEM_BYTES, stream, map, a, bg, r) != cudaSuccess)
+        return SASSD_ERR_LAUNCH;
     return sassd_check_launch();
 }
 
@@ -744,6 +832,8 @@ __global__ void conv2d_pack_kernel(const float* __restrict__ w, int taps, int ci
 }
 
 }  // namespace tma
+
+extern "C" int sassd_pdl_enabled(void) { return tc::pdl_enabled() ? 1 : 0; }
 
 extern "C" size_t sassd_conv2d_pack_bytes(int taps, int cin, int cout) {
     if (!(taps == 9 || taps == 1) || cin < 1 || cout < 1 || cout > 256) return 0;
@@ -809,6 +899,13 @@ extern "C" int sassd_conv2d_f16x3_occ_bg_status(const sassd_conv2d_desc* d, cons
     if (!(d->taps == 9 || d->taps == 1) || (d->cin_stored % 64) != 0 || d->cin_stored < d->cin) return SASSD_ERR_ARG;
     if (out_split && ((d->out_split_ch % 8) != 0 || d->out_split_ch < 32)) return SASSD_ERR_ARG;
     if (out_f32 && (d->out_f32_stride % 4) != 0) return SASSD_ERR_ARG;
+    // ready counters: BN = 128 launches only, without a zero tail (zero_split_tail's stores are not counted: every
+    // stored channel must belong to a unit, out_split_ch <= nsplit * 128), and a timed-out wait needs the status word
+    // to report it
+    if ((d->in_ready || d->out_ready) &&
+        (d->cout <= 64 || (out_split && d->out_split_ch > (d->cout > 128 ? 256 : 128))))
+        return SASSD_ERR_ARG;
+    if (d->in_ready && !d_status) return SASSD_ERR_ARG;
     EncodeTiledFn enc = get_encode();
     if (!enc) return SASSD_ERR_UNSUPPORTED;
     CUtensorMap map;
@@ -831,14 +928,16 @@ extern "C" int sassd_conv2d_f16x3_occ_bg_status(const sassd_conv2d_desc* d, cons
     a.tile_order = d->tile_order;
     a.nsplit = 1;
     a.status = d_status;
+    const Ready r = {d->in_ready, d->out_ready};
     const Background bg = {out_split ? (const __half*)bg_split : nullptr, out_f32 ? bg_f32 : nullptr};
     cudaStream_t stream = (cudaStream_t)stream_;
-    if (d->cout <= 32) return launch2<32>(map, a, bg, stream);
-    if (d->cout <= 64) return launch2<64>(map, a, bg, stream);
-    if (d->cout <= 128) return launch2<128>(map, a, bg, stream);
+    if (d->cout <= 32) return launch2<32>(map, a, bg, r, stream);
+    if (d->cout <= 64) return launch2<64>(map, a, bg, r, stream);
+    const bool ready = r.in_ready || r.out_ready;
+    if (d->cout <= 128) return ready ? launch2<128, true>(map, a, bg, r, stream) : launch2<128>(map, a, bg, r, stream);
     // 128 < cout <= 256: two units per tile, each 128 output channels of the 256-wide weight pack
     a.nsplit = 2;
-    return launch2<128>(map, a, bg, stream);
+    return ready ? launch2<128, true>(map, a, bg, r, stream) : launch2<128>(map, a, bg, r, stream);
 }
 
 // SparseConvTensor.dense() into the split BEV map: hi / lo*2048 fp16 planes [2,B,H,W,D*C] (channel d*C + c).

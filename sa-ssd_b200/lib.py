@@ -18,7 +18,8 @@ class VoxelParams(ctypes.Structure):
 
 class Conv2dDesc(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in ("batch", "H", "W", "cin", "cin_stored", "cout", "taps", "relu",
-                                              "out_f32_stride", "out_split_ch", "tile_order", "n_split")]
+                                              "out_f32_stride", "out_split_ch", "tile_order", "n_split")] + \
+               [("in_ready", c_void_p), ("out_ready", c_void_p)]
 
 
 class SpconvDesc(ctypes.Structure):
@@ -60,10 +61,11 @@ KITTI_DT_NOT_COUNTED, KITTI_DT_TP, KITTI_DT_FP, KITTI_DT_DONTCARE, KITTI_DT_IGNO
 OK = 0
 ERRORS = {-1: "SASSD_ERR_ARG", -2: "SASSD_ERR_LAUNCH", -3: "SASSD_ERR_WORKSPACE", -4: "SASSD_ERR_UNSUPPORTED"}
 FLAGS = {1: "VOXEL_CAP", 2: "ROWS_CAP", 4: "GUIDED_CAP", 8: "NMS_CAP", 16: "HASH_FULL", 32: "DET_CAP",
-         64: "GT_CAP", 128: "GATHER_CAP", 256: "POINTS_CAP", 512: "F16_RANGE"}
+         64: "GT_CAP", 128: "GATHER_CAP", 256: "POINTS_CAP", 512: "F16_RANGE", 1024: "TILE_WAIT"}
 F16_RANGE = 512                           # SASSD_FLAG_F16_RANGE: a finite value with |x| >= 65520 overflowed the fp16 split
 F16_SPLIT_MAX = 65520.0                   # the least magnitude the 3xFP16 split cannot hold (half_rn rounds it to inf)
 GATHER_CAP = 128                          # SASSD_FLAG_GATHER_CAP: sassd_points_in_rbboxes' rows exceed gather_cap
+TILE_WAIT = 1024                          # SASSD_FLAG_TILE_WAIT: a dense conv gave up waiting for its input tiles
 
 P = c_void_p
 _SIGNATURES = {
@@ -88,6 +90,7 @@ _SIGNATURES = {
     "sassd_rulebook_conv_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "sassd_rulebook_conv_outputs": (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, P, c_size_t, P]),
     "sassd_set_pdl": (c_int, [c_int]),
+    "sassd_pdl_enabled": (c_int, []),
     "sassd_rulebook_conv_outputs_hash": (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, P, P, c_int, P, P, c_int, P, P,
                                                  c_size_t, P]),
     "sassd_rulebook_conv_nbr": (c_int, [P, P, c_int, c_int, c_int, c_int, P, P, c_int, P, P, P]),
@@ -203,5 +206,8 @@ def raise_on_status(word):
     if word & F16_RANGE:
         raise SassdError("activation out of the fp16 split's range on device (|x| >= 65520), outputs that read it are "
                          "NaN: %s; run the model at set_precision(PREC_FP32) (fp32 range)" % decode_flags(word))
+    if word & TILE_WAIT:
+        raise SassdError("a dense conv waited over a second for its input tiles and went on without them, its outputs "
+                         "are undefined: %s; SASSD_TILE_FLAGS=0 turns the per-tile waits off" % decode_flags(word))
     if word:
         raise SassdError("capacity overflow on device: %s" % decode_flags(word))

@@ -137,13 +137,15 @@ def pack_conv2d_weight(w, dc_order=None):
     return p.contiguous().float()
 
 
-def conv2d_nhwc(x, weight_packed, scale, shift, relu, cout, precision=ops.PREC_FP32, out=None, split_out=False):
+def conv2d_nhwc(x, weight_packed, scale, shift, relu, cout, precision=ops.PREC_FP32, out=None, split_out=False,
+                in_ready=None, out_ready=None):
     """x [B,H,W,Cin] NHWC contiguous -> [B,H,W,cout_stride]; 3x3 (pad 1) when taps == 9, 1x1 when 1.
     A ``ops.SplitMap`` input selects the TMA tensor-core kernel (csrc/conv2d_tma.cu); ``split_out`` then keeps
-    the output in split form for the next such layer."""
+    the output in split form for the next such layer, and in_ready / out_ready are its tile counters
+    (ops.conv2d_split)."""
     if isinstance(x, ops.SplitMap):
         sp, f32 = ops.conv2d_split(x, weight_packed, scale, shift, relu, cout, out_split=split_out,
-                                   out_f32=not split_out)
+                                   out_f32=not split_out, in_ready=in_ready, out_ready=out_ready)
         return sp if split_out else f32
     B, H, W, cin = x.shape
     taps = weight_packed.shape[0]
@@ -186,14 +188,23 @@ class BEVNet(nn.Module):
         if self.training:
             raise NotImplementedError("sassd_b200 is inference-only: call .eval()")
         split = isinstance(x, ops.SplitMap)
-        for i in range(7):
-            scale, shift = fold_bn(getattr(self, "bn%d" % i))
-            x = conv2d_nhwc(x, self._weights(i, dc_order if i == 0 else None), scale, shift, True, self.num_filters,
-                            self.precision, split_out=split)
-        conv6 = x
-        scale, shift = fold_bn(self.bn7)
-        x = conv2d_nhwc(x, self._weights(7, None), scale, shift, True, self.num_filters, self.precision,
-                        split_out=split)
+        # conv1-conv7 start each tile once the tiles it reads of the previous map are stored: counters for the
+        # outputs of conv0-conv6.  A layer may then still read its input while later layers write theirs, so every
+        # map stays referenced until conv7 is queued: the allocator must not hand one to a later layer's output.
+        # Every layer's weights and folded BatchNorm before the first conv: on a cache miss they queue work, which must
+        # not come between a conv and the next (ops.conv2d_split, in_ready).
+        params = [(self._weights(i, dc_order if i == 0 else None),) + fold_bn(getattr(self, "bn%d" % i))
+                  for i in range(8)]
+        ready = ops.tile_ready_arena(x, 7) if split and self.num_filters > 64 else None
+        live = []
+        for i, (weight, scale, shift) in enumerate(params):
+            kw = {}
+            if ready is not None:
+                kw = dict(in_ready=ready[i - 1] if i > 0 else None, out_ready=ready[i] if i < 7 else None)
+                live.append(x)
+            x = conv2d_nhwc(x, weight, scale, shift, True, self.num_filters, self.precision, split_out=split, **kw)
+            if i == 6:
+                conv6 = x
         return x, conv6
 
     def forward(self, x):

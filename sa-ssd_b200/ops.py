@@ -341,6 +341,9 @@ def rulebook_pairs(nbr, d_rows):
 
 # ---------------------------------------------------------------------------- gathered conv
 _TC_PACKS = {}
+# Bumped by every fill of the dense conv's caches (weight pack, constant vector, background), each of which queues work
+# on the stream: conv2d_split sees from it whether its preparation launched anything after the input's producer.
+_CONV2D_FILLS = 0
 
 
 def check_f16_weight(weight, what):
@@ -397,6 +400,8 @@ def conv2d_pack_cached(weight):
         _call("sassd_conv2d_pack", None, _ptr(w), taps, cin, cout, _ptr(packed), _stream())
         ent = (packed, weight)
         _TC_PACKS[key] = ent
+        global _CONV2D_FILLS
+        _CONV2D_FILLS += 1
     return ent[0]
 
 
@@ -845,6 +850,14 @@ class SplitMap:
 TILE_OCCUPANCY = os.environ.get("SASSD_TMA_OCC", "1") != "0"     # constant-region tile skipping in the BEV convs
 CONV2D_TILE_ORDER = 0       # 1 while a latency-oriented step is captured (computed tiles first, see sassd_b200.h)
 CONV2D_COUNTERS = None     # bench instrumentation: {label: int32[2] device tensor} += tiles computed, += tiles
+# Per-tile ready counters between consecutive BN = 128 convs launched as programmatic dependents (tile_ready_arena):
+# a conv starts each tile once the tiles it reads are stored instead of waiting for the whole previous layer.  Results
+# are the same bit for bit either way; SASSD_TILE_FLAGS=0 turns them off for bisecting.
+CONV2D_TILE_FLAGS = os.environ.get("SASSD_TILE_FLAGS", "1") != "0"
+# Frames per step up to which the counters are used.  At batch 1 a 256-channel layer is about two units per SM and its
+# second half mostly idle; at batch 16 it is ~23 units per SM, the tail is small and the per-unit release fences cost
+# more than the early starts return (H100 80GB HBM3, 700 W: batch 1 +6 %, batch 16 -2 % with the counters).
+TILE_FLAGS_MAX_BATCH = 1
 _TILE_FAR = 1 << 20
 
 
@@ -891,6 +904,8 @@ def conv_constant(x_const, cin, weight, scale, shift, relu, cout):
         _, f = conv2d_split(SplitMap.from_float(m), weight, scale, shift, relu, cout, out_split=False, out_f32=True)
         ent = (f[0, h // 2, w // 2, :cout].clone().contiguous(), weight, scale, shift, x_const)   # keep keys alive
         _CONV_CONSTS[key] = ent
+        global _CONV2D_FILLS
+        _CONV2D_FILLS += 1
     return ent[0]
 
 
@@ -923,6 +938,8 @@ def conv_background(x, weight, scale, shift, relu, cout, out_split, out_f32):
         nbytes = sum(t.numel() * t.element_size() for t in (bg[0] and bg[0].planes, bg[1]) if t is not None)
         ent = (bg, nbytes, weight, scale, shift, src)       # keep the keys alive
         _BACKGROUNDS[key] = ent
+        global _CONV2D_FILLS
+        _CONV2D_FILLS += 1
         while len(_BACKGROUNDS) > 1 and sum(e[1] for e in _BACKGROUNDS.values()) > BACKGROUND_CACHE_BYTES:
             _BACKGROUNDS.popitem(last=False)
     else:
@@ -940,16 +957,37 @@ def sparse_to_bev_split(feat, coors, d_rows, C, D, H, W, batch, status=None):
     return SplitMap(planes, D * C, dist, status=status)
 
 
-def conv2d_split(x, weight, scale, shift, relu, cout, out_split=True, out_f32=False):
-    """x: SplitMap; weight [taps, cin, cout] fp32 (packed on first use).  Returns (SplitMap | None, fp32 map | None)."""
+def tile_ready_arena(x, maps):
+    """Ready counters for ``maps`` outputs of a chain of cout > 64 convs on split map x, each conv launched right after
+    the one that wrote its input (sassd_conv2d_desc.in_ready / out_ready): a list of int32 [tiles + 1] views of one
+    arena, zeroed here, once per call (the arena is a fresh allocation, a node of its own in a captured graph).  None
+    when the counters are off: CONV2D_TILE_FLAGS unset, launches not programmatic (without PDL every conv waits for
+    the previous one anyway), no status word to report a timed-out wait in, or more than TILE_FLAGS_MAX_BATCH
+    frames."""
+    B, H, W, _ = x.shape
+    if not CONV2D_TILE_FLAGS or x.status is None or B > TILE_FLAGS_MAX_BATCH or not _L().sassd_pdl_enabled():
+        return None
+    th, tw = _lib.CONV2D_TILE_H, _lib.CONV2D_TILE_W
+    n = B * ((H + th - 1) // th) * ((W + tw - 1) // tw) + 1
+    return list(torch.zeros((maps, n), dtype=torch.int32, device=x.device).unbind(0))
+
+
+def conv2d_split(x, weight, scale, shift, relu, cout, out_split=True, out_f32=False, in_ready=None, out_ready=None):
+    """x: SplitMap; weight [taps, cin, cout] fp32 (packed on first use).  Returns (SplitMap | None, fp32 map | None).
+    in_ready / out_ready (cout > 64): tile_ready_arena counters of x and of the output map.  in_ready requires that
+    the launch which wrote x is the last one on the stream before this call; work this call queues itself first (a
+    weight pack, constant or background not yet cached) breaks that, and the conv then waits for it to complete
+    instead of polling the counters."""
     B, H, W, cin = x.shape
     taps = weight.shape[0]
+    fills = _CONV2D_FILLS
     wp = conv2d_pack_cached(weight)
     d = Conv2dDesc()
     d.batch, d.H, d.W, d.cin, d.cin_stored = B, H, W, cin, x.planes.shape[-1]
     d.cout, d.taps, d.relu = cout, taps, 1 if relu else 0
     d.tile_order = CONV2D_TILE_ORDER
     d.n_split = 0        # the kernel picks its units (cout > 128: two 128-channel units per tile)
+    d.out_ready = None if out_ready is None else _ptr(out_ready).value
     osp = of = None
     if out_split:
         cs = (cout + 63) // 64 * 64
@@ -971,6 +1009,8 @@ def conv2d_split(x, weight, scale, shift, relu, cout, out_split=True, out_f32=Fa
         bg = conv_background(x, weight, scale, shift, relu, cout, out_split, out_f32)
         if bg is not None:
             bg_sp, bg_f = bg
+    # with a cache filled above, the kernel would read what that work writes without waiting for it
+    d.in_ready = None if in_ready is None or _CONV2D_FILLS != fills else _ptr(in_ready).value
     _call("sassd_conv2d_f16x3_occ_bg_status", label, ctypes.byref(d), _ptr(x.planes), _ptr(wp), _ptr(scale), _ptr(shift),
           _ptr(of), _ptr(osp), _ptr(dist), reach, _ptr(cvec), _ptr(bg_sp.planes if bg_sp is not None else None),
           _ptr(bg_f), _ptr(CONV2D_COUNTERS.get(label) if CONV2D_COUNTERS is not None else None), _ptr(x.status),
