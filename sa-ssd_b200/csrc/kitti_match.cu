@@ -182,10 +182,12 @@ __device__ __forceinline__ double min_overlap_of(const SassdKittiEvalDesc& e, co
 
 // Pass 1 (compute_fp=False): append the score of every true positive to its job's score region.  One thread per
 // (job, frame); `asg` is this thread's assigned-detection scratch, stride kScratchThreads.
+// With `frames`, each score's frame goes to the same slot of it.
 __global__ void __launch_bounds__(kMatchThreads) eval_tp_scores_kernel(SassdKittiEvalDesc e, long long njobs,
                                                                      char* __restrict__ asg_ws,
                                                                      double* __restrict__ scores,
-                                                                     int32_t* __restrict__ n_scores) {
+                                                                     int32_t* __restrict__ n_scores,
+                                                                     int32_t* __restrict__ frames = nullptr) {
     const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     char* asg = asg_ws + tid;
     for (long long w = tid; w < njobs * e.nframes; w += kScratchThreads) {
@@ -213,11 +215,43 @@ __global__ void __launch_bounds__(kMatchThreads) eval_tp_scores_kernel(SassdKitt
                 asg[det * kScratchThreads] = 1;
             } else {
                 const int slot = atomicAdd(&n_scores[job], 1);
-                if (slot < cap) scores[base + slot] = fr.score[det];
+                if (slot < cap) {
+                    scores[base + slot] = fr.score[det];
+                    if (frames) frames[base + slot] = (int32_t)(w % e.nframes);
+                }
                 asg[det * kScratchThreads] = 1;
             }
         }
     }
+}
+
+// Sort the first n of a job's P (a power of two) scores descending, bitonic over the whole region padded with -inf,
+// by the whole CTA; `tag` (or null) is permuted with them.
+__device__ void sort_desc(double* s, int32_t* tag, long long n, long long P) {
+    for (long long i = n + threadIdx.x; i < P; i += blockDim.x) {
+        s[i] = -INFINITY;
+        if (tag) tag[i] = -1;
+    }
+    __syncthreads();
+    for (long long k = 2; k <= P; k <<= 1)
+        for (long long jj = k >> 1; jj > 0; jj >>= 1) {
+            for (long long i = threadIdx.x; i < P; i += blockDim.x) {
+                const long long l = i ^ jj;
+                if (l > i) {
+                    const double a = s[i], b = s[l];
+                    if ((i & k) == 0 ? a < b : a > b) {      // descending runs where (i & k) == 0
+                        s[i] = b;
+                        s[l] = a;
+                        if (tag) {
+                            const int32_t t = tag[i];
+                            tag[i] = tag[l];
+                            tag[l] = t;
+                        }
+                    }
+                }
+            }
+            __syncthreads();
+        }
 }
 
 // get_thresholds (kitti_eval.py:17-36): sort each job's scores descending (bitonic, in its power-of-two region), then
@@ -230,22 +264,7 @@ __global__ void eval_thresholds_kernel(SassdKittiEvalDesc e, double* __restrict_
     double* s = scores + e.score_off[job];
     const long long P = e.score_off[job + 1] - e.score_off[job];
     const long long n = n_scores[job] < P ? n_scores[job] : P;
-    for (long long i = n + threadIdx.x; i < P; i += blockDim.x) s[i] = -INFINITY;
-    __syncthreads();
-    for (long long k = 2; k <= P; k <<= 1)
-        for (long long jj = k >> 1; jj > 0; jj >>= 1) {
-            for (long long i = threadIdx.x; i < P; i += blockDim.x) {
-                const long long l = i ^ jj;
-                if (l > i) {
-                    const double a = s[i], b = s[l];
-                    if ((i & k) == 0 ? a < b : a > b) {      // descending runs where (i & k) == 0
-                        s[i] = b;
-                        s[l] = a;
-                    }
-                }
-            }
-            __syncthreads();
-        }
+    sort_desc(s, nullptr, n, P);
     if (threadIdx.x != 0) return;
     const double num_gt = (double)e.n_valid[(long long)jb.c * e.ndiff + jb.d];
     const double step = 1.0 / (kThresh - 1.0);
@@ -518,6 +537,185 @@ __global__ void __launch_bounds__(kMatchThreads) eval_assign_kernel(SassdKittiEv
     }
 }
 
+
+// --------------------------------------------------------------------------------------------------- bootstrap
+// A bootstrap replicate is a list of the split's frames drawn with replacement.  Its matching needs no new overlaps:
+// pass 2 reads the threshold only through `score < thresh`, so a frame's (tp, fp, fn, similarity) at threshold t is its
+// state at the smallest of its own scores >= t, or the state with every scored detection inactive when there is none
+// (a NaN score is active at every threshold).  Each (job, frame) keeps that step table once; a replicate's per-threshold
+// sums are then lookups over its list.
+
+// The first table entry of (job, frame f): the job's block of tab_off, then set k's frames, nd + 1 entries each.
+__device__ __forceinline__ long long step_base(const SassdKittiEvalDesc& e, const Job& jb, long long job,
+                                               const int64_t* tab_off, int f) {
+    const int b0 = jb.k * e.nframes;
+    return tab_off[job] + (e.dt_off[b0 + f] - e.dt_off[b0]) + f;
+}
+
+// One thread per (job, frame): entry 0 is the state with every scored detection inactive (frame_statistics at +inf),
+// entries 1..m the states at the frame's distinct non-NaN scores of detections the job does not skip (flag != -1), in
+// descending score order; tab_n[job * nframes + f] = m.
+__global__ void __launch_bounds__(kMatchThreads) boot_steps_kernel(SassdKittiEvalDesc e, long long njobs,
+                                                                 char* __restrict__ asg_ws,
+                                                                 double* __restrict__ vals_ws,
+                                                                 const int64_t* __restrict__ tab_off,
+                                                                 double* __restrict__ tab_score,
+                                                                 int32_t* __restrict__ tab_cnt,
+                                                                 double* __restrict__ tab_sim,
+                                                                 int32_t* __restrict__ tab_n) {
+    const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    char* asg = asg_ws + tid;
+    double* vals = vals_ws + tid;
+    for (long long w = tid; w < njobs * e.nframes; w += kScratchThreads) {
+        const long long job = w / e.nframes;
+        const int f = (int)(w % e.nframes);
+        const Job jb = decode_job(e, job);
+        const Frame fr = frame_of(e, jb, f);
+        const double min_ov = min_overlap_of(e, jb);
+        const long long base = step_base(e, jb, job, tab_off, f);
+        double thresh = INFINITY;
+        int m = 0;
+        for (;;) {
+            int tp, fp, fn;
+            double sim;
+            frame_statistics<false>(fr, jb.m, min_ov, thresh, asg, vals, &tp, &fp, &fn, &sim);
+            tab_score[base + m] = thresh;
+            tab_cnt[3 * (base + m)] = tp;
+            tab_cnt[3 * (base + m) + 1] = fp;
+            tab_cnt[3 * (base + m) + 2] = fn;
+            tab_sim[base + m] = sim;
+            // the next distinct score down: the largest below the last one (any, +inf included, the first time)
+            bool found = false;
+            double next = 0.0;
+            for (int j = 0; j < fr.nd; ++j) {
+                const double sc = fr.score[j];
+                if (fr.idt[j] == -1 || sc != sc || (m > 0 && !(sc < thresh))) continue;
+                if (!found || sc > next) { next = sc; found = true; }
+            }
+            if (!found) break;
+            thresh = next;
+            ++m;
+        }
+        tab_n[w] = m;
+    }
+}
+
+// get_thresholds over replicate r's true positives: job's sorted scores, entry i counted weight[r, frame of i] times
+// (copies of one score are interchangeable), at recall positions over the replicate's valid GT count num_gt[r, cd].
+// One thread per (job, replicate), replicates fastest.
+__global__ void boot_thresholds_kernel(SassdKittiEvalDesc e, long long njobs, int nrep,
+                                       const int32_t* __restrict__ weight, const double* __restrict__ num_gt,
+                                       const double* __restrict__ scores, const int32_t* __restrict__ frames,
+                                       const int32_t* __restrict__ n_scores, double* __restrict__ thresholds,
+                                       int32_t* __restrict__ n_thresh) {
+    const long long w = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (w >= njobs * nrep) return;
+    const long long job = w / nrep;
+    const int r = (int)(w % nrep);
+    const Job jb = decode_job(e, job);
+    const long long s0 = e.score_off[job], P = e.score_off[job + 1] - s0;
+    const long long nj = n_scores[job] < P ? n_scores[job] : P;
+    const int32_t* wr = weight + (long long)r * e.nframes;
+    long long n = 0;
+    for (long long i = 0; i < nj; ++i) n += wr[frames[s0 + i]];
+    const double ngt = num_gt[(long long)r * e.nclass * e.ndiff + (long long)jb.c * e.ndiff + jb.d];
+    const double step = 1.0 / (kThresh - 1.0);
+    double* out = thresholds + ((long long)r * njobs + job) * kThresh;
+    double cur = 0.0;
+    int nt = 0;
+    long long i = 0;
+    for (long long q = 0; q < nj && nt < kThresh; ++q) {
+        const int c = wr[frames[s0 + q]];
+        const double sc = scores[s0 + q];
+        for (int copy = 0; copy < c && nt < kThresh; ++copy, ++i) {
+            const double l_recall = ddiv((double)(i + 1), ngt);
+            const double r_recall = i < n - 1 ? ddiv((double)(i + 2), ngt) : l_recall;
+            if (dsub(r_recall, cur) < dsub(cur, l_recall) && i < n - 1) continue;
+            out[nt++] = sc;
+            cur = dadd(cur, step);
+        }
+    }
+    for (int t = nt; t < kThresh; ++t) out[t] = 0.0;
+    n_thresh[(long long)r * njobs + job] = nt;
+}
+
+// Pass 2 of replicate r: one warp per (job, replicate), lane l at thresholds l and l + 32.  Each frame of the list, in
+// list order, adds the table entry of its smallest own score >= the threshold; the counts are integers (any order),
+// the similarity is added in list order as fused_compute_statistics adds it over the frames.
+constexpr int kBootWarps = 4;
+__global__ void __launch_bounds__(32 * kBootWarps) boot_pr_kernel(SassdKittiEvalDesc e, long long njobs, int nrep,
+                                                                  const int32_t* __restrict__ list,
+                                                                  const double* __restrict__ thresholds,
+                                                                  const int32_t* __restrict__ n_thresh,
+                                                                  const int64_t* __restrict__ tab_off,
+                                                                  const double* __restrict__ tab_score,
+                                                                  const int32_t* __restrict__ tab_cnt,
+                                                                  const double* __restrict__ tab_sim,
+                                                                  const int32_t* __restrict__ tab_n,
+                                                                  double* __restrict__ pr) {
+    const long long wid = blockIdx.x * (long long)kBootWarps + threadIdx.x / 32;
+    const int lane = threadIdx.x % 32;
+    if (wid >= njobs * nrep) return;
+    const long long job = wid / nrep;
+    const int r = (int)(wid % nrep);
+    const Job jb = decode_job(e, job);
+    const bool aos = jb.m == 0 && e.aos_table && e.compute_aos[jb.k];
+    const long long rj = (long long)r * njobs + job;
+    const int nt = n_thresh[rj];
+    constexpr int kPer = (kThresh + 31) / 32;
+    double th[kPer], sim[kPer];
+    long long tp[kPer], fp[kPer], fn[kPer];
+#pragma unroll
+    for (int u = 0; u < kPer; ++u) {
+        const int t = lane + 32 * u;
+        th[u] = t < nt ? thresholds[rj * kThresh + t] : INFINITY;
+        sim[u] = 0.0;
+        tp[u] = fp[u] = fn[u] = 0;
+    }
+    if (lane < nt) {
+        const int32_t* lr = list + (long long)r * e.nframes;
+        for (int p = 0; p < e.nframes; ++p) {
+            const int f = lr[p];
+            const long long base = step_base(e, jb, job, tab_off, f);
+            const int m = tab_n[job * e.nframes + f];
+#pragma unroll
+            for (int u = 0; u < kPer; ++u) {
+                if (lane + 32 * u >= nt) break;
+                int lo = 0, hi = m;                      // count the own scores >= th: entries 1..m descend
+                while (lo < hi) {
+                    const int mid = (lo + hi + 1) >> 1;
+                    if (tab_score[base + mid] >= th[u]) lo = mid; else hi = mid - 1;
+                }
+                const long long at = base + lo;
+                tp[u] += tab_cnt[3 * at];
+                fp[u] += tab_cnt[3 * at + 1];
+                fn[u] += tab_cnt[3 * at + 2];
+                if (aos) {
+                    const double s = tab_sim[at];
+                    if (s != -1.0) sim[u] = dadd(sim[u], s);
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int u = 0; u < kPer; ++u) {
+        const int t = lane + 32 * u;
+        if (t >= kThresh) break;
+        double* o = pr + (rj * kThresh + t) * 4;
+        o[0] = (double)tp[u];
+        o[1] = (double)fp[u];
+        o[2] = (double)fn[u];
+        o[3] = sim[u];
+    }
+}
+
+// The bootstrap's true-positive scores of each job sorted descending with their frames.  One CTA per job.
+__global__ void boot_sort_kernel(SassdKittiEvalDesc e, double* __restrict__ scores, int32_t* __restrict__ frames,
+                                 const int32_t* __restrict__ n_scores) {
+    const long long job = blockIdx.x, s0 = e.score_off[job], P = e.score_off[job + 1] - s0;
+    sort_desc(scores + s0, frames + s0, n_scores[job] < P ? n_scores[job] : P, P);
+}
+
 }  // namespace
 
 extern "C" int sassd_kitti_eval_flags(int ngt, const int32_t* gt_name, const double* gt_occ, const double* gt_trunc,
@@ -594,7 +792,7 @@ extern "C" int sassd_kitti_eval_match(const SassdKittiEvalDesc* e, double* score
         cudaMemsetAsync(pr, 0, sizeof(double) * 4 * kThresh * njobs, stream) != cudaSuccess)
         return SASSD_ERR_LAUNCH;
     if (e->nframes == 0) return SASSD_OK;
-    eval_tp_scores_kernel<<<kMatchCtas, kMatchThreads, 0, stream>>>(*e, njobs, asg, scores, n_scores);
+    eval_tp_scores_kernel<<<kMatchCtas, kMatchThreads, 0, stream>>>(*e, njobs, asg, scores, n_scores, nullptr);
     eval_thresholds_kernel<<<(unsigned)njobs, 1024, 0, stream>>>(*e, scores, n_scores, thresholds, n_thresh);
     eval_pr_kernel<<<kMatchCtas, kMatchThreads, 0, stream>>>(*e, njobs, asg, vals, thresholds, n_thresh, pr);
     return sassd_check_launch();
@@ -629,5 +827,53 @@ extern "C" int sassd_kitti_eval_assign(const SassdKittiEvalDesc* e, int row, int
     const long long njobs = (long long)e->nsets * e->nclass * ndiff * 3;
     eval_assign_kernel<<<kMatchCtas, kMatchThreads, 0, (cudaStream_t)stream>>>(*e, row, ndiff, njobs, (char*)ws, gt_cam,
                                                                              dt_cam, gt_det, gt_ov, dt_state, tp_err);
+    return sassd_check_launch();
+}
+
+static bool boot_desc_ok(const SassdKittiEvalDesc* e) {
+    return e && e->nsets >= 1 && e->nframes >= 1 && e->nclass >= 1 && e->ndiff >= 1 && e->nover >= 1 &&
+           e->max_nd >= 0 && e->max_ng >= 0 && e->gt_off && e->dt_off && e->ov_off && e->gt_dc && e->gt_bbox &&
+           e->dt_bbox && e->dt_score && e->ov_bbox && e->ov_bev && e->ov_3d && e->compute_aos && e->min_overlaps &&
+           e->ign_gt && e->ign_dt && e->n_valid && e->score_off;
+}
+
+extern "C" int sassd_kitti_boot_prepare(const SassdKittiEvalDesc* e, double* scores, int32_t* frames,
+                                        int32_t* n_scores, const int64_t* tab_off, double* tab_score,
+                                        int32_t* tab_cnt, double* tab_sim, int32_t* tab_n, void* ws, size_t ws_bytes,
+                                        sassd_stream_t stream_) {
+    if (!boot_desc_ok(e) || !scores || !frames || !n_scores || !tab_off || !tab_score || !tab_cnt || !tab_sim ||
+        !tab_n || !ws)
+        return SASSD_ERR_ARG;
+    const long long njobs = (long long)e->nsets * e->nclass * e->ndiff * 3 * e->nover;
+    if (njobs > 0x7fffffffLL) return SASSD_ERR_ARG;
+    if (ws_bytes < sassd_kitti_eval_workspace_bytes(e->max_nd, e->max_ng)) return SASSD_ERR_WORKSPACE;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    char* asg = (char*)ws;
+    double* vals = (double*)(asg + ((size_t)kScratchThreads * (size_t)(e->max_nd > 0 ? e->max_nd : 1) + 255) / 256 * 256);
+    if (cudaMemsetAsync(n_scores, 0, sizeof(int32_t) * njobs, stream) != cudaSuccess) return SASSD_ERR_LAUNCH;
+    eval_tp_scores_kernel<<<kMatchCtas, kMatchThreads, 0, stream>>>(*e, njobs, asg, scores, n_scores, frames);
+    boot_sort_kernel<<<(unsigned)njobs, 1024, 0, stream>>>(*e, scores, frames, n_scores);
+    boot_steps_kernel<<<kMatchCtas, kMatchThreads, 0, stream>>>(*e, njobs, asg, vals, tab_off, tab_score, tab_cnt,
+                                                                tab_sim, tab_n);
+    return sassd_check_launch();
+}
+
+extern "C" int sassd_kitti_boot_eval(const SassdKittiEvalDesc* e, int nrep, const int32_t* list,
+                                     const int32_t* weight, const double* num_gt, const double* scores,
+                                     const int32_t* frames, const int32_t* n_scores, const int64_t* tab_off,
+                                     const double* tab_score, const int32_t* tab_cnt, const double* tab_sim,
+                                     const int32_t* tab_n, double* thresholds, int32_t* n_thresh, double* pr,
+                                     sassd_stream_t stream_) {
+    if (!boot_desc_ok(e) || nrep < 1 || !list || !weight || !num_gt || !scores || !frames || !n_scores || !tab_off ||
+        !tab_score || !tab_cnt || !tab_sim || !tab_n || !thresholds || !n_thresh || !pr)
+        return SASSD_ERR_ARG;
+    const long long njobs = (long long)e->nsets * e->nclass * e->ndiff * 3 * e->nover;
+    const long long items = njobs * nrep;
+    if (njobs > 0x7fffffffLL || items > 0x7fffffffLL * (long long)kBootWarps) return SASSD_ERR_ARG;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    boot_thresholds_kernel<<<(unsigned)sassd_div_up(items, 128), 128, 0, stream>>>(
+        *e, njobs, nrep, weight, num_gt, scores, frames, n_scores, thresholds, n_thresh);
+    boot_pr_kernel<<<(unsigned)sassd_div_up(items, kBootWarps), 32 * kBootWarps, 0, stream>>>(
+        *e, njobs, nrep, list, thresholds, n_thresh, tab_off, tab_score, tab_cnt, tab_sim, tab_n, pr);
     return sassd_check_launch();
 }

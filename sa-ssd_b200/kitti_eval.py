@@ -22,10 +22,13 @@ the device (`read_block`, csrc/kitti_parse.cu).
 
 ``eval_many(..., ranges=[e0, e1, ...])`` adds every table per bin [e_i, e_i+1) of ground distance from the camera (more
 difficulty entries of the same evaluation), and ``match_table`` / ``eval_many(..., match=True)`` the evaluator's own
-per-object assignment with the 3-D true positives' ATE / ASE / AOE (``tp_errors``).
+per-object assignment with the 3-D true positives' ATE / ASE / AOE (``tp_errors``).  ``eval_many(...,
+bootstrap=idx)`` adds every table over bootstrap replicates of the frames (``bootstrap_indices``), each replicate bit for
+bit the evaluation of its resampled lists, with ``percentile_interval`` / ``paired_summary`` to summarise them.
 
     python -m sassd_b200.kitti_eval --data-root DIR [--split val] --results DIR [DIR ...] [--classes Car ...]
                                     [--r40] [--coco] [--json FILE] [--ranges EDGE ...] [--matches FILE.npz]
+                                    [--bootstrap R [--bootstrap-seed S]]
 
 evaluates directories of result files against a split's labels (`main`, `eval_dirs`).
 """
@@ -527,6 +530,17 @@ def _eval_device_full(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos
     ndiff) also the match table of the first ndiff entries at min-overlap row ``row`` (match_table's dicts, one per
     set), from the flags and overlaps already on the device.  ``ap`` False skips the AP matching (the arrays are then
     None).  Returns (arrays, tables)."""
+    st = _device_setup(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flags, bins, assign is not None)
+    return _device_arrays(st, assign, ap)
+
+
+def _device_setup(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos_flags, bins=None, ranged_out=False,
+                  aos_table=False):
+    """What every device evaluation of these sets starts from, built once: the blocks on the device, the flags, the
+    rotated and metric overlaps, the AOS cos table (when a set computes AOS, or ``aos_table``) and the matching
+    descriptor.  ``ranged_out``: also each row's ground range.  Returns a namespace."""
+    import types
+
     import torch
     from . import ops
     dev = _cuda_device()
@@ -554,7 +568,8 @@ def _eval_device_full(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos
              dt_bbox=dt_bbox, dt_score=torch.cat([d.score for d in dts]), gt_cam=gt.cam, dt_cam=dt_cam,
              min_overlaps=up(np.asarray(min_overlaps, np.float64)), compute_aos=up(np.asarray(aos_flags, np.int32)))
     ranged = bins is not None and any(b is not None for b in bins)
-    if ranged or assign is not None:
+    gt_range = dt_range = None
+    if ranged or ranged_out:
         # an entry without a bin has a lower edge of -inf: no range test
         ranges = up(np.array([(-np.inf, np.inf) if b is None else b for b in bins], np.float64)) if ranged else None
         ign_gt, ign_dt, n_valid, gt_range, dt_range = ops.kitti_eval_flags_ranged(
@@ -577,14 +592,14 @@ def _eval_device_full(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos
         rot.append(out)
     ov = ops.kitti_eval_overlaps(K, F, t["gt_off"], t["dt_off"], t["ov_off"], t["gt_cam"], t["dt_cam"], t["gt_bbox"],
                                  t["dt_bbox"], rot[0], rot[1], total, int(npairs.max()) if len(npairs) else 0)
-    aos_table = None
-    if any(aos_flags) and total:
+    aos_tab = None
+    if (any(aos_flags) or aos_table) and total:
         table = np.zeros((total,), np.float64)
         gt_alpha = gt.alpha.cpu().numpy()
         dt_alpha = torch.cat([d.alpha for d in dts]).cpu().numpy()
         _lib.check(_lib.load().sassd_kitti_aos_table(K, F, _p(gt_off), _p(dt_off), _p(ov_off), _p(gt_alpha),
                                                      _p(dt_alpha), _p(table)), "sassd_kitti_aos_table")
-        aos_table = up(table)
+        aos_tab = up(table)
     # each job's score region: the next power of two of its (class, difficulty)'s valid GT count
     nv = n_valid.cpu().numpy().astype(np.int64)
     region = np.broadcast_to((1 << np.ceil(np.log2(np.maximum(nv, 1))).astype(np.int64))[None, :, :, None, None],
@@ -593,16 +608,25 @@ def _eval_device_full(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos
     desc = _lib.KittiEvalDesc(nsets=K, nframes=F, nclass=C, ndiff=Dn, nover=M, max_nd=int(nd.max()) if len(nd) else 0,
                               max_ng=int(ng.max()) if len(ng) else 0)
     keep = dict(t, ign_gt=ign_gt, ign_dt=ign_dt, n_valid=n_valid, score_off=score_off, ov_bbox=ov[0], ov_bev=ov[1],
-                ov_3d=ov[2], aos_table=aos_table)
+                ov_3d=ov[2], aos_table=aos_tab)
     for name, _ in desc._fields_[7:]:
         setattr(desc, name, keep[name].data_ptr() if keep[name] is not None else None)
+    return types.SimpleNamespace(gt=gt, dts=dts, K=K, F=F, C=C, Dn=Dn, M=M, ng=ng, nd=nd, region=region, desc=desc,
+                                 keep=keep, dt_cam=dt_cam, gt_range=gt_range, dt_range=dt_range, aos_flags=aos_flags,
+                                 up=up)
+
+
+def _device_arrays(st, assign, ap):
+    """_eval_device_full's arrays and match tables from a _device_setup."""
+    from . import ops
+    K, C, Dn, M, gt, dts = st.K, st.C, st.Dn, st.M, st.gt, st.dts
     tables = None
     if assign is not None:
         row, nd_t = assign
-        gt_det, gt_ov, dt_state, tp_err = (x.cpu().numpy() for x in ops.kitti_eval_assign(desc, row, nd_t, gt.cam,
-                                                                                            dt_cam))
-        gt_flag, dt_flag = ign_gt[:, :nd_t].cpu().numpy(), ign_dt[:, :nd_t].cpu().numpy()
-        gt_range, dt_range = gt_range.cpu().numpy(), dt_range.cpu().numpy()
+        gt_det, gt_ov, dt_state, tp_err = (x.cpu().numpy() for x in ops.kitti_eval_assign(st.desc, row, nd_t, gt.cam,
+                                                                                            st.dt_cam))
+        gt_flag, dt_flag = st.keep["ign_gt"][:, :nd_t].cpu().numpy(), st.keep["ign_dt"][:, :nd_t].cpu().numpy()
+        gt_range, dt_range = st.gt_range.cpu().numpy(), st.dt_range.cpu().numpy()
         rows = _offsets([int(d.off[-1]) for d in dts], np.int64)
         tables = []
         for k in range(K):
@@ -613,28 +637,36 @@ def _eval_device_full(gt_annos, dt_sets, classes, difficultys, min_overlaps, aos
                                tp_errors=tp_err[k]))
     if not ap:
         return None, tables
-    _, n_thresh, pr = ops.kitti_eval_match(desc, len(region), int(region.sum()))
+    _, n_thresh, pr = ops.kitti_eval_match(st.desc, len(st.region), int(st.region.sum()))
     n_thresh = n_thresh.cpu().numpy().reshape(K, C, Dn, 3, M)
     pr = pr.cpu().numpy().reshape(K, C, Dn, 3, M, 41, 4)
-    # precision, recall and AOS of the sampled thresholds and their monotone envelope, as eval_class_many computes them
+    return _pr_arrays(pr, n_thresh, np.asarray(st.aos_flags, bool)), tables
+
+
+def _pr_arrays(pr, n_thresh, aos_flags):
+    """precision, recall and AOS of the sampled thresholds and their monotone envelope, as eval_class_many computes
+    them, from the per-threshold sums pr [..., K, C, Dn, 3, M, 41, 4] and threshold counts n_thresh [..., K, C, Dn, 3,
+    M]; ``aos_flags`` [..., K] bool.  Returns [metric][set] -> dict of [..., C, Dn, M, 41]."""
     past = np.arange(41) >= n_thresh[..., None]
     with np.errstate(divide="ignore", invalid="ignore"):
         recall = pr[..., 0] / (pr[..., 0] + pr[..., 2])
         precision = pr[..., 0] / (pr[..., 0] + pr[..., 1])
         aos = pr[..., 3] / (pr[..., 0] + pr[..., 1])
+    K = pr.shape[-7]
     out = []
     for m in range(3):
         per_set = []
         for k in range(K):
             res = {}
             for key, a in (("recall", recall), ("precision", precision), ("orientation", aos)):
-                v = np.where(past[k, :, :, m], 0.0, a[k, :, :, m])
-                if key == "orientation" and not (m == 0 and aos_flags[k]):
-                    v = np.zeros_like(v)
+                v = np.where(past[..., k, :, :, m, :, :], 0.0, a[..., k, :, :, m, :, :])
+                if key == "orientation":
+                    on = aos_flags[..., k] & (m == 0)
+                    v = np.where(np.reshape(on, np.shape(on) + (1,) * 4), v, 0.0)
                 res[key] = np.ascontiguousarray(np.maximum.accumulate(v[..., ::-1], axis=-1)[..., ::-1])
             per_set.append(res)
         out.append(per_set)
-    return out, tables
+    return out
 
 
 def get_mAP(prec):
@@ -713,7 +745,7 @@ def range_bins(edges):
 
 
 def eval_many(gt_annos, dt_sets, classes, tables=(11,), overlap_fn=None, difficultys=(0, 1, 2), ranges=None,
-              match=False):
+              match=False, bootstrap=None):
     """Every table of ``tables`` (11 and 40: the official tables at 11 / 40 recall positions; "coco": the COCO-style
     table) for each of the K detection sets of ``dt_sets`` against the same GT.  Returns one dict per set, {table:
     (text, ap)}.  The official and COCO overlap rows form one list of min overlaps, so the overlaps, the GT side and
@@ -723,11 +755,18 @@ def eval_many(gt_annos, dt_sets, classes, tables=(11,), overlap_fn=None, difficu
     ``ranges``: bin edges (check_ranges); each set's dict then also holds ``"ranges"``: [(lo, hi, {table: (text,
     ap)}), ...], the tables over the objects whose ground range (ground_range) lies in [lo, hi), each text naming its
     range.  The bins are more difficulty entries of the same evaluation: a GT or detection of the class outside a bin is
-    ignored there (clean_gt / clean_dt).  ``match``: each set's dict also holds ``"matches"``, its match_table."""
+    ignored there (clean_gt / clean_dt).  ``match``: each set's dict also holds ``"matches"``, its match_table.
+
+    ``bootstrap``: an int array [R, F] of frame indices (bootstrap_indices), replicate r the list of frames idx[r, 0],
+    idx[r, 1], ... (duplicates included).  Each set's dict then also holds ``"bootstrap"``: {table: ap} with a leading
+    R axis on every array, replicate r's AP bit for bit what this evaluation gives on the resampled GT and detection
+    lists (compute_aos decided per replicate; ``aos`` is NaN in a replicate without it, None when no replicate has
+    it); with ``ranges`` also ``"bootstrap_ranges"``, laid out like ``"ranges"``.  Every set uses the same lists, so
+    the replicates are paired (paired_summary)."""
     tables = tuple(tables)
     if not tables or any(t not in TABLES for t in tables):
         raise ValueError("tables must be among %r, not %r" % (TABLES, tables))
-    return _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, ranges, match)
+    return _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, ranges, match, bootstrap)
 
 
 def match_table(gt_annos, dt_sets, classes, difficultys=(0, 1, 2), overlap_fn=None):
@@ -797,11 +836,12 @@ def _table_host(gt_annos, dt_sets, classes, difficultys, row, overlap_fn, gt_sid
     return out
 
 
-def _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, ranges, match):
+def _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, ranges, match, bootstrap=None):
     """eval_many's work: the AP tables of ``tables`` (none: no AP matching) over the whole range and each bin of
-    ``ranges``, and with ``match`` the match table."""
+    ``ranges``, with ``match`` the match table, and with ``bootstrap`` the replicates' AP."""
     classes = _class_ids(classes)
     edges = None if ranges is None else check_ranges(ranges)
+    idx = None if bootstrap is None else check_bootstrap(bootstrap, len(gt_annos))
     diffs = list(difficultys)
     bins = [None] + ([] if edges is None else range_bins(edges))
     entries = [(d, b) for b in bins for d in diffs]     # difficulty entries: the whole range, then bin by bin
@@ -817,9 +857,18 @@ def _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, range
     n_off = 2 if official else 0
     aos_flags = [_aos_flag(d) for d in dt_sets]
     ent_diffs, ent_bins = [d for d, _ in entries], [b for _, b in entries]
+    Dn = len(diffs)
+    boot = None
     if overlap_fn is None:
-        prec, matches = _eval_device_full(gt_annos, dt_sets, classes, ent_diffs, min_overlaps, aos_flags,
-                                          ent_bins, (table_row, len(diffs)) if match else None, bool(tables))
+        boot_aos = None
+        if idx is not None:
+            dt_sets = [_as_block(d) for d in dt_sets]
+            boot_aos = _bootstrap_aos_flags(dt_sets, idx)
+        st = _device_setup(gt_annos, dt_sets, classes, ent_diffs, min_overlaps, aos_flags, ent_bins, match,
+                           boot_aos is not None and bool(boot_aos.any()))
+        prec, matches = _device_arrays(st, (table_row, Dn) if match else None, bool(tables))
+        if idx is not None:
+            boot = _bootstrap_device(st, idx, boot_aos, tables, Dn, len(bins), n_off)
     else:
         gt_annos, dt_sets = _as_annos(gt_annos), [_as_annos(d) for d in dt_sets]
         gt_sides = {(c, d, b): _GtSide(gt_annos, c, d, b) for c in classes for d, b in entries}
@@ -828,8 +877,9 @@ def _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, range
                 for metric in (0, 1, 2)] if tables else None
         matches = (_table_host(gt_annos, dt_sets, classes, diffs, min_overlaps[table_row], overlap_fn, gt_sides)
                    if match else None)
+        if idx is not None:
+            boot = _bootstrap_host(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, edges, idx)
     out = []
-    Dn = len(diffs)
     for s, compute_aos in enumerate(aos_flags):
         res = {}
         if tables:
@@ -841,28 +891,155 @@ def _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, range
                                  for b, (lo, hi) in enumerate(bins[1:])]
         if match:
             res["matches"] = matches[s]
+        if boot is not None:
+            res["bootstrap"] = boot[s][0]
+            if edges is not None:
+                res["bootstrap_ranges"] = [(lo, hi, boot[s][b + 1]) for b, (lo, hi) in enumerate(bins[1:])]
         out.append(res)
     return out
 
 
+# ------------------------------------------------------------------ bootstrap
+BOOTSTRAP_CHUNK = 64    # replicates per device pass: the device arrays of a pass grow with it, not with R
+
+
+def bootstrap_indices(nframes, replicates, seed=0):
+    """[replicates, nframes] int64 frame indices, row r the r-th draw of np.random.RandomState(seed).randint(0,
+    nframes, nframes): a row does not depend on how many rows follow it."""
+    rs = np.random.RandomState(seed)
+    return np.stack([rs.randint(0, nframes, nframes) for _ in range(int(replicates))]).astype(np.int64)
+
+
+def check_bootstrap(idx, nframes):
+    """The bootstrap indices as an int64 [R, nframes] array, R >= 1, every index in [0, nframes); else ValueError."""
+    a = np.asarray(idx)
+    if a.dtype.kind not in "iu":
+        raise ValueError("bootstrap indices must be integers, not %s" % a.dtype)
+    if a.ndim != 2 or a.shape[0] < 1 or a.shape[1] != nframes or nframes < 1:
+        raise ValueError("bootstrap indices must be [R >= 1, %d frames], not %r" % (nframes, a.shape))
+    if a.min() < 0 or a.max() >= nframes:
+        raise ValueError("bootstrap indices must lie in [0, %d)" % nframes)
+    return a.astype(np.int64)
+
+
+def percentile_interval(samples, lo=2.5, hi=97.5):
+    """[2, ...]: np.percentile of the replicates (axis 0) at ``lo`` and ``hi`` percent."""
+    return np.percentile(np.asarray(samples, np.float64), [lo, hi], axis=0)
+
+
+def paired_summary(ap, ap0, lo=2.5, hi=97.5):
+    """A set's replicate AP against the first set's, paired replicate by replicate: dict(interval=percentile_interval
+    of ap - ap0, better=the fraction of replicates with ap - ap0 > 0)."""
+    d = np.asarray(ap, np.float64) - np.asarray(ap0, np.float64)
+    return dict(interval=percentile_interval(d, lo, hi), better=np.mean(d > 0, axis=0))
+
+
+def _bootstrap_aos_flags(dt_blocks, idx):
+    """[R, K] compute_aos of every replicate and set, as _aos_flag decides it on the replicate's list: from its first
+    frame with detections."""
+    out = np.zeros((idx.shape[0], len(dt_blocks)), bool)
+    for k, d in enumerate(dt_blocks):
+        has = d.counts > 0
+        ok = np.zeros(len(d), bool)
+        if has.any():
+            ok[has] = d.alpha[d.off[:-1][has]].cpu().numpy() != -10
+        first = np.argmax(has[idx], axis=1)
+        out[:, k] = has[idx].any(1) & ok[idx[np.arange(len(idx)), first]]
+    return out
+
+
+def _with_aos(ap, flags):
+    """A bootstrap AP dict's aos: NaN in the replicates without compute_aos, None when no replicate has it."""
+    if not flags.any():
+        return dict(ap, aos=None)
+    return dict(ap, aos=np.where(flags.reshape((-1,) + (1,) * (ap["aos"].ndim - 1)), ap["aos"], np.nan))
+
+
+def _stack_aps(aps):
+    """One AP dict with a leading replicate axis from per-replicate AP dicts (a None aos becomes NaN)."""
+    out = {}
+    for key in aps[0]:
+        vals = [a[key] for a in aps]
+        some = next((v for v in vals if v is not None), None)
+        out[key] = None if some is None else np.stack([np.full_like(some, np.nan) if v is None else v for v in vals])
+    return out
+
+
+def _bootstrap_host(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, edges, idx):
+    """The reference implementation: the host evaluation of each replicate's lists.  [set][whole range, bins...] ->
+    {table: ap with a leading R axis}."""
+    per = [[] for _ in dt_sets]
+    for row in idx:
+        ev = _evaluate([gt_annos[i] for i in row], [[d[i] for i in row] for d in dt_sets], classes, tables, overlap_fn,
+                       difficultys, edges, False)
+        for s, e in enumerate(ev):
+            per[s].append([{t: e[t][1] for t in tables}] + [{t: r[t][1] for t in tables} for _, _, r in
+                                                            e.get("ranges", [])])
+    return [[{t: _stack_aps([rep[b][t] for rep in reps]) for t in tables} for b in range(len(reps[0]))]
+            for reps in per]
+
+
+def _bootstrap_device(st, idx, boot_aos, tables, Dn, nbins, n_off):
+    """The replicates on the device from the evaluation's set-up ``st``: each job's sorted true-positive scores and
+    each (job, frame)'s step table once (sassd_kitti_boot_prepare), then per chunk of BOOTSTRAP_CHUNK replicates their
+    thresholds and per-threshold sums (sassd_kitti_boot_eval) and eval_many's numpy tail on [R, ...] arrays.  Returns
+    _bootstrap_host's layout."""
+    from . import ops
+    K, F, C, D, M = st.K, st.F, st.C, st.Dn, st.M
+    njobs = len(st.region)
+    desc = _lib.KittiEvalDesc.from_buffer_copy(st.desc)
+    any_aos = st.up(boot_aos.any(0).astype(np.int32))
+    desc.compute_aos = any_aos.data_ptr()
+    # set k's block per job: one entry per detection row and one per frame
+    per_set = np.array([int(d.off[-1]) + F for d in st.dts], np.int64)
+    tab_off = st.up(_offsets(np.repeat(per_set, njobs // K), np.int64))
+    prep = ops.kitti_boot_prepare(desc, njobs, int(st.region.sum()), tab_off)
+    # each frame's valid GT count per (class, difficulty entry)
+    valid = (st.keep["ign_gt"] == 0).cpu().numpy().reshape(C * D, -1).astype(np.int64)
+    cs = np.concatenate([np.zeros((C * D, 1), np.int64), np.cumsum(valid, 1)], 1)
+    nv = cs[:, st.gt.off[1:]] - cs[:, st.gt.off[:-1]]
+    chunks = []
+    for r0 in range(0, len(idx), BOOTSTRAP_CHUNK):
+        rows = idx[r0:r0 + BOOTSTRAP_CHUNK]
+        R = len(rows)
+        w = np.bincount((rows + F * np.arange(R)[:, None]).reshape(-1), minlength=R * F).reshape(R, F)
+        n_thresh, pr = ops.kitti_boot_eval(desc, njobs, st.up(rows.astype(np.int32)), st.up(w.astype(np.int32)),
+                                           st.up((w @ nv.T).astype(np.float64)), prep, tab_off)
+        prec = _pr_arrays(pr.cpu().numpy().reshape(R, K, C, D, 3, M, 41, 4),
+                          n_thresh.cpu().numpy().reshape(R, K, C, D, 3, M), boot_aos[r0:r0 + R])
+        chunks.append([[_ap_dicts([p[k] for p in prec], b * Dn, Dn, tables, n_off, True) for b in range(nbins)]
+                       for k in range(K)])
+    return [[{t: _with_aos({key: np.concatenate([c[k][b][t][key] for c in chunks]) for key in chunks[0][k][b][t]},
+                           boot_aos[:, k]) for t in tables} for b in range(nbins)] for k in range(K)]
+
+
 def _ap_tables(r, e0, Dn, tables, classes, min_overlaps, n_off, compute_aos, rng):
     """{table: (text, ap)} of difficulty entries [e0, e0 + Dn) of one set's precision arrays r[metric]."""
-    r0, r1, r2 = ({k: v[:, e0:e0 + Dn] for k, v in m.items()} for m in r)
+    res = {}
+    for t, ap in _ap_dicts(r, e0, Dn, tables, n_off, compute_aos).items():
+        text = (_coco_text(ap, classes, compute_aos, rng) if t == "coco" else
+                _ap_text(ap, classes, min_overlaps[:n_off], compute_aos, "AP" if t == 11 else "AP_R40", rng))
+        res[t] = (text, ap)
+    return res
+
+
+def _ap_dicts(r, e0, Dn, tables, n_off, compute_aos):
+    """{table: ap} of difficulty entries [e0, e0 + Dn) of precision arrays r[metric] of [..., C, entries, M, 41] (any
+    leading axes, e.g. bootstrap replicates)."""
+    r0, r1, r2 = ({k: v[..., e0:e0 + Dn, :, :] for k, v in m.items()} for m in r)
     res = {}
     for rp in (t for t in tables if t in (11, 40)):
         get_mAP_n = get_mAP if rp == 11 else get_mAP_R40
-        ap = dict(bbox=get_mAP_n(r0["precision"][:, :, :n_off]),
-                  aos=get_mAP_n(r0["orientation"][:, :, :n_off]) if compute_aos else None,
-                  bev=get_mAP_n(r1["precision"][:, :, :n_off]), d3=get_mAP_n(r2["precision"][:, :, :n_off]))
-        res[rp] = (_ap_text(ap, classes, min_overlaps[:n_off], compute_aos, "AP" if rp == 11 else "AP_R40", rng), ap)
+        res[rp] = dict(bbox=get_mAP_n(r0["precision"][..., :n_off, :]),
+                       aos=get_mAP_n(r0["orientation"][..., :n_off, :]) if compute_aos else None,
+                       bev=get_mAP_n(r1["precision"][..., :n_off, :]), d3=get_mAP_n(r2["precision"][..., :n_off, :]))
     if "coco" in tables:
         # do_coco_style_eval (kitti_eval.py:711-729): the mean over the ten overlaps of get_mAP_v2
         c0 = n_off + 10
-        ap = dict(bbox=get_mAP(r0["precision"][:, :, n_off:c0]).mean(-1),
-                  aos=get_mAP(r0["orientation"][:, :, n_off:c0]).mean(-1) if compute_aos else None,
-                  bev=get_mAP(r1["precision"][:, :, n_off:c0]).mean(-1),
-                  d3=get_mAP(r2["precision"][:, :, n_off:c0]).mean(-1))
-        res["coco"] = (_coco_text(ap, classes, compute_aos, rng), ap)
+        res["coco"] = dict(bbox=get_mAP(r0["precision"][..., n_off:c0, :]).mean(-1),
+                           aos=get_mAP(r0["orientation"][..., n_off:c0, :]).mean(-1) if compute_aos else None,
+                           bev=get_mAP(r1["precision"][..., n_off:c0, :]).mean(-1),
+                           d3=get_mAP(r2["precision"][..., n_off:c0, :]).mean(-1))
     return res
 
 
@@ -991,6 +1168,98 @@ def range_report(entry, ev, class_names, log=print, tp_err=None):
     return fields
 
 
+def _interval_lists(ap):
+    """percentile_interval of each of a bootstrap AP dict's arrays as JSON-ready lists ([2, ...]: low, high)."""
+    return {k: (None if v is None else percentile_interval(v).tolist()) for k, v in ap.items()}
+
+
+def _strict(a):
+    """[R, C, 3] of an AP array: the class's strict (first) overlap row of an official table; COCO has no row axis."""
+    return a[..., 0] if a.ndim == 4 else a
+
+
+def bootstrap_report(ev, class_names, log=print):
+    """Print a set's bootstrap block (``ev``: eval_many's dict with ``bootstrap``): per table and class the 95 %
+    percentile interval of bbox / BEV / 3D / AOS AP for easy, moderate and hard at the class's strict overlap.  Returns
+    (the JSON entry {table: interval lists}, the summary fields: the moderate 3D interval per class and table)."""
+    boot = ev["bootstrap"]
+    nrep = len(boot[11]["d3"])
+    for t, ap in boot.items():
+        tag = "AP" if t == 11 else "AP_R40" if t == 40 else "coco AP"
+        for j, c in enumerate(class_names):
+            log("%s %s 95%% interval (%d replicates):" % (c, tag, nrep))
+            for key, label in (("bbox", "bbox AP"), ("bev", "bev  AP"), ("d3", "3d   AP"), ("aos", "aos  AP")):
+                if ap[key] is None:
+                    continue
+                iv = percentile_interval(_strict(ap[key])[:, j])
+                log("%s:%s" % (label, ", ".join("[%.2f, %.2f]" % (iv[0, d], iv[1, d]) for d in range(3))))
+    fields = []
+    for j, c in enumerate(class_names):
+        fields.append("%s 3d mod 95%% " % c + " ".join(
+            "%s [%.2f, %.2f]" % ((("R11", "R40", "COCO")[TABLES.index(t)],) + tuple(percentile_interval(
+                _strict(ap["d3"])[:, j, 1]))) for t, ap in boot.items()))
+    return {str(t): _interval_lists(ap) for t, ap in boot.items()}, fields
+
+
+def paired_report(labels, evs, class_names, log=print):
+    """Print each set's moderate 3D AP against the first set's, paired over the bootstrap replicates: per set and class
+    and table the 95 % interval of the difference and the share of replicates in which the set is better.  Returns the
+    JSON list."""
+    out = []
+    log("paired against %s (moderate 3D AP, %d replicates):" % (labels[0], len(evs[0]["bootstrap"][11]["d3"])))
+    for k in range(1, len(evs)):
+        for t in evs[0]["bootstrap"]:
+            name = ("R11", "R40", "COCO")[TABLES.index(t)]
+            for j, c in enumerate(class_names):
+                sm = paired_summary(_strict(evs[k]["bootstrap"][t]["d3"])[:, j, 1],
+                                    _strict(evs[0]["bootstrap"][t]["d3"])[:, j, 1])
+                log("%-24s %s %s dAP 95%% [%+.2f, %+.2f]  better in %.1f%% of replicates" % (
+                    labels[k], c, name, sm["interval"][0], sm["interval"][1], 100 * sm["better"]))
+                out.append(dict(set=str(labels[k]), against=str(labels[0]), table=str(t), cls=c,
+                                interval=sm["interval"].tolist(), better=float(sm["better"])))
+    return out
+
+
+def add_bootstrap_args(p):
+    """The --bootstrap / --bootstrap-seed options of the evaluation commands."""
+    p.add_argument("--bootstrap", type=int, default=None, metavar="R",
+                   help="also print 95%% intervals of the AP over R bootstrap replicates of the split's frames (and, "
+                        "for several sets, each set's paired difference against the first)")
+    p.add_argument("--bootstrap-seed", type=int, default=None, metavar="S",
+                   help="the seed of the replicates' frame draws (default 0)")
+
+
+def check_bootstrap_args(p, args, unlabelled=None):
+    """Refuse --bootstrap below 1, --bootstrap without labels (``unlabelled``: the option that has none) and
+    --bootstrap-seed without --bootstrap."""
+    if args.bootstrap is not None:
+        if args.bootstrap < 1:
+            p.error("--bootstrap must be at least 1")
+        if unlabelled:
+            p.error("--bootstrap needs a labelled split: %s has no labels" % unlabelled)
+    elif args.bootstrap_seed is not None:
+        p.error("--bootstrap-seed goes with --bootstrap")
+    if args.bootstrap is not None and args.bootstrap_seed is None:
+        args.bootstrap_seed = 0
+
+
+def bootstrap_kw(args, nframes):
+    """eval_many's bootstrap argument of the command's options."""
+    if args.bootstrap is None:
+        return {}
+    return dict(bootstrap=bootstrap_indices(nframes, args.bootstrap, args.bootstrap_seed))
+
+
+def pop_bootstrap(args, nframes, labels, entries):
+    """The --json ``bootstrap`` entry, taken out of report_sets' entries: R, seed, F, per set its label and {table:
+    intervals}, and the paired summaries against the first set (None without --bootstrap)."""
+    if args.bootstrap is None:
+        return None
+    return dict(replicates=args.bootstrap, seed=args.bootstrap_seed, frames=nframes,
+                sets=[dict(label=str(l), intervals=e.pop("bootstrap")) for l, e in zip(labels, entries)],
+                paired=entries[0].pop("bootstrap_paired", []))
+
+
 def write_matches(path, labels, tables):
     """Write each set's match_table to an .npz: set k's arrays as ``set<k>_<name>``, ``labels`` [K] the sets' labels
     and the KITTI_DT_* state names ``states``."""
@@ -1027,25 +1296,32 @@ def report_sets(entries, labels, evs, class_names, noun, log=print, extra=None, 
         if "ranges" in ev or "matches" in ev:
             tp_err = tp_error_summary(ev["matches"], class_names, ranges=ranges) if "matches" in ev else None
             line += range_report(entry, ev, class_names, log, tp_err)
+        if "bootstrap" in ev:
+            entry["bootstrap"], fields = bootstrap_report(ev, class_names, log)
+            line += fields
         if extra is not None:
             line += extra(k, entry)
         summary.append("  ".join(line))
     log("summary: %d %s (moderate 3D AP)" % (len(labels), noun))
     for line in summary:
         log(line)
+    if len(evs) > 1 and "bootstrap" in evs[0]:
+        entries[0]["bootstrap_paired"] = paired_report(labels, evs, class_names, log)
     return entries
 
 
-def eval_dirs(label_dir, result_dirs, ids, classes, tables=(11,), times=None, ranges=None, match=False):
+def eval_dirs(label_dir, result_dirs, ids, classes, tables=(11,), times=None, ranges=None, match=False,
+              bootstrap=None):
     """Every table of ``tables`` for each directory of KITTI result files in ``result_dirs`` against the label files
     of ``label_dir``, over the frames ``ids``: the GT is read once, every directory is read and parsed on the device
-    (read_block), and one eval_many evaluates them all (``ranges``, ``match``: eval_many's).  Returns eval_many's list,
+    (read_block), and one eval_many evaluates them all (``ranges``, ``match``, ``bootstrap``: eval_many's).  Returns
+    eval_many's list,
     one dict per directory.  ``times``: a dict whose "read", "parse" and "eval" entries accumulate seconds."""
     times = {} if times is None else times
     gt = read_block(label_dir, ids, times=times)
     dts = [read_block(d, ids, times=times) for d in result_dirs]
     t0 = time.perf_counter()
-    out = eval_many(gt, dts, classes, tables, ranges=ranges, match=match)
+    out = eval_many(gt, dts, classes, tables, ranges=ranges, match=match, bootstrap=bootstrap)
     times["eval"] = times.get("eval", 0.0) + time.perf_counter() - t0
     return out
 
@@ -1063,8 +1339,10 @@ def parse_args(argv=None):
                    help="also print the COCO-style AP table (AP averaged over ten IoU thresholds per class)")
     p.add_argument("--json", default=None, help="write the AP arrays and times here")
     add_range_args(p)
+    add_bootstrap_args(p)
     args = p.parse_args(argv)
     check_range_args(p, args)
+    check_bootstrap_args(p, args)
     unknown = [c for c in args.classes if c not in CLASS_TO_NAME.values()]
     if unknown:
         p.error("--classes: unknown class %s (known: %s)" % (", ".join(unknown), ", ".join(CLASS_TO_NAME.values())))
@@ -1102,14 +1380,17 @@ def main(argv=None, log=print):
     python -m sassd_b200.kitti_eval --data-root DIR [--split val] --results DIR [DIR ...]
                                     [--classes Car Pedestrian Cyclist] [--r40] [--coco] [--json FILE]
                                     [--ranges EDGE EDGE [...]] [--matches FILE.npz]
+                                    [--bootstrap R [--bootstrap-seed S]]
 
     The labels are ``training/label_2/%06d.txt`` and the frames those of ``ImageSets/<split>.txt``; files a result
     directory holds beyond them are ignored.  Every file is read into pinned memory, copied to the device once and
     parsed there (read_block), and all directories are evaluated in one pass (eval_many) on the device.  Prints each
     directory's tables under ``== DIR ==``, one summary line per directory and the seconds spent reading, parsing and
     evaluating.  ``--ranges`` adds each directory's tables per range bin and, with ``--matches``, the true positives'
-    TP errors to its summary line; ``--matches`` writes every directory's match table.  Returns the result dict that
-    ``--json`` writes."""
+    TP errors to its summary line; ``--matches`` writes every directory's match table.  ``--bootstrap R`` adds each
+    directory's 95 % AP intervals over R bootstrap replicates of the frames (bootstrap_indices, seed
+    ``--bootstrap-seed``) and, for two or more directories, each one's paired difference against the first.  Returns
+    the result dict that ``--json`` writes."""
     from .kitti_data import read_split
     args = parse_args(argv)
     ids = read_split(args.data_root, args.split)
@@ -1117,14 +1398,17 @@ def main(argv=None, log=print):
     times = {}
     match = args.ranges is not None or args.matches is not None
     evs = eval_dirs(os.path.join(args.data_root, "training", "label_2"), args.results, ids, args.classes, tables, times,
-                    args.ranges, match)
+                    args.ranges, match, **bootstrap_kw(args, len(ids)))
     entries = report_sets([dict(dir=d) for d in args.results], args.results, evs, args.classes, "directories", log,
                           ranges=args.ranges)
+    boot = pop_bootstrap(args, len(ids), args.results, entries)
     if args.matches:
         write_matches(args.matches, args.results, [ev["matches"] for ev in evs])
     log("frames: %d, directories: %d, read %.3f s, parse %.3f s, evaluate %.3f s" % (
         len(ids), len(args.results), times["read"], times["parse"], times["eval"]))
     result = dict(split=args.split, frames=len(ids), classes=args.classes, results=entries, times_s=times)
+    if boot is not None:
+        result["bootstrap"] = boot
     if args.json:
         with open(args.json, "w") as fh:
             json.dump(result, fh, indent=1)

@@ -53,7 +53,7 @@ def next_pow2(n):
 # kernels launched by each C-ABI entry point (memsets not counted)
 _KERNELS = {"sassd_voxelize": 4, "sassd_voxel_mean": 1, "sassd_frustum_crop": 1, "sassd_image_fov_crop": 1, "sassd_points_in_rbboxes": 1, "sassd_augment_drop_points": 1, "sassd_augment_noise_search": 1, "sassd_augment_assemble": 1, "sassd_anchor_mask": 4, "sassd_hash_build": 1,
             "sassd_rulebook_subm": 1, "sassd_rulebook_conv_outputs": 2, "sassd_rulebook_conv_outputs_hash": 2, "sassd_rulebook_conv_nbr": 1,
-            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_kitti_eval_flags": 1, "sassd_kitti_eval_flags_ranged": 1, "sassd_kitti_eval_assign": 1, "sassd_kitti_eval_overlaps": 1, "sassd_kitti_eval_match": 3, "sassd_kitti_scan_labels": 1, "sassd_kitti_parse_labels": 2, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_conv2d_f16x3_occ_bg_status": 1, "sassd_gconv_status": 1, "sassd_spconv_f16x3_status": 1, "sassd_features_to_split_status": 1, "sassd_sparse_to_bev_split_status": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
+            "sassd_rulebook_pairs": 1, "sassd_gconv": 1, "sassd_gconv_pack": 1, "sassd_spconv_pack": 1, "sassd_rotate_overlap_eval": 1, "sassd_kitti_eval_flags": 1, "sassd_kitti_eval_flags_ranged": 1, "sassd_kitti_eval_assign": 1, "sassd_kitti_eval_overlaps": 1, "sassd_kitti_eval_match": 3, "sassd_kitti_boot_prepare": 3, "sassd_kitti_boot_eval": 2, "sassd_kitti_scan_labels": 1, "sassd_kitti_parse_labels": 2, "sassd_conv2d_pack": 1, "sassd_conv2d_f16x3": 1, "sassd_conv2d_f16x3_occ": 1, "sassd_conv2d_f16x3_occ_bg": 1, "sassd_conv2d_f16x3_occ_bg_status": 1, "sassd_gconv_status": 1, "sassd_spconv_f16x3_status": 1, "sassd_features_to_split_status": 1, "sassd_sparse_to_bev_split_status": 1, "sassd_spconv_f16x3": 1, "sassd_features_to_split": 1, "sassd_split_rows_to_bev": 1, "sassd_sparse_to_bev_split": 1, "sassd_sparse_to_bev": 1, "sassd_decode_select": 2,
             "sassd_pswarp": 1, "sassd_rescore_nms": 3, "sassd_kitti_format": 1, "sassd_merge_detections": 1, "sassd_three_nn": 1, "sassd_point_aux_head": 1, "sassd_nms_mask": 1, "sassd_nms_sorted": 2,
             "sassd_boxes_iou_bev": 1, "sassd_points_in_boxes": 2, "sassd_assign_rpn": 3, "sassd_assign_pswarp": 3,
             "sassd_rpn_loss": 2, "sassd_pswarp_loss": 2, "sassd_aux_loss": 2}
@@ -593,6 +593,42 @@ def kitti_eval_assign(desc, row, ndiff, gt_cam, dt_cam, ws=None):
     _call("sassd_kitti_eval_assign", None, ctypes.byref(desc), int(row), int(ndiff), _ptr(gt_cam), _ptr(dt_cam),
           _ptr(gt_det), _ptr(gt_ov), _ptr(dt_state), _ptr(tp_err), _ptr(w), w.numel(), _stream())
     return gt_det, gt_ov, dt_state, tp_err
+
+
+def kitti_boot_prepare(desc, njobs, score_total, tab_off, ws=None):
+    """The bootstrap's per-job sorted true-positive scores with their frames and every (job, frame)'s step table
+    (csrc/kitti_match.cu; ``desc`` as kitti_eval_match's, tab_off [njobs+1] i64 device).  Returns (scores, frames,
+    n_scores, tab_score, tab_cnt, tab_sim, tab_n)."""
+    dev = tab_off.device
+    n = max(int(score_total), 1)
+    total = max(int(tab_off[-1]), 1)
+    scores = torch.empty((n,), dtype=torch.float64, device=dev)
+    frames = torch.empty((n,), dtype=torch.int32, device=dev)
+    n_scores = torch.empty((njobs,), dtype=torch.int32, device=dev)
+    tab_score = torch.empty((total,), dtype=torch.float64, device=dev)
+    tab_cnt = torch.empty((total, 3), dtype=torch.int32, device=dev)
+    tab_sim = torch.empty((total,), dtype=torch.float64, device=dev)
+    tab_n = torch.empty((njobs * desc.nframes,), dtype=torch.int32, device=dev)
+    w = (ws or _WS).get("kitti_eval", _L().sassd_kitti_eval_workspace_bytes(desc.max_nd, desc.max_ng), dev)
+    _call("sassd_kitti_boot_prepare", None, ctypes.byref(desc), _ptr(scores), _ptr(frames), _ptr(n_scores),
+          _ptr(tab_off), _ptr(tab_score), _ptr(tab_cnt), _ptr(tab_sim), _ptr(tab_n), _ptr(w), w.numel(), _stream())
+    return scores, frames, n_scores, tab_score, tab_cnt, tab_sim, tab_n
+
+
+def kitti_boot_eval(desc, njobs, lists, weight, num_gt, prep, tab_off):
+    """Thresholds and per-threshold sums of a chunk of bootstrap replicates (lists / weight [R, F] i32, num_gt
+    [R, nclass * ndiff] f64, ``prep`` kitti_boot_prepare's tuple).  Returns (n_thresh [R, njobs] i32,
+    pr [R, njobs, 41, 4] f64)."""
+    R = lists.shape[0]
+    dev = lists.device
+    scores, frames, n_scores, tab_score, tab_cnt, tab_sim, tab_n = prep
+    thresholds = torch.empty((R, njobs, 41), dtype=torch.float64, device=dev)
+    n_thresh = torch.empty((R, njobs), dtype=torch.int32, device=dev)
+    pr = torch.empty((R, njobs, 41, 4), dtype=torch.float64, device=dev)
+    _call("sassd_kitti_boot_eval", None, ctypes.byref(desc), R, _ptr(lists), _ptr(weight), _ptr(num_gt), _ptr(scores),
+          _ptr(frames), _ptr(n_scores), _ptr(tab_off), _ptr(tab_score), _ptr(tab_cnt), _ptr(tab_sim), _ptr(tab_n),
+          _ptr(thresholds), _ptr(n_thresh), _ptr(pr), _stream())
+    return n_thresh, pr
 
 
 def kitti_scan_labels(buf, file_off):

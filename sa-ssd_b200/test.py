@@ -3,6 +3,7 @@
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR [--split val] [--batch 16]
                               [--lidar velodyne|velodyne_reduced] [--out DIR] [--workers N] [--json FILE]
                               [--losses] [--r40] [--coco] [--ranges EDGE EDGE [...]] [--matches FILE.npz]
+                              [--bootstrap R [--bootstrap-seed S]]
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR --split test --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --drive DRIVE_DIR [--calib-dir DIR] --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --model CONFIG2 CHECKPOINT2 [--model ...] --data-root DIR [...]
@@ -20,6 +21,9 @@ kitti_eval.read_block parses them on the device.  ``--ranges 0 20 40 inf`` adds 
 distance from the camera after the whole-range ones (kitti_eval.eval_many(ranges=...)) and the true positives' mean
 ATE / ASE / AOE per class (kitti_eval.tp_error_summary); ``--matches FILE.npz`` writes every set's per-object match
 table (kitti_eval.match_table).  Both come from the same one evaluation, for every checkpoint and bin.
+``--bootstrap R [--bootstrap-seed S]`` adds 95 % intervals of the AP over R bootstrap replicates of the split's frames
+(kitti_eval.eval_many(bootstrap=...)) after the tables and, for a sweep, each checkpoint's paired difference against
+the first.
 
 ``--losses`` (labelled splits): every frame also carries its ground truth (kitti_data.gt_from_anno) and the captured
 step computes SA-SSD's six losses beside the detections (detect_stream(losses=True)); the result files and AP tables
@@ -95,10 +99,12 @@ def parse_args(argv=None):
                    help="one more single-class model, run with the first as one set (repeatable)")
     p.add_argument("--checkpoints", nargs="+", default=[], metavar="CHECKPOINT",
                    help="more checkpoints of CONFIG, validated with CHECKPOINT in one pass over a labelled split")
-    from .kitti_eval import add_range_args, check_range_args
+    from .kitti_eval import add_bootstrap_args, add_range_args, check_bootstrap_args, check_range_args
     add_range_args(p)
+    add_bootstrap_args(p)
     args = p.parse_args(argv)
     check_range_args(p, args)
+    check_bootstrap_args(p, args, "--drive" if args.drive else "--split test" if args.split == "test" else None)
     if args.batch < 1:
         p.error("--batch must be positive")
     if args.checkpoints:
@@ -308,15 +314,20 @@ def run(args, log=print):
         _write_json(args.json, result)
         D.barrier()
         return result
-    from .kitti_eval import ap_lists, eval_many, range_report, read_block, tp_error_summary, write_matches
+    from .kitti_eval import (ap_lists, bootstrap_kw, bootstrap_report, eval_many, pop_bootstrap, range_report,
+                             read_block, tp_error_summary, write_matches)
     gt = read_block(os.path.join(split.dir, "label_2"), split.ids)
     if sweep:
         result["checkpoints"] = _report_sweep(args, gt, dt_sets, class_names, per_batch, log)
+        boot = pop_bootstrap(args, len(split.ids), [os.path.basename(p) for p in [args.checkpoint] + args.checkpoints],
+                             result["checkpoints"])
+        if boot is not None:
+            result["bootstrap"] = boot
         log(rate)
         _write_json(args.json, result)
         D.barrier()
         return result
-    ev = eval_many(gt, [dt_annos], class_names, _tables(args), **_range_kw(args))[0]
+    ev = eval_many(gt, [dt_annos], class_names, _tables(args), **_range_kw(args), **bootstrap_kw(args, len(split.ids)))[0]
     text, ap = ev[11]
     log(text, end="")
     result.update(text=text, ap=ap_lists(ap))
@@ -326,10 +337,18 @@ def run(args, log=print):
     if args.coco:
         log(ev["coco"][0], end="")
         result.update(text_coco=ev["coco"][0], ap_coco=ap_lists(ev["coco"][1]))
+    fields = []
     if "matches" in ev:
         fields = range_report(result, ev, class_names, log,
                               tp_error_summary(ev["matches"], class_names, ranges=args.ranges))
+    if "bootstrap" in ev:
+        intervals, more = bootstrap_report(ev, class_names, log)
+        fields += more
+        result["bootstrap"] = dict(replicates=args.bootstrap, seed=args.bootstrap_seed, frames=len(split.ids),
+                                   sets=[dict(label=os.path.basename(args.checkpoint), intervals=intervals)], paired=[])
+    if fields:
         log("summary: " + "  ".join(fields))
+    if "matches" in ev:
         if args.matches:
             write_matches(args.matches, [os.path.basename(args.checkpoint)], [ev["matches"]])
     if args.losses:
@@ -378,7 +397,8 @@ def _report_sweep(args, gt, dt_sets, class_names, per_batch, log):
         entry.update(_loss_means([v[k * n:(k + 1) * n] for v in per_batch], args.batch, log))
         return ["rpn_cls_loss %.6f loss_cls %.6f" % (entry["losses"]["rpn_cls_loss"], entry["losses"]["loss_cls"])]
     from .kitti_eval import write_matches
-    evs = eval_many(gt, dt_sets, class_names, _tables(args), **_range_kw(args))
+    from .kitti_eval import bootstrap_kw
+    evs = eval_many(gt, dt_sets, class_names, _tables(args), **_range_kw(args), **bootstrap_kw(args, len(gt)))
     if args.matches:
         write_matches(args.matches, [os.path.basename(p) for p in paths], [ev["matches"] for ev in evs])
     return report_sets([dict(path=p) for p in paths], [os.path.basename(p) for p in paths], evs, class_names,
