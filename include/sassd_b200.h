@@ -690,8 +690,9 @@ size_t sassd_kitti_eval_workspace_bytes(int max_nd, int max_ng);
 int sassd_kitti_eval_match(const SassdKittiEvalDesc* desc, double* scores, int32_t* n_scores, double* thresholds,
                            int32_t* n_thresh, double* pr, void* ws, size_t ws_bytes, sassd_stream_t stream);
 
-/* Bootstrap replicates of the same evaluation (csrc/kitti_match.cu): a replicate is a list of nframes frames drawn
- * with replacement, and its sums are what sassd_kitti_eval_match gives on the GT and detections of that list.
+/* Bootstrap replicates of the same evaluation (csrc/kitti_match.cu): a replicate is a non-empty list of the nframes
+ * frames, drawn with replacement and of any length (frame-level: nframes draws; drive-level: the frames of the drawn
+ * drives), and its sums are what sassd_kitti_eval_match gives on the GT and detections of that list.
  *
  * sassd_kitti_boot_prepare, once per desc (compute_aos: [nsets] whether any replicate sums the similarity): each job's
  * true-positive scores sorted descending into scores[score_off[job] ..] with their frames in frames[same],
@@ -701,18 +702,19 @@ int sassd_kitti_eval_match(const SassdKittiEvalDesc* desc, double* scores, int32
  * its distinct non-NaN scores of unskipped detections, descending (tab_score; tab_cnt three int32 per entry; tab_sim).
  * ws as sassd_kitti_eval_match's.
  *
- * sassd_kitti_boot_eval, per chunk of nrep replicates: list[r * nframes + p] the p-th frame of replicate r,
- * weight[r * nframes + f] how often frame f occurs in it, num_gt[r * nclass * ndiff + cd] its valid GT count; out
+ * sassd_kitti_boot_eval, per chunk of nrep replicates: list[list_off[r] + p] the p-th frame of replicate r (list_off
+ * [nrep + 1] int64, non-decreasing from 0), weight[r * nframes + f] how often frame f occurs in it,
+ * num_gt[r * nclass * ndiff + cd] its valid GT count; out
  * thresholds[(r * jobs + job) * 41 + t], n_thresh[r * jobs + job] and pr[((r * jobs + job) * 41 + t) * 4 + ...] as
  * sassd_kitti_eval_match lays them out (rows past n_thresh zero), the similarity summed in list order. */
 int sassd_kitti_boot_prepare(const SassdKittiEvalDesc* desc, double* scores, int32_t* frames, int32_t* n_scores,
                              const int64_t* tab_off, double* tab_score, int32_t* tab_cnt, double* tab_sim,
                              int32_t* tab_n, void* ws, size_t ws_bytes, sassd_stream_t stream);
-int sassd_kitti_boot_eval(const SassdKittiEvalDesc* desc, int nrep, const int32_t* list, const int32_t* weight,
-                          const double* num_gt, const double* scores, const int32_t* frames, const int32_t* n_scores,
-                          const int64_t* tab_off, const double* tab_score, const int32_t* tab_cnt,
-                          const double* tab_sim, const int32_t* tab_n, double* thresholds, int32_t* n_thresh,
-                          double* pr, sassd_stream_t stream);
+int sassd_kitti_boot_eval(const SassdKittiEvalDesc* desc, int nrep, const int32_t* list, const int64_t* list_off,
+                          const int32_t* weight, const double* num_gt, const double* scores, const int32_t* frames,
+                          const int32_t* n_scores, const int64_t* tab_off, const double* tab_score,
+                          const int32_t* tab_cnt, const double* tab_sim, const int32_t* tab_n, double* thresholds,
+                          int32_t* n_thresh, double* pr, sassd_stream_t stream);
 
 /* Match-table states of a detection row (compute_statistics_jit's fate of the detection). */
 #define SASSD_KITTI_DT_NOT_COUNTED 0   /* flag -1 (other class) or 1 (ignored) and not assigned */

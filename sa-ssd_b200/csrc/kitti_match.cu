@@ -639,12 +639,14 @@ __global__ void boot_thresholds_kernel(SassdKittiEvalDesc e, long long njobs, in
     n_thresh[(long long)r * njobs + job] = nt;
 }
 
-// Pass 2 of replicate r: one warp per (job, replicate), lane l at thresholds l and l + 32.  Each frame of the list, in
-// list order, adds the table entry of its smallest own score >= the threshold; the counts are integers (any order),
-// the similarity is added in list order as fused_compute_statistics adds it over the frames.
+// Pass 2 of replicate r: one warp per (job, replicate), lane l at thresholds l and l + 32.  Each frame of the list
+// list[list_off[r] .. list_off[r + 1]), in list order, adds the table entry of its smallest own score >= the
+// threshold; the counts are integers (any order), the similarity is added in list order as fused_compute_statistics
+// adds it over the frames.  A list may have any length (a drive-level replicate is longer or shorter than nframes).
 constexpr int kBootWarps = 4;
 __global__ void __launch_bounds__(32 * kBootWarps) boot_pr_kernel(SassdKittiEvalDesc e, long long njobs, int nrep,
                                                                   const int32_t* __restrict__ list,
+                                                                  const int64_t* __restrict__ list_off,
                                                                   const double* __restrict__ thresholds,
                                                                   const int32_t* __restrict__ n_thresh,
                                                                   const int64_t* __restrict__ tab_off,
@@ -673,9 +675,9 @@ __global__ void __launch_bounds__(32 * kBootWarps) boot_pr_kernel(SassdKittiEval
         tp[u] = fp[u] = fn[u] = 0;
     }
     if (lane < nt) {
-        const int32_t* lr = list + (long long)r * e.nframes;
-        for (int p = 0; p < e.nframes; ++p) {
-            const int f = lr[p];
+        const long long p1 = list_off[r + 1];
+        for (long long p = list_off[r]; p < p1; ++p) {
+            const int f = list[p];
             const long long base = step_base(e, jb, job, tab_off, f);
             const int m = tab_n[job * e.nframes + f];
 #pragma unroll
@@ -859,13 +861,13 @@ extern "C" int sassd_kitti_boot_prepare(const SassdKittiEvalDesc* e, double* sco
 }
 
 extern "C" int sassd_kitti_boot_eval(const SassdKittiEvalDesc* e, int nrep, const int32_t* list,
-                                     const int32_t* weight, const double* num_gt, const double* scores,
-                                     const int32_t* frames, const int32_t* n_scores, const int64_t* tab_off,
-                                     const double* tab_score, const int32_t* tab_cnt, const double* tab_sim,
-                                     const int32_t* tab_n, double* thresholds, int32_t* n_thresh, double* pr,
-                                     sassd_stream_t stream_) {
-    if (!boot_desc_ok(e) || nrep < 1 || !list || !weight || !num_gt || !scores || !frames || !n_scores || !tab_off ||
-        !tab_score || !tab_cnt || !tab_sim || !tab_n || !thresholds || !n_thresh || !pr)
+                                     const int64_t* list_off, const int32_t* weight, const double* num_gt,
+                                     const double* scores, const int32_t* frames, const int32_t* n_scores,
+                                     const int64_t* tab_off, const double* tab_score, const int32_t* tab_cnt,
+                                     const double* tab_sim, const int32_t* tab_n, double* thresholds,
+                                     int32_t* n_thresh, double* pr, sassd_stream_t stream_) {
+    if (!boot_desc_ok(e) || nrep < 1 || !list || !list_off || !weight || !num_gt || !scores || !frames || !n_scores ||
+        !tab_off || !tab_score || !tab_cnt || !tab_sim || !tab_n || !thresholds || !n_thresh || !pr)
         return SASSD_ERR_ARG;
     const long long njobs = (long long)e->nsets * e->nclass * e->ndiff * 3 * e->nover;
     const long long items = njobs * nrep;
@@ -874,6 +876,6 @@ extern "C" int sassd_kitti_boot_eval(const SassdKittiEvalDesc* e, int nrep, cons
     boot_thresholds_kernel<<<(unsigned)sassd_div_up(items, 128), 128, 0, stream>>>(
         *e, njobs, nrep, weight, num_gt, scores, frames, n_scores, thresholds, n_thresh);
     boot_pr_kernel<<<(unsigned)sassd_div_up(items, kBootWarps), 32 * kBootWarps, 0, stream>>>(
-        *e, njobs, nrep, list, thresholds, n_thresh, tab_off, tab_score, tab_cnt, tab_sim, tab_n, pr);
+        *e, njobs, nrep, list, list_off, thresholds, n_thresh, tab_off, tab_score, tab_cnt, tab_sim, tab_n, pr);
     return sassd_check_launch();
 }

@@ -14,6 +14,9 @@ Raw drives (KittiDrive; the reference's KittiVideo, mmdet/datasets/kitti.py:356-
 ``image_02/data/%010d.png`` and ``velodyne_points/data/%010d.bin`` per frame, and one calibration for the drive from
 ``calib_cam_to_cam.txt`` and ``calib_velo_to_cam.txt`` in the recording day's directory (results.Calibration.from_video).
 No labels.
+
+The object devkit's ``mapping/`` directory (``train_mapping.txt``, ``train_rand.txt``) names each training frame's
+raw drive (read_drive_mapping, split_drives), for drive-level bootstrap intervals and per-drive AP.
 """
 import os
 import struct
@@ -32,6 +35,56 @@ def read_split(root, split):
     """Frame ids of ``ImageSets/<split>.txt`` (one integer per line), in file order."""
     with open(os.path.join(root, "ImageSets", split + ".txt")) as fh:
         return [int(line) for line in fh.read().split()]
+
+
+def read_drive_mapping(mapping_dir):
+    """The raw drive of every object training frame, from the object devkit's ``mapping/`` directory: a list whose
+    i-th entry is training frame i's drive (e.g. ``2011_09_26_drive_0005_sync``).  Each line of ``train_mapping.txt``
+    is ``date drive frame``; ``train_rand.txt`` is one comma-separated line whose i-th entry is the 1-based line of
+    train_mapping.txt for training frame i.  A line without three fields, or train_rand entries that are not a
+    permutation of 1..N (N the mapping's lines), is a ValueError naming the file and the line or entry."""
+    path = os.path.join(mapping_dir, "train_mapping.txt")
+    with open(path) as fh:
+        lines = fh.read().splitlines()
+    while lines and not lines[-1].strip():
+        lines.pop()
+    drives = []
+    for n, line in enumerate(lines, 1):
+        fields = line.split()
+        if len(fields) != 3:
+            raise ValueError("%s line %d: expected 'date drive frame', got %r" % (path, n, line))
+        drives.append(fields[1])
+    rand_path = os.path.join(mapping_dir, "train_rand.txt")
+    with open(rand_path) as fh:
+        entries = [e.strip() for e in fh.read().strip().split(",")]
+    order = []
+    for i, e in enumerate(entries):
+        try:
+            order.append(int(e))
+        except ValueError:
+            raise ValueError("%s entry %d: %r is not an integer" % (rand_path, i, e)) from None
+    seen = np.zeros(len(drives) + 1, bool)
+    for i, line in enumerate(order):
+        if not 1 <= line <= len(drives):
+            raise ValueError("%s entry %d: line %d is outside 1..%d, the lines of %s" % (rand_path, i, line,
+                                                                                    len(drives), path))
+        if seen[line]:
+            raise ValueError("%s entry %d: line %d appears twice" % (rand_path, i, line))
+        seen[line] = True
+    if len(order) != len(drives):
+        raise ValueError("%s has %d entries, not a permutation of the %d lines of %s" % (rand_path, len(order),
+                                                                                       len(drives), path))
+    return [drives[line - 1] for line in order]
+
+
+def split_drives(drives, ids):
+    """Each frame id of a split (``ids``) -> its raw drive (``drives``: read_drive_mapping's list), as a numpy string
+    array; an id past the mapping's end is a ValueError naming the frame."""
+    for i in ids:
+        if not 0 <= int(i) < len(drives):
+            raise ValueError("frame %06d is not in the drive mapping (it covers training frames 0..%d)" % (
+                i, len(drives) - 1))
+    return np.array([drives[int(i)] for i in ids], dtype=str)
 
 
 def png_shape(path):

@@ -24,11 +24,14 @@ the device (`read_block`, csrc/kitti_parse.cu).
 difficulty entries of the same evaluation), and ``match_table`` / ``eval_many(..., match=True)`` the evaluator's own
 per-object assignment with the 3-D true positives' ATE / ASE / AOE (``tp_errors``).  ``eval_many(...,
 bootstrap=idx)`` adds every table over bootstrap replicates of the frames (``bootstrap_indices``), each replicate bit for
-bit the evaluation of its resampled lists, with ``percentile_interval`` / ``paired_summary`` to summarise them.
+bit the evaluation of its resampled lists, with ``percentile_interval`` / ``paired_summary`` to summarise them.  The
+replicates may also be a ``ReplicateLists`` of lists of any length: ``bootstrap_groups`` draws whole raw drives
+(a drive-level bootstrap, from the devkit's frame mapping), and ``per_drive_report`` evaluates each drive's own frames.
 
     python -m sassd_b200.kitti_eval --data-root DIR [--split val] --results DIR [DIR ...] [--classes Car ...]
                                     [--r40] [--coco] [--json FILE] [--ranges EDGE ...] [--matches FILE.npz]
-                                    [--bootstrap R [--bootstrap-seed S]]
+                                    [--bootstrap R [--bootstrap-seed S] [--bootstrap-by frame|drive]]
+                                    [--mapping DIR [--per-drive]]
 
 evaluates directories of result files against a split's labels (`main`, `eval_dirs`).
 """
@@ -758,11 +761,12 @@ def eval_many(gt_annos, dt_sets, classes, tables=(11,), overlap_fn=None, difficu
     ignored there (clean_gt / clean_dt).  ``match``: each set's dict also holds ``"matches"``, its match_table.
 
     ``bootstrap``: an int array [R, F] of frame indices (bootstrap_indices), replicate r the list of frames idx[r, 0],
-    idx[r, 1], ... (duplicates included).  Each set's dict then also holds ``"bootstrap"``: {table: ap} with a leading
-    R axis on every array, replicate r's AP bit for bit what this evaluation gives on the resampled GT and detection
-    lists (compute_aos decided per replicate; ``aos`` is NaN in a replicate without it, None when no replicate has
-    it); with ``ranges`` also ``"bootstrap_ranges"``, laid out like ``"ranges"``.  Every set uses the same lists, so
-    the replicates are paired (paired_summary)."""
+    idx[r, 1], ... (duplicates included), or a ReplicateLists of lists of any length (bootstrap_groups: drive-level
+    replicates; or each drive's own frames, for per-drive AP).  Each set's dict then also holds ``"bootstrap"``:
+    {table: ap} with a leading R axis on every array, replicate r's AP bit for bit what this evaluation gives on the
+    resampled GT and detection lists (compute_aos decided per replicate; ``aos`` is NaN in a replicate without it, None
+    when no replicate has it); with ``ranges`` also ``"bootstrap_ranges"``, laid out like ``"ranges"``.  Every set uses
+    the same lists, so the replicates are paired (paired_summary)."""
     tables = tuple(tables)
     if not tables or any(t not in TABLES for t in tables):
         raise ValueError("tables must be among %r, not %r" % (TABLES, tables))
@@ -841,7 +845,7 @@ def _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, range
     ``ranges``, with ``match`` the match table, and with ``bootstrap`` the replicates' AP."""
     classes = _class_ids(classes)
     edges = None if ranges is None else check_ranges(ranges)
-    idx = None if bootstrap is None else check_bootstrap(bootstrap, len(gt_annos))
+    lists = None if bootstrap is None else check_bootstrap(bootstrap, len(gt_annos))
     diffs = list(difficultys)
     bins = [None] + ([] if edges is None else range_bins(edges))
     entries = [(d, b) for b in bins for d in diffs]     # difficulty entries: the whole range, then bin by bin
@@ -861,14 +865,14 @@ def _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, range
     boot = None
     if overlap_fn is None:
         boot_aos = None
-        if idx is not None:
+        if lists is not None:
             dt_sets = [_as_block(d) for d in dt_sets]
-            boot_aos = _bootstrap_aos_flags(dt_sets, idx)
+            boot_aos = _bootstrap_aos_flags(dt_sets, lists)
         st = _device_setup(gt_annos, dt_sets, classes, ent_diffs, min_overlaps, aos_flags, ent_bins, match,
                            boot_aos is not None and bool(boot_aos.any()))
         prec, matches = _device_arrays(st, (table_row, Dn) if match else None, bool(tables))
-        if idx is not None:
-            boot = _bootstrap_device(st, idx, boot_aos, tables, Dn, len(bins), n_off)
+        if lists is not None:
+            boot = _bootstrap_device(st, lists, boot_aos, tables, Dn, len(bins), n_off)
     else:
         gt_annos, dt_sets = _as_annos(gt_annos), [_as_annos(d) for d in dt_sets]
         gt_sides = {(c, d, b): _GtSide(gt_annos, c, d, b) for c in classes for d, b in entries}
@@ -877,8 +881,8 @@ def _evaluate(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, range
                 for metric in (0, 1, 2)] if tables else None
         matches = (_table_host(gt_annos, dt_sets, classes, diffs, min_overlaps[table_row], overlap_fn, gt_sides)
                    if match else None)
-        if idx is not None:
-            boot = _bootstrap_host(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, edges, idx)
+        if lists is not None:
+            boot = _bootstrap_host(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, edges, lists)
     out = []
     for s, compute_aos in enumerate(aos_flags):
         res = {}
@@ -910,8 +914,78 @@ def bootstrap_indices(nframes, replicates, seed=0):
     return np.stack([rs.randint(0, nframes, nframes) for _ in range(int(replicates))]).astype(np.int64)
 
 
+class ReplicateLists:
+    """R >= 1 bootstrap replicates, each a non-empty list of frame indices of any length (a drive-level replicate is
+    the frames of its drawn drives): ``flat`` int64 the lists concatenated, ``off`` int64 [R + 1] replicate r's slice
+    flat[off[r]:off[r + 1]].  Built from a sequence of 1-D integer arrays; an empty list, a non-integer index or no list
+    at all is a ValueError.  eval_many refuses an index outside the split's frames."""
+
+    def __init__(self, lists):
+        rows = [np.asarray(l) for l in lists]
+        if not rows:
+            raise ValueError("bootstrap replicate lists: need at least one replicate")
+        for r, row in enumerate(rows):
+            if row.ndim != 1 or not len(row):
+                raise ValueError("bootstrap replicate %d must be a non-empty 1-D list of frame indices, not shape %r"
+                                 % (r, row.shape))
+            if row.dtype.kind not in "iu":
+                raise ValueError("bootstrap replicate %d: frame indices must be integers, not %s" % (r, row.dtype))
+        self.flat = np.concatenate(rows).astype(np.int64)
+        self.off = _offsets([len(row) for row in rows], np.int64)
+
+    @classmethod
+    def _from(cls, flat, off):
+        out = cls.__new__(cls)
+        out.flat, out.off = flat, off
+        return out
+
+    @classmethod
+    def _of_array(cls, idx):
+        """The rows of an [R, F] index array: replicate r at offset r * F."""
+        return cls._from(np.ascontiguousarray(idx, np.int64).reshape(-1),
+                         np.arange(idx.shape[0] + 1, dtype=np.int64) * idx.shape[1])
+
+    def __len__(self):
+        return len(self.off) - 1
+
+    def __getitem__(self, r):
+        return self.flat[self.off[r]:self.off[r + 1]]
+
+    def __iter__(self):
+        return (self[r] for r in range(len(self)))
+
+    @property
+    def lengths(self):
+        return np.diff(self.off)
+
+    def rows(self, r0, r1):
+        """Replicates [r0, r1) as a ReplicateLists."""
+        return ReplicateLists._from(self.flat[self.off[r0]:self.off[r1]], self.off[r0:r1 + 1] - self.off[r0])
+
+
+def bootstrap_groups(groups, replicates, seed=0):
+    """Drive-level (cluster) bootstrap replicates as ReplicateLists: ``groups`` holds one label per split frame (its
+    raw drive).  The G distinct labels are sorted; replicate r draws G of them with the r-th
+    np.random.RandomState(seed).randint(0, G, G) and lists each drawn group's frame positions in ascending order, group
+    after group.  A row does not depend on how many rows follow it; with groups = np.arange(F) the rows are
+    bootstrap_indices(F, replicates, seed)'s."""
+    labels, inv = np.unique(np.asarray(groups), return_inverse=True)
+    inv = inv.reshape(-1)
+    G = len(labels)
+    if G < 1:
+        raise ValueError("bootstrap groups: need a label per frame, not an empty list")
+    members = [np.flatnonzero(inv == g) for g in range(G)]
+    rs = np.random.RandomState(seed)
+    return ReplicateLists([np.concatenate([members[g] for g in rs.randint(0, G, G)]) for _ in range(int(replicates))])
+
+
 def check_bootstrap(idx, nframes):
-    """The bootstrap indices as an int64 [R, nframes] array, R >= 1, every index in [0, nframes); else ValueError."""
+    """The bootstrap replicates as ReplicateLists.  An array must be an int [R >= 1, nframes] array; a ReplicateLists
+    may hold lists of any length; every index must lie in [0, nframes).  Anything else is a ValueError."""
+    if isinstance(idx, ReplicateLists):
+        if nframes < 1 or idx.flat.min() < 0 or idx.flat.max() >= nframes:
+            raise ValueError("bootstrap indices must lie in [0, %d)" % nframes)
+        return idx
     a = np.asarray(idx)
     if a.dtype.kind not in "iu":
         raise ValueError("bootstrap indices must be integers, not %s" % a.dtype)
@@ -919,7 +993,7 @@ def check_bootstrap(idx, nframes):
         raise ValueError("bootstrap indices must be [R >= 1, %d frames], not %r" % (nframes, a.shape))
     if a.min() < 0 or a.max() >= nframes:
         raise ValueError("bootstrap indices must lie in [0, %d)" % nframes)
-    return a.astype(np.int64)
+    return ReplicateLists._of_array(a)
 
 
 def percentile_interval(samples, lo=2.5, hi=97.5):
@@ -934,17 +1008,20 @@ def paired_summary(ap, ap0, lo=2.5, hi=97.5):
     return dict(interval=percentile_interval(d, lo, hi), better=np.mean(d > 0, axis=0))
 
 
-def _bootstrap_aos_flags(dt_blocks, idx):
-    """[R, K] compute_aos of every replicate and set, as _aos_flag decides it on the replicate's list: from its first
-    frame with detections."""
-    out = np.zeros((idx.shape[0], len(dt_blocks)), bool)
+def _bootstrap_aos_flags(dt_blocks, lists):
+    """[R, K] compute_aos of every replicate (ReplicateLists) and set, as _aos_flag decides it on the replicate's list:
+    from its first frame with detections."""
+    out = np.zeros((len(lists), len(dt_blocks)), bool)
     for k, d in enumerate(dt_blocks):
         has = d.counts > 0
         ok = np.zeros(len(d), bool)
         if has.any():
             ok[has] = d.alpha[d.off[:-1][has]].cpu().numpy() != -10
-        first = np.argmax(has[idx], axis=1)
-        out[:, k] = has[idx].any(1) & ok[idx[np.arange(len(idx)), first]]
+        hit = np.flatnonzero(has[lists.flat])               # list positions of frames with detections
+        j = np.searchsorted(hit, lists.off[:-1])            # each replicate's first such position, if in its slice
+        found = j < len(hit)
+        found[found] = hit[j[found]] < lists.off[1:][found]
+        out[found, k] = ok[lists.flat[hit[j[found]]]]
     return out
 
 
@@ -965,11 +1042,11 @@ def _stack_aps(aps):
     return out
 
 
-def _bootstrap_host(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, edges, idx):
-    """The reference implementation: the host evaluation of each replicate's lists.  [set][whole range, bins...] ->
-    {table: ap with a leading R axis}."""
+def _bootstrap_host(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys, edges, lists):
+    """The reference implementation: the host evaluation of each replicate's lists (ReplicateLists).  [set][whole
+    range, bins...] -> {table: ap with a leading R axis}."""
     per = [[] for _ in dt_sets]
-    for row in idx:
+    for row in lists:
         ev = _evaluate([gt_annos[i] for i in row], [[d[i] for i in row] for d in dt_sets], classes, tables, overlap_fn,
                        difficultys, edges, False)
         for s, e in enumerate(ev):
@@ -979,11 +1056,11 @@ def _bootstrap_host(gt_annos, dt_sets, classes, tables, overlap_fn, difficultys,
             for reps in per]
 
 
-def _bootstrap_device(st, idx, boot_aos, tables, Dn, nbins, n_off):
-    """The replicates on the device from the evaluation's set-up ``st``: each job's sorted true-positive scores and
-    each (job, frame)'s step table once (sassd_kitti_boot_prepare), then per chunk of BOOTSTRAP_CHUNK replicates their
-    thresholds and per-threshold sums (sassd_kitti_boot_eval) and eval_many's numpy tail on [R, ...] arrays.  Returns
-    _bootstrap_host's layout."""
+def _bootstrap_device(st, lists, boot_aos, tables, Dn, nbins, n_off):
+    """The replicates (ReplicateLists) on the device from the evaluation's set-up ``st``: each job's sorted
+    true-positive scores and each (job, frame)'s step table once (sassd_kitti_boot_prepare), then per chunk of
+    BOOTSTRAP_CHUNK replicates their thresholds and per-threshold sums (sassd_kitti_boot_eval) and eval_many's numpy
+    tail on [R, ...] arrays.  Returns _bootstrap_host's layout."""
     from . import ops
     K, F, C, D, M = st.K, st.F, st.C, st.Dn, st.M
     njobs = len(st.region)
@@ -999,12 +1076,14 @@ def _bootstrap_device(st, idx, boot_aos, tables, Dn, nbins, n_off):
     cs = np.concatenate([np.zeros((C * D, 1), np.int64), np.cumsum(valid, 1)], 1)
     nv = cs[:, st.gt.off[1:]] - cs[:, st.gt.off[:-1]]
     chunks = []
-    for r0 in range(0, len(idx), BOOTSTRAP_CHUNK):
-        rows = idx[r0:r0 + BOOTSTRAP_CHUNK]
-        R = len(rows)
-        w = np.bincount((rows + F * np.arange(R)[:, None]).reshape(-1), minlength=R * F).reshape(R, F)
-        n_thresh, pr = ops.kitti_boot_eval(desc, njobs, st.up(rows.astype(np.int32)), st.up(w.astype(np.int32)),
-                                           st.up((w @ nv.T).astype(np.float64)), prep, tab_off)
+    for r0 in range(0, len(lists), BOOTSTRAP_CHUNK):
+        part = lists.rows(r0, min(r0 + BOOTSTRAP_CHUNK, len(lists)))
+        R = len(part)
+        rep = np.repeat(np.arange(R), part.lengths)
+        w = np.bincount(part.flat + F * rep, minlength=R * F).reshape(R, F)
+        n_thresh, pr = ops.kitti_boot_eval(desc, njobs, st.up(part.flat.astype(np.int32)), st.up(part.off),
+                                           st.up(w.astype(np.int32)), st.up((w @ nv.T).astype(np.float64)), prep,
+                                           tab_off)
         prec = _pr_arrays(pr.cpu().numpy().reshape(R, K, C, D, 3, M, 41, 4),
                           n_thresh.cpu().numpy().reshape(R, K, C, D, 3, M), boot_aos[r0:r0 + R])
         chunks.append([[_ap_dicts([p[k] for p in prec], b * Dn, Dn, tables, n_off, True) for b in range(nbins)]
@@ -1178,16 +1257,23 @@ def _strict(a):
     return a[..., 0] if a.ndim == 4 else a
 
 
-def bootstrap_report(ev, class_names, log=print):
+def _replicates_text(nrep, groups=None):
+    """How the blocks name the replicates: "R replicates", or "R drive-level replicates of G drives" (``groups``: G
+    for a drive-level bootstrap)."""
+    return "%d replicates" % nrep if groups is None else "%d drive-level replicates of %d drives" % (nrep, groups)
+
+
+def bootstrap_report(ev, class_names, log=print, groups=None):
     """Print a set's bootstrap block (``ev``: eval_many's dict with ``bootstrap``): per table and class the 95 %
-    percentile interval of bbox / BEV / 3D / AOS AP for easy, moderate and hard at the class's strict overlap.  Returns
-    (the JSON entry {table: interval lists}, the summary fields: the moderate 3D interval per class and table)."""
+    percentile interval of bbox / BEV / 3D / AOS AP for easy, moderate and hard at the class's strict overlap
+    (``groups``: the drive count of a drive-level bootstrap, named in the headings).  Returns (the JSON entry {table:
+    interval lists}, the summary fields: the moderate 3D interval per class and table)."""
     boot = ev["bootstrap"]
     nrep = len(boot[11]["d3"])
     for t, ap in boot.items():
         tag = "AP" if t == 11 else "AP_R40" if t == 40 else "coco AP"
         for j, c in enumerate(class_names):
-            log("%s %s 95%% interval (%d replicates):" % (c, tag, nrep))
+            log("%s %s 95%% interval (%s):" % (c, tag, _replicates_text(nrep, groups)))
             for key, label in (("bbox", "bbox AP"), ("bev", "bev  AP"), ("d3", "3d   AP"), ("aos", "aos  AP")):
                 if ap[key] is None:
                     continue
@@ -1201,12 +1287,13 @@ def bootstrap_report(ev, class_names, log=print):
     return {str(t): _interval_lists(ap) for t, ap in boot.items()}, fields
 
 
-def paired_report(labels, evs, class_names, log=print):
+def paired_report(labels, evs, class_names, log=print, groups=None):
     """Print each set's moderate 3D AP against the first set's, paired over the bootstrap replicates: per set and class
-    and table the 95 % interval of the difference and the share of replicates in which the set is better.  Returns the
-    JSON list."""
+    and table the 95 % interval of the difference and the share of replicates in which the set is better (``groups``
+    as bootstrap_report's).  Returns the JSON list."""
     out = []
-    log("paired against %s (moderate 3D AP, %d replicates):" % (labels[0], len(evs[0]["bootstrap"][11]["d3"])))
+    log("paired against %s (moderate 3D AP, %s):" % (labels[0], _replicates_text(len(evs[0]["bootstrap"][11]["d3"]),
+                                                                                 groups)))
     for k in range(1, len(evs)):
         for t in evs[0]["bootstrap"]:
             name = ("R11", "R40", "COCO")[TABLES.index(t)]
@@ -1227,11 +1314,19 @@ def add_bootstrap_args(p):
                         "for several sets, each set's paired difference against the first)")
     p.add_argument("--bootstrap-seed", type=int, default=None, metavar="S",
                    help="the seed of the replicates' frame draws (default 0)")
+    p.add_argument("--bootstrap-by", default=None, choices=("frame", "drive"),
+                   help="resample the split's frames (default) or its raw drives, whole (needs --mapping)")
+    p.add_argument("--mapping", default=None, metavar="DIR",
+                   help="the KITTI object devkit's mapping/ directory (train_mapping.txt, train_rand.txt): each "
+                        "training frame's raw drive, for --bootstrap-by drive and --per-drive")
+    p.add_argument("--per-drive", action="store_true",
+                   help="also print each drive's frame count and moderate 3D AP (needs --mapping)")
 
 
 def check_bootstrap_args(p, args, unlabelled=None):
-    """Refuse --bootstrap below 1, --bootstrap without labels (``unlabelled``: the option that has none) and
-    --bootstrap-seed without --bootstrap."""
+    """Refuse --bootstrap below 1, --bootstrap, --bootstrap-by, --mapping or --per-drive without labels
+    (``unlabelled``: the option that has none), --bootstrap-seed or --bootstrap-by without --bootstrap,
+    --bootstrap-by drive or --per-drive without --mapping, and --mapping without either of them."""
     if args.bootstrap is not None:
         if args.bootstrap < 1:
             p.error("--bootstrap must be at least 1")
@@ -1239,25 +1334,91 @@ def check_bootstrap_args(p, args, unlabelled=None):
             p.error("--bootstrap needs a labelled split: %s has no labels" % unlabelled)
     elif args.bootstrap_seed is not None:
         p.error("--bootstrap-seed goes with --bootstrap")
+    for flag, given in (("--bootstrap-by", args.bootstrap_by is not None), ("--mapping", args.mapping is not None),
+                        ("--per-drive", args.per_drive)):
+        if given and unlabelled:
+            p.error("%s needs a labelled split: %s has no labels" % (flag, unlabelled))
+    if args.bootstrap_by is not None and args.bootstrap is None:
+        p.error("--bootstrap-by goes with --bootstrap")
+    if args.bootstrap_by == "drive" and args.mapping is None:
+        p.error("--bootstrap-by drive needs --mapping (the devkit's mapping/ directory)")
+    if args.per_drive and args.mapping is None:
+        p.error("--per-drive needs --mapping (the devkit's mapping/ directory)")
+    if args.mapping is not None and args.bootstrap_by != "drive" and not args.per_drive:
+        p.error("--mapping goes with --bootstrap-by drive or --per-drive")
     if args.bootstrap is not None and args.bootstrap_seed is None:
         args.bootstrap_seed = 0
+    if args.bootstrap is not None and args.bootstrap_by is None:
+        args.bootstrap_by = "frame"
 
 
-def bootstrap_kw(args, nframes):
-    """eval_many's bootstrap argument of the command's options."""
+def split_drives_of(args, ids):
+    """Each frame of ``ids``'s raw drive from --mapping (kitti_data.read_drive_mapping, split_drives), or None
+    without it."""
+    if args.mapping is None:
+        return None
+    from .kitti_data import read_drive_mapping, split_drives
+    return split_drives(read_drive_mapping(args.mapping), ids)
+
+
+def bootstrap_kw(args, nframes, drives=None):
+    """eval_many's bootstrap argument of the command's options (``drives``: split_drives_of's, for --bootstrap-by
+    drive)."""
     if args.bootstrap is None:
         return {}
+    if args.bootstrap_by == "drive":
+        return dict(bootstrap=bootstrap_groups(drives, args.bootstrap, args.bootstrap_seed))
     return dict(bootstrap=bootstrap_indices(nframes, args.bootstrap, args.bootstrap_seed))
 
 
-def pop_bootstrap(args, nframes, labels, entries):
+def bootstrap_groups_of(args, drives):
+    """The drive count G of a drive-level bootstrap (what the blocks name), None otherwise."""
+    if args.bootstrap is None or args.bootstrap_by != "drive":
+        return None
+    return len(np.unique(drives))
+
+
+def pop_bootstrap(args, nframes, labels, entries, kw=None, drives=None):
     """The --json ``bootstrap`` entry, taken out of report_sets' entries: R, seed, F, per set its label and {table:
-    intervals}, and the paired summaries against the first set (None without --bootstrap)."""
+    intervals}, and the paired summaries against the first set (None without --bootstrap).  A drive-level bootstrap
+    (``kw``: bootstrap_kw's, ``drives``: split_drives_of's) adds ``by``, the drive count ``groups`` and the replicate
+    lists' lengths (min, median, max)."""
     if args.bootstrap is None:
         return None
-    return dict(replicates=args.bootstrap, seed=args.bootstrap_seed, frames=nframes,
-                sets=[dict(label=str(l), intervals=e.pop("bootstrap")) for l, e in zip(labels, entries)],
-                paired=entries[0].pop("bootstrap_paired", []))
+    out = dict(replicates=args.bootstrap, seed=args.bootstrap_seed, frames=nframes,
+               sets=[dict(label=str(l), intervals=e.pop("bootstrap")) for l, e in zip(labels, entries)],
+               paired=entries[0].pop("bootstrap_paired", []))
+    if args.bootstrap_by == "drive":
+        n = kw["bootstrap"].lengths
+        out.update(by="drive", groups=bootstrap_groups_of(args, drives),
+                   lengths=dict(min=int(n.min()), median=float(np.median(n)), max=int(n.max())))
+    return out
+
+
+def per_drive_report(gt, dt_sets, labels, class_names, tables, drives, log=print):
+    """Print one line per drive after the tables: its name, frame count and, for every set (columns, in ``labels``
+    order), the moderate 3D AP per class of each table at the class's strict overlap.  One eval_many whose replicate r
+    is drive r's frame list (drives sorted by name), so each line is that drive's own evaluation.  Returns the --json
+    ``per_drive`` list: per drive its name, frame count and per set {table: AP dict}."""
+    names, inv = np.unique(np.asarray(drives), return_inverse=True)
+    lists = ReplicateLists([np.flatnonzero(inv.reshape(-1) == g) for g in range(len(names))])
+    evs = eval_many(gt, dt_sets, class_names, tables, bootstrap=lists)
+    tags = [("R11", "R40", "COCO")[TABLES.index(t)] for t in tables]
+    log("per drive (moderate 3D AP, %d drives; columns: %s):" % (len(names), " | ".join(str(l) for l in labels)))
+    out = []
+    for g, name in enumerate(names):
+        cols = []
+        for ev in evs:
+            d3 = [_strict(ev["bootstrap"][t]["d3"])[g] for t in tables]
+            cols.append("  ".join("%s 3d mod %s" % (c, " ".join("%s %6.2f" % (tag, a[j, 1])
+                                                              for tag, a in zip(tags, d3)))
+                                  for j, c in enumerate(class_names)))
+        log("%-32s %5d frames  %s" % (name, lists.lengths[g], " | ".join(cols)))
+        out.append(dict(drive=str(name), frames=int(lists.lengths[g]),
+                        sets=[dict(label=str(l), ap={str(t): ap_lists({k: None if v is None else v[g]
+                                                                       for k, v in ev["bootstrap"][t].items()})
+                                                     for t in tables}) for l, ev in zip(labels, evs)]))
+    return out
 
 
 def write_matches(path, labels, tables):
@@ -1270,12 +1431,13 @@ def write_matches(path, labels, tables):
     np.savez_compressed(path, **out)
 
 
-def report_sets(entries, labels, evs, class_names, noun, log=print, extra=None, ranges=None):
+def report_sets(entries, labels, evs, class_names, noun, log=print, extra=None, ranges=None, groups=None):
     """Print each evaluated set's tables (``evs``: eval_many's dicts, with table 11) under ``== label ==``, then one
     summary line per set: moderate 3D AP per class at the class's strict overlap (R11, and R40 / COCO when evaluated).
     Each set's texts and AP lists go into its dict of ``entries`` (returned).  ``extra(k, entry)`` may add to set k's
     entry after its tables and returns more summary fields.  A set evaluated with ranges or a match table also prints
-    its per-range tables, and its summary line gains range_report's fields (``ranges``: the bin edges)."""
+    its per-range tables, and its summary line gains range_report's fields (``ranges``: the bin edges).  ``groups``:
+    the drive count of a drive-level bootstrap (bootstrap_report's)."""
     summary = []
     for k, (entry, label, ev) in enumerate(zip(entries, labels, evs)):
         log("== %s ==" % label)
@@ -1297,7 +1459,7 @@ def report_sets(entries, labels, evs, class_names, noun, log=print, extra=None, 
             tp_err = tp_error_summary(ev["matches"], class_names, ranges=ranges) if "matches" in ev else None
             line += range_report(entry, ev, class_names, log, tp_err)
         if "bootstrap" in ev:
-            entry["bootstrap"], fields = bootstrap_report(ev, class_names, log)
+            entry["bootstrap"], fields = bootstrap_report(ev, class_names, log, groups)
             line += fields
         if extra is not None:
             line += extra(k, entry)
@@ -1306,8 +1468,13 @@ def report_sets(entries, labels, evs, class_names, noun, log=print, extra=None, 
     for line in summary:
         log(line)
     if len(evs) > 1 and "bootstrap" in evs[0]:
-        entries[0]["bootstrap_paired"] = paired_report(labels, evs, class_names, log)
+        entries[0]["bootstrap_paired"] = paired_report(labels, evs, class_names, log, groups)
     return entries
+
+
+def read_dirs(label_dir, result_dirs, ids, times=None):
+    """The AnnoBlocks of the label files and of every result directory over the frames ``ids`` (read_block)."""
+    return read_block(label_dir, ids, times=times), [read_block(d, ids, times=times) for d in result_dirs]
 
 
 def eval_dirs(label_dir, result_dirs, ids, classes, tables=(11,), times=None, ranges=None, match=False,
@@ -1318,8 +1485,7 @@ def eval_dirs(label_dir, result_dirs, ids, classes, tables=(11,), times=None, ra
     eval_many's list,
     one dict per directory.  ``times``: a dict whose "read", "parse" and "eval" entries accumulate seconds."""
     times = {} if times is None else times
-    gt = read_block(label_dir, ids, times=times)
-    dts = [read_block(d, ids, times=times) for d in result_dirs]
+    gt, dts = read_dirs(label_dir, result_dirs, ids, times)
     t0 = time.perf_counter()
     out = eval_many(gt, dts, classes, tables, ranges=ranges, match=match, bootstrap=bootstrap)
     times["eval"] = times.get("eval", 0.0) + time.perf_counter() - t0
@@ -1380,7 +1546,8 @@ def main(argv=None, log=print):
     python -m sassd_b200.kitti_eval --data-root DIR [--split val] --results DIR [DIR ...]
                                     [--classes Car Pedestrian Cyclist] [--r40] [--coco] [--json FILE]
                                     [--ranges EDGE EDGE [...]] [--matches FILE.npz]
-                                    [--bootstrap R [--bootstrap-seed S]]
+                                    [--bootstrap R [--bootstrap-seed S] [--bootstrap-by frame|drive]]
+                                    [--mapping DIR [--per-drive]]
 
     The labels are ``training/label_2/%06d.txt`` and the frames those of ``ImageSets/<split>.txt``; files a result
     directory holds beyond them are ignored.  Every file is read into pinned memory, copied to the device once and
@@ -1389,19 +1556,27 @@ def main(argv=None, log=print):
     evaluating.  ``--ranges`` adds each directory's tables per range bin and, with ``--matches``, the true positives'
     TP errors to its summary line; ``--matches`` writes every directory's match table.  ``--bootstrap R`` adds each
     directory's 95 % AP intervals over R bootstrap replicates of the frames (bootstrap_indices, seed
-    ``--bootstrap-seed``) and, for two or more directories, each one's paired difference against the first.  Returns
-    the result dict that ``--json`` writes."""
+    ``--bootstrap-seed``) and, for two or more directories, each one's paired difference against the first.
+    ``--mapping DIR`` is the object devkit's ``mapping/`` directory; with it ``--bootstrap-by drive`` resamples whole
+    raw drives (bootstrap_groups) and ``--per-drive`` prints each drive's frame count and moderate 3D AP, one column
+    per directory (per_drive_report).  Returns the result dict that ``--json`` writes."""
     from .kitti_data import read_split
     args = parse_args(argv)
     ids = read_split(args.data_root, args.split)
+    drives = split_drives_of(args, ids)
     tables = (11,) + ((40,) if args.r40 else ()) + (("coco",) if args.coco else ())
     times = {}
     match = args.ranges is not None or args.matches is not None
-    evs = eval_dirs(os.path.join(args.data_root, "training", "label_2"), args.results, ids, args.classes, tables, times,
-                    args.ranges, match, **bootstrap_kw(args, len(ids)))
+    gt, dts = read_dirs(os.path.join(args.data_root, "training", "label_2"), args.results, ids, times)
+    kw = bootstrap_kw(args, len(ids), drives)
+    t0 = time.perf_counter()
+    evs = eval_many(gt, dts, args.classes, tables, ranges=args.ranges, match=match, **kw)
+    times["eval"] = time.perf_counter() - t0
     entries = report_sets([dict(dir=d) for d in args.results], args.results, evs, args.classes, "directories", log,
-                          ranges=args.ranges)
-    boot = pop_bootstrap(args, len(ids), args.results, entries)
+                          ranges=args.ranges, groups=bootstrap_groups_of(args, drives))
+    boot = pop_bootstrap(args, len(ids), args.results, entries, kw, drives)
+    per_drive = (per_drive_report(gt, dts, args.results, args.classes, tables, drives, log) if args.per_drive
+                 else None)
     if args.matches:
         write_matches(args.matches, args.results, [ev["matches"] for ev in evs])
     log("frames: %d, directories: %d, read %.3f s, parse %.3f s, evaluate %.3f s" % (
@@ -1409,6 +1584,8 @@ def main(argv=None, log=print):
     result = dict(split=args.split, frames=len(ids), classes=args.classes, results=entries, times_s=times)
     if boot is not None:
         result["bootstrap"] = boot
+    if per_drive is not None:
+        result["per_drive"] = per_drive
     if args.json:
         with open(args.json, "w") as fh:
             json.dump(result, fh, indent=1)

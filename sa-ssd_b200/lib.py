@@ -118,7 +118,7 @@ _SIGNATURES = {
     "sassd_kitti_eval_match": (c_int, [ctypes.POINTER(KittiEvalDesc), P, P, P, P, P, P, c_size_t, P]),
     "sassd_kitti_eval_assign": (c_int, [ctypes.POINTER(KittiEvalDesc), c_int, c_int, P, P, P, P, P, P, P, c_size_t, P]),
     "sassd_kitti_boot_prepare": (c_int, [ctypes.POINTER(KittiEvalDesc), P, P, P, P, P, P, P, P, P, c_size_t, P]),
-    "sassd_kitti_boot_eval": (c_int, [ctypes.POINTER(KittiEvalDesc), c_int] + [P] * 15),
+    "sassd_kitti_boot_eval": (c_int, [ctypes.POINTER(KittiEvalDesc), c_int] + [P] * 16),
     "sassd_kitti_assign": (c_int, [c_int, P, P, P, P, P, P, P, P, P, P, c_int, ctypes.c_double, P, P, P]),
     "sassd_kitti_scan_labels": (c_int, [P, P, c_int, P, P, P]),
     "sassd_kitti_parse_workspace_bytes": (c_size_t, [c_int]),

@@ -615,19 +615,19 @@ def kitti_boot_prepare(desc, njobs, score_total, tab_off, ws=None):
     return scores, frames, n_scores, tab_score, tab_cnt, tab_sim, tab_n
 
 
-def kitti_boot_eval(desc, njobs, lists, weight, num_gt, prep, tab_off):
-    """Thresholds and per-threshold sums of a chunk of bootstrap replicates (lists / weight [R, F] i32, num_gt
-    [R, nclass * ndiff] f64, ``prep`` kitti_boot_prepare's tuple).  Returns (n_thresh [R, njobs] i32,
-    pr [R, njobs, 41, 4] f64)."""
-    R = lists.shape[0]
+def kitti_boot_eval(desc, njobs, lists, list_off, weight, num_gt, prep, tab_off):
+    """Thresholds and per-threshold sums of a chunk of bootstrap replicates (lists: the replicates' frames
+    concatenated, i32; list_off [R+1] i64 replicate r's slice of them; weight [R, F] i32, num_gt [R, nclass * ndiff]
+    f64, ``prep`` kitti_boot_prepare's tuple).  Returns (n_thresh [R, njobs] i32, pr [R, njobs, 41, 4] f64)."""
+    R = list_off.shape[0] - 1
     dev = lists.device
     scores, frames, n_scores, tab_score, tab_cnt, tab_sim, tab_n = prep
     thresholds = torch.empty((R, njobs, 41), dtype=torch.float64, device=dev)
     n_thresh = torch.empty((R, njobs), dtype=torch.int32, device=dev)
     pr = torch.empty((R, njobs, 41, 4), dtype=torch.float64, device=dev)
-    _call("sassd_kitti_boot_eval", None, ctypes.byref(desc), R, _ptr(lists), _ptr(weight), _ptr(num_gt), _ptr(scores),
-          _ptr(frames), _ptr(n_scores), _ptr(tab_off), _ptr(tab_score), _ptr(tab_cnt), _ptr(tab_sim), _ptr(tab_n),
-          _ptr(thresholds), _ptr(n_thresh), _ptr(pr), _stream())
+    _call("sassd_kitti_boot_eval", None, ctypes.byref(desc), R, _ptr(lists), _ptr(list_off), _ptr(weight),
+          _ptr(num_gt), _ptr(scores), _ptr(frames), _ptr(n_scores), _ptr(tab_off), _ptr(tab_score), _ptr(tab_cnt),
+          _ptr(tab_sim), _ptr(tab_n), _ptr(thresholds), _ptr(n_thresh), _ptr(pr), _stream())
     return n_thresh, pr
 
 

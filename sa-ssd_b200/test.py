@@ -3,7 +3,8 @@
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR [--split val] [--batch 16]
                               [--lidar velodyne|velodyne_reduced] [--out DIR] [--workers N] [--json FILE]
                               [--losses] [--r40] [--coco] [--ranges EDGE EDGE [...]] [--matches FILE.npz]
-                              [--bootstrap R [--bootstrap-seed S]]
+                              [--bootstrap R [--bootstrap-seed S] [--bootstrap-by frame|drive]]
+                              [--mapping DIR [--per-drive]]
     python -m sassd_b200.test CONFIG CHECKPOINT --data-root DIR --split test --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --drive DRIVE_DIR [--calib-dir DIR] --out DIR [...]
     python -m sassd_b200.test CONFIG CHECKPOINT --model CONFIG2 CHECKPOINT2 [--model ...] --data-root DIR [...]
@@ -23,7 +24,10 @@ ATE / ASE / AOE per class (kitti_eval.tp_error_summary); ``--matches FILE.npz`` 
 table (kitti_eval.match_table).  Both come from the same one evaluation, for every checkpoint and bin.
 ``--bootstrap R [--bootstrap-seed S]`` adds 95 % intervals of the AP over R bootstrap replicates of the split's frames
 (kitti_eval.eval_many(bootstrap=...)) after the tables and, for a sweep, each checkpoint's paired difference against
-the first.
+the first.  ``--mapping DIR`` reads the object devkit's ``mapping/`` directory (each training frame's raw drive,
+kitti_data.read_drive_mapping): ``--bootstrap-by drive`` then resamples whole drives (kitti_eval.bootstrap_groups)
+instead of frames, and ``--per-drive`` prints each drive's frame count and moderate 3D AP after the tables, every
+checkpoint of a sweep a column (kitti_eval.per_drive_report).
 
 ``--losses`` (labelled splits): every frame also carries its ground truth (kitti_data.gt_from_anno) and the captured
 step computes SA-SSD's six losses beside the detections (detect_stream(losses=True)); the result files and AP tables
@@ -227,6 +231,8 @@ def run(args, log=print):
         split = KittiSplit(args.data_root, args.split, args.lidar)
         if not split.ids:
             raise ValueError("split %s of %s lists no frames" % (args.split, args.data_root))
+    from .kitti_eval import split_drives_of
+    drives = split_drives_of(args, split.ids)       # read before detection: a bad mapping fails fast
     cfg = S.Config.fromfile(args.config)
     rank, world, local = D.init_from_env()
     batches = rank_batches(split.ids, rank, world, args.batch)
@@ -314,20 +320,25 @@ def run(args, log=print):
         _write_json(args.json, result)
         D.barrier()
         return result
-    from .kitti_eval import (ap_lists, bootstrap_kw, bootstrap_report, eval_many, pop_bootstrap, range_report,
-                             read_block, tp_error_summary, write_matches)
+    from .kitti_eval import (ap_lists, bootstrap_groups_of, bootstrap_kw, bootstrap_report, eval_many,
+                             per_drive_report, pop_bootstrap, range_report, read_block, tp_error_summary,
+                             write_matches)
     gt = read_block(os.path.join(split.dir, "label_2"), split.ids)
+    boot_kw = bootstrap_kw(args, len(split.ids), drives)
+    groups = bootstrap_groups_of(args, drives)
     if sweep:
-        result["checkpoints"] = _report_sweep(args, gt, dt_sets, class_names, per_batch, log)
-        boot = pop_bootstrap(args, len(split.ids), [os.path.basename(p) for p in [args.checkpoint] + args.checkpoints],
-                             result["checkpoints"])
+        labels = [os.path.basename(p) for p in [args.checkpoint] + args.checkpoints]
+        result["checkpoints"] = _report_sweep(args, gt, dt_sets, class_names, per_batch, log, boot_kw, groups)
+        boot = pop_bootstrap(args, len(split.ids), labels, result["checkpoints"], boot_kw, drives)
         if boot is not None:
             result["bootstrap"] = boot
+        if args.per_drive:
+            result["per_drive"] = per_drive_report(gt, dt_sets, labels, class_names, _tables(args), drives, log)
         log(rate)
         _write_json(args.json, result)
         D.barrier()
         return result
-    ev = eval_many(gt, [dt_annos], class_names, _tables(args), **_range_kw(args), **bootstrap_kw(args, len(split.ids)))[0]
+    ev = eval_many(gt, [dt_annos], class_names, _tables(args), **_range_kw(args), **boot_kw)[0]
     text, ap = ev[11]
     log(text, end="")
     result.update(text=text, ap=ap_lists(ap))
@@ -342,12 +353,15 @@ def run(args, log=print):
         fields = range_report(result, ev, class_names, log,
                               tp_error_summary(ev["matches"], class_names, ranges=args.ranges))
     if "bootstrap" in ev:
-        intervals, more = bootstrap_report(ev, class_names, log)
+        intervals, more = bootstrap_report(ev, class_names, log, groups)
         fields += more
-        result["bootstrap"] = dict(replicates=args.bootstrap, seed=args.bootstrap_seed, frames=len(split.ids),
-                                   sets=[dict(label=os.path.basename(args.checkpoint), intervals=intervals)], paired=[])
+        result["bootstrap"] = pop_bootstrap(args, len(split.ids), [os.path.basename(args.checkpoint)],
+                                            [dict(bootstrap=intervals)], boot_kw, drives)
     if fields:
         log("summary: " + "  ".join(fields))
+    if args.per_drive:
+        result["per_drive"] = per_drive_report(gt, [dt_annos], [os.path.basename(args.checkpoint)], class_names,
+                                               _tables(args), drives, log)
     if "matches" in ev:
         if args.matches:
             write_matches(args.matches, [os.path.basename(args.checkpoint)], [ev["matches"]])
@@ -381,11 +395,11 @@ def _loss_means(per_batch, batch, log):
                 losses_per_batch=[dict(zip(ops.LOSS_KEYS, v)) for v in per_batch])
 
 
-def _report_sweep(args, gt, dt_sets, class_names, per_batch, log):
-    """Evaluate and print each checkpoint of a sweep (one kitti_eval.eval_many for all of them), then one summary line
-    per checkpoint: moderate 3D AP per class at the class's strict overlap (R11, and R40 with --r40), the moderate 3D
-    COCO-style AP with --coco, and the rpn_cls_loss / loss_cls means.  Returns the result dict's ``checkpoints``
-    list."""
+def _report_sweep(args, gt, dt_sets, class_names, per_batch, log, boot_kw, groups):
+    """Evaluate and print each checkpoint of a sweep (one kitti_eval.eval_many for all of them, ``boot_kw`` its
+    bootstrap argument, ``groups`` the drive count of a drive-level bootstrap), then one summary line per checkpoint:
+    moderate 3D AP per class at the class's strict overlap (R11, and R40 with --r40), the moderate 3D COCO-style AP
+    with --coco, and the rpn_cls_loss / loss_cls means.  Returns the result dict's ``checkpoints`` list."""
     from . import ops
     from .kitti_eval import eval_many, report_sets
     paths = [args.checkpoint] + args.checkpoints
@@ -397,12 +411,11 @@ def _report_sweep(args, gt, dt_sets, class_names, per_batch, log):
         entry.update(_loss_means([v[k * n:(k + 1) * n] for v in per_batch], args.batch, log))
         return ["rpn_cls_loss %.6f loss_cls %.6f" % (entry["losses"]["rpn_cls_loss"], entry["losses"]["loss_cls"])]
     from .kitti_eval import write_matches
-    from .kitti_eval import bootstrap_kw
-    evs = eval_many(gt, dt_sets, class_names, _tables(args), **_range_kw(args), **bootstrap_kw(args, len(gt)))
+    evs = eval_many(gt, dt_sets, class_names, _tables(args), **_range_kw(args), **boot_kw)
     if args.matches:
         write_matches(args.matches, [os.path.basename(p) for p in paths], [ev["matches"] for ev in evs])
     return report_sets([dict(path=p) for p in paths], [os.path.basename(p) for p in paths], evs, class_names,
-                       "checkpoints", log, losses, ranges=args.ranges)
+                       "checkpoints", log, losses, ranges=args.ranges, groups=groups)
 
 
 def _write_json(path, result):
