@@ -70,11 +70,45 @@ def _segment_hit(p1, p2, i, j):
     return None
 
 
-def rotated_intersection(box1, box2):
-    """Area of the intersection polygon of two rotated boxes (x, y, dx, dy, angle) — `inter`, :366-380."""
+def _clipped_area(p1, p2, amin):
+    """csrc/kitti_eval.cu clipped_area: Sutherland-Hodgman clipping of p1 against p2's edges in float64 (Python float
+    operations in the kernel's order), rounded to float32 and clamped to [0, amin]."""
+    sx, sy = [float(x) for x, _ in p1], [float(y) for _, y in p1]
+    s2 = 0.0
+    for i in range(4):
+        k = (i + 1) % 4
+        s2 += float(p2[i][0]) * float(p2[k][1]) - float(p2[k][0]) * float(p2[i][1])
+    if not s2 != 0.0:
+        return F(0)
+    sg = 1.0 if s2 > 0.0 else -1.0
+    for e in range(4):
+        if not sx:
+            break
+        ax, ay = float(p2[e][0]), float(p2[e][1])
+        ex, ey = float(p2[(e + 1) % 4][0]) - ax, float(p2[(e + 1) % 4][1]) - ay
+        d = [sg * (ex * (y - ay) - ey * (x - ax)) for x, y in zip(sx, sy)]
+        n, tx, ty = len(sx), [], []
+        for i in range(n):
+            k = 0 if i + 1 == n else i + 1
+            if d[i] >= 0.0 and len(tx) < 16:
+                tx.append(sx[i]); ty.append(sy[i])
+            if (d[i] >= 0.0) != (d[k] >= 0.0) and len(tx) < 16:
+                t = d[i] / (d[i] - d[k])
+                tx.append(sx[i] + t * (sx[k] - sx[i])); ty.append(sy[i] + t * (sy[k] - sy[i]))
+        sx, sy = tx, ty
+    a = 0.0
+    for i in range(len(sx)):
+        k = 0 if i + 1 == len(sx) else i + 1
+        a += sx[i] * sy[k] - sx[k] * sy[i]
+    r = F(abs(a) * 0.5)
+    return r if r < amin else amin
+
+
+def collected_points(box1, box2):
+    """The points quadrilateral_intersection (:317-337) collects: corners inside the other box, then edge hits."""
     p1, p2 = _corners(box1), _corners(box2)
     pts = []
-    for i in range(4):                                   # :317-337
+    for i in range(4):
         if _inside(p1[i][0], p1[i][1], p2):
             pts.append(p1[i])
         if _inside(p2[i][0], p2[i][1], p1):
@@ -84,6 +118,16 @@ def rotated_intersection(box1, box2):
             hit = _segment_hit(p1, p2, i, j)
             if hit is not None:
                 pts.append(hit)
+    return p1, p2, pts
+
+
+def rotated_intersection(box1, box2):
+    """Area of the intersection polygon of two rotated boxes (x, y, dx, dy, angle) — `inter`, :366-380.  Past 8
+    collected points, where the reference overruns its 8-point buffer and is undefined, the kernel's fp64 clipping
+    (csrc/kitti_eval.cu, the comment at pts[24])."""
+    p1, p2, pts = collected_points(box1, box2)
+    if len(pts) > 8:
+        return _clipped_area(p1, p2, min(abs(F(box1[2]) * F(box1[3])), abs(F(box2[2]) * F(box2[3]))))
     n = len(pts)
     if n > 0:                                            # :169-206 sort by a monotone key of the polar angle
         cx = F(sum(p[0] for p in pts) / F(n))

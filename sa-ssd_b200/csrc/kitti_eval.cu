@@ -63,8 +63,58 @@ __device__ bool segment_hit(const P2f* p1, const P2f* p2, int i, int j, P2f* out
     return true;
 }
 
+// Intersection area of the quadrilaterals p1 and p2 by Sutherland-Hodgman clipping of p1 against p2's edges in fp64,
+// rounded to float and clamped to [0, amin].  Used only where the reference's result is undefined (see pts[24]
+// below).  A convex input gives at most 8 vertices; the 16-entry buffers only bound what rounding can add.
+__device__ float clipped_area(const P2f* p1, const P2f* p2, float amin) {
+    double sx[16], sy[16], tx[16], ty[16], d[16];
+    int n = 4;
+    for (int i = 0; i < 4; ++i) { sx[i] = p1[i].x; sy[i] = p1[i].y; }
+    double s2 = 0.0;      // twice p2's signed area: the side its interior is on
+    for (int i = 0; i < 4; ++i) {
+        const int k = (i + 1) & 3;
+        s2 = __dadd_rn(s2, __dsub_rn(__dmul_rn(p2[i].x, p2[k].y), __dmul_rn(p2[k].x, p2[i].y)));
+    }
+    if (!(s2 != 0.0)) return 0.f;
+    const double sg = s2 > 0.0 ? 1.0 : -1.0;
+    for (int e = 0; e < 4 && n > 0; ++e) {
+        const double ax = p2[e].x, ay = p2[e].y;
+        const double ex = __dsub_rn(p2[(e + 1) & 3].x, ax), ey = __dsub_rn(p2[(e + 1) & 3].y, ay);
+        for (int i = 0; i < n; ++i)
+            d[i] = sg * __dsub_rn(__dmul_rn(ex, __dsub_rn(sy[i], ay)), __dmul_rn(ey, __dsub_rn(sx[i], ax)));
+        int m = 0;
+        for (int i = 0; i < n; ++i) {
+            const int k = i + 1 == n ? 0 : i + 1;
+            if (d[i] >= 0.0 && m < 16) { tx[m] = sx[i]; ty[m] = sy[i]; ++m; }
+            if ((d[i] >= 0.0) != (d[k] >= 0.0) && m < 16) {
+                const double t = __ddiv_rn(d[i], __dsub_rn(d[i], d[k]));
+                tx[m] = __dadd_rn(sx[i], __dmul_rn(t, __dsub_rn(sx[k], sx[i])));
+                ty[m] = __dadd_rn(sy[i], __dmul_rn(t, __dsub_rn(sy[k], sy[i])));
+                ++m;
+            }
+        }
+        for (int i = 0; i < m; ++i) { sx[i] = tx[i]; sy[i] = ty[i]; }
+        n = m;
+    }
+    double a = 0.0;
+    for (int i = 0; i < n; ++i) {
+        const int k = i + 1 == n ? 0 : i + 1;
+        a = __dadd_rn(a, __dsub_rn(__dmul_rn(sx[i], sy[k]), __dmul_rn(sx[k], sy[i])));
+    }
+    const float r = __double2float_rn(__dmul_rn(fabs(a), 0.5));
+    return r < amin ? r : amin;
+}
+
 // area of the intersection polygon of two rotated boxes (x, y, dx, dy, angle) (:366-380)
 __device__ float rotated_intersection(const float* b1, const float* b2) {
+    // The reference collects the points into a 16-float local array, 8 points.  Where edges of the two boxes
+    // coincide up to rounding (a box against itself turned by pi, or by 1e-7) nearly parallel edges pass its
+    // crossing tests and it collects up to 24 points (8 corners, 16 hits): it writes past its array, so its value
+    // there is undefined, and its own arithmetic on those points gives intersections above the boxes' areas.
+    // pts[24] holds every point the collection can make.  Up to 8 points the result is the reference's, bit for
+    // bit; past 8 it is clipped_area's, which is within 2^-24 A + 2^-40 (M + 1)^2 of min(A, amin), A the exact
+    // intersection of the same float corners, M their largest |coordinate| and amin the smaller |dx * dy|; it never
+    // exceeds amin and is never negative or NaN for finite boxes (tests/test_kitti_eval_geometry.py).
     P2f p1[4], p2[4], pts[24];
     box_corners(b1, p1);
     box_corners(b2, p2);
@@ -78,6 +128,7 @@ __device__ float rotated_intersection(const float* b1, const float* b2) {
             P2f h;
             if (segment_hit(p1, p2, i, j, &h)) pts[n++] = h;
         }
+    if (n > 8) return clipped_area(p1, p2, fminf(fabsf(mul(b1[2], b1[3])), fabsf(mul(b2[2], b2[3]))));
     if (n > 0) {      // sort by a monotone key of the polar angle about the centroid (:169-206)
         float cx = 0.f, cy = 0.f;
         for (int i = 0; i < n; ++i) { cx = add(cx, pts[i].x); cy = add(cy, pts[i].y); }

@@ -30,6 +30,14 @@ __device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a,
 __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
 __device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
 
+// The reference's min(a, b) and max(a, b) (numba / Python: the second argument when it compares below / above the
+// first, else the first), in place of fmin / fmax, which drop a NaN from either side: a NaN coordinate then gives the
+// reference's overlap, NaN or a number, whichever side it is on.  In the DontCare test the order cannot change the
+// outcome (a NaN detection coordinate makes the quotient's denominator, the detection's area, NaN), but it is kept
+// the reference's there too, so that every min / max of the evaluation reads the same.
+__device__ __forceinline__ double ref_min(double a, double b) { return b < a ? b : a; }
+__device__ __forceinline__ double ref_max(double a, double b) { return b > a ? b : a; }
+
 // ------------------------------------------------------------------------------------------------------ flags
 // The ground distance of a camera-frame row (x, y, z, ...): sqrt(x * x + z * z), numpy's operation order.
 __device__ __forceinline__ double ground_range(const double* cam) {
@@ -104,8 +112,8 @@ __global__ void eval_overlaps_kernel(int nsets, int nframes, const int32_t* __re
             // image_box_overlap(dt, gt, criterion=-1) (kitti_eval.py:95-122, vectorised in kitti_eval.py)
             const double* b4 = dt_bbox + 4 * (long long)(d0 + j);
             const double* q4 = gt_bbox + 4 * (long long)(g0 + i);
-            const double iw = dsub(fmin(b4[2], q4[2]), fmax(b4[0], q4[0]));
-            const double ih = dsub(fmin(b4[3], q4[3]), fmax(b4[1], q4[1]));
+            const double iw = dsub(ref_min(b4[2], q4[2]), ref_max(b4[0], q4[0]));
+            const double ih = dsub(ref_min(b4[3], q4[3]), ref_max(b4[1], q4[1]));
             double v = 0.0;
             if (iw > 0 && ih > 0) {
                 const double area_b = dmul(dsub(b4[2], b4[0]), dsub(b4[3], b4[1]));
@@ -120,8 +128,9 @@ __global__ void eval_overlaps_kernel(int nsets, int nframes, const int32_t* __re
             const double* bc = dt_cam + 7 * (long long)(d0 + j);
             const double* qc = gt_cam + 7 * (long long)(g0 + i);
             const float rinc = bev_inter[o0 + p];
-            const double hw = dsub(fmin(bc[1], qc[1]), fmax(dsub(bc[1], bc[4]), dsub(qc[1], qc[4])));
-            double v3 = 0.0;
+            const double hw = dsub(ref_min(bc[1], qc[1]), ref_max(dsub(bc[1], bc[4]), dsub(qc[1], qc[4])));
+            // a BEV intersection that is not > 0 (0 or NaN) is kept, as d3_box_overlap_kernel leaves it
+            double v3 = rinc > 0.f ? 0.0 : (double)rinc;
             if (rinc > 0.f && hw > 0) {
                 const double inc = dmul(hw, (double)rinc);
                 const double a1 = dmul(dmul(bc[3], bc[4]), bc[5]), a2 = dmul(dmul(qc[3], qc[4]), qc[5]);
@@ -399,9 +408,9 @@ __device__ void frame_statistics(const Frame& fr, int metric, double min_ov, dou
             for (int j = 0; j < fr.nd; ++j) {
                 if (asg[j * S] || fr.idt[j] == -1 || fr.idt[j] == 1 || fr.score[j] < thresh) continue;
                 const double* b = fr.dt_bbox + 4 * j;    // image_box_overlap with criterion 0
-                const double iw = dsub(fmin(b[2], q[2]), fmax(b[0], q[0]));
+                const double iw = dsub(ref_min(b[2], q[2]), ref_max(b[0], q[0]));
                 if (iw <= 0) continue;
-                const double ih = dsub(fmin(b[3], q[3]), fmax(b[1], q[1]));
+                const double ih = dsub(ref_min(b[3], q[3]), ref_max(b[1], q[1]));
                 if (ih <= 0) continue;
                 if (ddiv(dmul(iw, ih), dmul(dsub(b[2], b[0]), dsub(b[3], b[1]))) > min_ov) {
                     asg[j * S] = 1;

@@ -110,19 +110,30 @@ def rotate_iou_gpu_eval(boxes, query_boxes, criterion=-1, device_id=0):
     return _rotated_overlaps([boxes], [query_boxes], criterion)[0]
 
 
+def _min(a, b):
+    """The reference's min(a, b) (numba's and Python's): b if b < a else a, so a NaN counts only as the first argument."""
+    return np.where(b < a, b, a)
+
+
+def _max(a, b):
+    """The reference's max(a, b): b if b > a else a."""
+    return np.where(b > a, b, a)
+
+
 def image_box_overlap(boxes, query_boxes, criterion=-1):
-    """Axis-aligned 2-D overlap, kitti_eval.py:95-122, vectorised (same expressions per element)."""
+    """Axis-aligned 2-D overlap, kitti_eval.py:95-122, vectorised (same expressions per element, min / max in the
+    reference's argument order, which decides what a NaN coordinate gives)."""
     b, q = boxes[:, None, :], query_boxes[None, :, :]
-    iw = np.minimum(b[..., 2], q[..., 2]) - np.maximum(b[..., 0], q[..., 0])
-    ih = np.minimum(b[..., 3], q[..., 3]) - np.maximum(b[..., 1], q[..., 1])
+    iw = _min(b[..., 2], q[..., 2]) - _max(b[..., 0], q[..., 0])
+    ih = _min(b[..., 3], q[..., 3]) - _max(b[..., 1], q[..., 1])
     area_b = (b[..., 2] - b[..., 0]) * (b[..., 3] - b[..., 1])
     area_q = (q[..., 2] - q[..., 0]) * (q[..., 3] - q[..., 1])
     if criterion == -1:
         ua = area_b + area_q - iw * ih
     elif criterion == 0:
-        ua = area_b + 0 * area_q
+        ua = np.broadcast_to(area_b, iw.shape)      # the other box's area, NaN or not, takes no part
     elif criterion == 1:
-        ua = area_q + 0 * area_b
+        ua = np.broadcast_to(area_q, iw.shape)
     else:
         ua = np.ones_like(iw)
     hit = (iw > 0) & (ih > 0)
@@ -136,20 +147,21 @@ def _d3_from_bev(boxes, qboxes, rinc, criterion=-1):
     # rinc stays float32 (rotate_iou_gpu_eval returns its float32 working copy's dtype) and the quotient is stored
     # back into it, i.e. rounded to float32, exactly as d3_box_overlap_kernel does
     rinc = np.asarray(rinc, np.float32)
-    iw = (np.minimum(boxes[:, None, 1], qboxes[None, :, 1])
-          - np.maximum(boxes[:, None, 1] - boxes[:, None, 4], qboxes[None, :, 1] - qboxes[None, :, 4]))
+    iw = (_min(boxes[:, None, 1], qboxes[None, :, 1])
+          - _max(boxes[:, None, 1] - boxes[:, None, 4], qboxes[None, :, 1] - qboxes[None, :, 4]))
     a1 = (boxes[:, 3] * boxes[:, 4] * boxes[:, 5])[:, None]
     a2 = (qboxes[:, 3] * qboxes[:, 4] * qboxes[:, 5])[None, :]
     inc = iw * rinc
     if criterion == -1:
         ua = a1 + a2 - inc
     elif criterion == 0:
-        ua = a1 + 0 * a2
+        ua = np.broadcast_to(a1, inc.shape)         # the other box's volume, NaN or not, takes no part
     elif criterion == 1:
-        ua = a2 + 0 * a1
+        ua = np.broadcast_to(a2, inc.shape)
     else:
         ua = np.ones_like(inc)
-    out = np.zeros(rinc.shape, np.float32)
+    # a pair whose BEV intersection is not > 0 (0 or NaN) keeps it; one whose heights do not overlap gets 0
+    out = np.where(rinc > 0, np.float32(0), rinc)
     hit = (rinc > 0) & (iw > 0)
     out[hit] = (inc[hit] / ua[hit]).astype(np.float32)
     return out
